@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""bench.py -- restarts/sec of the batched factorize hot path on B200 (BASELINE.json metric).
+"""bench.py -- restarts/sec of the batched factorize hot path on H100 (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload c3|c2] [--scaling strong|weak]
+                    [--dump-outputs DIR]
 
-Workload (default c3 = BASELINE.json configs[2], the north-star target; it fits one B200): synthetic 50 000 cells x
+Workload (default c3 = BASELINE.json configs[2], the north-star target; it fits one 80 GB H100): synthetic 50 000 cells x
 2 000 HVG, K = 5..13 x 100 seeds = 900 restarts, solver 'mu' (Frobenius), tol 1e-4, max_iter 1000 -- the reference's
 own restart loop (cnmf.py:735-745) with its own seed rule (cnmf.py:597-610).  `--workload c2` = configs[1]
 (20 000 x 2 000, K=10 x 100).  One "step" = factorizing the WHOLE job table to convergence.
@@ -18,11 +19,17 @@ Printed JSON (rank 0): `value` = restarts/s with X resident in HBM (random init 
 left in HBM); `e2e` = the same through the public call with HOST buffers (H2D of X and device-side preparation, the
 solve, the all-gather, D2H of all spectra inside the timed region); `with_consensus` = factorize + all-gather +
 cNMF.consensus numerics for every K (Ks sharded over the ranks) with its HBM roofline; `roofline` = the dominant
-kernel (the batched tcgen05 GEMM) from CUDA events inside the timed region (recorded on rank 0); `cpu_baseline` / `cd_default` = the
+kernel (the batched wgmma GEMM) from CUDA events inside the timed region (recorded on rank 0); `cpu_baseline` / `cd_default` = the
 reference's own scikit-learn call timed on the host cores.
 `--impl reference` times the reference's CPU implementation (oracle/reference_path.py: the reference's call
 sequence on scikit-learn, float64): one restart of the job table to convergence per step, K cycling through the
 sweep, on the best thread count of a short sweep.
+
+`--dump-outputs DIR` writes, after the timed steps, what the last timed step computed (rank 0): `spectra.npy`
+(float32, the stacked spectra of a fixed seeded sample of the job table's restarts, whole table when it fits 48 MB),
+`spectra_jobs.npy` (their job indices) and `n_iter.npy` (iteration count of every restart of the table, in job order,
+gathered from all ranks).
+The inputs are seeded, so two builds given the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -37,7 +44,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-METRIC = "NMF restarts/sec on NxG counts, K-sweep x100 seeds, 1/2/4/8 B200 vs sklearn CPU"
+METRIC = "NMF restarts/sec on NxG counts, K-sweep x100 seeds, 1/2/4/8 H100 vs sklearn CPU"
 WORKLOADS = {
     "c3": dict(n_cells=50000, n_genes=2000, ks=list(range(5, 14)), n_iter=100,
                desc="c3 = BASELINE configs[2] (north-star target): synthetic 50000x2000 (Poisson counts / gene std), "
@@ -78,7 +85,7 @@ def job_table(name, world, scaling):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -129,14 +136,14 @@ def measured_peaks():
         m = json.load(open(p))
         return m.get("bf16_tflops_sustained", m.get("bf16_tflops")) / 2.0, \
             "MEASURED_PEAKS.json bf16_tflops_sustained/2 (dense TF32 = half the bf16 rate), of measured"
-    return 1400.0 / 2.0, "fallback 1.4 PFLOP/s sustained bf16 / 2, of fallback"
+    return 989.0 / 2.0, "H100 SXM data sheet 989 TFLOP/s dense bf16 / 2 (700 W card; not a measured rate), of fallback"
 
 
 def measured_hbm():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (copy bandwidth), of measured"
-    return 6650.0, "fallback 6.65 TB/s copy bandwidth, of fallback"
+    return 3350.0, "H100 SXM data sheet 3.35 TB/s HBM3 (not a measured rate), of fallback"
 
 
 def host_threads():
@@ -213,6 +220,27 @@ def consensus_bytes(R, Rk, G, N, G_all, K, lloyd_iters, refit_iters):
     return 4.0 * b
 
 
+DUMP_SPECTRA_BYTES = 48 << 20
+
+
+def dump_outputs(out_dir, sharded, jobs_iter):
+    """The last timed step's results: spectra of a seeded sample of restarts (all of them when they fit), n_iter of every
+    restart.  jobs_iter: per rank, (its job indices, their n_iter)."""
+    os.makedirs(out_dir, exist_ok=True)
+    spectra = sharded.host()
+    jobs = np.arange(len(spectra))
+    total = sum(s.size for s in spectra) * 4
+    if total > DUMP_SPECTRA_BYTES:
+        keep = int(len(jobs) * DUMP_SPECTRA_BYTES / total)
+        jobs = np.sort(np.random.RandomState(0).choice(jobs, keep, replace=False))
+    np.save(os.path.join(out_dir, "spectra.npy"), np.vstack([spectra[j] for j in jobs]).astype(np.float32))
+    np.save(os.path.join(out_dir, "spectra_jobs.npy"), jobs.astype(np.float64))
+    n_iter = np.zeros(len(spectra), np.float64)
+    for jobs_r, iters_r in jobs_iter:
+        n_iter[np.asarray(jobs_r, dtype=np.int64)] = iters_r
+    np.save(os.path.join(out_dir, "n_iter.npy"), n_iter)
+
+
 def run_ours(args, rank, world, local):
     import torch
     import torch.distributed as dist
@@ -234,7 +262,7 @@ def run_ours(args, rank, world, local):
     eng = Engine(local)
     comm = SpectraComm(eng) if world > 1 else None
     # Python's cyclic collector walks every object of every imported package (torch, pandas, sklearn: ~10^6) when a
-    # generation-2 collection fires -- 60-90 ms at a random point of a timed region (seen in tools/probe_stalls.py).
+    # generation-2 collection fires -- tens of ms at a random point of a timed region (tools/probe_stalls.py finds such stalls).
     # Everything alive now is set-up state: move it out of the collector's reach.
     import gc
     gc.collect()
@@ -269,16 +297,25 @@ def run_ours(args, rank, world, local):
         clocks.start()
     launches0 = eng.launch_count
     # per-launch CUDA events (the roofline's kernel times) on the rank that reports them; on the other ranks they would
-    # only add their ~3 us per launch to a max-over-ranks time nobody reads them from
+    # only add their per-launch cost to a max-over-ranks time nobody reads them from
     eng.profile(rank == 0)
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     sync_all()
     e0.record()
     n_iter = None
     for _ in range(args.steps):
-        _, n_iter, my_jobs = step_resident()
+        sharded, n_iter, my_jobs = step_resident()
     e1.record()
     sync_all()
+    if args.dump_outputs:
+        mine = ([int(j) for j in my_jobs], [int(x) for x in n_iter])
+        jobs_iter = [mine]
+        if world > 1:
+            jobs_iter = [None] * world
+            dist.all_gather_object(jobs_iter, mine)
+        if rank == 0:
+            dump_outputs(args.dump_outputs, sharded, jobs_iter)
+    del sharded
     ms = max_over_ranks(e0.elapsed_time(e1))
     gemm_ms, gemm_launches, gemm_flops = eng.profile_get(0)
     upd_ms, upd_launches, upd_bytes = eng.profile_get(1)
@@ -395,16 +432,12 @@ def run_ours(args, rank, world, local):
         return
 
     peak, peak_src = measured_peaks()
-    if f16:           # kind::f16 runs at the bf16 rate: the denominator is the measured bf16 figure itself
-        peak, peak_src = 2.0 * peak, peak_src.replace("/2 (dense TF32 = half the bf16 rate)", " (kind::f16 = the bf16 rate)")
+    if f16:           # f16 MMAs run at the bf16 rate: the denominator is the bf16 figure itself
+        peak, peak_src = 2.0 * peak, peak_src.replace("/2 (dense TF32 = half the bf16 rate)", " (f16 = the bf16 rate)").replace(
+            "bf16 / 2", "bf16 (f16 = the bf16 rate)")
     hbm_peak, hbm_src = measured_hbm()
     upd_gbs = upd_bytes / (upd_ms * 1e-3) / 1e9 if upd_ms > 0 else 0.0
     achieved = gemm_flops / (gemm_ms * 1e-3) / 1e12 if gemm_ms > 0 else 0.0
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "gemm_traffic.json")
-    if os.path.exists(tp):
-        tj = json.load(open(tp))
-        traffic = tj.get("dram_bytes_per_launch_f16" if f16 else "dram_bytes_per_launch", tj.get("dram_bytes_per_launch"))
     out = {
         "metric": METRIC, "value": value, "unit": "restarts/s", "n_gpus": world, "steps": args.steps,
         "warmup": args.warmup, "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": args.scaling,
@@ -418,8 +451,8 @@ def run_ours(args, rank, world, local):
                 "ms_per_step": {k_: v_ / args.steps for k_, v_ in phases.items()},
                 "note": "public call with host buffers: Engine.dataset(X host) + parallel.factorize_sharded + D2H of all spectra"},
         "gpu_launches": int(launches),
-        "roofline": {"bound": "tensor", "kernel": "gemm_tf32x3_kernel<256,%s>" % ("3,exact-B,kind::f16" if f16 else "3,exact-B" if passes == 2 else "2,general"),
-                     "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak, "traffic": traffic,
+        "roofline": {"bound": "tensor", "kernel": "gemm_tf32x3_kernel<%s>" % ("4,exact-B,f16" if f16 else "4,exact-B" if passes == 2 else "3,general"),
+                     "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak, "traffic": None,
                      "mma_passes": passes, "mma_frac": passes * achieved / peak,
                      "note": "achieved = algorithmic 2*M*N*K per launch (counted once, not %dx for the passes) / "
                              "CUDA-event launch time; %d launches, %.1f ms of %.1f ms timed (rank 0); peak = %s; X %s" % (
@@ -472,8 +505,12 @@ def main():
     ap.add_argument("--no-consensus", action="store_true")
     ap.add_argument("--no-cd", action="store_true")
     ap.add_argument("--precision", type=str, default="f16x2", choices=["f16x2", "tf32x3", "tf32x3-general", "fp32"],
-                    help="f16x2 (default): 2 kind::f16 passes when X is scaled integer counts, else 3 kind::tf32 passes; tf32x3: 2 / 3 kind::tf32 passes")
+                    help="f16x2 (default): 2 f16 passes when X is scaled integer counts, else 3 tf32 passes; tf32x3: 2 / 3 tf32 passes")
+    ap.add_argument("--dump-outputs", type=str, default=None, metavar="DIR",
+                    help="write what the last timed step computed to DIR/<name>.npy (see the module docstring)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))

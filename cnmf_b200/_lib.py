@@ -2,7 +2,7 @@
 
 The CUDA library is the product: there is no Python / numpy / torch fallback.  Importing this
 module never needs a GPU (so CPU-only hosts can check the ABI), but every compute entry point
-raises ``CnmfError`` when no sm_100 device is present.
+raises ``CnmfError`` when no sm_90 (H100) device is present.
 """
 import ctypes
 import os

@@ -1,9 +1,9 @@
-"""In-tree build of libcnmf_b200.so (nvcc, sm_100a only).
+"""In-tree build of libcnmf_b200.so (nvcc, sm_90a: H100).
 
     python -m cnmf_b200.build [--force]
 
 nvcc cross-compiles without a GPU.  Objects go to build/ (git-ignored), the shared library to
-cnmf_b200/libcnmf_b200.so (git-ignored but NOT gpurun-ignored, so it travels to the GPU box).
+cnmf_b200/libcnmf_b200.so (git-ignored).
 """
 import concurrent.futures
 import os
@@ -17,8 +17,8 @@ OBJ_DIR = os.path.join(ROOT, "build", "obj")
 LIB_PATH = os.path.join(HERE, "libcnmf_b200.so")
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH + [ "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC,-ffp-contract=off", "--expt-relaxed-constexpr",
 ]
 
@@ -65,8 +65,7 @@ def build(force=False, verbose=True):
                 if verbose:
                     print("compiled", os.path.relpath(src, ROOT))
     if jobs or not os.path.exists(LIB_PATH):
-        cmd = [NVCC, "-shared", "-o", LIB_PATH] + objs + ["-gencode", "arch=compute_100a,code=sm_100a",
-                                                          "-Xcompiler", "-fPIC", "-lpthread", "-ldl"]
+        cmd = [NVCC, "-shared", "-o", LIB_PATH] + objs + ARCH + ["-Xcompiler", "-fPIC", "-lpthread", "-ldl"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("link failed\n" + r.stdout + r.stderr)

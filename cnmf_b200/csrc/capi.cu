@@ -163,8 +163,8 @@ int cnmf_create(cnmf_handle_t* out, int device) {
   CNMF_CUDA_CHECK(cudaSetDevice(device));
   cudaDeviceProp prop;
   CNMF_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    set_last_error("cnmf_b200 is built for sm_100a only; device reports sm_" + std::to_string(prop.major) +
+  if (prop.major != 9 || prop.minor != 0) {
+    set_last_error("cnmf_b200 is built for sm_90a only; device reports sm_" + std::to_string(prop.major) +
                    std::to_string(prop.minor));
     return -3;
   }
@@ -308,7 +308,7 @@ static int dataset_finish(cnmf_dataset_s* d, cudaStream_t s) {
       CNMF_TRY(launch_build_counts(d->X, d->n_rows, d->n_cols, d->ld_c, d->row_scale, d->col_scale, d->X_hi, s));
       CNMF_TRY(launch_transpose(d->X_hi, d->n_rows, d->n_cols, d->ld_c, d->Xt_hi, nullptr, nullptr, d->ld_r, s));
       h->launches += 2;
-      if (d->want_f16) {       // counts <= 2048 are exact in fp16: the B operands of the kind::f16 products
+      if (d->want_f16) {       // counts <= 2048 are exact in fp16: the B operands of the f16 products
         float *xh = nullptr, *xth = nullptr;
         CNMF_TRY(dataset_alloc(d, &xh, (nx + 1) / 2));
         CNMF_TRY(dataset_alloc(d, &xth, (nxt + 1) / 2));
@@ -340,7 +340,7 @@ static int dataset_finish(cnmf_dataset_s* d, cudaStream_t s) {
     CNMF_TRY(launch_transpose(d->X, d->n_rows, d->n_cols, d->ld_c, d->Xt, nullptr, nullptr, d->ld_r, s));
     h->launches += 1;
   }
-  const int scratch_len = 2 * 148 * 8 + 2;
+  const int scratch_len = 2 * cnmf::NUM_SMS * 8 + 2;
   double* scratch = static_cast<double*>(h->dev_buf("dataset.sums", sizeof(double) * (scratch_len + 2)));
   if (!scratch) return -2;
   CNMF_TRY(launch_matrix_sums(d->X, d->n_rows, d->n_cols, d->ld_c, scratch + scratch_len, scratch, scratch_len, s));

@@ -240,7 +240,7 @@ int cnmf_dataset_scale_rows(cnmf_dataset_t src, const float* row_scale_host, voi
   d->want_f16 = src->want_f16;
   int rc = cnmf_dataset_alloc_internal(d, &d->X, (size_t)d->n_rows * d->ld_c);
   if (rc == 0) {
-    scale_rows_kernel<<<148 * 8, 256, 0, s>>>(src->X, d->n_rows, d->n_cols, d->ld_c, d_rs, d->X);
+    scale_rows_kernel<<<NUM_SMS * 8, 256, 0, s>>>(src->X, d->n_rows, d->n_cols, d->ld_c, d_rs, d->X);
     h->launches += 1;
     if (cudaGetLastError() != cudaSuccess) rc = -2;
   }
@@ -287,7 +287,7 @@ int cnmf_refit(cnmf_dataset_t d, int transposed, int k, const float* fixed_host,
   if (p->solver == CNMF_SOLVER_MU) {
     // sklearn _nmf.py:1223-1226: W = full(sqrt(X.mean() / k))
     const double mean = v.sum / ((double)v.n_r * (double)v.n_c);
-    fill_kernel<<<148 * 4, 256, 0, s>>>(Fr, (float)std::sqrt(mean / k), k, v.n_r, v.ld_r);
+    fill_kernel<<<NUM_SMS * 4, 256, 0, s>>>(Fr, (float)std::sqrt(mean / k), k, v.n_r, v.ld_r);
     CNMF_CUDA_CHECK(cudaGetLastError());
     h->launches += 1;
   }  // 'cd': zeros (sklearn _nmf.py:1227-1228)
@@ -313,7 +313,7 @@ int cnmf_refit(cnmf_dataset_t d, int transposed, int k, const float* fixed_host,
 
   // Fr is k x n_r; the caller wants n_r x k (row-major).  Transposed on the device into a COMPACT n_r x k array and
   // copied back in one contiguous transfer through pinned memory: a pitched 2-D copy of 50 000 rows of ~40 bytes to
-  // pageable memory took 10 ms on a good day and 80 ms on a bad one -- ten times the solve itself.
+  // pageable memory can take longer than the solve itself.
   float* T = static_cast<float*>(h->dev_buf("refit.T", (size_t)v.n_r * k * 4));
   float* T_host = static_cast<float*>(h->host_buf("refit.T_host", (size_t)v.n_r * k * 4));
   if (!T || !T_host) return -2;

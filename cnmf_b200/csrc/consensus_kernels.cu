@@ -55,8 +55,8 @@ __global__ void l2_normalize_kernel(float* __restrict__ S, int R, int G, int ld)
 
 // ---------------------------------------------------------------- C2: D[i][j] = sqrt(sum_g (A_i - B_j)^2)
 // 64 x 64 output tile per block, 16 x 16 threads, 4 x 4 per thread, k-tiles of 16 through smem.  The inner product
-// runs on packed fp32 (FADD2 with a broadcast operand, FFMA2): one instruction per element pair instead of two --
-// this kernel is FP32-issue bound, not HBM-bound (profiles/r1h_ncu_consensus_summary.txt).  SYM (A == B, the R x R
+// runs on element pairs (add2 / fma2 of common.cuh: two round-to-nearest fp32 instructions per pair) -- this kernel
+// is FP32-issue bound, not HBM-bound (3 R^2 G FLOPs against R G 4 bytes).  SYM (A == B, the R x R
 // matrix of cnmf.py:891): only tiles on or above the diagonal are computed, each is also written transposed, so the
 // matrix is exactly symmetric with an exactly zero diagonal at half the work.
 template <bool SQRT, bool SYM>
@@ -141,8 +141,8 @@ pair_dist_kernel(const float* __restrict__ A, int RA, int lda, const float* __re
 // k-means++ candidate scoring (sklearn _kmeans.py:231-262): squared distances from every row of S to a handful of
 // candidate rows of S.  HBM-bound form: one warp per row streams it once with 16-byte loads against the (L1-hot)
 // candidate rows, differences in fp32, squares accumulated in fp64 (sklearn scores candidates in float64).  The
-// 64 x 64-tile kernel above needed 200 us for this shape (60 blocks, latency-bound); 19 calls per init made the
-// seeding, not Lloyd, the cost of KMeans (profiles/r1h_ncu_consensus_summary.txt).
+// 64 x 64-tile kernel above is latency-bound for this shape (a few dozen blocks), and it runs once per candidate round
+// of every init.
 template <int NC>
 __global__ void __launch_bounds__(256)
 cand_dist_kernel(const float* __restrict__ S, int R, int G, int ld, const int32_t* __restrict__ idx, int n_c,

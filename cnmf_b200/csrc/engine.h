@@ -11,7 +11,7 @@
 
 struct cnmf_handle_s {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = cnmf::NUM_SMS;
   long long launches = 0;                       // kernels launched by this library (bench: gpu_launches)
   // optional per-launch timing of the hot kernels (batched GEMM, fused update) with CUDA events on the
   // launching stream; read back by bench.py for the roofline lines

@@ -5,11 +5,11 @@
 namespace cnmf {
 
 // Multiplicative update of the row factor applied in the epilogue of  NUM = F_other * X^T  (north star: "update applied in
-// the GEMM epilogue"; sklearn _nmf.py:535-549, 610-624).  The product tile never leaves the SM: the accumulate warp
-// thread that owns packed row (o + c) of a restart and 128 items holds their numerators in registers, streams the
-// restart's K old factor rows at those items (one broadcast load per row and 4 items for all lanes of the restart),
-// forms den = sum_i Gram[c, i] F[o + i, item] and writes F_out = F * num / den, its two fp16 operand pieces with the
-// power-of-two scale of its 128-item group and -- when gram_part is given -- the K x K Gram partial of the NEW rows.
+// the GEMM epilogue"; sklearn _nmf.py:535-549, 610-624).  The product tile never leaves the SM: the consumer thread that
+// owns packed row (o + c) of a restart and 64 items (one column half of a 128-item tile) holds their numerators in
+// registers, reads the restart's K old factor rows at those items from shared memory, forms
+// den = sum_i Gram[c, i] F[o + i, item] and writes F_out = F * num / den, its two fp16 operand pieces with the
+// power-of-two scale of the tile's 128-item group and -- when gram_part is given -- the K x K Gram partial of the NEW rows.
 // F_in / F_out are different buffers (other threads read the old rows of the restart while this one writes).
 struct FuseW {
   const float* F_in;      // SK x ld fp32, old values
@@ -28,7 +28,7 @@ struct FuseW {
   const int* done;        // [rid]
   float l1, l2;           // regularisation (sklearn _nmf.py:611-614)
   int kmax;               // largest n_components in the batch (<= 16)
-  double* gram_part;      // optional: [(rid * n_tiles + item tile) * 256 + c * KP + i], KP = K rounded up to 4
+  double* gram_part;      // optional: [(rid * n_tiles + 128-item tile) * 256 + c * KP + i], KP = K rounded up to 4
   int active;             // 0 = plain product store (this struct is ignored)
 };
 
@@ -43,16 +43,15 @@ struct GemmArgs {
   long long c_split_stride;   // elements between consecutive split-K slices of C
   int splits;                 // requested split-K factor
   int splits_effective;       // gemm_effective_splits(Kd, splits): what the kernel will actually write
-  int chain_kb;               // tf32x3: k-blocks (of 32) accumulated in TMEM before draining to registers (0 -> 1)
-  int bn;                     // tf32x3: tile width (UMMA N); 0 = choose from (M, N, Kd, splits)
+  int chain_kb;               // tf32x3: k-blocks (of 32) per short MMA chain before it is added to the fp32 sums (0 -> default)
   int b_exact;                // tf32x3: B_hi holds B exactly (tf32-representable values); B_lo unused -> 2 passes
   const float* out_col_scale; // optional: C[:, n] *= out_col_scale[n] (length >= ldc, 16-byte aligned, zero padded)
-  // f16 = 1 (tcgen05 path, b_exact only): A_hi / A_lo / B_hi point to __half arrays (two fp16 pieces of the row-
-  // normalised A, the integer matrix B), lda / ldb are in half elements, k-blocks hold 64 elements; kind::f16 MMAs run
-  // at twice the kind::tf32 rate and carry the same 11-bit significand per piece
+  // f16 = 1 (tensor-core path, b_exact only): A_hi / A_lo / B_hi point to __half arrays (two fp16 pieces of the row-
+  // normalised A, the integer matrix B), lda / ldb are in half elements, k-blocks hold 64 elements; f16 MMAs run
+  // at twice the tf32 rate and carry the same 11-bit significand per piece
   int f16;
-  // f16: the A pieces were divided by a power of two per (row, group of 512 reduction elements); the accumulate warps
-  // multiply each drained TMEM chain (128 elements, never straddling a group) by a_tile_scale[m * a_tiles + group]
+  // f16: the A pieces were divided by a power of two per (row, group of 512 reduction elements); the consumers
+  // multiply each finished MMA chain (128 elements, never straddling a group) by a_tile_scale[m * a_tiles + group]
   const float* a_tile_scale;
   int a_tiles;                // groups per row = ceil(Kd / group size)
   int a_group_kb_shift;       // log2(k-blocks per scale group): 3 = groups of 512 elements (default), 1 = groups of 128
@@ -66,13 +65,7 @@ int gemm_effective_splits(int Kd, int splits, int f16 = 0);
 // restart's result does not depend on the batch it is solved in
 int gemm_fixed_splits(int Kd, int f16 = 0);
 
-// Choice of the split-K factor (gemm_fixed_splits) and the tile width for the tcgen05 kernel: minimises
-// (waves of the persistent grid) x (tile cost) x (k-blocks per item + pipeline fill) over the tile widths.
-void gemm_plan(int M, int N, int Kd, int sm_count, int* splits, int* bn, int f16 = 0, int b_exact = 0);
-// whether gemm_tf32x3 runs the CTA-pair (cta_group::2, 256-row tiles) kernel for this problem
-bool gemm_uses_pair(int M, int b_exact);
-
-// tcgen05 / TMEM / TMA path (gemm_tf32x3.cu)
+// wgmma / TMA path (gemm_tf32x3.cu), 128 x 128 output tiles
 int gemm_tf32x3(const GemmArgs& g, cudaStream_t stream);
 
 // plain fp32 FFMA path (gemm_simt.cu): A = A_hi, B = B_hi exactly; same split-K contract

@@ -1,7 +1,7 @@
 // Plain fp32 FFMA GEMM with the same contract as gemm_tf32x3 (precision mode "fp32"):
 //   C[z] (M x N) = A[:, Kz] (M x Kd, K-major) * B[:, Kz]^T (N x Kd, K-major)
 // Used for small problems, for the fp32 precision mode and as the on-device cross-check of the
-// tcgen05 kernel in tests.  128x128x16 tiles, 256 threads, 8x8 micro-tile per thread.
+// tensor-core kernel in tests.  128x128x16 tiles, 256 threads, 8x8 micro-tile per thread.
 #include <cuda_runtime.h>
 
 #include "common.cuh"

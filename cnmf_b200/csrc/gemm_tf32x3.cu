@@ -1,11 +1,13 @@
-// 3xTF32 tensor-core GEMM for sm_100a (tcgen05 + TMEM + TMA), hand-written PTX.
+// Split-operand tensor-core GEMM for sm_90a (wgmma + TMA + mbarrier), hand-written PTX.
 //
 //   C[z] (M x N, row-major, ldc) = A[:, Kz] * B[:, Kz]^T          z = split-K slice
 //
 // A (M x Kd) and B (N x Kd) are both K-major (row-major with the reduction index contiguous),
 // each given as two tf32-representable pieces  A = A_hi + A_lo,  B = B_hi + B_lo  and the
-// product is accumulated in fp32 in tensor memory as  A_hi*B_hi + A_lo*B_hi + A_hi*B_lo
-// (the dropped A_lo*B_lo term is <= 2^-22 relative): fp32-class accuracy from kind::tf32 MMAs.
+// product is accumulated in fp32 as  A_hi*B_hi + A_lo*B_hi + A_hi*B_lo
+// (the dropped A_lo*B_lo term is <= 2^-22 relative): fp32-class accuracy from tf32 MMAs.
+// With an exact B (integer counts) the A_hi*B_lo term vanishes (2 passes), and with f16 = 1 the two A pieces
+// are fp16 (row-normalised per 512-element group) against an fp16 B: the same 2 passes at twice the tf32 rate.
 //
 // This is the shape of both big products of an NMF multiplicative-update / coordinate-descent
 // iteration once the restarts are batched (SURVEY.md section 8a rows A2/A3):
@@ -13,19 +15,21 @@
 //   X H^T   (sklearn _nmf.py:538, :380)  ->  A = H_batch (SK x G),   B = X   (cells x G)
 //   W^T X   (sklearn _nmf.py:634, :380)  ->  A = W^T_batch (SK x N), B = X^T (G x cells), split-K
 //
-// Structure (one CTA per SM, persistent over a static tile schedule, 320 threads):
-//   warp 0     TMA producer: cp.async.bulk.tensor 2D, 128B-swizzled tiles, mbarrier full/empty ring
-//   warp 1     TMEM allocator + single-thread tcgen05.mma issuer (UMMA 128 x BN x 8, kind::tf32)
-//   warps 2-9  accumulate/epilogue: tcgen05.ld 32x32b -> fp32 register accumulators -> float4 stores
+// Structure (one CTA per SM, persistent over a static tile schedule, 384 threads = 3 warpgroups):
+//   warpgroup 0     TMA producer (one thread): cp.async.bulk.tensor 2D, 128B-swizzled tiles, mbarrier full/empty ring
+//   warpgroups 1-2  consumers: rows [0, 64) / [64, 128) of the 128 x 128 tile, wgmma.mma_async m64n128 from shared
+//                   memory descriptors, fp32 fragment in registers, float2 stores
 //
-// Accumulation accuracy.  The tensor core adds each MMA result into the TMEM accumulator with
-// truncation: measured on B200, a chain of n MMAs on non-negative data is biased low by about
-// n * 3e-8 relative (2.3e-5 at K = 2048), which is far outside the 1e-4 parity budget of an NMF
-// run.  So TMEM only ever holds SHORT chains (`chain_kb` k-blocks, at most 16 MMAs: 1 k-block of 12 MMAs
-// in the general 3-pass form, 2 k-blocks of 8 MMAs in the exact-B 2-pass form):
-// the MMA warp ping-pongs between two TMEM buffers, and the eight accumulate warps drain each
-// finished chain into round-to-nearest fp32 register accumulators (128 per thread) while the next
-// chain is being issued.  Result: ~4e-7 relative, the same class as an FFMA fp32 GEMM.
+// Accumulation accuracy.  The tensor core does not round its running sum to nearest: a long chain of MMAs on
+// non-negative data is biased low by about 3e-8 relative per MMA (2.3e-5 at K = 2048), far outside the 1e-4 parity
+// budget of an NMF run.  So the wgmma accumulator only ever holds SHORT chains (`chain_kb` k-blocks, at most 16 MMAs:
+// 1 k-block of 12 MMAs in the general 3-pass form, 2 k-blocks of 8 MMAs in the exact-B 2-pass forms): every chain
+// starts from zero (scale-d = 0) and is then added into a second set of round-to-nearest fp32 register accumulators.
+// Result: ~4e-7 relative, the same class as an FFMA fp32 GEMM.
+//
+// FUSE (gemm_fused_w_kernel): NUM = F_other * X^T with the multiplicative update of the row factor applied to the tile
+// before it leaves the SM (struct FuseW in gemm.h): the consumers pass their sums through shared memory into row layout
+// and run fused_w_epilogue instead of storing the product.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -44,30 +48,24 @@ namespace cnmf {
 
 namespace {
 
-constexpr int BM = 128;          // UMMA M (rows of A per tile) -- one TMEM lane per row
+constexpr int BM = 128;          // rows of A per tile: two consumer warpgroups of 64
+constexpr int BN = 128;          // rows of B per tile (wgmma N)
 constexpr int BK = 32;           // fp32 elements per k-block = 128 B = one swizzle row
-constexpr int UMMA_K = 8;        // kind::tf32: 32 B of K per instruction
-constexpr int NUM_EPI_WARPS = 8;                         // two per TMEM lane quadrant (column halves)
-constexpr int NUM_THREADS = 64 + 32 * NUM_EPI_WARPS;      // 320
+constexpr int NUM_THREADS = 384;
 constexpr long long WAIT_TIMEOUT_CYCLES = 4000000000LL;   // ~2 s: a dead pipeline traps instead of hanging
 
-// BEXACT: the B operand is exactly representable in tf32 (e.g. integer counts), so it needs no "lo" piece:
-// 2 MMAs per k-step instead of 3, 64 KB stages (3 of them) instead of 96 KB (2).
-// CTA2: a pair of CTAs (one cluster, two SMs of a TPC) works on a 256 x BN tile with tcgen05.mma.cta_group::2: each CTA
-// stages its own 128 rows of A and HALF of the B tile, so the operand bytes every SM pulls from L2 per MMA cycle drop
-// from 64 KB to 48 KB per k-block -- the feed the 1-CTA kernel is bound by (profiles/r1i_ncu_f16_summary.txt).
-template <int BN, int STAGES, bool BEXACT, bool CTA2 = false, int EPI_BYTES_OVERRIDE = 0>
+// BEXACT: the B operand is exactly representable in tf32 / fp16 (e.g. integer counts), so it needs no "lo" piece:
+// 2 MMAs per k-step instead of 3, 48 KB stages (4 of them) instead of 64 KB (3).
+template <int STAGES, bool BEXACT, int EPI_BYTES = 0>
 struct SmemLayout {
   static constexpr int A_BYTES = BM * BK * 4;              // 16 KB
-  static constexpr int B_BYTES = (CTA2 ? BN / 2 : BN) * BK * 4;
+  static constexpr int B_BYTES = BN * BK * 4;              // 16 KB
   static constexpr int STAGE_BYTES = 2 * A_BYTES + (BEXACT ? 1 : 2) * B_BYTES;
-  static constexpr int TILE_BYTES = STAGES * STAGE_BYTES;
-  static constexpr int BAR_OFFSET = TILE_BYTES;            // full[STAGES], empty[STAGES], tfull[2], tempty[2]
-  static constexpr int TMEM_PTR_OFFSET = BAR_OFFSET + (2 * STAGES + 4) * 8;
-  static constexpr int EPI_OFFSET = TMEM_PTR_OFFSET + 16;   // per accumulate warp: 32 x 20-float transpose patch
-  static constexpr int EPI_BYTES = EPI_BYTES_OVERRIDE > 0 ? EPI_BYTES_OVERRIDE : NUM_EPI_WARPS * 32 * 20 * 4;
+  static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;  // full[STAGES], empty[STAGES]
+  static constexpr int EPI_OFFSET = BAR_OFFSET + 2 * STAGES * 8;
   static constexpr int TOTAL = EPI_OFFSET + EPI_BYTES;
   static constexpr int DYN_BYTES = TOTAL + 1024;           // slack for manual 1024 B alignment
+  static_assert(DYN_BYTES <= 227 * 1024, "pipeline stages do not fit the shared memory of an SM");
 };
 
 // ------------------------------------------------------------------ PTX wrappers
@@ -91,14 +89,12 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int who) {
+// No printf on timeout: any call in the kernel makes ptxas serialise the wgmma pipeline.
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > WAIT_TIMEOUT_CYCLES) {
-      printf("cnmf gemm_tf32x3: mbarrier wait timed out (block %d, role %d, parity %u)\n", blockIdx.x, who, parity);
-      __trap();
-    }
+    if (clock64() - t0 > WAIT_TIMEOUT_CYCLES) __trap();
   }
 }
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
@@ -107,111 +103,67 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
-// ---- CTA-pair (cluster of 2) variants
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// address of the same shared-memory offset in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// both CTAs of a pair load into their OWN shared memory; the transaction bytes are signalled on the LEADER's barrier
-__device__ __forceinline__ void tma_load_2d_pair(uint32_t dst, const CUtensorMap* map, uint32_t leader_bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(leader_bar), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void umma_f16_pair(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void umma_tf32_pair(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-// arrives on the barrier at this offset in BOTH CTAs of the pair once the MMAs issued so far have completed
-__device__ __forceinline__ void umma_commit_pair(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"(static_cast<uint16_t>(3)) : "memory");
-}
 
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-// K-major, 128B-swizzled operand tile: rows of 128 B, 8-row groups 1024 B apart
-// (cute::UMMA::SmemDescriptor, canonical layout Swizzle<3,4,3> o ((8,m),(T,2)):((8T,SBO),(1,T))).
+// K-major, 128B-swizzled operand tile: rows of 128 B, 8-row groups 1024 B apart (wgmma matrix descriptor:
+// start address >> 4 in bits [0,14), leading offset (unused for swizzled K-major) [16,30), stride offset [32,46),
+// swizzle mode in bits [62,64): 1 = 128B).  Tiles are 1024 B aligned, so the base offset field stays 0.
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
   uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);   // start address   bits [0,14)
-  d |= static_cast<uint64_t>(1) << 16;                        // LBO (unused for swizzled K-major)
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;                // SBO = 1024 B    bits [32,46)
-  d |= static_cast<uint64_t>(1) << 46;                        // descriptor version 1 (sm_100)
-  d |= static_cast<uint64_t>(2) << 61;                        // SWIZZLE_128B
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
+  d |= static_cast<uint64_t>(1) << 16;
+  d |= static_cast<uint64_t>(1024 >> 4) << 32;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
 
-template <bool F16>
-__device__ __forceinline__ uint32_t make_idesc(int bn, int m = BM) {
-  // cute::UMMA::InstrDescriptor: c=F32 (1<<4), a/b format @7/@10 (TF32 = 2, F16 = 0), K-major A and B, N>>3 @17, M>>4 @24
-  // (M = 256 for cta_group::2: 128 rows in each CTA of the pair)
-  const uint32_t fmt = F16 ? 0u : 2u;
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | (static_cast<uint32_t>(bn >> 3) << 17) |
-         (static_cast<uint32_t>(m >> 4) << 24);
-}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+// D (64 x 128 fp32, warpgroup fragment) (+)= A (64 x k, smem) * B (128 x k, smem)^T, both K-major; acc = 0: D = A * B^T
+template <bool F16>
+__device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+  if constexpr (F16) {
+    asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63 "
+      "}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(acc));
+  } else {
+    asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63 "
+      "}, %64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(acc));
+  }
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // ------------------------------------------------------------------ fused W-half epilogue
 __device__ __forceinline__ void named_bar(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
@@ -221,17 +173,21 @@ __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool v
 }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
-// shared memory of the fused epilogue (after the pipeline stages and barriers): a staging area of 128 rows x 36 floats per
-// column half, and per accumulate thread its row of the other factor's Gram (16 floats) and of the new Gram (16 doubles)
+// shared memory of the fused epilogue (after the pipeline stages and barriers): the 128 x 128 product tile in row layout
+// (rows of 136 floats; the wgmma fragments are written into it, then every thread reads its row half), reused as the
+// staging area of 128 rows x 36 floats per column half; per consumer thread its row of the other factor's Gram
+// (16 floats) and of the new Gram (16 doubles); the group maxima of the two column halves
+constexpr int FUSE_XROW = 136;                                       // floats per product row (128 + pad)
 constexpr int FUSE_SROW = 36;                                        // floats per staging row (32 items + pad: conflict-free)
-constexpr int FUSE_STAGING_BYTES = 2 * 128 * FUSE_SROW * 4;          // 36 864
+constexpr int FUSE_STAGING_BYTES = 128 * FUSE_XROW * 4;              // 69 632 (>= 2 * 128 * FUSE_SROW * 4)
 constexpr int FUSE_G_BYTES = 16 * 256 * 4;                           // 16 384
 constexpr int FUSE_GD_BYTES = 16 * 256 * 8;                          // 32 768
-constexpr int FUSE_EPI_BYTES = FUSE_STAGING_BYTES + FUSE_G_BYTES + FUSE_GD_BYTES;
+constexpr int FUSE_MAX_BYTES = 256 * 4;
+constexpr int FUSE_EPI_BYTES = FUSE_STAGING_BYTES + FUSE_G_BYTES + FUSE_GD_BYTES + FUSE_MAX_BYTES;
 
 // The multiplicative update of the row factor, applied to the product tile while it is still in registers (struct
-// FuseW in gemm.h).  Thread = packed row (o + c) of a restart x the 128 items of one scale group; acc[] holds the
-// numerators on entry and the new factor values on exit.  The 128 threads that share a column half exchange rows
+// FuseW in gemm.h).  Thread = packed row (o + c) of a restart x 64 items, one column half of the tile's 128-item scale
+// group; acc[] holds the numerators on entry and the new factor values on exit.  The 128 threads that share a column half exchange rows
 // through a shared-memory staging area: per 32-item chunk every thread publishes the OLD values of its row (cp.async
 // straight from global memory), reads the K rows of its restart (den = sum_i Gram[c, i] F[o + i, item]), publishes the
 // NEW values, accumulates its row of the restart's K x K Gram of the new values (fp32 over 16 items, fp64 beyond: the
@@ -239,20 +195,20 @@ constexpr int FUSE_EPI_BYTES = FUSE_STAGING_BYTES + FUSE_G_BYTES + FUSE_GD_BYTES
 // Restarts never straddle a 128-row tile (the engine packs them that way), so every row a thread needs is in the
 // staging area.  All per-thread state that is indexed by the component lives in shared memory, the component loops are
 // rolled (small code, no local memory: with ~200 KB of shared memory per CTA the L1 is too small to hold spills).
-// Afterwards the thread emits the two fp16 operand pieces of its 128 values with the power-of-two scale of the group:
-// the same bits emit_f16_kernel would produce from F_out.
+// Afterwards the two halves of a row agree on the group maximum and each emits the two fp16 operand pieces of its 64
+// values with the power-of-two scale of the group: the same bits emit_f16_kernel would produce from F_out.
 template <int HALF>
 __device__ __forceinline__ void fused_w_epilogue(float (&acc)[HALF], const FuseW& fz, int M, int mt, int nt, int n_tiles,
                                                  int q, int half, int lane, const float* __restrict__ out_scale,
                                                  uint8_t* epi) {
-  static_assert(HALF == 128, "one thread owns one 128-item scale group");
+  static_assert(HALF == 64, "two threads (column halves) own one 128-item scale group");
   constexpr float EPS32 = 1.1920928955078125e-07f;     // np.finfo(np.float32).eps, sklearn _nmf.py:32
   constexpr float FMIN = 1.17549435e-38f;
   constexpr int SR = FUSE_SROW;
   const int r = q * 32 + lane;                          // row inside the 128-row tile
-  const int tid = half * 128 + r;                       // accumulate-thread index 0..255
+  const int tid = half * 128 + r;                       // consumer-thread index 0..255
   const int grow = mt * BM + r;
-  const int col0 = nt * 256 + half * HALF;              // first item of this thread's group (tile width 256)
+  const int col0 = nt * 128 + half * HALF;              // first item of this thread's half (tile width 128)
   float* S = reinterpret_cast<float*>(epi) + half * (128 * SR);     // staging of this column half
   float* Sr = S + r * SR;
   float* gs = reinterpret_cast<float*>(epi + FUSE_STAGING_BYTES) + tid;                       // gs[i * 256]
@@ -298,7 +254,7 @@ __device__ __forceinline__ void fused_w_epilogue(float (&acc)[HALF], const FuseW
   const int sub_r = lane >> 3, sub_c = (lane & 7) * 4;  // coalesced store: 4 rows x 128 B per instruction
 
 #pragma unroll
-  for (int ch = 0; ch < 4; ++ch) {                      // 32 items per chunk
+  for (int ch = 0; ch < HALF / 32; ++ch) {              // 32 items per chunk
     cp_async_wait_all();
     named_bar(bar_id, 128);                             // old rows of the chunk are published
 #pragma unroll
@@ -370,7 +326,7 @@ __device__ __forceinline__ void fused_w_epilogue(float (&acc)[HALF], const FuseW
       }
     }
     named_bar(bar_id, 128);                             // staging free for the next chunk
-    if (ch < 3) {
+    if (ch < HALF / 32 - 1) {
 #pragma unroll
       for (int t = 0; t < 8; ++t) {
         const int cc = (ch + 1) * 32 + 4 * t;
@@ -401,15 +357,19 @@ __device__ __forceinline__ void fused_w_epilogue(float (&acc)[HALF], const FuseW
   }
 #pragma unroll
   for (int j = 0; j < HALF; ++j) m = fmaxf(m, acc[j]);
+  float* gmax = reinterpret_cast<float*>(epi + FUSE_STAGING_BYTES + FUSE_G_BYTES + FUSE_GD_BYTES);
+  gmax[tid] = m;
+  named_bar(3, 256);
+  m = fmaxf(m, gmax[tid ^ 128]);                        // the other column half of the row
   const float sc = f16_group_scale(m);
   const float inv = 1.f / sc;                           // power of two: exact
-  if (row_ok && col0 < ld) fz.tile_scale[static_cast<long long>(grow) * fz.n_groups + (col0 >> 7)] = sc;
+  if (half == 0 && row_ok && col0 < ld) fz.tile_scale[static_cast<long long>(grow) * fz.n_groups + (col0 >> 7)] = sc;
   __half* ph = static_cast<__half*>(fz.P_hi);
   __half* pm = static_cast<__half*>(fz.P_mid);
   uint32_t* Su = reinterpret_cast<uint32_t*>(Sr);
   const int sub_r8 = lane >> 2, sub_q = lane & 3;       // 8 rows x 64 B per instruction
 #pragma unroll
-  for (int cc = 0; cc < 4; ++cc) {                      // 32 items = 64 B of halves per row and piece
+  for (int cc = 0; cc < HALF / 32; ++cc) {              // 32 items = 64 B of halves per row and piece
 #pragma unroll
     for (int pc = 0; pc < 2; ++pc) {
       __syncwarp();
@@ -446,27 +406,22 @@ __device__ __forceinline__ void fused_w_epilogue(float (&acc)[HALF], const FuseW
 
 // ------------------------------------------------------------------ the kernel
 // F16 (with BEXACT): operands are fp16 (two pieces of A, one exact B); a k-block is still 128 B per row = 64 elements,
-// a k-step still 32 B = 16 elements (UMMA_K of kind::f16), so the smem / TMA / descriptor byte geometry is unchanged.
+// a k-step still 32 B = 16 elements (wgmma K of f16), so the smem / TMA / descriptor byte geometry is unchanged.
 //
-// CTA2: the grid is made of clusters of two CTAs (ranks 0 / 1 = the two SMs of a TPC).  A work item is a 256 x bn tile:
-// rank r stages rows [256 i + 128 r, +128) of both A pieces and rows [r bn/2, +bn/2) of the B tile; rank 0's MMA thread
-// issues tcgen05.mma.cta_group::2 (M = 256) which reads A from each CTA's own shared memory, the two B halves from both,
-// and leaves rows 0-127 of the product in rank 0's TMEM and rows 128-255 in rank 1's.  Barrier protocol (the one of
-// CUTLASS / DeepGEMM 2-SM kernels): `full` lives in rank 0 (both producers arrive on it, both CTAs' TMA bytes are
-// signalled on it), `empty` and `tfull` exist in both CTAs and are arrived by multicast commits, `tempty` lives in
-// rank 0 and is arrived by the accumulate warps of both CTAs.
-template <int BN, int STAGES, bool BEXACT, bool F16, bool CTA2, bool FUSE = false>
+// Fragment of consumer thread (warp w of its warpgroup, lane l): d[4j + e] is row 16w + l/4 (+8 for e >= 2),
+// column 8j + 2(l%4) + (e & 1) of the warpgroup's 64 x 128 block.
+template <int STAGES, bool BEXACT, bool F16, bool FUSE>
 __device__ __forceinline__ void
 gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMap& tmB_hi, const CUtensorMap& tmB_lo,
-          float* __restrict__ C, int M, int N, int ldc, long long c_split_stride,
-          int m_tiles, int n_tiles, int splits, int total_kb, int kb_per_split, int chain_kb, int bn,
+          float* __restrict__ C, int M, int ldc, long long c_split_stride,
+          int m_tiles, int n_tiles, int splits, int total_kb, int kb_per_split, int chain_kb,
           const float* __restrict__ out_scale, const float* __restrict__ a_tile_scale, int a_tiles, int a_gshift,
-          const FuseW* __restrict__ fz = nullptr) {
+          const FuseW* __restrict__ fz) {
   static_assert(!F16 || BEXACT, "the fp16 path exists for exact integer B operands only");
-  static_assert(!FUSE || (F16 && !CTA2 && BN == 256), "the fused W-half epilogue is built for the kind::f16 1-CTA kernel");
-  static_assert(!CTA2 || BEXACT, "the CTA-pair kernel is built for the exact-B (2-pass) forms");
+  static_assert(!FUSE || (F16 && STAGES == 2), "the fused W-half epilogue is built for the 2-stage f16 kernel");
   constexpr int BKE = F16 ? 2 * BK : BK;                        // elements per k-block
-  using L = SmemLayout<BN, STAGES, BEXACT, CTA2, FUSE ? FUSE_EPI_BYTES : 0>;
+  constexpr int KSTEP_BYTES = 32;                               // wgmma K: 8 tf32 or 16 fp16 elements
+  using L = SmemLayout<STAGES, BEXACT, FUSE ? FUSE_EPI_BYTES : 0>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;     // SWIZZLE_128B needs 1024 B alignment
   uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
@@ -474,293 +429,179 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
   const uint32_t bar_base = smem_base + L::BAR_OFFSET;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + 2 + a); };
-  volatile uint32_t* tmem_ptr_smem = reinterpret_cast<volatile uint32_t*>(smem_gen + L::TMEM_PTR_OFFSET);
 
-  const int warp = threadIdx.x >> 5;
+  const int wg = threadIdx.x >> 7;
+  const int warp = (threadIdx.x >> 5) & 3;                      // warp inside its warpgroup
   const int lane = threadIdx.x & 31;
-  constexpr uint32_t TMEM_COLS = 2 * BN;                      // two accumulators (power of two: 256 or 512)
-  const uint32_t rank = CTA2 ? cluster_ctarank() : 0u;       // 0 = leader of the pair
-  const int worker = CTA2 ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-  const int n_workers = CTA2 ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
-  // CTA2: m_tiles counts 256-row tile PAIRS; this CTA's 128-row tile is 2 * (pair) + rank
 
-  if constexpr (CTA2) cluster_sync_all();                     // both CTAs are running before either touches the pair state
-
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar(s), CTA2 ? 2 : 1);                   // CTA2 (used in rank 0): one arrival per producer
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), 1);
-      mbar_init(tempty_bar(a), (CTA2 ? 2 : 1) * NUM_EPI_WARPS);   // one arrival per accumulate warp (of both CTAs)
+      mbar_init(full_bar(s), 1);
+      mbar_init(empty_bar(s), 8);                               // one arrival per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    if constexpr (CTA2) {
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;"
-                   ::"r"(smem_base + L::TMEM_PTR_OFFSET), "r"(TMEM_COLS) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                   ::"r"(smem_base + L::TMEM_PTR_OFFSET), "r"(TMEM_COLS) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-  }
-  tc_fence_before();
   __syncthreads();
-  if constexpr (CTA2) cluster_sync_all();                     // the peer's barriers are initialised before anyone arrives
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
   const int items = m_tiles * n_tiles * splits;
-  const int bnl = CTA2 ? bn >> 1 : bn;                        // B rows this CTA stages
 
-  if (warp == 0) {
+  if constexpr (FUSE) {     // the epilogue's state needs more than 168 registers: move them from the producer warpgroup
+    if (wg == 0) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    else asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+  }
+  if (wg == 0) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int w = worker; w < items; w += n_workers) {
-        const int mt = (w % m_tiles) * (CTA2 ? 2 : 1) + static_cast<int>(rank);
+      constexpr uint32_t stage_tx = static_cast<uint32_t>(L::STAGE_BYTES);
+      for (int w = blockIdx.x; w < items; w += gridDim.x) {
+        const int mt = w % m_tiles;
         const int nt = (w / m_tiles) % n_tiles;
         const int z = w / (m_tiles * n_tiles);
         const int kb0 = z * kb_per_split;
         const int kb1 = min(total_kb, kb0 + kb_per_split);
         for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(empty_bar(stage), phase ^ 1u, 0);
+          mbar_wait(empty_bar(stage), phase ^ 1u);
           const uint32_t st = smem_base + stage * L::STAGE_BYTES;
-          const uint32_t stage_tx = 2u * L::A_BYTES + (BEXACT ? 1u : 2u) * static_cast<uint32_t>(bnl) * BK * 4u;
-          if constexpr (CTA2) {
-            const uint32_t lead_full = mapa_shared(full_bar(stage), 0);
-            if (rank == 0) mbar_arrive_expect_tx(full_bar(stage), 2u * stage_tx);      // both CTAs' bytes
-            tma_load_2d_pair(st, &tmA_hi, lead_full, kb * BKE, mt * BM);
-            tma_load_2d_pair(st + L::A_BYTES, &tmA_lo, lead_full, kb * BKE, mt * BM);
-            tma_load_2d_pair(st + 2 * L::A_BYTES, &tmB_hi, lead_full, kb * BKE, nt * bn + static_cast<int>(rank) * bnl);
-            if (rank != 0) mbar_arrive_cluster(lead_full);
-          } else {
-            mbar_arrive_expect_tx(full_bar(stage), stage_tx);
-            tma_load_2d(st, &tmA_hi, full_bar(stage), kb * BKE, mt * BM);
-            tma_load_2d(st + L::A_BYTES, &tmA_lo, full_bar(stage), kb * BKE, mt * BM);
-            tma_load_2d(st + 2 * L::A_BYTES, &tmB_hi, full_bar(stage), kb * BKE, nt * bn);
-            if constexpr (!BEXACT) tma_load_2d(st + 2 * L::A_BYTES + L::B_BYTES, &tmB_lo, full_bar(stage), kb * BKE, nt * bn);
-          }
+          mbar_arrive_expect_tx(full_bar(stage), stage_tx);
+          tma_load_2d(st, &tmA_hi, full_bar(stage), kb * BKE, mt * BM);
+          tma_load_2d(st + L::A_BYTES, &tmA_lo, full_bar(stage), kb * BKE, mt * BM);
+          tma_load_2d(st + 2 * L::A_BYTES, &tmB_hi, full_bar(stage), kb * BKE, nt * BN);
+          if constexpr (!BEXACT) tma_load_2d(st + 2 * L::A_BYTES + L::B_BYTES, &tmB_lo, full_bar(stage), kb * BKE, nt * BN);
           if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-      }
-      if constexpr (CTA2) {
-        // the MMA thread's last commits arrive on this CTA's `empty` barriers from the other SM: see every slot
-        // released before this CTA may retire its shared memory
-        for (int i = 0; i < STAGES; ++i) {
-          mbar_wait(empty_bar(stage), phase ^ 1u, 0);
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (one thread; the leader CTA of a pair) =====================
-    if (lane == 0 && rank == 0) {
-      const uint32_t idesc = make_idesc<F16>(bn, CTA2 ? 2 * BM : BM);   // UMMA N = bn (multiple of 16, <= BN)
-      int stage = 0;
-      uint32_t phase = 0;
-      int buf = 0;
-      uint32_t buf_phase = 0;
-      for (int w = worker; w < items; w += n_workers) {
-        const int z = w / (m_tiles * n_tiles);
-        const int kb0 = z * kb_per_split;
-        const int kb1 = min(total_kb, kb0 + kb_per_split);
-        for (int c0 = kb0; c0 < kb1; c0 += chain_kb) {          // one short accumulation chain per TMEM buffer
-          const int c1 = min(kb1, c0 + chain_kb);
-          mbar_wait(tempty_bar(buf), buf_phase ^ 1u, 1);
-          tc_fence_after();
-          const uint32_t tmem_d = tmem_base + static_cast<uint32_t>(buf * BN);
-          for (int kb = c0; kb < c1; ++kb) {
-            mbar_wait(full_bar(stage), phase, 2);
-            tc_fence_after();
-            const uint32_t st = smem_base + stage * L::STAGE_BYTES;
-            const uint64_t a_hi = make_smem_desc(st);
-            const uint64_t a_lo = make_smem_desc(st + L::A_BYTES);
-            const uint64_t b_hi = make_smem_desc(st + 2 * L::A_BYTES);
-            const uint64_t b_lo = make_smem_desc(st + 2 * L::A_BYTES + L::B_BYTES);
-#pragma unroll
-            for (int k = 0; k < BK / UMMA_K; ++k) {
-              const uint64_t koff = static_cast<uint64_t>((k * UMMA_K * 4) >> 4);   // +32 B per k-step inside the swizzle row
-              const uint32_t acc0 = (kb > c0 || k > 0) ? 1u : 0u;
-              if constexpr (CTA2) {
-                if constexpr (F16) {
-                  umma_f16_pair(tmem_d, a_lo + koff, b_hi + koff, idesc, acc0);     // small terms first
-                  umma_f16_pair(tmem_d, a_hi + koff, b_hi + koff, idesc, 1u);
-                } else {
-                  umma_tf32_pair(tmem_d, a_lo + koff, b_hi + koff, idesc, acc0);
-                  umma_tf32_pair(tmem_d, a_hi + koff, b_hi + koff, idesc, 1u);
-                }
-              } else if constexpr (F16) {
-                umma_f16(tmem_d, a_lo + koff, b_hi + koff, idesc, acc0);    // small terms first
-                umma_f16(tmem_d, a_hi + koff, b_hi + koff, idesc, 1u);
-              } else {
-                umma_tf32(tmem_d, a_lo + koff, b_hi + koff, idesc, acc0);   // small terms first
-                if constexpr (!BEXACT) umma_tf32(tmem_d, a_hi + koff, b_lo + koff, idesc, 1u);
-                umma_tf32(tmem_d, a_hi + koff, b_hi + koff, idesc, 1u);
-              }
-            }
-            // smem slot is free once these MMAs have read it (CTA2: in both CTAs)
-            if constexpr (CTA2) umma_commit_pair(empty_bar(stage)); else umma_commit(empty_bar(stage));
-            if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-          }
-          // chain complete -> accumulate warps (CTA2: of both CTAs)
-          if constexpr (CTA2) umma_commit_pair(tfull_bar(buf)); else umma_commit(tfull_bar(buf));
-          if (++buf == 2) { buf = 0; buf_phase ^= 1u; }
-        }
-      }
-      if constexpr (CTA2) {
-        // every chain has been drained by both CTAs before the leader lets go of its barriers
-        for (int i = 0; i < 2; ++i) {
-          mbar_wait(tempty_bar(buf), buf_phase ^ 1u, 1);
-          if (++buf == 2) { buf = 0; buf_phase ^= 1u; }
         }
       }
     }
   } else {
-    // ===================== accumulate + epilogue (8 warps) =====================
-    // tcgen05.ld: warp w may touch TMEM lanes 32*(w%4) .. +31.  Warps 2-5 own columns [0, BN/2),
-    // warps 6-9 own [BN/2, BN) of their lane quadrant.
-    constexpr int HALF = BN / 2;
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    int buf = 0;
-    uint32_t buf_phase = 0;
-    for (int w = worker; w < items; w += n_workers) {
-      const int mt = (w % m_tiles) * (CTA2 ? 2 : 1) + static_cast<int>(rank);
+    // ===================== consumers: MMA chains + drain + epilogue =====================
+    const int cw = wg - 1;                                      // rows [64 cw, 64 cw + 64) of the tile
+    const uint32_t a_off = static_cast<uint32_t>(cw * 64 * 128);
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int w = blockIdx.x; w < items; w += gridDim.x) {
+      const int mt = w % m_tiles;
       const int nt = (w / m_tiles) % n_tiles;
       const int z = w / (m_tiles * n_tiles);
       const int kb0 = z * kb_per_split;
       const int kb1 = min(total_kb, kb0 + kb_per_split);
-      float acc[HALF];
+      const int row0 = mt * BM + cw * 64 + warp * 16 + (lane >> 2);   // and row0 + 8
+      float acc[64];
 #pragma unroll
-      for (int i = 0; i < HALF; ++i) acc[i] = 0.f;
-      // f16: power-of-two scale of this thread's A row for the 512-element group a chain belongs to (8 k-blocks)
-      const int arow = mt * BM + q * 32 + lane;
-      const float* sc_row = (F16 && a_tile_scale && arow < M) ? a_tile_scale + static_cast<long long>(arow) * a_tiles : nullptr;
-      for (int c0 = kb0; c0 < kb1; c0 += chain_kb) {
-        float sc = 1.f;
-        if (F16 && sc_row) sc = sc_row[c0 >> a_gshift];
-        mbar_wait(tfull_bar(buf), buf_phase, 3);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) +
-                               static_cast<uint32_t>(buf * BN + half * HALF);
+      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+      // f16: power-of-two scale of this thread's two A rows for the scale group (2^a_gshift k-blocks) of a chain
+      const float* sc_row0 = (F16 && a_tile_scale && row0 < M) ? a_tile_scale + static_cast<long long>(row0) * a_tiles : nullptr;
+      const float* sc_row1 = (F16 && a_tile_scale && row0 + 8 < M) ? a_tile_scale + static_cast<long long>(row0 + 8) * a_tiles : nullptr;
+      for (int c0 = kb0; c0 < kb1; c0 += chain_kb) {            // one short accumulation chain
+        const int c1 = min(kb1, c0 + chain_kb);
+        float d[64];
+        int prev = -1;
+        for (int kb = c0; kb < c1; ++kb) {
+          mbar_wait(full_bar(stage), phase);
+          const uint32_t st = smem_base + stage * L::STAGE_BYTES;
+          const uint64_t a_hi = make_smem_desc(st + a_off);
+          const uint64_t a_lo = make_smem_desc(st + L::A_BYTES + a_off);
+          const uint64_t b_hi = make_smem_desc(st + 2 * L::A_BYTES);
+          const uint64_t b_lo = make_smem_desc(st + 2 * L::A_BYTES + L::B_BYTES);
+          wgmma_fence();
 #pragma unroll
-        for (int c = 0; c < HALF; c += 32) {
-          if (half * HALF + c < bn) {                  // warp-uniform: columns >= bn were not computed
-            uint32_t r[32];
-            tmem_ld32(taddr + c, r);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              if constexpr (F16) acc[c + i] = fmaf(__uint_as_float(r[i]), sc, acc[c + i]);   // exact scaling, one rounding
-              else acc[c + i] += __uint_as_float(r[i]);   // round-to-nearest fp32
-            }
+          for (int k = 0; k < BK * 4 / KSTEP_BYTES; ++k) {
+            const uint64_t koff = static_cast<uint64_t>((k * KSTEP_BYTES) >> 4);   // +32 B per k-step inside the swizzle row
+            const uint32_t acc0 = (kb > c0 || k > 0) ? 1u : 0u;
+            wgmma_m64n128<F16>(d, a_lo + koff, b_hi + koff, acc0);     // small terms first
+            if constexpr (!BEXACT) wgmma_m64n128<F16>(d, a_hi + koff, b_lo + koff, 1u);
+            wgmma_m64n128<F16>(d, a_hi + koff, b_hi + koff, 1u);
           }
+          wgmma_commit();
+          if (prev >= 0) {                                      // the previous k-block's MMAs have read their slot
+            wgmma_wait<1>();
+            if (lane == 0) mbar_arrive(empty_bar(prev));
+          }
+          prev = stage;
+          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) {                                // one arrival per warp, on the leader's barrier
-          if constexpr (CTA2) mbar_arrive_cluster(mapa_shared(tempty_bar(buf), 0));
-          else mbar_arrive(tempty_bar(buf));
+        wgmma_wait<0>();
+        if (lane == 0) mbar_arrive(empty_bar(prev));
+        if constexpr (F16) {                                    // exact power-of-two scaling, one rounding
+          const float s0 = sc_row0 ? sc_row0[c0 >> a_gshift] : 1.f;
+          const float s1 = sc_row1 ? sc_row1[c0 >> a_gshift] : 1.f;
+#pragma unroll
+          for (int i = 0; i < 64; i += 4) {
+            acc[i] = fmaf(d[i], s0, acc[i]);
+            acc[i + 1] = fmaf(d[i + 1], s0, acc[i + 1]);
+            acc[i + 2] = fmaf(d[i + 2], s1, acc[i + 2]);
+            acc[i + 3] = fmaf(d[i + 3], s1, acc[i + 3]);
+          }
+        } else {
+#pragma unroll
+          for (int i = 0; i < 64; ++i) acc[i] += d[i];          // round-to-nearest fp32
         }
-        if (++buf == 2) { buf = 0; buf_phase ^= 1u; }
       }
       if constexpr (FUSE) {
-        // W-half update applied to the tile in registers; the product itself is never stored (gemm.h, struct FuseW)
-        fused_w_epilogue<HALF>(acc, *fz, M, mt, nt, n_tiles, q, half, lane, out_scale, smem_gen + L::EPI_OFFSET);
+        // fragments -> row layout: consumer thread ct owns tile row ct % 128, items [64 (ct / 128), +64)
+        const int ct = static_cast<int>(threadIdx.x) - 128;
+        float* X = reinterpret_cast<float*>(smem_gen + L::EPI_OFFSET);
+        named_bar(4, 256);                                      // the previous tile's epilogue is done with X
+        const int lr = cw * 64 + warp * 16 + (lane >> 2);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const int lc = 8 * j + 2 * (lane & 3);
+          *reinterpret_cast<float2*>(X + lr * FUSE_XROW + lc) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(X + (lr + 8) * FUSE_XROW + lc) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+        named_bar(4, 256);
+        float rowv[64];
+        const float4* src = reinterpret_cast<const float4*>(X + (ct & 127) * FUSE_XROW + (ct >> 7) * 64);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const float4 v = src[j];
+          rowv[4 * j] = v.x; rowv[4 * j + 1] = v.y; rowv[4 * j + 2] = v.z; rowv[4 * j + 3] = v.w;
+        }
+        named_bar(4, 256);                                      // X is reused as the epilogue's staging area
+        fused_w_epilogue<64>(rowv, *fz, M, mt, nt, n_tiles, (ct & 127) >> 5, ct >> 7, lane, out_scale,
+                             smem_gen + L::EPI_OFFSET);
         continue;
       }
-      // Epilogue.  A thread owns one output row, so a direct store touches 32 rows x 16 B per instruction (32 cache
-      // lines: the LSU, not the tensor pipe, then paces short tiles -- the 720-tile W half ran at 0.76 of the MMA rate
-      // against 0.92 for the long-K H half).  Each warp transposes 16-column chunks through a private 32 x 20-float
-      // shared-memory patch instead, so that one store instruction writes 8 rows x 64 B.
-      {
-        float* patch = reinterpret_cast<float*>(smem_gen + L::EPI_OFFSET) + (warp - 2) * (32 * 20);
-        const int row0 = mt * BM + q * 32;
-        const int col0 = nt * bn + half * HALF;
-        const int sub_r = lane >> 2, sub_c = (lane & 3) * 4;
-        float* cbase = C + static_cast<long long>(z) * c_split_stride;
+      // Epilogue: a quad of lanes writes 32 contiguous bytes of a row per instruction (whole sectors)
+      float* cbase = C + static_cast<long long>(z) * c_split_stride;
+      const int colq = nt * BN + 2 * (lane & 3);
 #pragma unroll
-        for (int c = 0; c < HALF; c += 16) {
-          if (half * HALF + c < bn) {                     // warp-uniform (bn is a multiple of 16)
-#pragma unroll
-            for (int i = 0; i < 16; i += 4) {
-              float4 v = make_float4(acc[c + i], acc[c + i + 1], acc[c + i + 2], acc[c + i + 3]);
-              if (out_scale && col0 + c + i + 3 < ldc) {  // per-output-column scale (length >= ldc, zero padded)
-                const float4 sc = *reinterpret_cast<const float4*>(out_scale + col0 + c + i);
-                v.x *= sc.x; v.y *= sc.y; v.z *= sc.z; v.w *= sc.w;
-              }
-              *reinterpret_cast<float4*>(patch + lane * 20 + i) = v;
-            }
-            __syncwarp();
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const int r = sub_r + 8 * j;
-              const float4 v = *reinterpret_cast<const float4*>(patch + r * 20 + sub_c);
-              const int grow = row0 + r, gcol = col0 + c + sub_c;
-              if (grow < M && gcol + 3 < ldc) *reinterpret_cast<float4*>(cbase + static_cast<long long>(grow) * ldc + gcol) = v;
-            }
-            __syncwarp();
-          }
-        }
+      for (int j = 0; j < 16; ++j) {
+        const int col = colq + 8 * j;
+        if (col >= ldc) continue;                               // ldc % 4 == 0 and col even: col + 1 < ldc too
+        float2 sc = make_float2(1.f, 1.f);
+        if (out_scale) sc = *reinterpret_cast<const float2*>(out_scale + col);   // length >= ldc, zero padded
+        if (row0 < M)
+          *reinterpret_cast<float2*>(cbase + static_cast<long long>(row0) * ldc + col) =
+              make_float2(acc[4 * j] * sc.x, acc[4 * j + 1] * sc.y);
+        if (row0 + 8 < M)
+          *reinterpret_cast<float2*>(cbase + static_cast<long long>(row0 + 8) * ldc + col) =
+              make_float2(acc[4 * j + 2] * sc.x, acc[4 * j + 3] * sc.y);
       }
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if constexpr (CTA2) cluster_sync_all();       // neither CTA retires while the other may still signal it
-  if (warp == 1) {
-    tc_fence_after();
-    if constexpr (CTA2)
-      asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-    else
-      asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-  }
 }
 
-// 320 threads = 10 warps, allocated as 12 (granularity 4): at most 65536 / (12 * 32) = 170 registers per thread --
-// __launch_bounds__ makes ptxas pick 168; a higher __maxnreg__ compiles but cannot launch
-template <int BN, int STAGES, bool BEXACT, bool F16>
+template <int STAGES, bool BEXACT, bool F16>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                    const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
-                   float* __restrict__ C, int M, int N, int ldc, long long c_split_stride,
-                   int m_tiles, int n_tiles, int splits, int total_kb, int kb_per_split, int chain_kb, int bn,
+                   float* __restrict__ C, int M, int ldc, long long c_split_stride,
+                   int m_tiles, int n_tiles, int splits, int total_kb, int kb_per_split, int chain_kb,
                    const float* __restrict__ out_scale, const float* __restrict__ a_tile_scale, int a_tiles, int a_gshift) {
-  gemm_body<BN, STAGES, BEXACT, F16, false>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, C, M, N, ldc, c_split_stride, m_tiles, n_tiles,
-                                            splits, total_kb, kb_per_split, chain_kb, bn, out_scale, a_tile_scale, a_tiles,
-                                            a_gshift);
+  gemm_body<STAGES, BEXACT, F16, false>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, C, M, ldc, c_split_stride, m_tiles, n_tiles, splits,
+                                        total_kb, kb_per_split, chain_kb, out_scale, a_tile_scale, a_tiles, a_gshift,
+                                        nullptr);
 }
 
-// NUM = F_other * X^T with the multiplicative update of the row factor in the epilogue (kind::f16, 256-wide tiles, no split-K)
+// NUM = F_other * X^T with the multiplicative update of the row factor in the epilogue (f16, 128-wide tiles, no split-K)
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_fused_w_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
-                    const __grid_constant__ CUtensorMap tmB_hi, int M, int N,
-                    int m_tiles, int n_tiles, int total_kb, const float* __restrict__ out_scale,
-                    const float* __restrict__ a_tile_scale, int a_tiles, int a_gshift, const __grid_constant__ FuseW fz) {
-  gemm_body<256, 2, true, true, false, true>(tmA_hi, tmA_lo, tmB_hi, tmB_hi, nullptr, M, N, 0, 0, m_tiles, n_tiles, 1, total_kb,
-                                             total_kb + (total_kb & 1), 2, 256, out_scale, a_tile_scale, a_tiles, a_gshift, &fz);
-}
-
-// the CTA-pair form: clusters of two CTAs, m_tiles = number of 256-row tile pairs
-template <int BN, int STAGES, bool F16>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NUM_THREADS, 1)
-gemm_pair_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
-                 const __grid_constant__ CUtensorMap tmB_hi,
-                 float* __restrict__ C, int M, int N, int ldc, long long c_split_stride,
-                 int m_tiles, int n_tiles, int splits, int total_kb, int kb_per_split, int chain_kb, int bn,
-                 const float* __restrict__ out_scale, const float* __restrict__ a_tile_scale, int a_tiles, int a_gshift) {
-  gemm_body<BN, STAGES, true, F16, true>(tmA_hi, tmA_lo, tmB_hi, tmB_hi, C, M, N, ldc, c_split_stride, m_tiles, n_tiles,
-                                         splits, total_kb, kb_per_split, chain_kb, bn, out_scale, a_tile_scale, a_tiles,
-                                         a_gshift);
+                    const __grid_constant__ CUtensorMap tmB_hi, int M, int m_tiles, int n_tiles, int total_kb,
+                    const float* __restrict__ out_scale, const float* __restrict__ a_tile_scale, int a_tiles, int a_gshift,
+                    const __grid_constant__ FuseW fz) {
+  gemm_body<2, true, true, true>(tmA_hi, tmA_lo, tmB_hi, tmB_hi, nullptr, M, 0, 0, m_tiles, n_tiles, 1, total_kb,
+                                 total_kb + (total_kb & 1), 2, out_scale, a_tile_scale, a_tiles, a_gshift, &fz);
 }
 
 // ------------------------------------------------------------------ host side
@@ -781,7 +622,7 @@ PFN_encodeTiled get_encode_fn() {
   return fn;
 }
 
-// 2D fp32 tensor (rows x cols, row stride ld elements), box = 32 cols x box_rows rows, 128B swizzle, zero OOB fill.
+// 2D fp32 / fp16 tensor (rows x cols, row stride ld elements), box = 128 B x box_rows rows, 128B swizzle, zero OOB fill.
 // Encoded maps are cached by (pointer, shape, box): the solver relaunches the same few operand views a thousand
 // times per solve, and the driver call costs more than the launch itself.
 struct MapKey {
@@ -825,8 +666,8 @@ static int env_int(const char* name, int dflt) {
   return e ? std::atoi(e) : dflt;
 }
 
-// k-blocks per TMEM accumulation chain: at most 16 MMAs between drains (general: 1 k-block = 12 MMAs,
-// exact-B: 2 k-blocks = 16 MMAs; with 8 MMAs per chain the drain, not the tensor pipe, paced the kernel)
+// k-blocks per accumulation chain: at most 16 MMAs between drains (general: 1 k-block = 12 MMAs,
+// exact-B: 2 k-blocks = 16 MMAs)
 template <bool BEXACT, bool F16>
 static int pick_chain_kb(const GemmArgs& g) {
   int chain_kb = g.chain_kb;
@@ -838,42 +679,21 @@ static int pick_chain_kb(const GemmArgs& g) {
   return chain_kb;
 }
 
-template <int BN, int STAGES, bool BEXACT, bool F16>
+template <int STAGES, bool BEXACT, bool F16>
 int launch(const GemmArgs& g, cudaStream_t stream) {
-  using L = SmemLayout<BN, STAGES, BEXACT>;
+  using L = SmemLayout<STAGES, BEXACT>;
   constexpr int BKE = F16 ? 2 * BK : BK;
   CUtensorMap mAh, mAl, mBh, mBl;
   int rc;
   if ((rc = make_map(&mAh, g.A_hi, g.M, g.Kd, g.lda, BM, F16))) return rc;
   if ((rc = make_map(&mAl, g.A_lo, g.M, g.Kd, g.lda, BM, F16))) return rc;
+  if ((rc = make_map(&mBh, g.B_hi, g.N, g.Kd, g.ldb, BN, F16))) return rc;
+  if ((rc = make_map(&mBl, BEXACT ? g.B_hi : g.B_lo, g.N, g.Kd, g.ldb, BN, F16))) return rc;
   int dev = 0, sms = 0;
   CNMF_CUDA_CHECK(cudaGetDevice(&dev));
   CNMF_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const int m_tiles = (g.M + BM - 1) / BM;
-  // Tile width: the UMMA N is a runtime value (multiple of 16, <= BN), normally supplied by gemm_plan().
-  int bn = g.bn;
-  if (bn <= 0 || bn > BN || bn % 16 != 0) {
-    const int sp = gemm_effective_splits(g.Kd, g.splits, F16 ? 1 : 0);
-    if (g.N <= BN) {
-      bn = ((g.N + 15) / 16) * 16;
-    } else {
-      long long best = -1;
-      bn = BN;
-      for (int cand = BN; cand >= 192; cand -= 16) {
-        const long long tiles = (long long)m_tiles * ((g.N + cand - 1) / cand) * sp;
-        const long long cost = ((tiles + sms - 1) / sms) * (cand + 64);
-        if (best < 0 || cost < best) { best = cost; bn = cand; }
-      }
-    }
-  }
-  {
-    static const int env_bn = env_int("CNMF_GEMM_BN", 0);
-    if (env_bn >= 16 && env_bn <= BN && env_bn % 16 == 0) bn = env_bn;
-  }
-  if ((rc = make_map(&mBh, g.B_hi, g.N, g.Kd, g.ldb, bn, F16))) return rc;
-  if ((rc = make_map(&mBl, BEXACT ? g.B_hi : g.B_lo, g.N, g.Kd, g.ldb, bn, F16))) return rc;
-
-  const int n_tiles = (g.N + bn - 1) / bn;
+  const int n_tiles = (g.N + BN - 1) / BN;
   const int total_kb = (g.Kd + BKE - 1) / BKE;
   int splits = g.splits < 1 ? 1 : g.splits;
   if (splits > total_kb) splits = total_kb;
@@ -882,7 +702,7 @@ int launch(const GemmArgs& g, cudaStream_t stream) {
   splits = (total_kb + kb_per_split - 1) / kb_per_split;      // no empty slices
   if (splits != g.splits_effective) { set_last_error("gemm: splits_effective mismatch (use gemm_effective_splits)"); return -1; }
 
-  auto kern = gemm_tf32x3_kernel<BN, STAGES, BEXACT, F16>;
+  auto kern = gemm_tf32x3_kernel<STAGES, BEXACT, F16>;
   static bool attr_set[64] = {};              // per device: a second GPU in the same process needs its own call
   if (dev < 0 || dev >= 64 || !attr_set[dev]) {
     CNMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::DYN_BYTES));
@@ -891,27 +711,26 @@ int launch(const GemmArgs& g, cudaStream_t stream) {
   const int items = m_tiles * n_tiles * splits;
   const int grid = items < sms ? items : sms;
   const int chain_kb = pick_chain_kb<BEXACT, F16>(g);
-  kern<<<grid, NUM_THREADS, L::DYN_BYTES, stream>>>(mAh, mAl, mBh, mBl, g.C, g.M, g.N, g.ldc, g.c_split_stride,
-                                                    m_tiles, n_tiles, splits, total_kb, kb_per_split,
-                                                    chain_kb, bn, g.out_col_scale, g.a_tile_scale, g.a_tiles,
+  kern<<<grid, NUM_THREADS, L::DYN_BYTES, stream>>>(mAh, mAl, mBh, mBl, g.C, g.M, g.ldc, g.c_split_stride,
+                                                    m_tiles, n_tiles, splits, total_kb, kb_per_split, chain_kb,
+                                                    g.out_col_scale, g.a_tile_scale, g.a_tiles,
                                                     g.a_group_kb_shift > 0 ? g.a_group_kb_shift : 3);
   CNMF_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
 
-// fused W-half launch: 128 x 256 tiles, the whole reduction in one item (no split-K), kind::f16
+// fused W-half launch: 128 x 128 tiles, the whole reduction in one item (no split-K), f16
 int launch_fused_w(const GemmArgs& g, cudaStream_t stream) {
-  using L = SmemLayout<256, 2, true, false, FUSE_EPI_BYTES>;     // 2 stages of 64 KB leave room for the epilogue's state
-  static_assert(L::DYN_BYTES <= 227 * 1024, "fused epilogue state does not fit the shared memory of an SM");
+  using L = SmemLayout<2, true, FUSE_EPI_BYTES>;     // 2 stages of 48 KB leave room for the epilogue's state
   CUtensorMap mAh, mAl, mBh;
   int rc;
   if ((rc = make_map(&mAh, g.A_hi, g.M, g.Kd, g.lda, BM, true))) return rc;
   if ((rc = make_map(&mAl, g.A_lo, g.M, g.Kd, g.lda, BM, true))) return rc;
-  if ((rc = make_map(&mBh, g.B_hi, g.N, g.Kd, g.ldb, 256, true))) return rc;
+  if ((rc = make_map(&mBh, g.B_hi, g.N, g.Kd, g.ldb, BN, true))) return rc;
   int dev = 0, sms = 0;
   CNMF_CUDA_CHECK(cudaGetDevice(&dev));
   CNMF_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const int m_tiles = (g.M + BM - 1) / BM, n_tiles = (g.N + 255) / 256;
+  const int m_tiles = (g.M + BM - 1) / BM, n_tiles = (g.N + BN - 1) / BN;
   const int total_kb = (g.Kd + 2 * BK - 1) / (2 * BK);
   static bool attr_set[64] = {};
   if (dev < 0 || dev >= 64 || !attr_set[dev]) {
@@ -920,74 +739,9 @@ int launch_fused_w(const GemmArgs& g, cudaStream_t stream) {
   }
   const int items = m_tiles * n_tiles;
   const int grid = items < sms ? items : sms;
-  gemm_fused_w_kernel<<<grid, NUM_THREADS, L::DYN_BYTES, stream>>>(mAh, mAl, mBh, g.M, g.N, m_tiles, n_tiles, total_kb,
+  gemm_fused_w_kernel<<<grid, NUM_THREADS, L::DYN_BYTES, stream>>>(mAh, mAl, mBh, g.M, m_tiles, n_tiles, total_kb,
                                                                    g.out_col_scale, g.a_tile_scale, g.a_tiles,
                                                                    g.a_group_kb_shift > 0 ? g.a_group_kb_shift : 3, g.fuse);
-  CNMF_CUDA_CHECK(cudaGetLastError());
-  return 0;
-}
-
-// CTA-pair launch (exact-B forms): 256 x bn tiles, one cluster of two CTAs per tile, 4 stages of 48 KB
-template <int BN, int STAGES, bool F16>
-int launch_pair(const GemmArgs& g, cudaStream_t stream) {
-  using L = SmemLayout<BN, STAGES, true, true>;
-  static_assert(L::DYN_BYTES <= 227 * 1024, "CTA-pair stages do not fit the shared memory of an SM");
-  constexpr int BKE = F16 ? 2 * BK : BK;
-  CUtensorMap mAh, mAl, mBh;
-  int rc;
-  if ((rc = make_map(&mAh, g.A_hi, g.M, g.Kd, g.lda, BM, F16))) return rc;
-  if ((rc = make_map(&mAl, g.A_lo, g.M, g.Kd, g.lda, BM, F16))) return rc;
-  int dev = 0, sms = 0;
-  CNMF_CUDA_CHECK(cudaGetDevice(&dev));
-  CNMF_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const int m_pairs = (g.M + 2 * BM - 1) / (2 * BM);
-  int bn = g.bn;
-  if (bn <= 0 || bn > BN || bn % 16 != 0) bn = g.N <= BN ? ((g.N + 15) / 16) * 16 : BN;
-  {
-    static const int env_bn = env_int("CNMF_GEMM_BN", 0);
-    if (env_bn >= 16 && env_bn <= BN && env_bn % 16 == 0) bn = env_bn;
-  }
-  if ((rc = make_map(&mBh, g.B_hi, g.N, g.Kd, g.ldb, bn / 2, F16))) return rc;    // each CTA stages half of the B tile
-
-  const int n_tiles = (g.N + bn - 1) / bn;
-  const int total_kb = (g.Kd + BKE - 1) / BKE;
-  int splits = g.splits < 1 ? 1 : g.splits;
-  if (splits > total_kb) splits = total_kb;
-  int kb_per_split = (total_kb + splits - 1) / splits;
-  if (F16 && (kb_per_split & 1)) ++kb_per_split;
-  splits = (total_kb + kb_per_split - 1) / kb_per_split;
-  if (splits != g.splits_effective) { set_last_error("gemm: splits_effective mismatch (use gemm_effective_splits)"); return -1; }
-
-  auto kern = gemm_pair_kernel<BN, STAGES, F16>;
-  static bool attr_set[64] = {};
-  static int max_clusters[64] = {};
-  const int di = (dev >= 0 && dev < 64) ? dev : 0;
-  if (!attr_set[di]) {
-    CNMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::DYN_BYTES));
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(sms & ~1);
-    cfg.blockDim = dim3(NUM_THREADS);
-    cfg.dynamicSmemBytes = L::DYN_BYTES;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at;
-    cfg.numAttrs = 1;
-    int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess || n < 1) {
-      cudaGetLastError();
-      n = sms / 2;
-    }
-    max_clusters[di] = n;
-    attr_set[di] = true;
-  }
-  const int items = m_pairs * n_tiles * splits;
-  const int clusters = items < max_clusters[di] ? items : max_clusters[di];
-  const int chain_kb = pick_chain_kb<true, F16>(g);
-  kern<<<2 * clusters, NUM_THREADS, L::DYN_BYTES, stream>>>(mAh, mAl, mBh, g.C, g.M, g.N, g.ldc, g.c_split_stride,
-                                                            m_pairs, n_tiles, splits, total_kb, kb_per_split,
-                                                            chain_kb, bn, g.out_col_scale, g.a_tile_scale, g.a_tiles,
-                                                            g.a_group_kb_shift > 0 ? g.a_group_kb_shift : 3);
   CNMF_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
@@ -1004,44 +758,6 @@ int gemm_fixed_splits(int Kd, int f16) {
   const int total_kb = (Kd + bke - 1) / bke;
   const int s = std::max(1, std::min(16, (total_kb + 63) / 64));
   return gemm_effective_splits(Kd, s, f16);
-}
-
-// CTA pairs (cta_group::2): each SM pulls 48 KB instead of 64 KB of operands per k-block from L2.  MEASURED (run r2b,
-// profiles/r2b_gemm_pair_vs_1cta.log): correct (same bits as the 1-CTA kernel) but 0.65x its speed -- 387 vs 608 TFLOP/s on
-// the c2 W half, 487 vs 740 on 4096 x 16384 x 2000.  The 1-CTA kernel already runs at ~0.9 of the MMA rate its two passes
-// allow when timed alone, so the operand feed was not the limiter; what the pair adds is a cross-SM round trip (remote
-// mbarrier arrive + multicast commit) on EVERY 16-MMA accumulation chain, and with chains that short (the TMEM
-// truncation fix) the handshake, not the tensor pipe, paces the pair.  Kept as an opt-in (CNMF_GEMM_PAIR=1).
-bool gemm_uses_pair(int M, int b_exact) {
-  static const int env_pair = env_int("CNMF_GEMM_PAIR", 0);
-  return env_pair != 0 && b_exact && M > BM;
-}
-
-void gemm_plan(int M, int N, int Kd, int sm_count, int* splits_out, int* bn_out, int f16, int b_exact) {
-  const bool pair = gemm_uses_pair(M, b_exact || f16);
-  const int m_tiles = pair ? (M + 2 * BM - 1) / (2 * BM) : (M + BM - 1) / BM;
-  if (pair) sm_count /= 2;                                   // workers are CTA pairs
-  const int bke = f16 ? 2 * BK : BK;
-  const int total_kb = (Kd + bke - 1) / bke;
-  const int s = gemm_fixed_splits(Kd, f16);
-  const int kbps = (total_kb + s - 1) / s;
-  double best = -1.0;
-  int best_bn = 256;
-  // the tile width only groups output columns (no effect on any sum): narrow tiles (down to 128 columns; below
-  // that the accumulate warps, not the MMA chain, pace a tile) pay off when a compacted batch leaves less than
-  // one wave of 256-wide tiles
-  const int bn_lo = N <= 256 ? ((N + 15) / 16) * 16 : 128;
-  const int bn_hi = N <= 256 ? bn_lo : 256;
-  for (int bn = bn_hi; bn >= bn_lo; bn -= 16) {
-    const long long items = (long long)m_tiles * ((N + bn - 1) / bn) * s;
-    const long long waves = (items + sm_count - 1) / sm_count;
-    // tile cost bn + 64: per-tile A traffic / fill that does not shrink with bn; + 6 k-blocks of pipeline
-    // fill and epilogue per item
-    const double cost = (double)waves * (bn + 64) * (kbps + 6);
-    if (best < 0 || cost < best) { best = cost; best_bn = bn; }
-  }
-  *splits_out = s;
-  *bn_out = best_bn;
 }
 
 int gemm_effective_splits(int Kd, int splits, int f16) {
@@ -1061,7 +777,6 @@ int gemm_tf32x3(const GemmArgs& g, cudaStream_t stream) {
                 reinterpret_cast<uintptr_t>(g.B_hi) | reinterpret_cast<uintptr_t>(g.B_lo) |
                 reinterpret_cast<uintptr_t>(g.C) | reinterpret_cast<uintptr_t>(g.out_col_scale)) % 16 == 0,
                "gemm: pointers must be 16-byte aligned");
-  const bool pair = gemm_uses_pair(g.M, g.b_exact);
   if (g.f16) {
     CNMF_REQUIRE(g.b_exact, "gemm: the fp16 path needs an exact B operand");
     CNMF_REQUIRE(g.lda % 8 == 0 && g.ldb % 8 == 0, "gemm: fp16 leading dimensions must be multiples of 8 halves");
@@ -1073,14 +788,10 @@ int gemm_tf32x3(const GemmArgs& g, cudaStream_t stream) {
                    "gemm: incomplete fused-update arguments");
       return launch_fused_w(g, stream);
     }
-    if (pair) return launch_pair<256, 4, true>(g, stream);
-    return launch<256, 3, true, true>(g, stream);
+    return launch<4, true, true>(g, stream);
   }
-  if (g.b_exact) {
-    if (pair) return launch_pair<256, 4, false>(g, stream);
-    return launch<256, 3, true, false>(g, stream);
-  }
-  return launch<256, 2, false, false>(g, stream);
+  if (g.b_exact) return launch<4, true, false>(g, stream);
+  return launch<3, false, false>(g, stream);
 }
 
 }  // namespace cnmf

@@ -389,7 +389,7 @@ __global__ void __launch_bounds__(256) matrix_min_kernel(const float* __restrict
 }  // namespace
 
 int matrix_min(cnmf_handle_s* h, const float* X, int rows, int cols, int ld, float* out_host, cudaStream_t s) {
-  const int blocks = std::min(rows, 148 * 8);
+  const int blocks = std::min(rows, NUM_SMS * 8);
   float* d = static_cast<float*>(h->dev_buf("beta.min", sizeof(float) * blocks));
   if (!d) return -2;
   matrix_min_kernel<<<blocks, 256, 0, s>>>(X, rows, cols, ld, d);

@@ -44,7 +44,6 @@ namespace {
 
 struct GemmPlan {
   int splits;
-  int bn;                   // tile width for the tcgen05 kernel (0 = let the launcher choose)
   long long split_stride;   // elements
 };
 
@@ -59,7 +58,6 @@ int run_gemm(cnmf_handle_s* h, int precision, const float* A, const float* A_hi,
   g.c_split_stride = plan.split_stride;
   g.splits = plan.splits;
   g.splits_effective = plan.splits;
-  g.bn = plan.bn;
   h->launches += 1;
   const int slot = h->prof_begin(s, 2.0 * (double)g.M * (double)g.N * (double)g.Kd);
   int rc;
@@ -99,7 +97,7 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
   CNMF_REQUIRE(p.solver == CNMF_SOLVER_MU || p.solver == CNMF_SOLVER_CD, "solve: unknown solver");
   CNMF_REQUIRE(p.max_iter >= 1, "solve: max_iter must be >= 1");
   const bool tf32 = p.precision == CNMF_PRECISION_TF32X3;
-  const bool f16 = tf32 && v.f16;       // exact-count dataset created with CNMF_PRECISION_F16X2: kind::f16 products
+  const bool f16 = tf32 && v.f16;       // exact-count dataset created with CNMF_PRECISION_F16X2: f16 products
   const bool mu = p.solver == CNMF_SOLVER_MU;
 
   // ---- slot tables (host mirrors); slot s holds restart rid[s] at packed rows [off[s], off[s]+k[s])
@@ -116,10 +114,9 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
   const int kp = kmax <= 16 ? 16 : 32;
   // MU, f16x2, K <= 16, both factors iterated, whole gene reduction in one slice: the W-half update can run in the
   // epilogue of its own GEMM (gemm.h, struct FuseW) so that the product NUM_r is never materialised.  Parity-green
-  // (same n_iter, same accuracy class) but MEASURED SLOWER than GEMM + separate update kernel (c3: 715 vs 870
-  // restarts/s, run r2f): the epilogue's ~50 k warp-instructions per tile run on the 8 accumulate warps only (2 per
-  // scheduler, 168 registers of which 128 hold the tile) and do not overlap the tensor pipe beyond the two TMEM chain
-  // buffers.  Opt-in with CNMF_FUSE_W=1 until the update runs as a third warp role under the next tile's main loop.
+  // (same n_iter, same accuracy class); opt-in with CNMF_FUSE_W=1 because the epilogue runs on the two consumer
+  // warpgroups between tiles, not under the next tile's main loop, and GEMM + separate update kernel is faster
+  // (README.md: c2 on one H100).
   static const bool env_fuse_w = [] { const char* e = std::getenv("CNMF_FUSE_W"); return e && e[0] == '1'; }();
   const bool fuse_w = env_fuse_w && f16 && mu && kp == 16 && io.update_cols && gemm_fixed_splits(v.n_c, 1) == 1;
   // packing rule of the fused path: a restart never straddles a 128-row GEMM tile (its K rows meet in one CTA's
@@ -143,12 +140,13 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
   // restarts left a block should hold one tile, so that the work spreads over many SMs
   int cpb_r = 0, cpb_c = 0, chunks_r = 0, chunks_c = 0;
   auto plan_blocks = [&](int r_live) {
-    cpb_r = pick_cols_per_block(v.n_r, r_live, 4 * tile, tile, 148 * 8);
-    cpb_c = pick_cols_per_block(v.n_c, r_live, 4 * tile, tile, 148 * 8);
+    cpb_r = pick_cols_per_block(v.n_r, r_live, 4 * tile, tile, h->sm_count * 8);
+    cpb_c = pick_cols_per_block(v.n_c, r_live, 4 * tile, tile, h->sm_count * 8);
     chunks_r = (v.n_r + cpb_r - 1) / cpb_r;
     chunks_c = (v.n_c + cpb_c - 1) / cpb_c;
   };
-  const int gcpb_r = pick_cols_per_block(v.n_r, R0, 8192, 1024, 148 * 2), gcpb_c = pick_cols_per_block(v.n_c, R0, 8192, 1024, 148 * 2);
+  const int gcpb_r = pick_cols_per_block(v.n_r, R0, 8192, 1024, h->sm_count * 2);
+  const int gcpb_c = pick_cols_per_block(v.n_c, R0, 8192, 1024, h->sm_count * 2);
   const int chunks_cap = std::max((v.n_r + tile - 1) / tile, (v.n_c + tile - 1) / tile);   // finest chunking possible
   const int gchunks_max = std::max((v.n_r + gcpb_r - 1) / gcpb_r, (v.n_c + gcpb_c - 1) / gcpb_c);
   size_t fused_part_slots = 0;      // slot-indexed partials of the fused kernels: max over live counts of R * chunks
@@ -166,7 +164,7 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
   // per-block Gram partials of each factor (summed by the last block of the producing launch)
   const size_t gpart_elems0 = std::max((size_t)R0 * std::max(gchunks_max, std::max((v.n_r + 1023) / 1024, (v.n_c + 1023) / 1024)),
                                       fused_part_slots) * kp * kp;
-  const int ntiles_r = (v.n_r + 255) / 256;                 // item tiles of the fused W-half GEMM (one Gram partial each)
+  const int ntiles_r = (v.n_r + 127) / 128;                 // item tiles of the fused W-half GEMM (one Gram partial each)
   const size_t gpart_elems = std::max(gpart_elems0, fuse_w ? (size_t)R0 * ntiles_r * kp * kp : (size_t)0);
   double* d_gram_part = static_cast<double*>(h->dev_buf("solve.gram_part", sizeof(double) * 2 * gpart_elems));
   double* d_scal_part = static_cast<double*>(h->dev_buf("solve.scal_part", sizeof(double) * 2 * (size_t)R0 * chunks_cap));
@@ -174,18 +172,11 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
 
   GemmPlan plan_r, plan_c;   // plan_r: NUM_r = Fc * B_rows^T (reduce over n_c); plan_c: NUM_c = Fr * B_cols^T
   float *NUMr = nullptr, *NUMc = nullptr;
-  auto plan_one = [&](int sk, int n, int kd, GemmPlan* pl) {
-    if (tf32) {
-      gemm_plan(sk, n, kd, h->sm_count, &pl->splits, &pl->bn, f16 ? 1 : 0, v.exact ? 1 : 0);
-    } else {
-      pl->splits = gemm_fixed_splits(kd, 0);
-      pl->bn = 0;
-    }
-  };
+  // the split-K factor is a function of the reduction length only (gemm_fixed_splits)
   auto plan_gemms = [&]() -> int {
-    plan_one(SK, v.n_r, v.n_c, &plan_r);
+    plan_r.splits = gemm_fixed_splits(v.n_c, f16 ? 1 : 0);
     plan_r.split_stride = (long long)SK * v.ld_r;
-    plan_one(SK, v.n_c, v.n_r, &plan_c);
+    plan_c.splits = gemm_fixed_splits(v.n_r, f16 ? 1 : 0);
     plan_c.split_stride = (long long)SK * v.ld_c;
     return 0;
   };
@@ -193,11 +184,8 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
   // size the product buffers: the split-K factor depends on the reduction length only, the rows never exceed SKcap
   // (padded packing of the fused path included)
   {
-    GemmPlan a, b2;
-    plan_one(SKcap, v.n_r, v.n_c, &a);
-    plan_one(SKcap, v.n_c, v.n_r, &b2);
-    const size_t need_r = (size_t)a.splits * (size_t)SKcap * v.ld_r;
-    const size_t need_c = (size_t)b2.splits * (size_t)SKcap * v.ld_c;
+    const size_t need_r = (size_t)plan_r.splits * (size_t)SKcap * v.ld_r;
+    const size_t need_c = (size_t)plan_c.splits * (size_t)SKcap * v.ld_c;
     NUMr = fuse_w ? nullptr : static_cast<float*>(h->dev_buf("solve.NUMr", sizeof(float) * need_r));
     NUMc = io.update_cols ? static_cast<float*>(h->dev_buf("solve.NUMc", sizeof(float) * need_c)) : nullptr;
     if ((!fuse_w && !NUMr) || (io.update_cols && !NUMc)) return -2;
@@ -358,7 +346,7 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
     fz.gram_part = d_gpartR;
     fz.active = 1;
     GemmPlan pl = plan_r;
-    pl.splits = 1; pl.bn = 256;
+    pl.splits = 1;
     return run_gemm(h, p.precision, wFc, wFc_hi, wFc_lo, SK, v.ld_c, v.B_rows, nullptr, v.ld_r, pl, v.exact, v.scale_r,
                     f16, d_rs_c, s, 512, &fz);
   };

@@ -174,17 +174,17 @@ __global__ void sums_final_kernel(const double* __restrict__ part, int nblocks, 
 }
 
 // ------------------------------------------------------------------ fp16 operand pieces (f16x2 precision)
-// kind::f16 MMAs run at twice the kind::tf32 rate and fp16 carries the same 11-bit significand as tf32; what it
+// f16 MMAs run at twice the tf32 rate and fp16 carries the same 11-bit significand as tf32; what it
 // lacks is exponent range.  So every group of 512 reduction elements of a packed factor row is divided by a power
 // of two that puts its largest entry (times the per-column scale of the exact-count path) in [2^14, 2^15) -- far
 // above fp16's subnormals -- and split into hi = fp16(x), mid = fp16(x - hi): 22 significant bits like the tf32 pair,
-// absolute error <= 2^-39 of the group maximum for entries too small to keep them.  The GEMM multiplies each drained
-// 128-element chain by the group's power of two.
+// absolute error <= 2^-39 of the group maximum for entries too small to keep them.  The GEMM multiplies each finished
+// 128-element MMA chain by the group's power of two.
 // The pieces are a pure function of the factor values: this stand-alone kernel (initial factors, re-packing after a
 // compaction, K > 16 batches) and the in-update emission (emit_tile_f16) produce the same bits, so a restart's
 // operands do not depend on when the batch around it was compacted.
 // One block per row, one warp per group of 128 * QUADS columns (512: what the update kernels' tiles emit; 128: what the
-// fused GEMM epilogue emits, one group per thread), a lane owns QUADS 16-byte quads of the group.
+// fused GEMM epilogue emits, one group per 128-item tile), a lane owns QUADS 16-byte quads of the group.
 template <int QUADS>
 __global__ void __launch_bounds__(256)
 emit_f16_kernel(const float* __restrict__ F, int n, int ld, const float* __restrict__ pscale, __half* __restrict__ hi,
@@ -245,22 +245,20 @@ __global__ void to_half_kernel(const float* __restrict__ src, __half* __restrict
 }
 
 // ------------------------------------------------------------------ update kernels (fused with the Gram)
-// Thread = VEC consecutive items (cells / genes) of one restart, held as packed fp32 pairs: every array is
-// touched with one 16-byte (VEC = 4) access per component, and the K x K contraction with the Gram of the
-// other factor runs on FFMA2 (two items per instruction, the Gram entry a broadcast operand read from shared
-// memory as LDS.128 = 4 entries x 2 pairs = 8 packed FMAs per shared-memory instruction).  The quotient is
+// Thread = VEC consecutive items (cells / genes) of one restart, held as fp32 pairs: every array is touched with
+// one 16-byte (VEC = 4) access per component, and the K x K contraction with the Gram of the other factor runs on
+// item pairs (fma2 of common.cuh: two round-to-nearest FFMAs, the Gram entry read from shared memory as LDS.128 =
+// 4 entries x 2 pairs = 8 pair-FMAs per shared-memory instruction).  The quotient is
 // the branch-free MUFU.RCP + Newton sequence of common.cuh.  The unrolled body is instantiated per K rounded
 // up to 4 and dispatched per restart inside the kernel (block-uniform switch), so a K = 10 restart runs the
 // 12 x 12 body even when the batch also holds K = 13 restarts.
 //
 // The Gram of the UPDATED factor (needed by the next half-iteration's update and by the trace-form error) is
 // accumulated in the same launch: the block parks its new values in a shared-memory tile (components x
-// tile columns), the warps split the K x K entries by rows and walk the tile with packed FMAs, per-thread
+// tile columns), the warps split the K x K entries by rows and walk the tile with pair FMAs, per-thread
 // fp32 sums over at most 16 columns go through shared memory into per-block fp64 sums (fixed order), and the
-// last block of a restart adds the per-block partials in chunk order (FusedOut).  The first version -- a scalar
-// thread-per-item update (1 052 warp instructions per item at K = 10: 4-byte accesses, 3-register FFMA,
-// IEEE division) plus a separate Gram launch re-reading the factor -- spent 168 us per W half at c2 against 107 us
-// of DRAM time; see profiles/r1e_ncu_full_summary.txt.
+// last block of a restart adds the per-block partials in chunk order (FusedOut), so the factor is not re-read by a
+// separate Gram launch.
 template <int VEC> struct VecIO;
 template <> struct VecIO<4> {
   static constexpr int NP = 2;
@@ -642,8 +640,8 @@ __device__ __forceinline__ float2 mu_components(float* __restrict__ pFc, float* 
   constexpr int NP = VecIO<VEC>::NP;
   constexpr int TILE = UPD_THREADS * VEC;
   float2 sacc = make_float2(0.f, 0.f);
-  // products of components c + 1 and c + 2 in flight: one component of lead (~80 instructions) left the quotient
-  // waiting on the load (15 % of the kernel's stall samples, profiles/r2s_ncu_update_summary.txt)
+  // products of components c + 1 and c + 2 in flight: with one component of lead (~80 instructions) the quotient
+  // waits on the load
   float2 nvn[NP], nvn2[NP];
   VecIO<VEC>::ld(pNc, nvn);
   VecIO<VEC>::ld(pNc + (1 < K ? ld : 0u), nvn2);
@@ -713,7 +711,7 @@ __device__ __forceinline__ float2 mu_components(float* __restrict__ pFc, float* 
 // the thread's items -- are read back from the shared-memory tiles the load phase parked them in (tileF doubles as
 // the Gram tile: row c is overwritten with the new values once iteration c is done with it).  One compact loop
 // body (~80 instructions) instead of K unrolled copies: no per-component predicates for K < KP, and the code
-// stays resident in the instruction cache (the unrolled version stalled on instruction fetch, profiles/r1g_*).
+// stays resident in the instruction cache (an unrolled body is tens of KB per K).
 // Returns <NUM, F_new> over the thread's items (fp32 within a tile, fp64 across tiles).
 template <int KP, int VEC, bool GRAM, bool STREAMN>
 __device__ __forceinline__ double mu_body(const FactorView& f, const float* __restrict__ NUM, int nsplit,
@@ -1284,7 +1282,7 @@ int launch_split_tf32(const float* src, float* hi, float* lo, long long n_elems,
   CNMF_REQUIRE(n_elems % 4 == 0, "split_tf32: element count must be a multiple of 4");
   const long long n4 = n_elems / 4;
   if (n4 == 0) return 0;
-  const int blocks = (int)((n4 + 255) / 256 < 148 * 16 ? (n4 + 255) / 256 : 148 * 16);
+  const int blocks = (int)((n4 + 255) / 256 < NUM_SMS * 16 ? (n4 + 255) / 256 : NUM_SMS * 16);
   split_tf32_kernel<<<blocks, 256, 0, s>>>(src, hi, lo, n4);
   CNMF_CUDA_CHECK(cudaGetLastError());
   return 0;
@@ -1294,7 +1292,7 @@ int launch_split_scaled(const float* src, float* hi, float* lo, int rows, int ld
   CNMF_REQUIRE(ld % 4 == 0, "split_scaled: ld must be a multiple of 4");
   const long long n4 = (long long)rows * (ld / 4);
   if (n4 == 0) return 0;
-  const int blocks = (int)((n4 + 255) / 256 < 148 * 16 ? (n4 + 255) / 256 : 148 * 16);
+  const int blocks = (int)((n4 + 255) / 256 < NUM_SMS * 16 ? (n4 + 255) / 256 : NUM_SMS * 16);
   split_scaled_kernel<<<blocks, 256, 0, s>>>(src, hi, lo, rows, ld, col_scale);
   CNMF_CUDA_CHECK(cudaGetLastError());
   return 0;
@@ -1319,7 +1317,7 @@ int launch_to_half(const float* src, void* dst, long long n_elems, cudaStream_t 
   CNMF_REQUIRE(n_elems % 4 == 0, "to_half: element count must be a multiple of 4");
   const long long n4 = n_elems / 4;
   if (n4 == 0) return 0;
-  const int blocks = (int)((n4 + 255) / 256 < 148 * 16 ? (n4 + 255) / 256 : 148 * 16);
+  const int blocks = (int)((n4 + 255) / 256 < NUM_SMS * 16 ? (n4 + 255) / 256 : NUM_SMS * 16);
   to_half_kernel<<<blocks, 256, 0, s>>>(src, static_cast<__half*>(dst), n4);
   CNMF_CUDA_CHECK(cudaGetLastError());
   return 0;
@@ -1337,14 +1335,14 @@ int launch_min_positive(const float* X, int rows, int cols, int ld, float* col_m
 
 int launch_check_scaled_int(const float* X, int rows, int cols, int ld, const float* row_scale, const float* col_scale,
                             int* n_bad, cudaStream_t s) {
-  check_scaled_int_kernel<<<148 * 8, 256, 0, s>>>(X, rows, cols, ld, row_scale, col_scale, n_bad);
+  check_scaled_int_kernel<<<NUM_SMS * 8, 256, 0, s>>>(X, rows, cols, ld, row_scale, col_scale, n_bad);
   CNMF_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
 
 int launch_build_counts(const float* X, int rows, int cols, int ld, const float* row_scale, const float* col_scale,
                         float* C, cudaStream_t s) {
-  build_counts_kernel<<<148 * 8, 256, 0, s>>>(X, rows, cols, ld, row_scale, col_scale, C);
+  build_counts_kernel<<<NUM_SMS * 8, 256, 0, s>>>(X, rows, cols, ld, row_scale, col_scale, C);
   CNMF_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
@@ -1366,7 +1364,7 @@ int launch_transpose(const float* src, int rows, int cols, int ld_src, float* ds
 
 int launch_matrix_sums(const float* X, int rows, int cols, int ld, double* out2, double* scratch, int scratch_len,
                        cudaStream_t s) {
-  int blocks = 148 * 8;
+  int blocks = NUM_SMS * 8;
   if (2 * blocks > scratch_len) blocks = scratch_len / 2;
   CNMF_REQUIRE(blocks >= 1, "matrix_sums: scratch too small");
   sums_partial_kernel<<<blocks, 256, 0, s>>>(X, rows, cols, ld, scratch);
@@ -1406,9 +1404,7 @@ static int launch_update_inst(dim3 grid, const FactorView& f, const float* NUM, 
 // MU with the fused Gram at kp == 16, CNMF_UPD_VARIANT: 2 (default) = products streamed from global memory one
 // component ahead of their use, no product tile in shared memory, 4 blocks per SM (128 registers); 0 = round 1's
 // layout (products staged in a second shared-memory tile, 3 blocks per SM); 1 / 3 = streamed at 3 / 5 blocks per SM.
-// Measured on c3 (profiles/r2m_update_variants.log): update launches 1031 / 1085 / 962 / 1065 ms per 3 steps for
-// variants 0 / 1 / 2 / 3 -- the kernel is bound by its instruction count, not by occupancy; every variant computes the
-// same bits.
+// Every variant computes the same bits.
 static int upd_variant() {
   static int v = -1;
   if (v < 0) {

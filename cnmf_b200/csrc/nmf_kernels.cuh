@@ -36,7 +36,7 @@ struct FactorView {
 };
 
 // block granularity: large enough to amortise the per-block prologue, small enough that
-// (column chunks) x (restarts) fills the 148 SMs a few times over even for a single refit
+// (column chunks) x (restarts) fills the SMs a few times over even for a single refit
 inline int pick_cols_per_block(int n, int n_restarts, int max_cols, int min_cols, int min_blocks) {
   int c = max_cols;
   while (c > min_cols && (long long)((n + c - 1) / c) * n_restarts < min_blocks) c /= 2;

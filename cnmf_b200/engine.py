@@ -11,14 +11,14 @@ from . import _lib
 from ._lib import (LOSS_FROBENIUS, LOSS_ITAKURA_SAITO, LOSS_KULLBACK_LEIBLER, NmfParams, PRECISION_FP32,
                    PRECISION_F16X2, PRECISION_TF32X3, PRECISION_TF32X3_GENERAL, SOLVER_CD, SOLVER_MU, check, f32c, ptr)
 
-# default: split-operand tensor-core products with fp32-class accuracy -- 2 kind::f16 passes when X is recognised as
-# scaled integer counts (what the reference factorizes), 3 kind::tf32 passes otherwise
+# default: split-operand tensor-core products with fp32-class accuracy -- 2 f16 passes when X is recognised as
+# scaled integer counts (what the reference factorizes), 3 tf32 passes otherwise
 _DEFAULT_PRECISION = PRECISION_F16X2
 
 
 def precision_code(p):
     """'fp32' | 'tf32x3' (default; 2-pass products when X is scaled integer counts) | 'f16x2' (like tf32x3, but the
-    2-pass products of scaled-integer-count matrices run on kind::f16 MMAs) | 'tf32x3-general' (always 3-pass)."""
+    2-pass products of scaled-integer-count matrices run on f16 MMAs) | 'tf32x3-general' (always 3-pass)."""
     if p in (PRECISION_FP32, PRECISION_TF32X3, PRECISION_TF32X3_GENERAL, PRECISION_F16X2):
         return p
     return {"fp32": PRECISION_FP32, "tf32x3": PRECISION_TF32X3, "tf32x3-general": PRECISION_TF32X3_GENERAL,
@@ -284,7 +284,7 @@ class Dataset:
 
     @property
     def f16(self):
-        """True when the big products run as 2 kind::f16 passes (exact dataset created with precision='f16x2')."""
+        """True when the big products run as 2 f16 passes (exact dataset created with precision='f16x2')."""
         return self.lib.cnmf_dataset_is_exact(self._d) == 2
 
     def min(self):

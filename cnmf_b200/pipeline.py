@@ -1,5 +1,5 @@
 """`cNMF` facade: the reference's class / file ledger / method signatures (cnmf.py:265-1210) over the
-B200 engine.  Host logic only (paths, seeds, job split, DataFrame labelling, file I/O); the numerics of
+H100 engine.  Host logic only (paths, seeds, job split, DataFrame labelling, file I/O); the numerics of
 factorize and consensus run in libcnmf_b200.so.  Nothing here falls back to scikit-learn.
 
 Drop-in points (reference file:line -> here)
@@ -128,7 +128,7 @@ class cNMF:
                       else os.path.join(base, self.name + suffix) for key, tmp, suffix in _PATH_SPECS}
 
     def engine(self):
-        """The GPU engine (created on first use; raises without a B200 -- there is no CPU path)."""
+        """The GPU engine (created on first use; raises without an H100 -- there is no CPU path)."""
         if self._engine is None:
             from .engine import Engine
             dev = self.device
@@ -600,7 +600,7 @@ def main():
     ap.add_argument("--prepare-on-device", dest="prepare_on_device", action="store_true", default=False,
                     help="[cnmf_b200] prepare: cell totals, TPM gene statistics and the HVG matrix computed on the GPU")
     ap.add_argument("--precision", type=str, choices=["f16x2", "tf32x3", "fp32"], default="f16x2",
-                    help="[cnmf_b200] big products: split-fp16 tcgen05 MMAs for scaled-integer-count matrices, split-TF32 "
+                    help="[cnmf_b200] big products: split-fp16 wgmma MMAs for scaled-integer-count matrices, split-TF32 "
                          "otherwise (default); split-TF32 always; or FFMA fp32")
     a = ap.parse_args()
     obj = cNMF(output_dir=a.output_dir, name=a.name, precision=a.precision)

@@ -1,9 +1,9 @@
-/* cnmf_b200 -- C ABI of the B200-native consensus-NMF hot path.
+/* cnmf_b200 -- C ABI of the H100-native consensus-NMF hot path.
  *
  * Plain C, plain pointers and sizes, no torch / C++ types.  This is the boundary a reference
  * maintainer binds instead of scikit-learn at the seam
  *
- *     cNMF._nmf(X, nmf_kwargs) -> (spectra, usages)          /root/reference/src/cnmf/cnmf.py:661-674
+ *     cNMF._nmf(X, nmf_kwargs) -> (spectra, usages)          cnmf.py:661-674
  *
  * which the reference calls from cNMF.factorize (cnmf.py:735-745, one call per (k, seed)
  * restart) and cNMF.refit_usage (cnmf.py:776-802, update_H=False), plus the numeric steps of
@@ -35,11 +35,11 @@ typedef struct cnmf_handle_s* cnmf_handle_t;
 typedef struct cnmf_dataset_s* cnmf_dataset_t;
 
 enum { CNMF_SOLVER_MU = 0, CNMF_SOLVER_CD = 1 };            /* yaml 'solver': cnmf.py:618-631 */
-/* FFMA | tcgen05 3xTF32 with exact-count detection (default: 2 passes when X is scaled integers, else 3) |
- * tcgen05 3xTF32 always in the general 3-pass form.  Params for a dataset created with 2 use precision 1. */
+/* FFMA | wgmma 3xTF32 with exact-count detection (default: 2 passes when X is scaled integers, else 3) |
+ * wgmma 3xTF32 always in the general 3-pass form.  Params for a dataset created with 2 use precision 1. */
 enum { CNMF_PRECISION_FP32 = 0, CNMF_PRECISION_TF32X3 = 1, CNMF_PRECISION_TF32X3_GENERAL = 2,
        /* dataset_create only: like TF32X3, but when X is recognised as scaled integer counts the big products run as
-        * 2 kind::f16 tensor-core passes (integer operand exact in fp16, factor = two fp16 pieces of its row-normalised
+        * 2 f16 tensor-core passes (integer operand exact in fp16, factor = two fp16 pieces of its row-normalised
         * values: the same 22 significant bits as the tf32 pair at twice the MMA rate); params.precision stays TF32X3 */
        CNMF_PRECISION_F16X2 = 3 };
 
@@ -109,7 +109,7 @@ int cnmf_dataset_min(cnmf_dataset_t d, float* min_host, void* stream);
  * HVG-normalised counts (cnmf.py:542) and TPM (cnmf.py:245-251) are -- and therefore runs the 2-pass
  * tensor-core products (the integer operand needs no tf32 "lo" piece); 0 = general 3-pass 3xTF32.
  * CNMF_EXACT=0 in the environment disables the detection.  Returns 2 when, in addition, the dataset was created with
- * CNMF_PRECISION_F16X2 and the 2 passes therefore run on kind::f16 MMAs. */
+ * CNMF_PRECISION_F16X2 and the 2 passes therefore run on f16 MMAs. */
 int cnmf_dataset_is_exact(cnmf_dataset_t d);
 /* per-column mean and population variance (StandardScaler(with_mean=False), cnmf.py:131-134) */
 int cnmf_dataset_col_stats(cnmf_dataset_t d, double* mean_host, double* var_host, void* stream);
@@ -197,7 +197,7 @@ int cnmf_refit(cnmf_dataset_t d, int transposed, int k, const float* fixed_host,
 int cnmf_project_rows(cnmf_dataset_t d, int k, const float* Ut_host, float* out_host, void* stream);
 
 /* test / micro-benchmark hook: C (M x N) = A (M x Kd) * B (N x Kd)^T through the same GEMM kernels the
- * solver uses (precision selects FFMA or tcgen05 3xTF32); reps > 1 reports mean device ms per launch. */
+ * solver uses (precision selects FFMA or wgmma 3xTF32); reps > 1 reports mean device ms per launch. */
 int cnmf_gemm_abt_host(cnmf_handle_t h, int precision, const float* A, const float* B, int M, int N, int Kd,
                        int splits, float* C, int reps, float* ms_out, void* stream);
 

@@ -1,6 +1,6 @@
 """ORACLE (test infrastructure) -- numpy restatement of the numerics of ``cNMF.consensus``
 (cnmf.py:823-985) and of the scikit-learn 1.9.0 routines it calls (``SK/`` = site-packages/
-sklearn; third-party, not under /root/reference).  Each function cites what it restates.
+sklearn; third-party, not part of the reference).  Each function cites what it restates.
 Pinned by tests/test_oracle_golden.py against fixtures the reference itself produced
 (oracle/make_golden.py).
 """

@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Generate tests/golden/*.npz by running the UNMODIFIED reference
-(/root/reference/src/cnmf/cnmf.py, loaded through oracle/refshim.py) in the build container.
+(src/cnmf/cnmf.py of a dylkot/cNMF checkout, loaded through oracle/refshim.py).
 
-    python -m oracle.make_golden            # from the repo root; needs /root/reference
+    CNMF_REFERENCE=<cNMF checkout> python -m oracle.make_golden      # from the repo root
 
 Test infrastructure (see oracle/__init__.py).  The reference's own golden tarballs are
 network downloads (download_pytest_data.py:38-52) and are not available offline, so these
@@ -23,9 +23,11 @@ BASELINE.json configs[0] -- 1 000 cells x 500 HVG, K=7, 10 restarts -- in full) 
   fp32dev_k<K>    per restart: rel-L2 between scikit-learn's OWN float32 path and the reference (float64)
                   spectra for the same seed -- a conditioning yardstick for fp32-class implementations
                   (computed with a direct sklearn call; the reference itself always runs float64)
+``path_table.json``: the reference cNMF object's ``paths`` table (output_dir-relative, name "run").
 Everything derives from RandomState seeds, so the script is reproducible bit for bit on the
 same library versions (numpy 2.3.5, scikit-learn 1.9.0, pandas 3.0.2).
 """
+import json
 import os
 import shutil
 import sys
@@ -119,7 +121,21 @@ def run_case(tag, spec):
     print(tag, "->", {k: getattr(v, "shape", v) for k, v in out.items()})
 
 
+def path_table():
+    tmp = tempfile.mkdtemp()
+    try:
+        paths = refshim.load_reference().cNMF(output_dir=tmp, name="run").paths
+        rel = {k: os.path.relpath(v, tmp) for k, v in paths.items()}
+    finally:
+        shutil.rmtree(tmp, ignore_errors=True)
+    with open(os.path.join(GOLDEN_DIR, "path_table.json"), "w") as f:
+        json.dump(rel, f, indent=1, sort_keys=True)
+        f.write("\n")
+
+
 if __name__ == "__main__":
+    if len(sys.argv) == 1 or "path_table" in sys.argv[1:]:
+        path_table()
     for tag, spec in CASES.items():
         if len(sys.argv) == 1 or tag in sys.argv[1:]:      # `python -m oracle.make_golden sim_kl` regenerates one
             run_case(tag, spec)

@@ -2,14 +2,15 @@
 """Generate tests/golden/big_samples.npz: the reference's own NMF call on SAMPLED restarts of the
 BASELINE.json configurations whose full run would take hours on the host.
 
-    python -m oracle.make_golden_big [case ...]        # from the repo root, build container
+    python -m oracle.make_golden_big [case ...]        # from the repo root (scikit-learn only)
 
 Test infrastructure (see oracle/__init__.py).  What the reference executes per (k, seed) job is one
 `sklearn.decomposition.non_negative_factorization(X, **kwargs)` (cnmf.py:661-674, called at cnmf.py:741
 with the kwargs of cnmf.py:618-631) on the float64 normalised counts (cnmf.py:534-542);
 `oracle/reference_path.factorize` issues exactly that call.  Inputs are the deterministic synthetic
 matrices of SURVEY.md section 8d (cnmf_b200.synth, seeds of cnmf.py:597-610), so only the OUTPUTS are
-stored: per sample `H_<name>` (k x G float64), `it_<name>` (n_iter) and `meta_<name>` =
+stored: per sample `H_<name>` (k x G, the reference's float64 result rounded to float32: 6e-8 relative, far
+inside the 1e-4 tolerance, and it keeps the file under 1 MB), `it_<name>` (n_iter) and `meta_<name>` =
 [n_cells, n_genes, k, iter index, seed, solver is cd].
 
 Cases (name: shape, K-list of the job table, sampled (k, iter) jobs, solver)
@@ -60,7 +61,7 @@ def main():
             seed = lookup[(k, it)]
             t0 = time.perf_counter()
             H, n_it, _ = reference_path.factorize(X, [(k, seed)], solver)
-            out["H_" + tag] = H[0]
+            out["H_" + tag] = H[0].astype(np.float32)
             out["it_" + tag] = np.int64(n_it[0])
             out["meta_" + tag] = np.array([X.shape[0], X.shape[1], k, it, seed, int(solver == "cd")], dtype=np.int64)
             print(tag, "n_iter", n_it[0], "%.1f s" % (time.perf_counter() - t0), flush=True)

@@ -1,7 +1,7 @@
 """ORACLE (test infrastructure) -- numpy restatement of the NMF solvers the reference
 reaches through ``cNMF._nmf`` (cnmf.py:661-674 -> sklearn.decomposition.non_negative_factorization).
 
-The arithmetic lives in scikit-learn 1.9.0 (third-party, NOT under /root/reference;
+The arithmetic lives in scikit-learn 1.9.0 (third-party, NOT part of the reference;
 ``SK/`` below = site-packages/sklearn).  Each function cites the lines it restates.
 Pinned by tests/test_oracle_golden.py against fixtures produced by the reference itself
 (oracle/make_golden.py) and against live sklearn calls.

@@ -1,12 +1,12 @@
 """ORACLE / CPU BASELINE (test infrastructure) -- the reference's own call sequence for the hot path,
-executed on scikit-learn exactly as /root/reference/src/cnmf/cnmf.py does:
+executed on scikit-learn exactly as the reference's src/cnmf/cnmf.py does:
 
   factorize : one `non_negative_factorization(X, **kwargs)` per (k, seed) job, sequentially
               (cnmf.py:735-745 -> _nmf, cnmf.py:661-674), kwargs from get_nmf_iter_params (cnmf.py:618-631)
   consensus : the numeric steps of cnmf.py:871-975 with sklearn KMeans / euclidean_distances
 
 scikit-learn is a third-party dependency of the reference that IS part of the image, so this module
-travels to the GPU box (unlike /root/reference itself).  Only tests/, __graft_entry__.smoke() and
+runs anywhere (unlike the reference checkout itself).  Only tests/, __graft_entry__.smoke() and
 bench.py's cpu_baseline / --impl reference arm may call it.
 """
 import time

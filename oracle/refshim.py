@@ -1,5 +1,5 @@
-"""Load the UNMODIFIED reference module /root/reference/src/cnmf/cnmf.py in the build
-container (test infrastructure; see oracle/__init__.py).
+"""Load the UNMODIFIED reference module src/cnmf/cnmf.py of a dylkot/cNMF checkout named by the CNMF_REFERENCE
+environment variable (test infrastructure for the fixture generators; see oracle/__init__.py).
 
 The reference imports ``scanpy`` and ``matplotlib`` at module level (cnmf.py:24,26); neither
 is installed here and there is no network.  This file registers minimal stand-ins in
@@ -15,8 +15,8 @@ is installed here and there is no network.  This file registers minimal stand-in
 and then loads cnmf.py by file path so that ``cnmf/__init__.py`` (which imports
 preprocess.py -> scanpy/harmonypy) is not executed.
 
-This module only works where /root/reference exists (the build container).  Nothing
-that runs on the GPU box may import it.
+This module only works where such a checkout exists.  No test imports it: the tests compare against the fixtures
+it produced (tests/golden/).
 """
 import importlib.util
 import os
@@ -28,7 +28,12 @@ import numpy as np
 import pandas as pd
 import scipy.sparse as sp
 
-REFERENCE_FILE = "/root/reference/src/cnmf/cnmf.py"
+def reference_file():
+    """src/cnmf/cnmf.py of the checkout named by CNMF_REFERENCE (an explicit error when the variable is unset)."""
+    root = os.environ.get("CNMF_REFERENCE")
+    if not root:
+        raise RuntimeError("CNMF_REFERENCE is not set: point it at a dylkot/cNMF checkout")
+    return os.path.join(root, "src", "cnmf", "cnmf.py")
 
 
 class AnnDataLite:
@@ -118,10 +123,11 @@ def load_reference():
     global _REF
     if _REF is not None:
         return _REF
-    if not os.path.exists(REFERENCE_FILE):
-        raise RuntimeError("reference source not present (only available in the build container)")
+    path = reference_file()
+    if not os.path.exists(path):
+        raise RuntimeError("reference source not found: %s (CNMF_REFERENCE)" % path)
     _install_stubs()
-    spec = importlib.util.spec_from_file_location("cnmf_reference_module", REFERENCE_FILE)
+    spec = importlib.util.spec_from_file_location("cnmf_reference_module", path)
     mod = importlib.util.module_from_spec(spec)
     # AnnDataLite must be picklable under a stable module name
     spec.loader.exec_module(mod)

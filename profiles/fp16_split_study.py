@@ -1,8 +1,8 @@
 """CPU emulation: does a 2-piece fp16 factor split (per-row power-of-two normalisation) keep the MU iteration within
 the parity budget?  Compared with the current 2-piece tf32 split.  Products accumulate in float64 here (the operand
 representation is what is being tested)."""
-import sys, numpy as np
-sys.path.insert(0, '/root/repo')
+import os, sys, numpy as np
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from cnmf_b200.synth import make_counts, normalise, restart_table
 EPS = np.finfo(np.float32).eps
 

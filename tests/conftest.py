@@ -13,7 +13,7 @@ from cnmf_golden import load_golden  # noqa: E402  (tests/cnmf_golden.py; unique
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90)")
 
 
 @pytest.fixture(scope="session", params=["sim_mu", "sim_cd", "sim_kl", "sim_nndsvd", "c1_mu", "c1_cd"])

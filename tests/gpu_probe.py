@@ -1,12 +1,13 @@
 #!/usr/bin/env python
 """GPU bring-up probe (not a pytest file): run one stage per process so that a hung kernel
-only costs its own `timeout`.  Usage on the GPU box:
+only costs its own `timeout`.  Usage on a machine with an H100:
 
     for s in gemm_fp32 gemm_tf32 nmf_fp32 nmf_tf32 perf; do timeout 300 python tests/gpu_probe.py $s; done
 """
 import json
 import os
 import sys
+import tempfile
 import time
 import warnings
 
@@ -167,8 +168,8 @@ def stage_consensus_c4():
 
 
 def stage_consensus_kernels():
-    """One pass over the consensus kernels at BASELINE configs[3] size (R = 4000 x 2000, K = 20) -- the launch set
-    `ncu --set full -k regex:...` captures for the HBM roofline table in profiles/."""
+    """One pass over the consensus kernels at BASELINE configs[3] size (R = 4000 x 2000, K = 20): the launch set to
+    profile for the consensus stage's HBM roofline."""
     from cnmf_b200 import consensus as cs
     eng = Engine()
     rng = np.random.RandomState(11)
@@ -299,8 +300,9 @@ def stage_perf():
                     print("   oracle restart %d: n_iter %d (gpu %d) rel-L2 %.3e  cpu %.1fs" % (
                         r, it, n_iter[r], rel(sp[r], H), time.time() - t3), flush=True)
         ds.close()
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    json.dump(out, open(os.path.join(ROOT, "gpurun_out", "probe_perf.json"), "w"), indent=1)
+    out_dir = os.environ.get("PROBE_OUT", tempfile.gettempdir())
+    os.makedirs(out_dir, exist_ok=True)
+    json.dump(out, open(os.path.join(out_dir, "probe_perf.json"), "w"), indent=1)
 
 
 def stage_consensus():

@@ -1,5 +1,6 @@
 """CPU tests: C-ABI surface, host RNG, file ledger, prepare(), job sharding, gloo all-gather."""
 import ctypes
+import json
 import os
 import re
 import subprocess
@@ -68,11 +69,10 @@ def test_path_table_matches_reference(tmp_path):
     obj = cNMF(output_dir=str(tmp_path), name="run")
     assert obj.paths["iter_spectra"] % (7, 3) == os.path.join(str(tmp_path), "run", "cnmf_tmp", "run.spectra.k_7.iter_3.df.npz")
     assert obj.paths["consensus_usages__txt"] % (7, "0_1") == os.path.join(str(tmp_path), "run", "run.usages.k_7.dt_0_1.consensus.txt")
-    ref_file = "/root/reference/src/cnmf/cnmf.py"
-    if os.path.exists(ref_file):          # build container only: compare against the reference's own table
-        from oracle import refshim
-        ref = refshim.load_reference().cNMF(output_dir=str(tmp_path), name="run")
-        assert ref.paths == obj.paths
+    # the reference's own table (oracle/make_golden.py path_table), stored relative to output_dir
+    with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "path_table.json")) as f:
+        ref = {k: os.path.join(str(tmp_path), v) for k, v in json.load(f).items()}
+    assert ref == obj.paths
 
 
 def test_worker_split_rules():

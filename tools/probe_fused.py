@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""GPU probe: fused W-half epilogue on a multi-tile, mixed-K batch (small enough for compute-sanitizer) against the
-numpy oracle.  CNMF_FUSE_W=0/1 selects the path."""
+"""GPU probe: a multi-tile, mixed-K batch against the numpy oracle, for whichever kernel variant the environment
+selects (CNMF_FUSE_W, CNMF_UPD_VARIANT)."""
 import json, os, sys, time
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -19,7 +19,7 @@ kw = dict(solver="mu", beta_loss=2.0, tol=1e-4, max_iter=400)
 t0 = time.perf_counter()
 sp, _, n_iter, err = ds.factorize([r[0] for r in rows], [r[2] for r in rows], kw)
 dt = time.perf_counter() - t0
-out = {"fuse": os.environ.get("CNMF_FUSE_W", "1"), "SK": int(sum(r[0] for r in rows)), "sec": round(dt, 3), "n_iter": [int(x) for x in n_iter]}
+out = {"fuse": os.environ.get("CNMF_FUSE_W", "0"), "variant": os.environ.get("CNMF_UPD_VARIANT", ""), "SK": int(sum(r[0] for r in rows)), "sec": round(dt, 3), "n_iter": [int(x) for x in n_iter]}
 worst, bad = 0.0, []
 for i in range(0, len(rows), 4):
     k, _, seed = rows[i]

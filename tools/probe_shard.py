@@ -1,8 +1,7 @@
 """One rank's share of the c3 job table (idx % WORLD == 0) on ONE GPU: where the time of a small shard goes.
 
-The strong-scaling loss from 1 to 8 GPUs (5.83 x, profiles/r2i_strong_scaling.log) is the part of a solve that does
-not shrink with the number of restarts; this probe times the shard alone (wall, CUDA events, per-class kernel time) so
-that `wall - GEMM - update` can be read off, and is the command the ncu launch list of a shard is taken from.
+The strong-scaling loss from 1 to N GPUs is the part of a solve that does not shrink with the number of restarts; this
+probe times the shard alone (wall, CUDA events, per-class kernel time) so that `wall - GEMM - update` can be read off.
 usage: python tools/probe_shard.py [world=8] [reps=3]      env: SHARD_RANKS=0,1,.. (default 0), PROFILE=0 (no per-launch events)"""
 import json
 import os
