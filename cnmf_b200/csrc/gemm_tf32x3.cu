@@ -404,6 +404,30 @@ __device__ __forceinline__ void fused_w_epilogue(float (&acc)[HALF], const FuseW
   __syncwarp();
 }
 
+// ------------------------------------------------------------------ tile order
+// Work item w -> (m-tile, n-tile, split-K slice z).  The slice is outermost.  Inside a slice the tiles run in groups of
+// `group` consecutive m-tiles (n-tiles if group_n), the grouped index fastest, and each group sweeps every tile of the
+// other dimension: the group's operand panels stay in the L2 while the other operand streams past them (DESIGN.md
+// section 4.1; pick_tile_order chooses the group).  group = m_tiles, group_n = 0 is the plain m-tile-fastest order.
+// The producer and the consumers both decode through this function, so they always agree on a CTA's tiles.
+struct TileOrder {
+  int m_tiles, n_tiles, group, group_n;
+};
+
+__host__ __device__ __forceinline__ void decode_item(int w, const TileOrder& o, int& mt, int& nt, int& z) {
+  const int per_slice = o.m_tiles * o.n_tiles;
+  z = w / per_slice;
+  int r = w - z * per_slice;
+  const int q_tiles = o.group_n ? o.n_tiles : o.m_tiles;      // grouped dimension
+  const int p_tiles = o.group_n ? o.m_tiles : o.n_tiles;      // swept dimension
+  const int g0 = r / (o.group * p_tiles) * o.group;           // first grouped tile of w's group (earlier groups are full)
+  r -= g0 * p_tiles;
+  const int gq = q_tiles - g0 < o.group ? q_tiles - g0 : o.group;   // the last group may be partial
+  const int p = r / gq, q = g0 + r % gq;
+  mt = o.group_n ? p : q;
+  nt = o.group_n ? q : p;
+}
+
 // ------------------------------------------------------------------ the kernel
 // F16 (with BEXACT): operands are fp16 (two pieces of A, one exact B); a k-block is still 128 B per row = 64 elements,
 // a k-step still 32 B = 16 elements (wgmma K of f16), so the smem / TMA / descriptor byte geometry is unchanged.
@@ -414,7 +438,7 @@ template <int STAGES, bool BEXACT, bool F16, bool FUSE>
 __device__ __forceinline__ void
 gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMap& tmB_hi, const CUtensorMap& tmB_lo,
           float* __restrict__ C, int M, int ldc, long long c_split_stride,
-          int m_tiles, int n_tiles, int splits, int total_kb, int kb_per_split, int chain_kb,
+          const TileOrder& ord, int splits, int total_kb, int kb_per_split, int chain_kb,
           const float* __restrict__ out_scale, const float* __restrict__ a_tile_scale, int a_tiles, int a_gshift,
           const FuseW* __restrict__ fz) {
   static_assert(!F16 || BEXACT, "the fp16 path exists for exact integer B operands only");
@@ -443,7 +467,7 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
   }
   __syncthreads();
 
-  const int items = m_tiles * n_tiles * splits;
+  const int items = ord.m_tiles * ord.n_tiles * splits;
 
   if constexpr (FUSE) {     // the epilogue's state needs more than 168 registers: move them from the producer warpgroup
     if (wg == 0) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
@@ -456,9 +480,8 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
       uint32_t phase = 0;
       constexpr uint32_t stage_tx = static_cast<uint32_t>(L::STAGE_BYTES);
       for (int w = blockIdx.x; w < items; w += gridDim.x) {
-        const int mt = w % m_tiles;
-        const int nt = (w / m_tiles) % n_tiles;
-        const int z = w / (m_tiles * n_tiles);
+        int mt, nt, z;
+        decode_item(w, ord, mt, nt, z);
         const int kb0 = z * kb_per_split;
         const int kb1 = min(total_kb, kb0 + kb_per_split);
         for (int kb = kb0; kb < kb1; ++kb) {
@@ -480,9 +503,8 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
     int stage = 0;
     uint32_t phase = 0;
     for (int w = blockIdx.x; w < items; w += gridDim.x) {
-      const int mt = w % m_tiles;
-      const int nt = (w / m_tiles) % n_tiles;
-      const int z = w / (m_tiles * n_tiles);
+      int mt, nt, z;
+      decode_item(w, ord, mt, nt, z);
       const int kb0 = z * kb_per_split;
       const int kb1 = min(total_kb, kb0 + kb_per_split);
       const int row0 = mt * BM + cw * 64 + warp * 16 + (lane >> 2);   // and row0 + 8
@@ -558,7 +580,7 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
           rowv[4 * j] = v.x; rowv[4 * j + 1] = v.y; rowv[4 * j + 2] = v.z; rowv[4 * j + 3] = v.w;
         }
         named_bar(4, 256);                                      // X is reused as the epilogue's staging area
-        fused_w_epilogue<64>(rowv, *fz, M, mt, nt, n_tiles, (ct & 127) >> 5, ct >> 7, lane, out_scale,
+        fused_w_epilogue<64>(rowv, *fz, M, mt, nt, ord.n_tiles, (ct & 127) >> 5, ct >> 7, lane, out_scale,
                              smem_gen + L::EPI_OFFSET);
         continue;
       }
@@ -587,9 +609,9 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                    const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
                    float* __restrict__ C, int M, int ldc, long long c_split_stride,
-                   int m_tiles, int n_tiles, int splits, int total_kb, int kb_per_split, int chain_kb,
+                   const TileOrder ord, int splits, int total_kb, int kb_per_split, int chain_kb,
                    const float* __restrict__ out_scale, const float* __restrict__ a_tile_scale, int a_tiles, int a_gshift) {
-  gemm_body<STAGES, BEXACT, F16, false>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, C, M, ldc, c_split_stride, m_tiles, n_tiles, splits,
+  gemm_body<STAGES, BEXACT, F16, false>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, C, M, ldc, c_split_stride, ord, splits,
                                         total_kb, kb_per_split, chain_kb, out_scale, a_tile_scale, a_tiles, a_gshift,
                                         nullptr);
 }
@@ -597,10 +619,10 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_cons
 // NUM = F_other * X^T with the multiplicative update of the row factor in the epilogue (f16, 128-wide tiles, no split-K)
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_fused_w_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
-                    const __grid_constant__ CUtensorMap tmB_hi, int M, int m_tiles, int n_tiles, int total_kb,
+                    const __grid_constant__ CUtensorMap tmB_hi, int M, const TileOrder ord, int total_kb,
                     const float* __restrict__ out_scale, const float* __restrict__ a_tile_scale, int a_tiles, int a_gshift,
                     const __grid_constant__ FuseW fz) {
-  gemm_body<2, true, true, true>(tmA_hi, tmA_lo, tmB_hi, tmB_hi, nullptr, M, 0, 0, m_tiles, n_tiles, 1, total_kb,
+  gemm_body<2, true, true, true>(tmA_hi, tmA_lo, tmB_hi, tmB_hi, nullptr, M, 0, 0, ord, 1, total_kb,
                                  total_kb + (total_kb & 1), 2, out_scale, a_tile_scale, a_tiles, a_gshift, &fz);
 }
 
@@ -679,6 +701,39 @@ static int pick_chain_kb(const GemmArgs& g) {
   return chain_kb;
 }
 
+// Modelled HBM bytes of one split-K slice in a grouped tile order (tools/probe_gemm.py restates this model): the
+// `group` panels of the grouped operand q are read once if they fit the L2 budget, else once per wave of the grid that
+// passes over them; every panel of the swept operand p is read once per group (its readers run side by side).
+static double order_bytes(int q_tiles, int p_tiles, double q_panel, double p_panel, int group, int grid, double budget) {
+  const long long waves = (static_cast<long long>(group) * p_tiles + grid - 1) / grid;
+  const double q_reads = group * q_panel <= budget ? 1.0 : static_cast<double>(std::min<long long>(p_tiles, waves));
+  return q_tiles * q_panel * q_reads + static_cast<double>((q_tiles + group - 1) / group) * p_tiles * p_panel;
+}
+
+// The tile order with the least modelled traffic, over both orientations and every balanced group size, with half of
+// the L2 as the budget of the resident panels (the other half holds the streamed operand and the output lines).
+// a_panel / b_panel: bytes of one 128-row operand panel of a slice, all pieces.  Ties keep the m-tile-fastest order,
+// which is what a problem whose factor operand fits the L2 gets.  The order decides only which CTA computes a tile
+// when: every output element is still formed by the same chains in the same order.
+static TileOrder pick_tile_order(int m_tiles, int n_tiles, double a_panel, double b_panel, int grid, long long l2_bytes) {
+  const double budget = 0.5 * static_cast<double>(l2_bytes);
+  TileOrder best{m_tiles, n_tiles, m_tiles, 0};
+  double best_bytes = order_bytes(m_tiles, n_tiles, a_panel, b_panel, m_tiles, grid, budget);
+  for (int gn = 0; gn < 2; ++gn) {
+    const int q = gn ? n_tiles : m_tiles, p = gn ? m_tiles : n_tiles;
+    const double qb = gn ? b_panel : a_panel, pb = gn ? a_panel : b_panel;
+    int prev = 0;
+    for (int ng = 1; ng <= q; ++ng) {                 // groups of ceil(q / ng) tiles, the last one possibly shorter
+      const int g = (q + ng - 1) / ng;
+      if (g == prev) continue;
+      prev = g;
+      const double b = order_bytes(q, p, qb, pb, g, grid, budget);
+      if (b < best_bytes) { best_bytes = b; best = TileOrder{m_tiles, n_tiles, g, gn}; }
+    }
+  }
+  return best;
+}
+
 template <int STAGES, bool BEXACT, bool F16>
 int launch(const GemmArgs& g, cudaStream_t stream) {
   using L = SmemLayout<STAGES, BEXACT>;
@@ -689,9 +744,10 @@ int launch(const GemmArgs& g, cudaStream_t stream) {
   if ((rc = make_map(&mAl, g.A_lo, g.M, g.Kd, g.lda, BM, F16))) return rc;
   if ((rc = make_map(&mBh, g.B_hi, g.N, g.Kd, g.ldb, BN, F16))) return rc;
   if ((rc = make_map(&mBl, BEXACT ? g.B_hi : g.B_lo, g.N, g.Kd, g.ldb, BN, F16))) return rc;
-  int dev = 0, sms = 0;
+  int dev = 0, sms = 0, l2 = 0;
   CNMF_CUDA_CHECK(cudaGetDevice(&dev));
   CNMF_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  CNMF_CUDA_CHECK(cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, dev));
   const int m_tiles = (g.M + BM - 1) / BM;
   const int n_tiles = (g.N + BN - 1) / BN;
   const int total_kb = (g.Kd + BKE - 1) / BKE;
@@ -711,8 +767,11 @@ int launch(const GemmArgs& g, cudaStream_t stream) {
   const int items = m_tiles * n_tiles * splits;
   const int grid = items < sms ? items : sms;
   const int chain_kb = pick_chain_kb<BEXACT, F16>(g);
+  const double kslice_row = static_cast<double>(kb_per_split) * BK * 4;       // bytes of one slice row, one piece
+  const TileOrder ord = pick_tile_order(m_tiles, n_tiles, BM * kslice_row * 2, BN * kslice_row * (BEXACT ? 1 : 2),
+                                        grid, l2);
   kern<<<grid, NUM_THREADS, L::DYN_BYTES, stream>>>(mAh, mAl, mBh, mBl, g.C, g.M, g.ldc, g.c_split_stride,
-                                                    m_tiles, n_tiles, splits, total_kb, kb_per_split, chain_kb,
+                                                    ord, splits, total_kb, kb_per_split, chain_kb,
                                                     g.out_col_scale, g.a_tile_scale, g.a_tiles,
                                                     g.a_group_kb_shift > 0 ? g.a_group_kb_shift : 3);
   CNMF_CUDA_CHECK(cudaGetLastError());
@@ -727,9 +786,10 @@ int launch_fused_w(const GemmArgs& g, cudaStream_t stream) {
   if ((rc = make_map(&mAh, g.A_hi, g.M, g.Kd, g.lda, BM, true))) return rc;
   if ((rc = make_map(&mAl, g.A_lo, g.M, g.Kd, g.lda, BM, true))) return rc;
   if ((rc = make_map(&mBh, g.B_hi, g.N, g.Kd, g.ldb, BN, true))) return rc;
-  int dev = 0, sms = 0;
+  int dev = 0, sms = 0, l2 = 0;
   CNMF_CUDA_CHECK(cudaGetDevice(&dev));
   CNMF_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  CNMF_CUDA_CHECK(cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, dev));
   const int m_tiles = (g.M + BM - 1) / BM, n_tiles = (g.N + BN - 1) / BN;
   const int total_kb = (g.Kd + 2 * BK - 1) / (2 * BK);
   static bool attr_set[64] = {};
@@ -739,7 +799,9 @@ int launch_fused_w(const GemmArgs& g, cudaStream_t stream) {
   }
   const int items = m_tiles * n_tiles;
   const int grid = items < sms ? items : sms;
-  gemm_fused_w_kernel<<<grid, NUM_THREADS, L::DYN_BYTES, stream>>>(mAh, mAl, mBh, g.M, m_tiles, n_tiles, total_kb,
+  const double k_row = static_cast<double>(total_kb) * 2 * BK * 2;             // bytes of one fp16 row, one piece
+  const TileOrder ord = pick_tile_order(m_tiles, n_tiles, BM * k_row * 2, BN * k_row, grid, l2);
+  gemm_fused_w_kernel<<<grid, NUM_THREADS, L::DYN_BYTES, stream>>>(mAh, mAl, mBh, g.M, ord, total_kb,
                                                                    g.out_col_scale, g.a_tile_scale, g.a_tiles,
                                                                    g.a_group_kb_shift > 0 ? g.a_group_kb_shift : 3, g.fuse);
   CNMF_CUDA_CHECK(cudaGetLastError());

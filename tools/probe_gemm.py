@@ -1,23 +1,108 @@
 #!/usr/bin/env python
-"""GPU probe: the batched GEMM alone on BASELINE-shaped problems (f16x2 path), mean device time per launch."""
+"""GPU probe: the batched GEMM alone (f16x2 path), mean device time per launch, accuracy, and the modelled HBM operand
+traffic of two tile orders: the m-tile-fastest order of the first kernel versions and the grouped order the launcher
+picks now (the same rule as pick_tile_order in csrc/gemm_tf32x3.cu, restated here).
+
+Cases: c2-shaped problems, a 4 096-row problem, the c3 shapes at full SK (8 100 packed rows: factor operand larger
+than the L2) and the same c3 shapes with 1 024 rows (factor operand resident in the L2)."""
 import json, os, sys
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from cnmf_b200.engine import Engine
 
-eng = Engine(0)
-rng = np.random.RandomState(0)
-out = {}
-for name, (M, N, K, sp) in {"c2_W_half": (1000, 20000, 2000, 1), "c2_H_half": (1000, 2000, 20000, 5),
-                            "mid_W_half": (4096, 16384, 2000, 1), "mid_H_half": (4096, 2000, 16384, 4),
-                            "tail_H_half": (128, 2000, 20000, 5)}.items():
-    A = np.abs(rng.standard_normal((M, K))).astype(np.float32)
-    B = rng.poisson(1.5, size=(N, K)).astype(np.float32)
-    C, ms = eng.gemm_abt(A, B, precision="f16x2", splits=sp, reps=20)
-    ref = A[:64].astype(np.float64) @ B.astype(np.float64).T
-    err = float(np.linalg.norm(C[:64] - ref) / np.linalg.norm(ref))
-    tail = A[-64:].astype(np.float64) @ B.astype(np.float64).T
-    err2 = float(np.linalg.norm(C[-64:] - tail) / np.linalg.norm(tail))
-    out[name] = {"ms": round(ms, 4), "tflops": round(2.0 * M * N * K / (ms * 1e-3) / 1e12, 1), "rel_err_first_rows": err, "rel_err_last_rows": err2}
-print(json.dumps(out))
+BM = BN = 128            # output tile
+KB_ELEMS = 64            # fp16 elements per k-block
+
+
+def slices(Kd, splits):
+    """k-blocks per split-K slice, as the launcher partitions them (slices start on even k-blocks)."""
+    total_kb = -(-Kd // KB_ELEMS)
+    splits = max(1, min(splits, total_kb))
+    kbps = -(-total_kb // splits)
+    kbps += kbps & 1
+    return [min(kbps, total_kb - z * kbps) for z in range(-(-total_kb // kbps))]
+
+
+def order_bytes(q_tiles, p_tiles, q_panel, p_panel, group, grid, budget):
+    """Operand bytes one slice reads from HBM when groups of `group` panels of one operand (q) each sweep every panel of
+    the other (p): the group is read once if it fits the L2 budget, else once per wave of the grid that passes over it;
+    each p panel is read once per group."""
+    if group * q_panel <= budget:
+        q_reads = 1
+    else:
+        q_reads = min(p_tiles, -(-group * p_tiles // grid))
+    return q_tiles * q_panel * q_reads + -(-q_tiles // group) * p_tiles * p_panel
+
+
+def pick_order(m_tiles, n_tiles, a_panel, b_panel, grid, budget):
+    """(bytes, group, group_n) of the cheapest grouped order; ties keep the m-tile-fastest order (group = m_tiles)."""
+    best = None
+    for group_n, q, p, qb, pb in ((0, m_tiles, n_tiles, a_panel, b_panel), (1, n_tiles, m_tiles, b_panel, a_panel)):
+        for ng in range(1, q + 1):
+            g = -(-q // ng)
+            if ng > 1 and g == -(-q // (ng - 1)):
+                continue
+            b = order_bytes(q, p, qb, pb, g, grid, budget)
+            if best is None or b < best[0]:
+                best = (b, g, group_n)
+    return best
+
+
+def model(M, N, Kd, splits, l2, sms):
+    """Modelled operand bytes of the launch (A = two fp16 pieces, B = one exact fp16 operand) in both orders."""
+    m_tiles, n_tiles = -(-M // BM), -(-N // BN)
+    kbs = slices(Kd, splits)
+    items = m_tiles * n_tiles * len(kbs)
+    grid = min(items, sms)
+    budget = l2 // 2
+    a_panel, b_panel = (BM * kbs[0] * KB_ELEMS * 4, BN * kbs[0] * KB_ELEMS * 2)
+    _, g, gn = pick_order(m_tiles, n_tiles, a_panel, b_panel, grid, budget)
+    flat = grouped = 0
+    for kb in kbs:
+        ap, bp = BM * kb * KB_ELEMS * 4, BN * kb * KB_ELEMS * 2
+        flat += order_bytes(m_tiles, n_tiles, ap, bp, m_tiles, grid, budget)
+        grouped += (order_bytes(n_tiles, m_tiles, bp, ap, g, grid, budget) if gn else
+                    order_bytes(m_tiles, n_tiles, ap, bp, g, grid, budget))
+    minimum = sum(m_tiles * BM * kb * KB_ELEMS * 4 + n_tiles * BN * kb * KB_ELEMS * 2 for kb in kbs)
+    return {"m_fastest_GB": round(flat / 1e9, 3), "grouped_GB": round(grouped / 1e9, 3), "min_GB": round(minimum / 1e9, 3),
+            "grouped_order": "%d %s-tiles per group" % (g, "n" if gn else "m"), "slices": len(kbs)}
+
+
+def main():
+    import torch
+    props = torch.cuda.get_device_properties(0)
+    l2, sms = props.L2_cache_size, props.multi_processor_count
+    eng = Engine(0)
+    rng = np.random.RandomState(0)
+    out = {"device": props.name, "l2_bytes": l2, "sms": sms}
+    cases = {"c2_W_half": (1000, 20000, 2000, 1), "c2_H_half": (1000, 2000, 20000, 5),
+             "mid_W_half": (4096, 16384, 2000, 1), "mid_H_half": (4096, 2000, 16384, 4),
+             "tail_H_half": (128, 2000, 20000, 5),
+             "c3_W_half_full": (8100, 50000, 2000, 1), "c3_H_half_full": (8100, 2000, 50000, 13),
+             "c3_W_half_1024": (1024, 50000, 2000, 1), "c3_H_half_1024": (1024, 2000, 50000, 13)}
+    only = sys.argv[1:]
+    for name, (M, N, K, sp) in cases.items():
+        if only and name not in only:
+            continue
+        if M * K > 10 ** 8 or N * K > 10 ** 8:      # c3 sizes: float32 draws directly (the float64 ones need 3+ GB)
+            g = np.random.default_rng(0)
+            A = g.random((M, K), dtype=np.float32)
+            B = g.poisson(1.5, size=(N, K)).astype(np.float32)
+        else:
+            A = np.abs(rng.standard_normal((M, K))).astype(np.float32)
+            B = rng.poisson(1.5, size=(N, K)).astype(np.float32)
+        C, ms = eng.gemm_abt(A, B, precision="f16x2", splits=sp, reps=20)
+        ref = A[:64].astype(np.float64) @ B.astype(np.float64).T
+        err = float(np.linalg.norm(C[:64] - ref) / np.linalg.norm(ref))
+        tail = A[-64:].astype(np.float64) @ B.astype(np.float64).T
+        err2 = float(np.linalg.norm(C[-64:] - tail) / np.linalg.norm(tail))
+        out[name] = {"shape": [M, N, K, sp], "ms": round(ms, 4), "tflops": round(2.0 * M * N * K / (ms * 1e-3) / 1e12, 1),
+                     "rel_err_first_rows": err, "rel_err_last_rows": err2, "model": model(M, N, K, sp, l2, sms)}
+        print(name, json.dumps(out[name]), flush=True)
+        del A, B, C
+    print(json.dumps(out))
+
+
+if __name__ == "__main__":
+    main()
