@@ -214,8 +214,7 @@ long long cnmf_solve_bytes_per_row(cnmf_dataset_t d) {
   // product NUM_r along the cells; the same along the genes with one product slice per split-K slice
   const long long splits_c = gemm_fixed_splits(d->n_rows, d->f16 ? 1 : 0);
   const long long splits_r = gemm_fixed_splits(d->n_cols, d->f16 ? 1 : 0);
-  // (+ the second ping-pong set and the output buffer of the fused W-half epilogue)
-  return 4LL * ((11 + splits_r) * (long long)d->ld_r + (10 + splits_c) * (long long)d->ld_c);
+  return 4LL * ((7 + splits_r) * (long long)d->ld_r + (7 + splits_c) * (long long)d->ld_c);
 }
 
 int cnmf_profile_enable(cnmf_handle_t h, int on) {

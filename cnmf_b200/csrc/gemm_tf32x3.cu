@@ -26,17 +26,11 @@
 // 1 k-block of 12 MMAs in the general 3-pass form, 2 k-blocks of 8 MMAs in the exact-B 2-pass forms): every chain
 // starts from zero (scale-d = 0) and is then added into a second set of round-to-nearest fp32 register accumulators.
 // Result: ~4e-7 relative, the same class as an FFMA fp32 GEMM.
-//
-// FUSE (gemm_fused_w_kernel): NUM = F_other * X^T with the multiplicative update of the row factor applied to the tile
-// before it leaves the SM (struct FuseW in gemm.h): the consumers pass their sums through shared memory into row layout
-// and run fused_w_epilogue instead of storing the product.
 #include <cuda.h>
-#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>
 #include <algorithm>
-#include <cstdlib>
 #include <map>
 #include <mutex>
 #include <tuple>
@@ -56,14 +50,13 @@ constexpr long long WAIT_TIMEOUT_CYCLES = 4000000000LL;   // ~2 s: a dead pipeli
 
 // BEXACT: the B operand is exactly representable in tf32 / fp16 (e.g. integer counts), so it needs no "lo" piece:
 // 2 MMAs per k-step instead of 3, 48 KB stages (4 of them) instead of 64 KB (3).
-template <int STAGES, bool BEXACT, int EPI_BYTES = 0>
+template <int STAGES, bool BEXACT>
 struct SmemLayout {
   static constexpr int A_BYTES = BM * BK * 4;              // 16 KB
   static constexpr int B_BYTES = BN * BK * 4;              // 16 KB
   static constexpr int STAGE_BYTES = 2 * A_BYTES + (BEXACT ? 1 : 2) * B_BYTES;
   static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;  // full[STAGES], empty[STAGES]
-  static constexpr int EPI_OFFSET = BAR_OFFSET + 2 * STAGES * 8;
-  static constexpr int TOTAL = EPI_OFFSET + EPI_BYTES;
+  static constexpr int TOTAL = BAR_OFFSET + 2 * STAGES * 8;
   static constexpr int DYN_BYTES = TOTAL + 1024;           // slack for manual 1024 B alignment
   static_assert(DYN_BYTES <= 227 * 1024, "pipeline stages do not fit the shared memory of an SM");
 };
@@ -165,245 +158,6 @@ __device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t adesc, ui
   }
 }
 
-// ------------------------------------------------------------------ fused W-half epilogue
-__device__ __forceinline__ void named_bar(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool valid) {
-  const int sz = valid ? 16 : 0;                       // src-size 0: the 16 bytes are zero-filled
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(sz) : "memory");
-}
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
-
-// shared memory of the fused epilogue (after the pipeline stages and barriers): the 128 x 128 product tile in row layout
-// (rows of 136 floats; the wgmma fragments are written into it, then every thread reads its row half), reused as the
-// staging area of 128 rows x 36 floats per column half; per consumer thread its row of the other factor's Gram
-// (16 floats) and of the new Gram (16 doubles); the group maxima of the two column halves
-constexpr int FUSE_XROW = 136;                                       // floats per product row (128 + pad)
-constexpr int FUSE_SROW = 36;                                        // floats per staging row (32 items + pad: conflict-free)
-constexpr int FUSE_STAGING_BYTES = 128 * FUSE_XROW * 4;              // 69 632 (>= 2 * 128 * FUSE_SROW * 4)
-constexpr int FUSE_G_BYTES = 16 * 256 * 4;                           // 16 384
-constexpr int FUSE_GD_BYTES = 16 * 256 * 8;                          // 32 768
-constexpr int FUSE_MAX_BYTES = 256 * 4;
-constexpr int FUSE_EPI_BYTES = FUSE_STAGING_BYTES + FUSE_G_BYTES + FUSE_GD_BYTES + FUSE_MAX_BYTES;
-
-// The multiplicative update of the row factor, applied to the product tile while it is still in registers (struct
-// FuseW in gemm.h).  Thread = packed row (o + c) of a restart x 64 items, one column half of the tile's 128-item scale
-// group; acc[] holds the numerators on entry and the new factor values on exit.  The 128 threads that share a column half exchange rows
-// through a shared-memory staging area: per 32-item chunk every thread publishes the OLD values of its row (cp.async
-// straight from global memory), reads the K rows of its restart (den = sum_i Gram[c, i] F[o + i, item]), publishes the
-// NEW values, accumulates its row of the restart's K x K Gram of the new values (fp32 over 16 items, fp64 beyond: the
-// summation granularity of the stand-alone update kernel) and the warp stores its 32 rows of the chunk coalesced.
-// Restarts never straddle a 128-row tile (the engine packs them that way), so every row a thread needs is in the
-// staging area.  All per-thread state that is indexed by the component lives in shared memory, the component loops are
-// rolled (small code, no local memory: with ~200 KB of shared memory per CTA the L1 is too small to hold spills).
-// Afterwards the two halves of a row agree on the group maximum and each emits the two fp16 operand pieces of its 64
-// values with the power-of-two scale of the group: the same bits emit_f16_kernel would produce from F_out.
-template <int HALF>
-__device__ __forceinline__ void fused_w_epilogue(float (&acc)[HALF], const FuseW& fz, int M, int mt, int nt, int n_tiles,
-                                                 int q, int half, int lane, const float* __restrict__ out_scale,
-                                                 uint8_t* epi) {
-  static_assert(HALF == 64, "two threads (column halves) own one 128-item scale group");
-  constexpr float EPS32 = 1.1920928955078125e-07f;     // np.finfo(np.float32).eps, sklearn _nmf.py:32
-  constexpr float FMIN = 1.17549435e-38f;
-  constexpr int SR = FUSE_SROW;
-  const int r = q * 32 + lane;                          // row inside the 128-row tile
-  const int tid = half * 128 + r;                       // consumer-thread index 0..255
-  const int grow = mt * BM + r;
-  const int col0 = nt * 128 + half * HALF;              // first item of this thread's half (tile width 128)
-  float* S = reinterpret_cast<float*>(epi) + half * (128 * SR);     // staging of this column half
-  float* Sr = S + r * SR;
-  float* gs = reinterpret_cast<float*>(epi + FUSE_STAGING_BYTES) + tid;                       // gs[i * 256]
-  double* gd = reinterpret_cast<double*>(epi + FUSE_STAGING_BYTES + FUSE_G_BYTES) + tid;      // gd[i * 256]
-  const int bar_id = 1 + half;
-  const int ld = fz.ld;
-
-  int slot = -1;
-  if (grow < M) slot = __ldg(fz.row_slot + grow);
-  int K = 0, o = grow, rid = 0;
-  bool upd = false, cpy = false;
-  if (slot >= 0) {
-    rid = __ldg(fz.rid + slot);
-    K = __ldg(fz.k + slot);
-    o = __ldg(fz.off + slot);
-    if (__ldg(fz.done + rid)) cpy = true; else upd = true;
-  }
-  const int c = grow - o;
-  const int lr0 = o - mt * BM;                          // tile-local row of the restart's first component
-  const int Kl = upd ? K : 0;
-  const bool want_gram = fz.gram_part != nullptr;
-  const bool row_ok = grow < M;
-  const float* pin = fz.F_in + static_cast<long long>(row_ok ? grow : 0) * ld + col0;
-  const uint32_t sr_addr = smem_u32(Sr);
-
-  // old values of the first chunk on their way while the per-thread state is set up
-#pragma unroll
-  for (int t = 0; t < 8; ++t) cp_async16(sr_addr + 16 * t, pin + 4 * t, row_ok && col0 + 4 * t + 3 < ld);
-  for (int i = 0; i < 16; ++i) {
-    gs[i * 256] = (i < Kl) ? static_cast<float>(fz.gram_in[static_cast<long long>(rid) * (KMAX * KMAX) + c * KMAX + i]) : 0.f;
-    gd[i * 256] = 0.0;
-  }
-  if (out_scale) {                                      // per-item scale of the product (exact-count datasets)
-#pragma unroll
-    for (int j = 0; j < HALF; j += 4) {
-      if (col0 + j + 3 < ld) {
-        const float4 sc = *reinterpret_cast<const float4*>(out_scale + col0 + j);
-        acc[j] *= sc.x; acc[j + 1] *= sc.y; acc[j + 2] *= sc.z; acc[j + 3] *= sc.w;
-      }
-    }
-  }
-  float* pout = fz.F_out;
-  const int sub_r = lane >> 3, sub_c = (lane & 7) * 4;  // coalesced store: 4 rows x 128 B per instruction
-
-#pragma unroll
-  for (int ch = 0; ch < HALF / 32; ++ch) {              // 32 items per chunk
-    cp_async_wait_all();
-    named_bar(bar_id, 128);                             // old rows of the chunk are published
-#pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {                    // 16 items at a time (register budget)
-      float2 den[8];
-#pragma unroll
-      for (int t = 0; t < 8; ++t) den[t] = make_float2(0.f, 0.f);
-#pragma unroll 2
-      for (int i = 0; i < Kl; ++i) {                    // summed in component order, like the reference's W @ HHt row
-        const float2 gi = bcast2(gs[i * 256]);
-        const float4* sp = reinterpret_cast<const float4*>(S + (lr0 + i) * SR + hh * 16);
-#pragma unroll
-        for (int t = 0; t < 4; ++t) {
-          const float4 w = sp[t];
-          den[2 * t] = fma2(gi, make_float2(w.x, w.y), den[2 * t]);
-          den[2 * t + 1] = fma2(gi, make_float2(w.z, w.w), den[2 * t + 1]);
-        }
-      }
-#pragma unroll
-      for (int t = 0; t < 4; ++t) {
-        const float4 own = *reinterpret_cast<const float4*>(Sr + hh * 16 + 4 * t);
-        const int j = ch * 32 + hh * 16 + 4 * t;
-        const float2 own0 = make_float2(own.x, own.y), own1 = make_float2(own.z, own.w);
-        const float2 num0 = make_float2(acc[j], acc[j + 1]), num1 = make_float2(acc[j + 2], acc[j + 3]);
-        // regularisation terms unconditionally (adding 0 is exact); zero denominators -> eps (sklearn _nmf.py:615)
-        float2 d0 = fma2(bcast2(fz.l2), own0, add2(den[2 * t], bcast2(fz.l1)));
-        float2 d1 = fma2(bcast2(fz.l2), own1, add2(den[2 * t + 1], bcast2(fz.l1)));
-        d0.x = (d0.x < FMIN) ? EPS32 : d0.x; d0.y = (d0.y < FMIN) ? EPS32 : d0.y;
-        d1.x = (d1.x < FMIN) ? EPS32 : d1.x; d1.y = (d1.y < FMIN) ? EPS32 : d1.y;
-        float2 o0 = mul2(own0, div_nr2(num0, d0));
-        float2 o1 = mul2(own1, div_nr2(num1, d1));
-        if (!upd) {                                     // converged restart: carried over unchanged; padding row: zero
-          o0 = cpy ? own0 : make_float2(0.f, 0.f);
-          o1 = cpy ? own1 : make_float2(0.f, 0.f);
-        }
-        acc[j] = o0.x; acc[j + 1] = o0.y; acc[j + 2] = o1.x; acc[j + 3] = o1.y;
-      }
-    }
-    named_bar(bar_id, 128);                             // everybody has read the old rows
-#pragma unroll
-    for (int t = 0; t < 8; ++t)
-      *reinterpret_cast<float4*>(Sr + 4 * t) = make_float4(acc[ch * 32 + 4 * t], acc[ch * 32 + 4 * t + 1],
-                                                           acc[ch * 32 + 4 * t + 2], acc[ch * 32 + 4 * t + 3]);
-    named_bar(bar_id, 128);                             // new rows of the chunk are published
-    if (want_gram) {
-#pragma unroll 2
-      for (int i = 0; i < Kl; ++i) {
-        const float4* sp = reinterpret_cast<const float4*>(S + (lr0 + i) * SR);
-        float2 sa = make_float2(0.f, 0.f), sb = make_float2(0.f, 0.f);   // two 16-item partial sums
-#pragma unroll
-        for (int t = 0; t < 4; ++t) {
-          const float4 w = sp[t], w2 = sp[t + 4];
-          const int j = ch * 32 + 4 * t;
-          sa = fma2(make_float2(acc[j], acc[j + 1]), make_float2(w.x, w.y), sa);
-          sa = fma2(make_float2(acc[j + 2], acc[j + 3]), make_float2(w.z, w.w), sa);
-          sb = fma2(make_float2(acc[j + 16], acc[j + 17]), make_float2(w2.x, w2.y), sb);
-          sb = fma2(make_float2(acc[j + 18], acc[j + 19]), make_float2(w2.z, w2.w), sb);
-        }
-        gd[i * 256] += static_cast<double>(sa.x + sa.y) + static_cast<double>(sb.x + sb.y);
-      }
-    }
-    {                                                   // this warp's 32 rows x 32 items, 4 rows x 128 B per instruction
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const int rr = q * 32 + sub_r + 4 * j;
-        const float4 v = *reinterpret_cast<const float4*>(S + rr * SR + sub_c);
-        const int grow2 = mt * BM + rr, gcol = col0 + ch * 32 + sub_c;
-        if (grow2 < M && gcol + 3 < ld) *reinterpret_cast<float4*>(pout + static_cast<long long>(grow2) * ld + gcol) = v;
-      }
-    }
-    named_bar(bar_id, 128);                             // staging free for the next chunk
-    if (ch < HALF / 32 - 1) {
-#pragma unroll
-      for (int t = 0; t < 8; ++t) {
-        const int cc = (ch + 1) * 32 + 4 * t;
-        cp_async16(sr_addr + 16 * t, pin + cc, row_ok && col0 + cc + 3 < ld);
-      }
-    }
-  }
-
-  if (want_gram) {                                      // the two column halves of a row meet in shared memory
-    named_bar(3, 256);
-    if (half == 0 && upd) {
-      const int KP = (K + 3) & ~3;                      // layout finalize_kernel reads: [c * KP + i]
-      double* dst = fz.gram_part + (static_cast<long long>(rid) * n_tiles + nt) * 256 + c * KP;
-      for (int i = 0; i < KP; ++i) dst[i] = (i < K) ? gd[i * 256] + gd[i * 256 + 128] : 0.0;
-    }
-    named_bar(3, 256);
-  }
-
-  // ---- fp16 operand pieces of the new values, group scale = power of two from the group maximum
-  float m = 0.f;
-  if (fz.piece_scale) {
-#pragma unroll
-    for (int j = 0; j < HALF; j += 4) {
-      float4 ps = make_float4(1.f, 1.f, 1.f, 1.f);
-      if (col0 + j + 3 < ld) ps = *reinterpret_cast<const float4*>(fz.piece_scale + col0 + j);
-      acc[j] *= ps.x; acc[j + 1] *= ps.y; acc[j + 2] *= ps.z; acc[j + 3] *= ps.w;
-    }
-  }
-#pragma unroll
-  for (int j = 0; j < HALF; ++j) m = fmaxf(m, acc[j]);
-  float* gmax = reinterpret_cast<float*>(epi + FUSE_STAGING_BYTES + FUSE_G_BYTES + FUSE_GD_BYTES);
-  gmax[tid] = m;
-  named_bar(3, 256);
-  m = fmaxf(m, gmax[tid ^ 128]);                        // the other column half of the row
-  const float sc = f16_group_scale(m);
-  const float inv = 1.f / sc;                           // power of two: exact
-  if (half == 0 && row_ok && col0 < ld) fz.tile_scale[static_cast<long long>(grow) * fz.n_groups + (col0 >> 7)] = sc;
-  __half* ph = static_cast<__half*>(fz.P_hi);
-  __half* pm = static_cast<__half*>(fz.P_mid);
-  uint32_t* Su = reinterpret_cast<uint32_t*>(Sr);
-  const int sub_r8 = lane >> 2, sub_q = lane & 3;       // 8 rows x 64 B per instruction
-#pragma unroll
-  for (int cc = 0; cc < HALF / 32; ++cc) {              // 32 items = 64 B of halves per row and piece
-#pragma unroll
-    for (int pc = 0; pc < 2; ++pc) {
-      __syncwarp();
-#pragma unroll
-      for (int e = 0; e < 16; e += 4) {
-        uint32_t u[4];
-#pragma unroll
-        for (int k2 = 0; k2 < 4; ++k2) {
-          const float x0 = acc[cc * 32 + 2 * (e + k2)] * inv, x1 = acc[cc * 32 + 2 * (e + k2) + 1] * inv;
-          const __half2 h = __floats2half2_rn(x0, x1);
-          if (pc == 0) {
-            u[k2] = *reinterpret_cast<const uint32_t*>(&h);
-          } else {
-            const float2 hf = __half22float2(h);
-            const __half2 md = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
-            u[k2] = *reinterpret_cast<const uint32_t*>(&md);
-          }
-        }
-        *reinterpret_cast<uint4*>(Su + e) = make_uint4(u[0], u[1], u[2], u[3]);
-      }
-      __syncwarp();
-      __half* dstp = pc == 0 ? ph : pm;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int rr = q * 32 + sub_r8 + 8 * j;
-        const uint4 v = *reinterpret_cast<const uint4*>(reinterpret_cast<const uint32_t*>(S + rr * SR) + sub_q * 4);
-        const int grow2 = mt * BM + rr, gcol = col0 + cc * 32 + sub_q * 8;
-        if (grow2 < M && gcol + 7 < ld) *reinterpret_cast<uint4*>(dstp + static_cast<long long>(grow2) * ld + gcol) = v;
-      }
-    }
-  }
-  __syncwarp();
-}
-
 // ------------------------------------------------------------------ tile order
 // Work item w -> (m-tile, n-tile, split-K slice z).  The slice is outermost.  Inside a slice the tiles run in groups of
 // `group` consecutive m-tiles (n-tiles if group_n), the grouped index fastest, and each group sweeps every tile of the
@@ -434,21 +188,18 @@ __host__ __device__ __forceinline__ void decode_item(int w, const TileOrder& o, 
 //
 // Fragment of consumer thread (warp w of its warpgroup, lane l): d[4j + e] is row 16w + l/4 (+8 for e >= 2),
 // column 8j + 2(l%4) + (e & 1) of the warpgroup's 64 x 128 block.
-template <int STAGES, bool BEXACT, bool F16, bool FUSE>
+template <int STAGES, bool BEXACT, bool F16>
 __device__ __forceinline__ void
 gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMap& tmB_hi, const CUtensorMap& tmB_lo,
           float* __restrict__ C, int M, int ldc, long long c_split_stride,
           const TileOrder& ord, int splits, int total_kb, int kb_per_split, int chain_kb,
-          const float* __restrict__ out_scale, const float* __restrict__ a_tile_scale, int a_tiles, int a_gshift,
-          const FuseW* __restrict__ fz) {
+          const float* __restrict__ out_scale, const float* __restrict__ a_tile_scale, int a_tiles, int a_gshift) {
   static_assert(!F16 || BEXACT, "the fp16 path exists for exact integer B operands only");
-  static_assert(!FUSE || (F16 && STAGES == 2), "the fused W-half epilogue is built for the 2-stage f16 kernel");
   constexpr int BKE = F16 ? 2 * BK : BK;                        // elements per k-block
   constexpr int KSTEP_BYTES = 32;                               // wgmma K: 8 tf32 or 16 fp16 elements
-  using L = SmemLayout<STAGES, BEXACT, FUSE ? FUSE_EPI_BYTES : 0>;
+  using L = SmemLayout<STAGES, BEXACT>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;     // SWIZZLE_128B needs 1024 B alignment
-  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
 
   const uint32_t bar_base = smem_base + L::BAR_OFFSET;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
@@ -469,10 +220,6 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
 
   const int items = ord.m_tiles * ord.n_tiles * splits;
 
-  if constexpr (FUSE) {     // the epilogue's state needs more than 168 registers: move them from the producer warpgroup
-    if (wg == 0) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
-    else asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
-  }
   if (wg == 0) {
     // ===================== TMA producer =====================
     if (threadIdx.x == 0) {
@@ -559,31 +306,6 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
           for (int i = 0; i < 64; ++i) acc[i] += d[i];          // round-to-nearest fp32
         }
       }
-      if constexpr (FUSE) {
-        // fragments -> row layout: consumer thread ct owns tile row ct % 128, items [64 (ct / 128), +64)
-        const int ct = static_cast<int>(threadIdx.x) - 128;
-        float* X = reinterpret_cast<float*>(smem_gen + L::EPI_OFFSET);
-        named_bar(4, 256);                                      // the previous tile's epilogue is done with X
-        const int lr = cw * 64 + warp * 16 + (lane >> 2);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const int lc = 8 * j + 2 * (lane & 3);
-          *reinterpret_cast<float2*>(X + lr * FUSE_XROW + lc) = make_float2(acc[4 * j], acc[4 * j + 1]);
-          *reinterpret_cast<float2*>(X + (lr + 8) * FUSE_XROW + lc) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-        }
-        named_bar(4, 256);
-        float rowv[64];
-        const float4* src = reinterpret_cast<const float4*>(X + (ct & 127) * FUSE_XROW + (ct >> 7) * 64);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const float4 v = src[j];
-          rowv[4 * j] = v.x; rowv[4 * j + 1] = v.y; rowv[4 * j + 2] = v.z; rowv[4 * j + 3] = v.w;
-        }
-        named_bar(4, 256);                                      // X is reused as the epilogue's staging area
-        fused_w_epilogue<64>(rowv, *fz, M, mt, nt, ord.n_tiles, (ct & 127) >> 5, ct >> 7, lane, out_scale,
-                             smem_gen + L::EPI_OFFSET);
-        continue;
-      }
       // Epilogue: a quad of lanes writes 32 contiguous bytes of a row per instruction (whole sectors)
       float* cbase = C + static_cast<long long>(z) * c_split_stride;
       const int colq = nt * BN + 2 * (lane & 3);
@@ -611,19 +333,8 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_cons
                    float* __restrict__ C, int M, int ldc, long long c_split_stride,
                    const TileOrder ord, int splits, int total_kb, int kb_per_split, int chain_kb,
                    const float* __restrict__ out_scale, const float* __restrict__ a_tile_scale, int a_tiles, int a_gshift) {
-  gemm_body<STAGES, BEXACT, F16, false>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, C, M, ldc, c_split_stride, ord, splits,
-                                        total_kb, kb_per_split, chain_kb, out_scale, a_tile_scale, a_tiles, a_gshift,
-                                        nullptr);
-}
-
-// NUM = F_other * X^T with the multiplicative update of the row factor in the epilogue (f16, 128-wide tiles, no split-K)
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_fused_w_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
-                    const __grid_constant__ CUtensorMap tmB_hi, int M, const TileOrder ord, int total_kb,
-                    const float* __restrict__ out_scale, const float* __restrict__ a_tile_scale, int a_tiles, int a_gshift,
-                    const __grid_constant__ FuseW fz) {
-  gemm_body<2, true, true, true>(tmA_hi, tmA_lo, tmB_hi, tmB_hi, nullptr, M, 0, 0, ord, 1, total_kb,
-                                 total_kb + (total_kb & 1), 2, out_scale, a_tile_scale, a_tiles, a_gshift, &fz);
+  gemm_body<STAGES, BEXACT, F16>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, C, M, ldc, c_split_stride, ord, splits, total_kb,
+                                 kb_per_split, chain_kb, out_scale, a_tile_scale, a_tiles, a_gshift);
 }
 
 // ------------------------------------------------------------------ host side
@@ -681,24 +392,6 @@ int make_map(CUtensorMap* map, const float* ptr, int rows, int cols, int ld, int
   if (cache.size() >= 512) cache.clear();             // views are few; a runaway caller just re-encodes
   cache.emplace(key, *map);
   return 0;
-}
-
-static int env_int(const char* name, int dflt) {
-  const char* e = std::getenv(name);
-  return e ? std::atoi(e) : dflt;
-}
-
-// k-blocks per accumulation chain: at most 16 MMAs between drains (general: 1 k-block = 12 MMAs,
-// exact-B: 2 k-blocks = 16 MMAs)
-template <bool BEXACT, bool F16>
-static int pick_chain_kb(const GemmArgs& g) {
-  int chain_kb = g.chain_kb;
-  if (chain_kb <= 0) {
-    static const int env_chain = [] { const int v = env_int("CNMF_CHAIN_KB", 0); return v >= 1 ? v : 0; }();   // tuning knob
-    chain_kb = env_chain > 0 ? env_chain : (BEXACT ? 2 : 1);
-  }
-  if (F16) chain_kb = 2;     // scale groups of 512 elements = 8 k-blocks: chains of 2 never straddle one
-  return chain_kb;
 }
 
 // Modelled HBM bytes of one split-K slice in a grouped tile order (tools/probe_gemm.py restates this model): the
@@ -766,44 +459,14 @@ int launch(const GemmArgs& g, cudaStream_t stream) {
   }
   const int items = m_tiles * n_tiles * splits;
   const int grid = items < sms ? items : sms;
-  const int chain_kb = pick_chain_kb<BEXACT, F16>(g);
   const double kslice_row = static_cast<double>(kb_per_split) * BK * 4;       // bytes of one slice row, one piece
   const TileOrder ord = pick_tile_order(m_tiles, n_tiles, BM * kslice_row * 2, BN * kslice_row * (BEXACT ? 1 : 2),
                                         grid, l2);
+  // chain_kb: at most 16 MMAs between drains (3-pass form: 1 k-block = 12 MMAs, exact-B forms: 2 k-blocks = 16; f16
+  // chains of 2 never straddle a scale group).  a_gshift = 3: f16 scale groups of 8 k-blocks = 512 elements.
   kern<<<grid, NUM_THREADS, L::DYN_BYTES, stream>>>(mAh, mAl, mBh, mBl, g.C, g.M, g.ldc, g.c_split_stride,
-                                                    ord, splits, total_kb, kb_per_split, chain_kb,
-                                                    g.out_col_scale, g.a_tile_scale, g.a_tiles,
-                                                    g.a_group_kb_shift > 0 ? g.a_group_kb_shift : 3);
-  CNMF_CUDA_CHECK(cudaGetLastError());
-  return 0;
-}
-
-// fused W-half launch: 128 x 128 tiles, the whole reduction in one item (no split-K), f16
-int launch_fused_w(const GemmArgs& g, cudaStream_t stream) {
-  using L = SmemLayout<2, true, FUSE_EPI_BYTES>;     // 2 stages of 48 KB leave room for the epilogue's state
-  CUtensorMap mAh, mAl, mBh;
-  int rc;
-  if ((rc = make_map(&mAh, g.A_hi, g.M, g.Kd, g.lda, BM, true))) return rc;
-  if ((rc = make_map(&mAl, g.A_lo, g.M, g.Kd, g.lda, BM, true))) return rc;
-  if ((rc = make_map(&mBh, g.B_hi, g.N, g.Kd, g.ldb, BN, true))) return rc;
-  int dev = 0, sms = 0, l2 = 0;
-  CNMF_CUDA_CHECK(cudaGetDevice(&dev));
-  CNMF_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  CNMF_CUDA_CHECK(cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, dev));
-  const int m_tiles = (g.M + BM - 1) / BM, n_tiles = (g.N + BN - 1) / BN;
-  const int total_kb = (g.Kd + 2 * BK - 1) / (2 * BK);
-  static bool attr_set[64] = {};
-  if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-    CNMF_CUDA_CHECK(cudaFuncSetAttribute(gemm_fused_w_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L::DYN_BYTES));
-    if (dev >= 0 && dev < 64) attr_set[dev] = true;
-  }
-  const int items = m_tiles * n_tiles;
-  const int grid = items < sms ? items : sms;
-  const double k_row = static_cast<double>(total_kb) * 2 * BK * 2;             // bytes of one fp16 row, one piece
-  const TileOrder ord = pick_tile_order(m_tiles, n_tiles, BM * k_row * 2, BN * k_row, grid, l2);
-  gemm_fused_w_kernel<<<grid, NUM_THREADS, L::DYN_BYTES, stream>>>(mAh, mAl, mBh, g.M, ord, total_kb,
-                                                                   g.out_col_scale, g.a_tile_scale, g.a_tiles,
-                                                                   g.a_group_kb_shift > 0 ? g.a_group_kb_shift : 3, g.fuse);
+                                                    ord, splits, total_kb, kb_per_split, BEXACT ? 2 : 1,
+                                                    g.out_col_scale, g.a_tile_scale, g.a_tiles, 3);
   CNMF_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
@@ -843,13 +506,6 @@ int gemm_tf32x3(const GemmArgs& g, cudaStream_t stream) {
     CNMF_REQUIRE(g.b_exact, "gemm: the fp16 path needs an exact B operand");
     CNMF_REQUIRE(g.lda % 8 == 0 && g.ldb % 8 == 0, "gemm: fp16 leading dimensions must be multiples of 8 halves");
     CNMF_REQUIRE(!g.a_tile_scale || g.a_tiles * 512 >= g.Kd, "gemm: a_tiles does not cover the reduction length");
-    CNMF_REQUIRE(g.chain_kb == 0 || g.chain_kb == 2, "gemm: the fp16 path drains chains of 2 k-blocks");
-    if (g.fuse.active) {
-      CNMF_REQUIRE(g.fuse.F_in && g.fuse.F_out && g.fuse.F_in != g.fuse.F_out && g.fuse.P_hi && g.fuse.P_mid &&
-                       g.fuse.tile_scale && g.fuse.gram_in && g.fuse.row_slot && g.fuse.ld % 32 == 0,
-                   "gemm: incomplete fused-update arguments");
-      return launch_fused_w(g, stream);
-    }
     return launch<4, true, true>(g, stream);
   }
   if (g.b_exact) return launch<4, true, false>(g, stream);

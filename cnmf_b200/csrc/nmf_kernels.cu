@@ -183,8 +183,8 @@ __global__ void sums_final_kernel(const double* __restrict__ part, int nblocks, 
 // The pieces are a pure function of the factor values: this stand-alone kernel (initial factors, re-packing after a
 // compaction, K > 16 batches) and the in-update emission (emit_tile_f16) produce the same bits, so a restart's
 // operands do not depend on when the batch around it was compacted.
-// One block per row, one warp per group of 128 * QUADS columns (512: what the update kernels' tiles emit; 128: what the
-// fused GEMM epilogue emits, one group per 128-item tile), a lane owns QUADS 16-byte quads of the group.
+// One block per row, one warp per group of 128 * QUADS columns (512: what the update kernels' tiles emit), a lane owns
+// QUADS 16-byte quads of the group.
 template <int QUADS>
 __global__ void __launch_bounds__(256)
 emit_f16_kernel(const float* __restrict__ F, int n, int ld, const float* __restrict__ pscale, __half* __restrict__ hi,
@@ -631,7 +631,7 @@ __device__ __forceinline__ float4 lds128(unsigned addr) {
 // item group of a row (n % 4 != 0: product columns >= n are undefined) as its own instantiation so that the common
 // case carries no selects.  SIMPLE = one product slice and no tf32 pieces to write (the W half of the default f16x2
 // path): the slice loop and the piece pointers drop out of the body.  Same arithmetic, same order as the rolled loop
-// of round 1.
+// of mu_body.
 template <int KP, int VEC, bool GRAM, bool RAGGED, bool SIMPLE>
 __device__ __forceinline__ float2 mu_components(float* __restrict__ pFc, float* pH, float* pL, const float* __restrict__ pNc,
                                                 int nsplit, long long sstride, unsigned ld, unsigned g_row, int K, float l1,
@@ -1299,16 +1299,11 @@ int launch_split_scaled(const float* src, float* hi, float* lo, int rows, int ld
 }
 
 int launch_emit_f16(const float* F, int rows, int n, int ld, const float* pscale, void* hi, void* mid, float* tile_scale,
-                    int n_ktiles, cudaStream_t s, int group) {
-  CNMF_REQUIRE(group == 512 || group == 128, "emit_f16: scale groups hold 512 or 128 elements");
-  CNMF_REQUIRE(ld % 8 == 0 && (long long)n_ktiles * group >= ld, "emit_f16: bad ld / n_ktiles");
+                    int n_ktiles, cudaStream_t s) {
+  CNMF_REQUIRE(ld % 8 == 0 && (long long)n_ktiles * 512 >= ld, "emit_f16: bad ld / n_ktiles");
   if (rows <= 0) return 0;
-  if (group == 512)
-    emit_f16_kernel<4><<<rows, 256, 0, s>>>(F, n, ld, pscale, static_cast<__half*>(hi), static_cast<__half*>(mid), tile_scale,
-                                            n_ktiles);
-  else
-    emit_f16_kernel<1><<<rows, 256, 0, s>>>(F, n, ld, pscale, static_cast<__half*>(hi), static_cast<__half*>(mid), tile_scale,
-                                            n_ktiles);
+  emit_f16_kernel<4><<<rows, 256, 0, s>>>(F, n, ld, pscale, static_cast<__half*>(hi), static_cast<__half*>(mid), tile_scale,
+                                          n_ktiles);
   CNMF_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
@@ -1401,33 +1396,16 @@ static int launch_update_inst(dim3 grid, const FactorView& f, const float* NUM, 
   return 0;
 }
 
-// MU with the fused Gram at kp == 16, CNMF_UPD_VARIANT: 2 (default) = products streamed from global memory one
-// component ahead of their use, no product tile in shared memory, 4 blocks per SM (128 registers); 0 = round 1's
-// layout (products staged in a second shared-memory tile, 3 blocks per SM); 1 / 3 = streamed at 3 / 5 blocks per SM.
-// Every variant computes the same bits.
-static int upd_variant() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("CNMF_UPD_VARIANT");
-    v = e ? atoi(e) : 2;
-    if (v < 0 || v > 3) v = 2;
-  }
-  return v;
-}
-
+// MU with the fused Gram at kp == 16: products streamed from global memory one component ahead of their use, no
+// product tile in shared memory, 4 blocks per SM (128 registers).  Everything else stages the products in shared memory.
 template <int KPMAX, bool CD, bool GRAM>
 static int launch_update_variant(dim3 grid, const FactorView& f, const float* NUM, int nsplit, long long sstride,
                                  const double* gram_in, const BatchMeta& b, float l1, float l2, const FusedOut& out,
                                  cudaStream_t s) {
-  if constexpr (KPMAX == 16 && !CD && GRAM) {
-    switch (upd_variant()) {
-      case 1: return launch_update_inst<KPMAX, CD, GRAM, 3, true>(grid, f, NUM, nsplit, sstride, gram_in, b, l1, l2, out, s);
-      case 2: return launch_update_inst<KPMAX, CD, GRAM, 4, true>(grid, f, NUM, nsplit, sstride, gram_in, b, l1, l2, out, s);
-      case 3: return launch_update_inst<KPMAX, CD, GRAM, 5, true>(grid, f, NUM, nsplit, sstride, gram_in, b, l1, l2, out, s);
-      default: break;
-    }
-  }
-  return launch_update_inst<KPMAX, CD, GRAM, (KPMAX == 32 ? 2 : 3), false>(grid, f, NUM, nsplit, sstride, gram_in, b, l1, l2, out, s);
+  if constexpr (KPMAX == 16 && !CD && GRAM)
+    return launch_update_inst<KPMAX, CD, GRAM, 4, true>(grid, f, NUM, nsplit, sstride, gram_in, b, l1, l2, out, s);
+  else
+    return launch_update_inst<KPMAX, CD, GRAM, (KPMAX == 32 ? 2 : 3), false>(grid, f, NUM, nsplit, sstride, gram_in, b, l1, l2, out, s);
 }
 
 template <bool CD>

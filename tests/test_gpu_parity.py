@@ -763,21 +763,3 @@ def test_two_gpu_sharded_factorize_allgather_consensus():
     assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-4000:]
     assert r.stdout.count("merged spectra match the reference fixture") == 2, r.stdout[-2000:]
 
-
-# explicit ids: the ids these cases have always had
-@pytest.mark.parametrize("env", [{"CNMF_FUSE_W": "1"}, {"CNMF_UPD_VARIANT": "0"}], ids=["env0", "env2"])
-def test_opt_in_kernel_variants_keep_parity(env):
-    """The opt-in kernel variants -- the W-half multiplicative update applied in the GEMM epilogue (CNMF_FUSE_W=1) and
-    the first update-kernel layout (CNMF_UPD_VARIANT=0) -- on a multi-tile, mixed-K batch (45 restarts, K = 5..13,
-    405 packed rows) against the numpy oracle: identical n_iter, spectra within 1e-4.  They are opt-in because the
-    default kernels are faster, not because they are less exact."""
-    import json
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    e = dict(os.environ, **env)
-    r = subprocess.run([sys.executable, os.path.join(root, "tools", "probe_fused.py")], capture_output=True, text=True,
-                       env=e, timeout=600)
-    assert r.returncode == 0, r.stdout[-1000:] + r.stderr[-3000:]
-    out = json.loads([l for l in r.stdout.splitlines() if l.startswith("{")][-1])
-    assert out["bad"] == [] and out["worst_rel"] < 1e-4, out
