@@ -18,7 +18,9 @@
 // Structure (one CTA per SM, persistent over a static tile schedule, 384 threads = 3 warpgroups):
 //   warpgroup 0     TMA producer (one thread): cp.async.bulk.tensor 2D, 128B-swizzled tiles, mbarrier full/empty ring
 //   warpgroups 1-2  consumers: rows [0, 64) / [64, 128) of the 128 x 128 tile, wgmma.mma_async m64n128 from shared
-//                   memory descriptors, fp32 fragment in registers, float2 stores
+//                   memory descriptors, fp32 fragment in registers, float2 stores.  Two named barriers make them take
+//                   turns issuing one k-block of MMAs each (ping-pong), so one warpgroup's chain drain and tile stores
+//                   run while the other's MMAs keep the tensor pipe busy.
 //
 // Accumulation accuracy.  The tensor core does not round its running sum to nearest: a long chain of MMAs on
 // non-negative data is biased low by about 3e-8 relative per MMA (2.3e-5 at K = 2048), far outside the 1e-4 parity
@@ -107,6 +109,15 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
   d |= static_cast<uint64_t>(1024 >> 4) << 32;
   d |= static_cast<uint64_t>(1) << 62;
   return d;
+}
+
+// Named barriers (id 0 is __syncthreads): bar.sync blocks until `count` threads have reached the barrier, bar.arrive
+// counts this warp without waiting.  Here 128 threads sync and the other warpgroup's 128 arrive.
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
@@ -245,8 +256,15 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
     }
   } else {
     // ===================== consumers: MMA chains + drain + epilogue =====================
+    // The two warpgroups take turns issuing one k-block of MMAs each (warpgroup 1 first): barrier TURN_BAR + cw is this
+    // warpgroup's turn, and it hands the turn over right after its commit.  Each chain's drain, sums and tile stores
+    // then run while the other warpgroup's k-block is still in the tensor pipe.  Both walk the same items, so they take
+    // the same number of turns; warpgroup 2's hand-off before the first turn and warpgroup 1's sync after the last one
+    // pair the ends.  Only the issue time changes, not which MMAs form a chain or the order of the sums.
+    constexpr uint32_t TURN_BAR = 1, TURN_THREADS = 256;
     const int cw = wg - 1;                                      // rows [64 cw, 64 cw + 64) of the tile
     const uint32_t a_off = static_cast<uint32_t>(cw * 64 * 128);
+    if (cw == 1) named_bar_arrive(TURN_BAR, TURN_THREADS);
     int stage = 0;
     uint32_t phase = 0;
     for (int w = blockIdx.x; w < items; w += gridDim.x) {
@@ -267,6 +285,7 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
         int prev = -1;
         for (int kb = c0; kb < c1; ++kb) {
           mbar_wait(full_bar(stage), phase);
+          named_bar_sync(TURN_BAR + cw, TURN_THREADS);
           const uint32_t st = smem_base + stage * L::STAGE_BYTES;
           const uint64_t a_hi = make_smem_desc(st + a_off);
           const uint64_t a_lo = make_smem_desc(st + L::A_BYTES + a_off);
@@ -282,6 +301,7 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
             wgmma_m64n128<F16>(d, a_hi + koff, b_hi + koff, 1u);
           }
           wgmma_commit();
+          named_bar_arrive(TURN_BAR + (cw ^ 1), TURN_THREADS);
           if (prev >= 0) {                                      // the previous k-block's MMAs have read their slot
             wgmma_wait<1>();
             if (lane == 0) mbar_arrive(empty_bar(prev));
@@ -306,23 +326,36 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
           for (int i = 0; i < 64; ++i) acc[i] += d[i];          // round-to-nearest fp32
         }
       }
-      // Epilogue: a quad of lanes writes 32 contiguous bytes of a row per instruction (whole sectors)
+      // Epilogue: a quad of lanes writes 32 contiguous bytes of a row per instruction (whole sectors).  The column
+      // scales are loaded EPI_J at a time ahead of their stores, so the epilogue waits for 2 load latencies, not for 16
+      // in a row, and fits better under the other warpgroup's last k-block (all 16 at once would need 168 registers
+      // and spill).
+      constexpr int EPI_J = 8;
       float* cbase = C + static_cast<long long>(z) * c_split_stride;
       const int colq = nt * BN + 2 * (lane & 3);
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int col = colq + 8 * j;
-        if (col >= ldc) continue;                               // ldc % 4 == 0 and col even: col + 1 < ldc too
-        float2 sc = make_float2(1.f, 1.f);
-        if (out_scale) sc = *reinterpret_cast<const float2*>(out_scale + col);   // length >= ldc, zero padded
-        if (row0 < M)
-          *reinterpret_cast<float2*>(cbase + static_cast<long long>(row0) * ldc + col) =
-              make_float2(acc[4 * j] * sc.x, acc[4 * j + 1] * sc.y);
-        if (row0 + 8 < M)
-          *reinterpret_cast<float2*>(cbase + static_cast<long long>(row0 + 8) * ldc + col) =
-              make_float2(acc[4 * j + 2] * sc.x, acc[4 * j + 3] * sc.y);
+      for (int j0 = 0; j0 < 16; j0 += EPI_J) {
+        float2 sc[EPI_J];
+#pragma unroll
+        for (int j = 0; j < EPI_J; ++j) {                       // length >= ldc, zero padded
+          const int col = colq + 8 * (j0 + j);
+          sc[j] = out_scale && col < ldc ? *reinterpret_cast<const float2*>(out_scale + col) : make_float2(1.f, 1.f);
+        }
+#pragma unroll
+        for (int j = 0; j < EPI_J; ++j) {
+          const int col = colq + 8 * (j0 + j);
+          if (col >= ldc) continue;                             // ldc % 4 == 0 and col even: col + 1 < ldc too
+          const float* a = acc + 4 * (j0 + j);
+          if (row0 < M)
+            *reinterpret_cast<float2*>(cbase + static_cast<long long>(row0) * ldc + col) =
+                make_float2(a[0] * sc[j].x, a[1] * sc[j].y);
+          if (row0 + 8 < M)
+            *reinterpret_cast<float2*>(cbase + static_cast<long long>(row0 + 8) * ldc + col) =
+                make_float2(a[2] * sc[j].x, a[3] * sc[j].y);
+        }
       }
     }
+    if (cw == 0) named_bar_sync(TURN_BAR, TURN_THREADS);
   }
 }
 

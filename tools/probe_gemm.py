@@ -1,26 +1,32 @@
 #!/usr/bin/env python
-"""GPU probe: the batched GEMM alone (f16x2 path), mean device time per launch, accuracy, and the modelled HBM operand
-traffic of two tile orders: the m-tile-fastest order of the first kernel versions and the grouped order the launcher
-picks now (the same rule as pick_tile_order in csrc/gemm_tf32x3.cu, restated here).
+"""GPU probe: the batched GEMM alone, mean device time per launch, accuracy, and the modelled HBM operand traffic of two
+tile orders: the m-tile-fastest order of the first kernel versions and the grouped order the launcher picks now (the
+same rule as pick_tile_order in csrc/gemm_tf32x3.cu, restated here).
+
+    python tools/probe_gemm.py [--precision f16x2|tf32x3|tf32x3-general] [case ...]
+
+--precision (default f16x2) is passed to Engine.gemm_abt.  f16x2 runs gemm_tf32x3_kernel<4,exact-B,f16>.  The raw GEMM
+hook does not assume B exact in tf32, so tf32x3 and tf32x3-general both run the 3-pass <3,general> form there.
 
 Cases: c2-shaped problems, a 4 096-row problem, the c3 shapes at full SK (8 100 packed rows: factor operand larger
 than the L2) and the same c3 shapes with 1 024 rows (factor operand resident in the L2)."""
-import json, os, sys
+import argparse, json, os, sys
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from cnmf_b200.engine import Engine
 
 BM = BN = 128            # output tile
-KB_ELEMS = 64            # fp16 elements per k-block
+KB_BYTES = 128           # bytes of one operand piece per row and k-block: 64 fp16 or 32 tf32 elements
 
 
-def slices(Kd, splits):
-    """k-blocks per split-K slice, as the launcher partitions them (slices start on even k-blocks)."""
-    total_kb = -(-Kd // KB_ELEMS)
+def slices(Kd, splits, f16):
+    """k-blocks per split-K slice, as the launcher partitions them (f16 slices start on even k-blocks)."""
+    total_kb = -(-Kd // (64 if f16 else 32))
     splits = max(1, min(splits, total_kb))
     kbps = -(-total_kb // splits)
-    kbps += kbps & 1
+    if f16:
+        kbps += kbps & 1
     return [min(kbps, total_kb - z * kbps) for z in range(-(-total_kb // kbps))]
 
 
@@ -49,39 +55,46 @@ def pick_order(m_tiles, n_tiles, a_panel, b_panel, grid, budget):
     return best
 
 
-def model(M, N, Kd, splits, l2, sms):
-    """Modelled operand bytes of the launch (A = two fp16 pieces, B = one exact fp16 operand) in both orders."""
+def model(M, N, Kd, splits, l2, sms, f16):
+    """Modelled operand bytes of the launch in both orders.  A is two pieces; B is one exact fp16 operand (f16) or two
+    tf32 pieces (the 3-pass form)."""
     m_tiles, n_tiles = -(-M // BM), -(-N // BN)
-    kbs = slices(Kd, splits)
+    kbs = slices(Kd, splits, f16)
     items = m_tiles * n_tiles * len(kbs)
     grid = min(items, sms)
     budget = l2 // 2
-    a_panel, b_panel = (BM * kbs[0] * KB_ELEMS * 4, BN * kbs[0] * KB_ELEMS * 2)
+    b_pieces = 1 if f16 else 2
+    a_panel, b_panel = (BM * kbs[0] * KB_BYTES * 2, BN * kbs[0] * KB_BYTES * b_pieces)
     _, g, gn = pick_order(m_tiles, n_tiles, a_panel, b_panel, grid, budget)
     flat = grouped = 0
     for kb in kbs:
-        ap, bp = BM * kb * KB_ELEMS * 4, BN * kb * KB_ELEMS * 2
+        ap, bp = BM * kb * KB_BYTES * 2, BN * kb * KB_BYTES * b_pieces
         flat += order_bytes(m_tiles, n_tiles, ap, bp, m_tiles, grid, budget)
         grouped += (order_bytes(n_tiles, m_tiles, bp, ap, g, grid, budget) if gn else
                     order_bytes(m_tiles, n_tiles, ap, bp, g, grid, budget))
-    minimum = sum(m_tiles * BM * kb * KB_ELEMS * 4 + n_tiles * BN * kb * KB_ELEMS * 2 for kb in kbs)
+    minimum = sum(m_tiles * BM * kb * KB_BYTES * 2 + n_tiles * BN * kb * KB_BYTES * b_pieces for kb in kbs)
     return {"m_fastest_GB": round(flat / 1e9, 3), "grouped_GB": round(grouped / 1e9, 3), "min_GB": round(minimum / 1e9, 3),
             "grouped_order": "%d %s-tiles per group" % (g, "n" if gn else "m"), "slices": len(kbs)}
 
 
 def main():
+    ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
+    ap.add_argument("--precision", choices=("f16x2", "tf32x3", "tf32x3-general"), default="f16x2")
+    ap.add_argument("cases", nargs="*", help="case names to run (default: all)")
+    args = ap.parse_args()
+    f16 = args.precision == "f16x2"
     import torch
     props = torch.cuda.get_device_properties(0)
     l2, sms = props.L2_cache_size, props.multi_processor_count
     eng = Engine(0)
     rng = np.random.RandomState(0)
-    out = {"device": props.name, "l2_bytes": l2, "sms": sms}
+    out = {"device": props.name, "l2_bytes": l2, "sms": sms, "precision": args.precision}
     cases = {"c2_W_half": (1000, 20000, 2000, 1), "c2_H_half": (1000, 2000, 20000, 5),
              "mid_W_half": (4096, 16384, 2000, 1), "mid_H_half": (4096, 2000, 16384, 4),
              "tail_H_half": (128, 2000, 20000, 5),
              "c3_W_half_full": (8100, 50000, 2000, 1), "c3_H_half_full": (8100, 2000, 50000, 13),
              "c3_W_half_1024": (1024, 50000, 2000, 1), "c3_H_half_1024": (1024, 2000, 50000, 13)}
-    only = sys.argv[1:]
+    only = args.cases
     for name, (M, N, K, sp) in cases.items():
         if only and name not in only:
             continue
@@ -92,13 +105,13 @@ def main():
         else:
             A = np.abs(rng.standard_normal((M, K))).astype(np.float32)
             B = rng.poisson(1.5, size=(N, K)).astype(np.float32)
-        C, ms = eng.gemm_abt(A, B, precision="f16x2", splits=sp, reps=20)
+        C, ms = eng.gemm_abt(A, B, precision=args.precision, splits=sp, reps=20)
         ref = A[:64].astype(np.float64) @ B.astype(np.float64).T
         err = float(np.linalg.norm(C[:64] - ref) / np.linalg.norm(ref))
         tail = A[-64:].astype(np.float64) @ B.astype(np.float64).T
         err2 = float(np.linalg.norm(C[-64:] - tail) / np.linalg.norm(tail))
         out[name] = {"shape": [M, N, K, sp], "ms": round(ms, 4), "tflops": round(2.0 * M * N * K / (ms * 1e-3) / 1e12, 1),
-                     "rel_err_first_rows": err, "rel_err_last_rows": err2, "model": model(M, N, K, sp, l2, sms)}
+                     "rel_err_first_rows": err, "rel_err_last_rows": err2, "model": model(M, N, K, sp, l2, sms, f16)}
         print(name, json.dumps(out[name]), flush=True)
         del A, B, C
     print(json.dumps(out))
