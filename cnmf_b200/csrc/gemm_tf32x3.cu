@@ -15,8 +15,10 @@
 //   X H^T   (sklearn _nmf.py:538, :380)  ->  A = H_batch (SK x G),   B = X   (cells x G)
 //   W^T X   (sklearn _nmf.py:634, :380)  ->  A = W^T_batch (SK x N), B = X^T (G x cells), split-K
 //
-// Structure (one CTA per SM, persistent over a static tile schedule, 384 threads = 3 warpgroups):
-//   warpgroup 0     TMA producer (one thread): cp.async.bulk.tensor 2D, 128B-swizzled tiles, mbarrier full/empty ring
+// Structure (one CTA per SM, persistent over a static tile schedule, 384 threads = 3 warpgroups; the CTAs run in
+// clusters of 2 whose tiles share an m-tile, and each CTA loads half of the shared A panel and multicasts it to both):
+//   warpgroup 0     TMA producer (one thread): cp.async.bulk.tensor 2D, 128B-swizzled tiles, mbarrier full/empty ring,
+//                   a stage refilled only once both CTAs of the pair have released it
 //   warpgroups 1-2  consumers: rows [0, 64) / [64, 128) of the 128 x 128 tile, wgmma.mma_async m64n128 from shared
 //                   memory descriptors, fp32 fragment in registers, float2 stores.  Two named barriers make them take
 //                   turns issuing one k-block of MMAs each (ping-pong), so one warpgroup's chain drain and tile stores
@@ -57,8 +59,8 @@ struct SmemLayout {
   static constexpr int A_BYTES = BM * BK * 4;              // 16 KB
   static constexpr int B_BYTES = BN * BK * 4;              // 16 KB
   static constexpr int STAGE_BYTES = 2 * A_BYTES + (BEXACT ? 1 : 2) * B_BYTES;
-  static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;  // full[STAGES], empty[STAGES]
-  static constexpr int TOTAL = BAR_OFFSET + 2 * STAGES * 8;
+  static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;  // full[STAGES], empty[STAGES], peer_free[STAGES]
+  static constexpr int TOTAL = BAR_OFFSET + 3 * STAGES * 8;
   static constexpr int DYN_BYTES = TOTAL + 1024;           // slack for manual 1024 B alignment
   static_assert(DYN_BYTES <= 227 * 1024, "pipeline stages do not fit the shared memory of an SM");
 };
@@ -97,6 +99,34 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
+}
+// The same box written to the same CTA-relative `dst` in every CTA of `mask`, each CTA's copy signalling its own
+// mbarrier at the CTA-relative address `bar`.
+__device__ __forceinline__ void tma_load_2d_multicast(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1,
+                                                      uint16_t mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "h"(mask)
+      : "memory");
+}
+
+// Arrive on the mbarrier at the same offset in the CTA of cluster rank `rank`.  Default (CTA-scope) semantics, as for
+// the local arrivals: the arrival only signals that this CTA's consumers have finished reading a stage, and what follows
+// it is a TMA write, not a generic load.  With .release.cluster (and .acquire.cluster on the wait) ptxas emits
+// MEMBAR.ALL.GPU and an L1 invalidate around every k-block of the producer, which made the kernel slower than unpaired.
+__device__ __forceinline__ void mbar_arrive_remote(uint32_t bar, uint32_t rank) {
+  asm volatile(
+      "{\n\t.reg .b32 remote;\n\t"
+      "mapa.shared::cluster.u32 remote, %0, %1;\n\t"
+      "mbarrier.arrive.shared::cluster.b64 _, [remote];\n\t}"
+      ::"r"(bar), "r"(rank)
+      : "memory");
+}
+// All threads of both CTAs: release what this CTA did before, acquire what the peer did before its arrival.  Not
+// .aligned: the producer warp's lanes may reach it diverged.
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
 }
 
 // K-major, 128B-swizzled operand tile: rows of 128 B, 8-row groups 1024 B apart (wgmma matrix descriptor:
@@ -170,27 +200,29 @@ __device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t adesc, ui
 }
 
 // ------------------------------------------------------------------ tile order
-// Work item w -> (m-tile, n-tile, split-K slice z).  The slice is outermost.  Inside a slice the tiles run in groups of
-// `group` consecutive m-tiles (n-tiles if group_n), the grouped index fastest, and each group sweeps every tile of the
+// The CTAs run in clusters of 2 (a pair), and a pair's work item is an m-tile and two adjacent n-tiles: the CTA of
+// cluster rank r computes n-tile 2 * n-pair + r, and the two share the m-tile's A panel (multicast, see gemm_body).
+// Pair item w -> (m-tile, n-pair, split-K slice z).  The slice is outermost.  Inside a slice the items run in groups of
+// `group` consecutive m-tiles (n-pairs if group_n), the grouped index fastest, and each group sweeps every tile of the
 // other dimension: the group's operand panels stay in the L2 while the other operand streams past them (DESIGN.md
 // section 4.1; pick_tile_order chooses the group).  group = m_tiles, group_n = 0 is the plain m-tile-fastest order.
 // The producer and the consumers both decode through this function, so they always agree on a CTA's tiles.
 struct TileOrder {
-  int m_tiles, n_tiles, group, group_n;
+  int m_tiles, n_pairs, group, group_n;
 };
 
-__host__ __device__ __forceinline__ void decode_item(int w, const TileOrder& o, int& mt, int& nt, int& z) {
-  const int per_slice = o.m_tiles * o.n_tiles;
+__host__ __device__ __forceinline__ void decode_item(int w, const TileOrder& o, int& mt, int& np, int& z) {
+  const int per_slice = o.m_tiles * o.n_pairs;
   z = w / per_slice;
   int r = w - z * per_slice;
-  const int q_tiles = o.group_n ? o.n_tiles : o.m_tiles;      // grouped dimension
-  const int p_tiles = o.group_n ? o.m_tiles : o.n_tiles;      // swept dimension
+  const int q_tiles = o.group_n ? o.n_pairs : o.m_tiles;      // grouped dimension
+  const int p_tiles = o.group_n ? o.m_tiles : o.n_pairs;      // swept dimension
   const int g0 = r / (o.group * p_tiles) * o.group;           // first grouped tile of w's group (earlier groups are full)
   r -= g0 * p_tiles;
   const int gq = q_tiles - g0 < o.group ? q_tiles - g0 : o.group;   // the last group may be partial
   const int p = r / gq, q = g0 + r % gq;
   mt = o.group_n ? p : q;
-  nt = o.group_n ? q : p;
+  np = o.group_n ? q : p;
 }
 
 // ------------------------------------------------------------------ the kernel
@@ -203,7 +235,7 @@ template <int STAGES, bool BEXACT, bool F16>
 __device__ __forceinline__ void
 gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMap& tmB_hi, const CUtensorMap& tmB_lo,
           float* __restrict__ C, int M, int ldc, long long c_split_stride,
-          const TileOrder& ord, int splits, int total_kb, int kb_per_split, int chain_kb,
+          const TileOrder& ord, int n_tiles, int splits, int total_kb, int kb_per_split, int chain_kb,
           const float* __restrict__ out_scale, const float* __restrict__ a_tile_scale, int a_tiles, int a_gshift) {
   static_assert(!F16 || BEXACT, "the fp16 path exists for exact integer B operands only");
   constexpr int BKE = F16 ? 2 * BK : BK;                        // elements per k-block
@@ -215,39 +247,54 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
   const uint32_t bar_base = smem_base + L::BAR_OFFSET;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
+  auto peer_free_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + s); };
 
   const int wg = threadIdx.x >> 7;
   const int warp = (threadIdx.x >> 5) & 3;                      // warp inside its warpgroup
   const int lane = threadIdx.x & 31;
+  // __cluster_dims__(2, 1, 1): blocks 2c and 2c + 1 form cluster c, with ranks 0 and 1.
+  const int rank = blockIdx.x & 1, cluster = blockIdx.x >> 1, clusters = gridDim.x >> 1;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
       mbar_init(empty_bar(s), 8);                               // one arrival per consumer warp
+      mbar_init(peer_free_bar(s), 1);                           // the peer's producer
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  __syncthreads();
+  cluster_sync();                                               // both CTAs' barriers exist before any remote use
 
-  const int items = ord.m_tiles * ord.n_tiles * splits;
+  const int items = ord.m_tiles * ord.n_pairs * splits;
 
   if (wg == 0) {
     // ===================== TMA producer =====================
+    // Both CTAs of the pair need the whole 128-row A panel of the m-tile: each loads its 64-row half of A_hi and A_lo
+    // once from L2 and multicasts it to the same stage offset in both CTAs; B is the CTA's own n-tile, a local load.
+    // So a stage of this CTA is written by both producers, and may be refilled only once the consumers of BOTH CTAs
+    // have released it: after its local `empty` wait, the producer tells the peer (remote arrival on the peer's
+    // `peer_free`) and waits for the peer to say the same.  `full` still expects the whole stage; the peer's half may
+    // land before the local expect_tx, which the transaction count allows.  Both CTAs walk the same k-blocks.
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       constexpr uint32_t stage_tx = static_cast<uint32_t>(L::STAGE_BYTES);
-      for (int w = blockIdx.x; w < items; w += gridDim.x) {
-        int mt, nt, z;
-        decode_item(w, ord, mt, nt, z);
+      constexpr uint32_t HALF_A = L::A_BYTES / 2;
+      for (int w = cluster; w < items; w += clusters) {
+        int mt, np, z;
+        decode_item(w, ord, mt, np, z);
+        const int nt = 2 * np + rank;                           // past the last n-tile: B is zero-filled
         const int kb0 = z * kb_per_split;
         const int kb1 = min(total_kb, kb0 + kb_per_split);
         for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(empty_bar(stage), phase ^ 1u);
+          mbar_arrive_remote(peer_free_bar(stage), rank ^ 1);
+          mbar_wait(peer_free_bar(stage), phase);
           const uint32_t st = smem_base + stage * L::STAGE_BYTES;
           mbar_arrive_expect_tx(full_bar(stage), stage_tx);
-          tma_load_2d(st, &tmA_hi, full_bar(stage), kb * BKE, mt * BM);
-          tma_load_2d(st + L::A_BYTES, &tmA_lo, full_bar(stage), kb * BKE, mt * BM);
+          tma_load_2d_multicast(st + rank * HALF_A, &tmA_hi, full_bar(stage), kb * BKE, mt * BM + rank * (BM / 2), 0x3);
+          tma_load_2d_multicast(st + L::A_BYTES + rank * HALF_A, &tmA_lo, full_bar(stage), kb * BKE,
+                                mt * BM + rank * (BM / 2), 0x3);
           tma_load_2d(st + 2 * L::A_BYTES, &tmB_hi, full_bar(stage), kb * BKE, nt * BN);
           if constexpr (!BEXACT) tma_load_2d(st + 2 * L::A_BYTES + L::B_BYTES, &tmB_lo, full_bar(stage), kb * BKE, nt * BN);
           if (++stage == STAGES) { stage = 0; phase ^= 1u; }
@@ -267,9 +314,10 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
     if (cw == 1) named_bar_arrive(TURN_BAR, TURN_THREADS);
     int stage = 0;
     uint32_t phase = 0;
-    for (int w = blockIdx.x; w < items; w += gridDim.x) {
-      int mt, nt, z;
-      decode_item(w, ord, mt, nt, z);
+    for (int w = cluster; w < items; w += clusters) {
+      int mt, np, z;
+      decode_item(w, ord, mt, np, z);
+      const int nt = 2 * np + rank;
       const int kb0 = z * kb_per_split;
       const int kb1 = min(total_kb, kb0 + kb_per_split);
       const int row0 = mt * BM + cw * 64 + warp * 16 + (lane >> 2);   // and row0 + 8
@@ -326,6 +374,7 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
           for (int i = 0; i < 64; ++i) acc[i] += d[i];          // round-to-nearest fp32
         }
       }
+      if (nt >= n_tiles) continue;                              // second CTA of a pair past the last n-tile
       // Epilogue: a quad of lanes writes 32 contiguous bytes of a row per instruction (whole sectors).  The column
       // scales are loaded EPI_J at a time ahead of their stores, so the epilogue waits for 2 load latencies, not for 16
       // in a row, and fits better under the other warpgroup's last k-block (all 16 at once would need 168 registers
@@ -357,17 +406,18 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
     }
     if (cw == 0) named_bar_sync(TURN_BAR, TURN_THREADS);
   }
+  cluster_sync();                 // neither CTA exits while the peer may still write its shared memory or barriers
 }
 
 template <int STAGES, bool BEXACT, bool F16>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NUM_THREADS, 1)
 gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                    const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
                    float* __restrict__ C, int M, int ldc, long long c_split_stride,
-                   const TileOrder ord, int splits, int total_kb, int kb_per_split, int chain_kb,
+                   const TileOrder ord, int n_tiles, int splits, int total_kb, int kb_per_split, int chain_kb,
                    const float* __restrict__ out_scale, const float* __restrict__ a_tile_scale, int a_tiles, int a_gshift) {
-  gemm_body<STAGES, BEXACT, F16>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, C, M, ldc, c_split_stride, ord, splits, total_kb,
-                                 kb_per_split, chain_kb, out_scale, a_tile_scale, a_tiles, a_gshift);
+  gemm_body<STAGES, BEXACT, F16>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, C, M, ldc, c_split_stride, ord, n_tiles, splits,
+                                 total_kb, kb_per_split, chain_kb, out_scale, a_tile_scale, a_tiles, a_gshift);
 }
 
 // ------------------------------------------------------------------ host side
@@ -438,15 +488,16 @@ static double order_bytes(int q_tiles, int p_tiles, double q_panel, double p_pan
 
 // The tile order with the least modelled traffic, over both orientations and every balanced group size, with half of
 // the L2 as the budget of the resident panels (the other half holds the streamed operand and the output lines).
-// a_panel / b_panel: bytes of one 128-row operand panel of a slice, all pieces.  Ties keep the m-tile-fastest order,
-// which is what a problem whose factor operand fits the L2 gets.  The order decides only which CTA computes a tile
-// when: every output element is still formed by the same chains in the same order.
-static TileOrder pick_tile_order(int m_tiles, int n_tiles, double a_panel, double b_panel, int grid, long long l2_bytes) {
+// a_panel: bytes of one 128-row A panel of a slice, b_panel: of the 256 rows of B one n-pair covers, all pieces;
+// grid: the number of pairs (clusters) that run at once.  Ties keep the m-tile-fastest order, which is what a problem
+// whose factor operand fits the L2 gets.  The order decides only which CTA computes a tile when: every output element
+// is still formed by the same chains in the same order.
+static TileOrder pick_tile_order(int m_tiles, int n_pairs, double a_panel, double b_panel, int grid, long long l2_bytes) {
   const double budget = 0.5 * static_cast<double>(l2_bytes);
-  TileOrder best{m_tiles, n_tiles, m_tiles, 0};
-  double best_bytes = order_bytes(m_tiles, n_tiles, a_panel, b_panel, m_tiles, grid, budget);
+  TileOrder best{m_tiles, n_pairs, m_tiles, 0};
+  double best_bytes = order_bytes(m_tiles, n_pairs, a_panel, b_panel, m_tiles, grid, budget);
   for (int gn = 0; gn < 2; ++gn) {
-    const int q = gn ? n_tiles : m_tiles, p = gn ? m_tiles : n_tiles;
+    const int q = gn ? n_pairs : m_tiles, p = gn ? m_tiles : n_pairs;
     const double qb = gn ? b_panel : a_panel, pb = gn ? a_panel : b_panel;
     int prev = 0;
     for (int ng = 1; ng <= q; ++ng) {                 // groups of ceil(q / ng) tiles, the last one possibly shorter
@@ -454,7 +505,7 @@ static TileOrder pick_tile_order(int m_tiles, int n_tiles, double a_panel, doubl
       if (g == prev) continue;
       prev = g;
       const double b = order_bytes(q, p, qb, pb, g, grid, budget);
-      if (b < best_bytes) { best_bytes = b; best = TileOrder{m_tiles, n_tiles, g, gn}; }
+      if (b < best_bytes) { best_bytes = b; best = TileOrder{m_tiles, n_pairs, g, gn}; }
     }
   }
   return best;
@@ -466,16 +517,16 @@ int launch(const GemmArgs& g, cudaStream_t stream) {
   constexpr int BKE = F16 ? 2 * BK : BK;
   CUtensorMap mAh, mAl, mBh, mBl;
   int rc;
-  if ((rc = make_map(&mAh, g.A_hi, g.M, g.Kd, g.lda, BM, F16))) return rc;
-  if ((rc = make_map(&mAl, g.A_lo, g.M, g.Kd, g.lda, BM, F16))) return rc;
+  if ((rc = make_map(&mAh, g.A_hi, g.M, g.Kd, g.lda, BM / 2, F16))) return rc;     // each CTA of a pair loads half
+  if ((rc = make_map(&mAl, g.A_lo, g.M, g.Kd, g.lda, BM / 2, F16))) return rc;
   if ((rc = make_map(&mBh, g.B_hi, g.N, g.Kd, g.ldb, BN, F16))) return rc;
   if ((rc = make_map(&mBl, BEXACT ? g.B_hi : g.B_lo, g.N, g.Kd, g.ldb, BN, F16))) return rc;
-  int dev = 0, sms = 0, l2 = 0;
+  int dev = 0, l2 = 0;
   CNMF_CUDA_CHECK(cudaGetDevice(&dev));
-  CNMF_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   CNMF_CUDA_CHECK(cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, dev));
   const int m_tiles = (g.M + BM - 1) / BM;
   const int n_tiles = (g.N + BN - 1) / BN;
+  const int n_pairs = (n_tiles + 1) / 2;
   const int total_kb = (g.Kd + BKE - 1) / BKE;
   int splits = g.splits < 1 ? 1 : g.splits;
   if (splits > total_kb) splits = total_kb;
@@ -485,20 +536,29 @@ int launch(const GemmArgs& g, cudaStream_t stream) {
   if (splits != g.splits_effective) { set_last_error("gemm: splits_effective mismatch (use gemm_effective_splits)"); return -1; }
 
   auto kern = gemm_tf32x3_kernel<STAGES, BEXACT, F16>;
-  static bool attr_set[64] = {};              // per device: a second GPU in the same process needs its own call
-  if (dev < 0 || dev >= 64 || !attr_set[dev]) {
+  // Per device (a second GPU in the same process needs its own calls): the shared-memory attribute, then how many
+  // pairs fit at once (66 on a 132-SM H100 SXM).
+  static int max_clusters[64] = {};
+  int clusters_cap = dev >= 0 && dev < 64 ? max_clusters[dev] : 0;
+  if (clusters_cap == 0) {
     CNMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::DYN_BYTES));
-    if (dev >= 0 && dev < 64) attr_set[dev] = true;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(2, 1, 1);
+    cfg.blockDim = dim3(NUM_THREADS, 1, 1);
+    cfg.dynamicSmemBytes = L::DYN_BYTES;
+    CNMF_CUDA_CHECK(cudaOccupancyMaxActiveClusters(&clusters_cap, kern, &cfg));
+    if (clusters_cap < 1) { set_last_error("gemm: no 2-CTA cluster of this kernel fits the device"); return -1; }
+    if (dev >= 0 && dev < 64) max_clusters[dev] = clusters_cap;
   }
-  const int items = m_tiles * n_tiles * splits;
-  const int grid = items < sms ? items : sms;
+  const int items = m_tiles * n_pairs * splits;
+  const int clusters = items < clusters_cap ? items : clusters_cap;
   const double kslice_row = static_cast<double>(kb_per_split) * BK * 4;       // bytes of one slice row, one piece
-  const TileOrder ord = pick_tile_order(m_tiles, n_tiles, BM * kslice_row * 2, BN * kslice_row * (BEXACT ? 1 : 2),
-                                        grid, l2);
+  const TileOrder ord = pick_tile_order(m_tiles, n_pairs, BM * kslice_row * 2, 2 * BN * kslice_row * (BEXACT ? 1 : 2),
+                                        clusters, l2);
   // chain_kb: at most 16 MMAs between drains (3-pass form: 1 k-block = 12 MMAs, exact-B forms: 2 k-blocks = 16; f16
   // chains of 2 never straddle a scale group).  a_gshift = 3: f16 scale groups of 8 k-blocks = 512 elements.
-  kern<<<grid, NUM_THREADS, L::DYN_BYTES, stream>>>(mAh, mAl, mBh, mBl, g.C, g.M, g.ldc, g.c_split_stride,
-                                                    ord, splits, total_kb, kb_per_split, BEXACT ? 2 : 1,
+  kern<<<2 * clusters, NUM_THREADS, L::DYN_BYTES, stream>>>(mAh, mAl, mBh, mBl, g.C, g.M, g.ldc, g.c_split_stride,
+                                                            ord, n_tiles, splits, total_kb, kb_per_split, BEXACT ? 2 : 1,
                                                     g.out_col_scale, g.a_tile_scale, g.a_tiles, 3);
   CNMF_CUDA_CHECK(cudaGetLastError());
   return 0;

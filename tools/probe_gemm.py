@@ -1,7 +1,12 @@
 #!/usr/bin/env python
-"""GPU probe: the batched GEMM alone, mean device time per launch, accuracy, and the modelled HBM operand traffic of two
+"""GPU probe: the batched GEMM alone, mean device time per launch, accuracy, the modelled HBM operand traffic of two
 tile orders: the m-tile-fastest order of the first kernel versions and the grouped order the launcher picks now (the
-same rule as pick_tile_order in csrc/gemm_tf32x3.cu, restated here).
+same rule as pick_tile_order in csrc/gemm_tf32x3.cu, restated here), and the operand bytes the launch moves from the L2
+into shared memory, with and without the A multicast of the CTA pairs, with the rate the measured time gives.
+
+The kernel runs in clusters of 2 CTAs: a pair's work item is an m-tile and two adjacent n-tiles (an n-pair), so the
+tile order is over m-tiles x n-pairs, a B panel is 256 rows, and the grid of the order is the number of pairs that
+run at once (taken here as half the SMs; the launcher asks the device).
 
     python tools/probe_gemm.py [--precision f16x2|tf32x3|tf32x3-general] [case ...]
 
@@ -56,25 +61,33 @@ def pick_order(m_tiles, n_tiles, a_panel, b_panel, grid, budget):
 
 
 def model(M, N, Kd, splits, l2, sms, f16):
-    """Modelled operand bytes of the launch in both orders.  A is two pieces; B is one exact fp16 operand (f16) or two
-    tf32 pieces (the 3-pass form)."""
+    """Modelled operand bytes of the launch in both orders, and its L2 -> shared memory operand bytes.  A is two pieces;
+    B is one exact fp16 operand (f16) or two tf32 pieces (the 3-pass form)."""
     m_tiles, n_tiles = -(-M // BM), -(-N // BN)
+    n_pairs = -(-n_tiles // 2)
     kbs = slices(Kd, splits, f16)
-    items = m_tiles * n_tiles * len(kbs)
-    grid = min(items, sms)
+    items = m_tiles * n_pairs * len(kbs)
+    grid = min(items, sms // 2)
     budget = l2 // 2
     b_pieces = 1 if f16 else 2
-    a_panel, b_panel = (BM * kbs[0] * KB_BYTES * 2, BN * kbs[0] * KB_BYTES * b_pieces)
-    _, g, gn = pick_order(m_tiles, n_tiles, a_panel, b_panel, grid, budget)
+    a_panel, b_panel = (BM * kbs[0] * KB_BYTES * 2, 2 * BN * kbs[0] * KB_BYTES * b_pieces)
+    _, g, gn = pick_order(m_tiles, n_pairs, a_panel, b_panel, grid, budget)
     flat = grouped = 0
     for kb in kbs:
-        ap, bp = BM * kb * KB_BYTES * 2, BN * kb * KB_BYTES * b_pieces
-        flat += order_bytes(m_tiles, n_tiles, ap, bp, m_tiles, grid, budget)
-        grouped += (order_bytes(n_tiles, m_tiles, bp, ap, g, grid, budget) if gn else
-                    order_bytes(m_tiles, n_tiles, ap, bp, g, grid, budget))
+        ap, bp = BM * kb * KB_BYTES * 2, 2 * BN * kb * KB_BYTES * b_pieces
+        flat += order_bytes(m_tiles, n_pairs, ap, bp, m_tiles, grid, budget)
+        grouped += (order_bytes(n_pairs, m_tiles, bp, ap, g, grid, budget) if gn else
+                    order_bytes(m_tiles, n_pairs, ap, bp, g, grid, budget))
     minimum = sum(m_tiles * BM * kb * KB_BYTES * 2 + n_tiles * BN * kb * KB_BYTES * b_pieces for kb in kbs)
+    # L2 -> SM: every CTA loads its B tile each k-block; A (16 KB per piece and tile k-block) once per CTA unpaired,
+    # once per pair with the multicast (each CTA of the pair loads half and receives the other half).
+    piece = BM * KB_BYTES
+    kb_total = sum(kbs)
+    unpaired = m_tiles * n_tiles * kb_total * piece * (2 + b_pieces)
+    paired = m_tiles * kb_total * piece * (2 * n_pairs + b_pieces * n_tiles)
     return {"m_fastest_GB": round(flat / 1e9, 3), "grouped_GB": round(grouped / 1e9, 3), "min_GB": round(minimum / 1e9, 3),
-            "grouped_order": "%d %s-tiles per group" % (g, "n" if gn else "m"), "slices": len(kbs)}
+            "grouped_order": "%d %s per group" % (g, "n-pairs" if gn else "m-tiles"), "slices": len(kbs),
+            "l2_to_smem_unpaired_GB": round(unpaired / 1e9, 2), "l2_to_smem_paired_GB": round(paired / 1e9, 2)}
 
 
 def main():
@@ -110,8 +123,10 @@ def main():
         err = float(np.linalg.norm(C[:64] - ref) / np.linalg.norm(ref))
         tail = A[-64:].astype(np.float64) @ B.astype(np.float64).T
         err2 = float(np.linalg.norm(C[-64:] - tail) / np.linalg.norm(tail))
+        mdl = model(M, N, K, sp, l2, sms, f16)
         out[name] = {"shape": [M, N, K, sp], "ms": round(ms, 4), "tflops": round(2.0 * M * N * K / (ms * 1e-3) / 1e12, 1),
-                     "rel_err_first_rows": err, "rel_err_last_rows": err2, "model": model(M, N, K, sp, l2, sms, f16)}
+                     "l2_to_smem_TBps": round(mdl["l2_to_smem_paired_GB"] / ms, 2),
+                     "rel_err_first_rows": err, "rel_err_last_rows": err2, "model": mdl}
         print(name, json.dumps(out[name]), flush=True)
         del A, B, C
     print(json.dumps(out))
