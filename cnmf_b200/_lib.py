@@ -49,6 +49,8 @@ SIGNATURES = {
     "cnmf_profile_get_class": (_i, [_vp, _i, _pp(_d), _pp(_ll), _pp(_d)]),
     "cnmf_last_timing": (_i, [_vp, _pp(_d), _pp(_d), _pp(_d), _pp(_d)]),
     "cnmf_dataset_create": (_i, [_vp, _vp, _i, _i, _ll, _i, _i, _vp, _pp(_vp)]),
+    "cnmf_dataset_create_csc": (_i, [_vp, _i, _i, _ll, _vp, _vp, _vp, _i, _vp, _pp(_vp)]),
+    "cnmf_dataset_dense_bytes": (_i, [_i, _i, _i, _pp(_ll)]),
     "cnmf_dataset_from_columns": (_i, [_vp, _vp, _vp, _i, _vp, _pp(_vp)]),
     "cnmf_dataset_destroy": (_i, [_vp]),
     "cnmf_dataset_shape": (_i, [_vp, _pp(_i), _pp(_i)]),
@@ -88,7 +90,7 @@ SIGNATURES = {
 _lib = None
 
 
-ABI_VERSION = 7      # include/cnmf_b200.h CNMF_B200_ABI_VERSION
+ABI_VERSION = 8      # include/cnmf_b200.h CNMF_B200_ABI_VERSION
 
 
 def load():

@@ -406,8 +406,30 @@ int cnmf_dataset_create(cnmf_handle_t h, const float* X, int n_rows, int n_cols,
 
 int cnmf_dataset_finish_internal(cnmf_dataset_t d, void* stream) { return dataset_finish(d, as_stream(stream)); }
 
+int cnmf_dataset_dense_bytes(int n_rows, int n_cols, int precision, long long* peak) {
+  CNMF_REQUIRE(peak && n_rows > 0 && n_cols > 0, "dataset_dense_bytes: bad arguments");
+  // what dataset_alloc hands out for one array of `elems` floats
+  auto bytes = [](size_t elems) { return (long long)(std::max<size_t>(elems, 64) * sizeof(float)); };
+  const size_t nx = (size_t)n_rows * pad_ld(n_cols), nxt = (size_t)n_cols * pad_ld(n_rows);
+  if (precision == CNMF_PRECISION_FP32) {
+    *peak = bytes(nx) + bytes(nxt);                                        // X, Xt
+    return 0;
+  }
+  CNMF_REQUIRE(precision == CNMF_PRECISION_TF32X3 || precision == CNMF_PRECISION_TF32X3_GENERAL ||
+                   precision == CNMF_PRECISION_F16X2, "dataset_dense_bytes: bad precision");
+  // dataset_finish: the general form holds X, X_hi, X_lo, Xt_hi, Xt_lo; the exact tf32 form X, C, C^T and the
+  // detection's two scale vectors; the exact f16 form, while it is built, those plus C and C^T as fp16
+  const long long scales = precision == CNMF_PRECISION_TF32X3_GENERAL ? 0 : bytes(pad_ld(n_cols)) + bytes(pad_ld(n_rows));
+  const long long general = bytes(nx) * 3 + bytes(nxt) * 2 + scales;
+  const long long exact_tf32 = bytes(nx) * 2 + bytes(nxt) + scales;
+  const long long exact_f16 = exact_tf32 + bytes((nx + 1) / 2) + bytes((nxt + 1) / 2);
+  *peak = std::max(general, std::max(exact_tf32, exact_f16));
+  return 0;
+}
+
 int cnmf_dataset_min(cnmf_dataset_t d, float* min_host, void* stream) {
   CNMF_REQUIRE(d && min_host, "dataset_min: NULL argument");
+  CNMF_TRY(require_dense(d, "dataset_min"));
   CNMF_CUDA_CHECK(cudaSetDevice(d->h->device));
   return cnmf::matrix_min(d->h, d->X, d->n_rows, d->n_cols, d->ld_c, min_host, as_stream(stream));
 }
@@ -426,7 +448,7 @@ int cnmf_dataset_shape(cnmf_dataset_t d, int* n_rows, int* n_cols) {
   return 0;
 }
 
-int cnmf_dataset_is_exact(cnmf_dataset_t d) { return (d && d->exact) ? (d->f16 ? 2 : 1) : 0; }
+int cnmf_dataset_is_exact(cnmf_dataset_t d) { return (d && d->exact && !d->sparse) ? (d->f16 ? 2 : 1) : 0; }
 
 int cnmf_dataset_sums(cnmf_dataset_t d, double* sum, double* sum_sq) {
   CNMF_REQUIRE(d, "dataset_sums: NULL dataset");
@@ -533,6 +555,7 @@ int check_params(cnmf_dataset_s* d, const cnmf_nmf_params* p) {
   CNMF_REQUIRE(d && p, "NULL dataset or params");
   CNMF_REQUIRE(p->precision == d->precision, "params.precision must match the precision the dataset was created with");
   CNMF_REQUIRE(p->reserved2 == 0, "params.reserved2 must be 0");
+  CNMF_TRY(require_dense(d, "factorize"));
   if (p->beta_loss != CNMF_LOSS_FROBENIUS) CNMF_TRY(cnmf::dataset_ensure_full_transpose(d, nullptr));
   return 0;
 }
@@ -708,6 +731,7 @@ int cnmf_factorize_dev(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, c
 int cnmf_random_init_dev(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, const uint32_t* seeds, float* Wt_dev,
                          float* H_dev, void* stream) {
   CNMF_REQUIRE(d && n_restarts > 0 && ks_in && seeds && Wt_dev && H_dev, "random_init_dev: bad arguments");
+  CNMF_TRY(require_dense(d, "random_init_dev"));
   cnmf_handle_s* h = d->h;
   cudaStream_t s = as_stream(stream);
   CNMF_CUDA_CHECK(cudaSetDevice(h->device));

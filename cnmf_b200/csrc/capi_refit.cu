@@ -107,21 +107,25 @@ static int col_stats_impl(cnmf_dataset_t d, const double* row_scale_host, double
   cnmf_handle_s* h = d->h;
   cudaStream_t s = as_stream(stream);
   CNMF_CUDA_CHECK(cudaSetDevice(h->device));
-  const int strips = std::max(1, std::min(64, d->n_rows / 64));
-  double* part = static_cast<double*>(h->dev_buf("colstats.part", sizeof(double) * 2 * (size_t)strips * d->n_cols));
-  double* buf = static_cast<double*>(h->dev_buf("colstats", sizeof(double) * 2 * d->n_cols));
-  double* d_rs = nullptr;
-  if (row_scale_host) {
-    d_rs = static_cast<double*>(h->dev_buf("colstats.rs", sizeof(double) * d->n_rows));
-    if (!d_rs) return -2;
-    CNMF_CUDA_CHECK(cudaMemcpyAsync(d_rs, row_scale_host, sizeof(double) * d->n_rows, cudaMemcpyHostToDevice, s));
+  if (row_scale_host) CNMF_TRY(require_dense(d, "scaled_col_stats"));
+  double* buf = d->col_sums;        // sparse datasets: csc_col_stats_kernel ran at creation
+  if (!d->sparse) {
+    const int strips = std::max(1, std::min(64, d->n_rows / 64));
+    double* part = static_cast<double*>(h->dev_buf("colstats.part", sizeof(double) * 2 * (size_t)strips * d->n_cols));
+    buf = static_cast<double*>(h->dev_buf("colstats", sizeof(double) * 2 * d->n_cols));
+    double* d_rs = nullptr;
+    if (row_scale_host) {
+      d_rs = static_cast<double*>(h->dev_buf("colstats.rs", sizeof(double) * d->n_rows));
+      if (!d_rs) return -2;
+      CNMF_CUDA_CHECK(cudaMemcpyAsync(d_rs, row_scale_host, sizeof(double) * d->n_rows, cudaMemcpyHostToDevice, s));
+    }
+    if (!part || !buf) return -2;
+    dim3 grid((d->n_cols + 127) / 128, strips);
+    col_stats_kernel<<<grid, 128, 0, s>>>(d->X, d->n_rows, d->n_cols, d->ld_c, d_rs, part);
+    col_stats_reduce_kernel<<<(d->n_cols + 127) / 128, 128, 0, s>>>(part, strips, d->n_cols, buf);
+    CNMF_CUDA_CHECK(cudaGetLastError());
+    h->launches += 2;
   }
-  if (!part || !buf) return -2;
-  dim3 grid((d->n_cols + 127) / 128, strips);
-  col_stats_kernel<<<grid, 128, 0, s>>>(d->X, d->n_rows, d->n_cols, d->ld_c, d_rs, part);
-  col_stats_reduce_kernel<<<(d->n_cols + 127) / 128, 128, 0, s>>>(part, strips, d->n_cols, buf);
-  CNMF_CUDA_CHECK(cudaGetLastError());
-  h->launches += 2;
   CNMF_CUDA_CHECK(cudaMemcpyAsync(mean_host, buf, sizeof(double) * d->n_cols, cudaMemcpyDeviceToHost, s));
   CNMF_CUDA_CHECK(cudaMemcpyAsync(var_host, buf + d->n_cols, sizeof(double) * d->n_cols, cudaMemcpyDeviceToHost, s));
   CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
@@ -146,6 +150,7 @@ int cnmf_dataset_scaled_col_stats(cnmf_dataset_t d, const double* row_scale_host
 
 int cnmf_dataset_row_sums(cnmf_dataset_t d, double* row_sums_host, void* stream) {
   CNMF_REQUIRE(d && row_sums_host, "row_sums: NULL argument");
+  CNMF_TRY(require_dense(d, "row_sums"));
   cnmf_handle_s* h = d->h;
   cudaStream_t s = as_stream(stream);
   CNMF_CUDA_CHECK(cudaSetDevice(h->device));
@@ -190,7 +195,9 @@ int cnmf_dataset_from_columns(cnmf_dataset_t src, const int32_t* cols_host, cons
     cudaError_t e = cudaMemsetAsync(d->X, 0, (size_t)d->n_rows * d->ld_c * sizeof(float), s);
     if (e != cudaSuccess) rc = -2;
   }
-  if (rc == 0) {
+  if (rc == 0 && src->sparse) {
+    rc = csc_gather_cols(src, d_cols, d_scale, n_cols, d->X, d->ld_c, s);
+  } else if (rc == 0) {
     dim3 grid((n_cols + 127) / 128, std::min(d->n_rows, 16384));
     gather_cols_kernel<<<grid, 128, 0, s>>>(src->X, d->n_rows, src->ld_c, d_cols, d_scale, n_cols, d->X, d->ld_c);
     h->launches += 1;
@@ -223,6 +230,7 @@ int cnmf_dataset_from_columns(cnmf_dataset_t src, const int32_t* cols_host, cons
 
 int cnmf_dataset_scale_rows(cnmf_dataset_t src, const float* row_scale_host, void* stream, cnmf_dataset_t* out) {
   CNMF_REQUIRE(src && row_scale_host && out, "dataset_scale_rows: bad arguments");
+  CNMF_TRY(require_dense(src, "scale_rows"));
   cnmf_handle_s* h = src->h;
   cudaStream_t s = as_stream(stream);
   CNMF_CUDA_CHECK(cudaSetDevice(h->device));
@@ -260,13 +268,23 @@ int cnmf_refit(cnmf_dataset_t d, int transposed, int k, const float* fixed_host,
   CNMF_REQUIRE(d && fixed_host && p && out_host, "refit: NULL argument");
   CNMF_REQUIRE(p->precision == d->precision, "params.precision must match the precision the dataset was created with");
   CNMF_REQUIRE(k >= 1 && k <= KMAX, "refit: n_components must be in [1, 32] on the CUDA path");
+  if (d->sparse && !transposed) CNMF_TRY(require_dense(d, "refit with transposed = 0"));
+  if (d->sparse && p->beta_loss != CNMF_LOSS_FROBENIUS) CNMF_TRY(require_dense(d, "refit with a KL / IS beta_loss"));
   const auto t_enter = std::chrono::steady_clock::now();
   cnmf_handle_s* h = d->h;
   cudaStream_t s = as_stream(stream);
   CNMF_CUDA_CHECK(cudaSetDevice(h->device));
-  const bool tf32 = p->precision == CNMF_PRECISION_TF32X3;
+  // sparse datasets: the one product X^T W is formed by csc_project_kernel in fp64 before the solve, which then
+  // iterates on K x K Grams only -- no GEMM runs, so no operand pieces are made (fp32 solver code)
+  cnmf_nmf_params pp = *p;
+  if (d->sparse) pp.precision = CNMF_PRECISION_FP32;
+  const bool tf32 = pp.precision == CNMF_PRECISION_TF32X3;
   if (p->beta_loss != CNMF_LOSS_FROBENIUS) CNMF_TRY(dataset_ensure_full_transpose(d, s));
   DataView v = make_view(d, transposed != 0);
+  if (d->sparse) {
+    v.exact = v.f16 = false;
+    v.scale_r = v.scale_c = nullptr;
+  }
 
   const size_t nr = (size_t)k * v.ld_r, nc = (size_t)k * v.ld_c;
   float* Fr = static_cast<float*>(h->dev_buf("refit.Fr", nr * 4));
@@ -302,13 +320,23 @@ int cnmf_refit(cnmf_dataset_t d, int transposed, int k, const float* fixed_host,
   io.Fr = Fr; io.Fr_hi = Fr_hi; io.Fr_lo = Fr_lo;
   io.Fc = Fc; io.Fc_hi = Fc_hi; io.Fc_lo = Fc_lo;
   io.update_cols = false;
+  if (d->sparse) {
+    const int kp = round_up(k, 4);
+    float* U = static_cast<float*>(h->dev_buf("refit.U", (size_t)v.n_c * kp * 4));
+    float* NUM = static_cast<float*>(h->dev_buf("refit.NUM", nr * 4));
+    if (!U || !NUM) return -2;
+    CNMF_CUDA_CHECK(cudaMemsetAsync(NUM, 0, nr * 4, s));
+    CNMF_TRY(stage_rows(h, Fc, k, v.n_c, v.ld_c, kp, U, s));
+    CNMF_TRY(csc_project(d, U, k, kp, NUM, v.ld_r, s));
+    io.num_rows = NUM;
+  }
   auto t_solve = std::chrono::steady_clock::now();
   if (h->profile) {
     CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
     h->t_h2d_ms = std::chrono::duration<double, std::milli>(t_solve - t_enter).count();
     t_solve = std::chrono::steady_clock::now();
   }
-  CNMF_TRY(solve_batched(h, v, io, *p, s));
+  CNMF_TRY(solve_batched(h, v, io, pp, s));
   if (h->profile) h->t_solve_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_solve).count();
 
   // Fr is k x n_r; the caller wants n_r x k (row-major).  Transposed on the device into a COMPACT n_r x k array and
@@ -334,6 +362,21 @@ int cnmf_project_rows(cnmf_dataset_t d, int k, const float* Ut_host, float* out_
   cnmf_handle_s* h = d->h;
   cudaStream_t s = as_stream(stream);
   CNMF_CUDA_CHECK(cudaSetDevice(h->device));
+  if (d->sparse) {       // fp64 products and sums in a fixed order (csc_project_kernel), one rounding to fp32
+    CNMF_REQUIRE(k <= KMAX, "project_rows: k must be <= 32 on a sparse dataset");
+    const int kp = round_up(k, 4);
+    float* Ut = static_cast<float*>(h->dev_buf("proj.Ut", (size_t)k * d->n_rows * 4));
+    float* U = static_cast<float*>(h->dev_buf("proj.U", (size_t)d->n_rows * kp * 4));
+    float* C = static_cast<float*>(h->dev_buf("proj.C", (size_t)k * d->ld_c * 4));
+    if (!Ut || !U || !C) return -2;
+    CNMF_CUDA_CHECK(cudaMemcpyAsync(Ut, Ut_host, (size_t)k * d->n_rows * 4, cudaMemcpyHostToDevice, s));
+    CNMF_TRY(stage_rows(h, Ut, k, d->n_rows, d->n_rows, kp, U, s));
+    CNMF_TRY(csc_project(d, U, k, kp, C, d->ld_c, s));
+    CNMF_CUDA_CHECK(cudaMemcpy2DAsync(out_host, (size_t)d->n_cols * 4, C, (size_t)d->ld_c * 4, (size_t)d->n_cols * 4, k,
+                                      cudaMemcpyDeviceToHost, s));
+    CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
+    return 0;
+  }
   const bool tf32 = d->precision == CNMF_PRECISION_TF32X3;
   const size_t nr = (size_t)k * d->ld_r;
   float* A = static_cast<float*>(h->dev_buf("proj.A", nr * 4));

@@ -28,10 +28,11 @@ struct cnmf_handle_s {
   cudaStream_t prof_last_stream = nullptr;
   std::vector<Pending> ev_pending;
   size_t ev_used = 0;
-  // kernel classes: 0 = batched GEMM (work = algorithmic FLOPs), 1 = fused update kernels (work = algorithmic bytes)
-  static constexpr int PROF_CLASSES = 2;
-  double prof_ms[PROF_CLASSES] = {0.0, 0.0}, prof_work[PROF_CLASSES] = {0.0, 0.0};
-  long long prof_launches[PROF_CLASSES] = {0, 0};
+  // kernel classes: 0 = batched GEMM (work = algorithmic FLOPs), 1 = fused update kernels (work = algorithmic bytes),
+  // 2 = sparse products csc_project (work = algorithmic bytes)
+  static constexpr int PROF_CLASSES = 3;
+  double prof_ms[PROF_CLASSES] = {0.0, 0.0, 0.0}, prof_work[PROF_CLASSES] = {0.0, 0.0, 0.0};
+  long long prof_launches[PROF_CLASSES] = {0, 0, 0};
   double t_rng_ms = 0, t_h2d_ms = 0, t_solve_ms = 0, t_d2h_ms = 0;   // host wall-clock phases of the last cnmf_factorize
   int prof_begin(cudaStream_t s, double work, int cls = 0);    // start event (recorded or shared); returns slot or -1
   void prof_end(cudaStream_t s, int slot);
@@ -75,6 +76,19 @@ struct cnmf_dataset_s {
   void *X_h16 = nullptr, *Xt_h16 = nullptr;
   float *row_scale = nullptr, *col_scale = nullptr;    // lengths ld_r / ld_c, zero padded
   double sum = 0.0, sum_sq = 0.0;
+  // sparse datasets (cnmf_dataset_create_csc): X stays canonical CSC and none of the dense forms above exist
+  // (X == nullptr).  `exact` and the scales are still detected, so that cnmf_dataset_from_columns builds the same
+  // dense dataset from it as from the dense form of the matrix.  col_sums: per column sum(x) then sum(x^2), fp64.
+  // Columns are cut into chunks of at most CSC_CHUNK entries (item_ptr: first chunk of each column, n_cols + 1):
+  // csc_project_kernel gives one warp to a chunk.
+  bool sparse = false;
+  long long nnz = 0;
+  long long* col_ptr = nullptr;
+  int* row_idx = nullptr;
+  float* vals = nullptr;
+  double* col_sums = nullptr;
+  int* item_ptr = nullptr;
+  int n_items = 0;
   std::vector<std::pair<void*, size_t>> owned;
 };
 
@@ -112,6 +126,9 @@ struct SolveIO {
   float *Fr = nullptr, *Fr_hi = nullptr, *Fr_lo = nullptr;
   float *Fc = nullptr, *Fc_hi = nullptr, *Fc_lo = nullptr;
   bool update_cols = true;  // false: Fc fixed (refit)
+  // the row product, computed by the caller (refits of sparse datasets: NUM_r = Fc * X^T, SK x ld_r, one split).
+  // Requires update_cols = false; the solver then runs no GEMM and reads no B operand.
+  const float* num_rows = nullptr;
   std::vector<int> n_iter;  // out
   std::vector<double> last; // out: last convergence statistic (mu: error, cd: violation)
   std::vector<double> err;  // out: final ||X - Fr^T Fc||_F
@@ -125,5 +142,22 @@ int matrix_min(cnmf_handle_s* h, const float* X, int rows, int cols, int ld, flo
 // the streaming beta-divergence kernels read X in both orientations in full fp32: builds d->Xt if the dataset
 // (tf32x3 mode) only holds the pieces
 int dataset_ensure_full_transpose(cnmf_dataset_s* d, cudaStream_t s);
+
+// ---- sparse (CSC) datasets: sparse_kernels.cu
+constexpr int CSC_CHUNK = 4096;     // most entries of a column one warp of csc_project_kernel reduces
+// -3 with a message naming the entry point when d is sparse
+int require_dense(const cnmf_dataset_s* d, const char* what);
+// out (k x ld, first n_cols columns written) = U^T * X with U staged on the device as n_rows x kp floats
+// (kp = k rounded up to 4, zero padded); fp64 products and sums in a fixed order, rounded to fp32 once
+int csc_project(const cnmf_dataset_s* d, const float* U, int k, int kp, float* out, int ld, cudaStream_t s);
+// U (n x kp) <- F^T for a device matrix F (k x ld), zero in the columns k..kp-1: the layout csc_project reads
+int stage_rows(cnmf_handle_s* h, const float* F, int k, int n, int ld, int kp, float* U, cudaStream_t s);
+// per column sum(x), sum(x^2) into d->col_sums and the dataset totals into d->sum / d->sum_sq (synchronises)
+int csc_col_stats(cnmf_dataset_s* d, cudaStream_t s);
+// exact-count detection on the stored entries: the test dataset_finish runs on the dense form (synchronises)
+int csc_detect_exact(cnmf_dataset_s* d, cudaStream_t s);
+// dst (n_rows x ld_dst, zeroed by the caller)[:, c] = X[:, cols[c]] * scale[c]
+int csc_gather_cols(const cnmf_dataset_s* d, const int* cols, const float* scale, int n_cols, float* dst, int ld_dst,
+                    cudaStream_t s);
 
 }  // namespace cnmf

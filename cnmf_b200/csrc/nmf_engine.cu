@@ -93,6 +93,7 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
   CNMF_REQUIRE(R0 > 0 && (int)io.ks.size() == R0, "solve: bad restart list");
   CNMF_REQUIRE(p.solver == CNMF_SOLVER_MU || p.solver == CNMF_SOLVER_CD, "solve: unknown solver");
   CNMF_REQUIRE(p.max_iter >= 1, "solve: max_iter must be >= 1");
+  CNMF_REQUIRE(!io.num_rows || !io.update_cols, "solve: a caller-computed row product needs update_cols = false");
   const bool tf32 = p.precision == CNMF_PRECISION_TF32X3;
   const bool f16 = tf32 && v.f16;       // exact-count dataset created with CNMF_PRECISION_F16X2: f16 products
   const bool mu = p.solver == CNMF_SOLVER_MU;
@@ -159,7 +160,7 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
   float *NUMr = nullptr, *NUMc = nullptr;
   // the split-K factor is a function of the reduction length only (gemm_fixed_splits)
   auto plan_gemms = [&]() -> int {
-    plan_r.splits = gemm_fixed_splits(v.n_c, f16 ? 1 : 0);
+    plan_r.splits = io.num_rows ? 1 : gemm_fixed_splits(v.n_c, f16 ? 1 : 0);
     plan_r.split_stride = (long long)SK * v.ld_r;
     plan_c.splits = gemm_fixed_splits(v.n_r, f16 ? 1 : 0);
     plan_c.split_stride = (long long)SK * v.ld_c;
@@ -170,7 +171,7 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
   {
     const size_t need_r = (size_t)plan_r.splits * (size_t)SK0 * v.ld_r;
     const size_t need_c = (size_t)plan_c.splits * (size_t)SK0 * v.ld_c;
-    NUMr = static_cast<float*>(h->dev_buf("solve.NUMr", sizeof(float) * need_r));
+    NUMr = io.num_rows ? const_cast<float*>(io.num_rows) : static_cast<float*>(h->dev_buf("solve.NUMr", sizeof(float) * need_r));
     NUMc = io.update_cols ? static_cast<float*>(h->dev_buf("solve.NUMc", sizeof(float) * need_c)) : nullptr;
     if (!NUMr || (io.update_cols && !NUMc)) return -2;
   }
@@ -295,6 +296,7 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
     return launch_finalize(nullptr, nullptr, part, out, chunks, bm(), s);
   };
   auto gemm_rows = [&]() -> int {   // NUM_r = Fc * B_rows^T
+    if (io.num_rows) return 0;      // computed by the caller
     return run_gemm(h, p.precision, wFc, wFc_hi, wFc_lo, SK, v.ld_c, v.B_rows, NUMr, v.ld_r, plan_r, v.exact, v.scale_r,
                     f16, d_rs_c, s);
   };

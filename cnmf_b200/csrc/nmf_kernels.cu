@@ -86,12 +86,7 @@ __global__ void check_scaled_int_kernel(const float* __restrict__ X, int rows, i
     const int r = (int)(i / cols), c = (int)(i % cols);
     const float v = X[(long long)r * ld + c];
     if (v == 0.f) continue;
-    const float sc = (rs ? rs[r] : 1.f) * (cs ? cs[c] : 1.f);
-    const float q = v / sc;
-    const float n = rintf(q);
-    // fp32 rounding of a genuinely scaled integer: v, sc and the quotient each carry <= 2^-24 relative error, i.e.
-    // |q - n| <= 1.8e-7 n; anything further away (soft-corrected counts, arbitrary matrices) takes the general path
-    if (!(v > 0.f) || !(n >= 1.f) || n > 2048.f || fabsf(q - n) > 5e-7f * n) ++bad;
+    if (!is_scaled_int(v, (rs ? rs[r] : 1.f) * (cs ? cs[c] : 1.f))) ++bad;
   }
   bad = warp_sum(bad);
   if ((threadIdx.x & 31) == 0 && bad) atomicAdd(n_bad, bad);

@@ -1,0 +1,370 @@
+// Sparse (CSC) datasets: the TPM matrix of the consensus step (cnmf.py:950-969) kept as canonical CSC on the device
+// instead of the dense forms, for matrices whose dense forms do not fit.  Every use of the TPM in consensus touches it
+// in a single product or a column pass, so three kernels cover them:
+//   csc_project_kernel     out (k x G) = U^T X : the OLS accumulator (cnmf.py:119) and the one product X^T W of
+//                          refit_spectra (cnmf.py:952), after which the refit iterates on K x K Grams only
+//   csc_col_stats_kernel   per-column sum(x), sum(x^2) in fp64: col_stats and the refit's ||X||^2 and mean(X)
+//   csc_gather_cols_kernel X[:, cols] * scale into a dense matrix: the HVG dataset of cnmf.py:965-969
+// Products and sums run in fp64 in a fixed order, without floating-point atomics: two runs are bit-identical.
+#include <algorithm>
+#include <cstdlib>
+#include <string>
+#include <type_traits>
+#include <vector>
+
+#include "engine.h"
+#include "nmf_kernels.cuh"
+
+using namespace cnmf;
+
+extern "C" int cnmf_dataset_alloc_internal(cnmf_dataset_t d, float** p, size_t elems);   // capi.cu
+
+#define CNMF_TRY(expr)            \
+  do {                            \
+    int _rc = (expr);             \
+    if (_rc != 0) return _rc;     \
+  } while (0)
+
+namespace {
+
+constexpr int WARPS = 8;    // warps per block of the warp-per-column / warp-per-chunk kernels
+
+// One warp per chunk item (at most CSC_CHUNK entries of one column).  The kp / 4 lanes of a strand share one entry:
+// lane q of the strand gathers float4 number q of the entry's U row, so an entry costs one contiguous kp-float read.
+// The 32 / (kp / 4) strands take the chunk's entries round robin; their fp64 partials are added in strand order.
+__global__ void __launch_bounds__(WARPS * 32) csc_project_kernel(const long long* __restrict__ col_ptr,
+                                                                 const int* __restrict__ row_idx,
+                                                                 const float* __restrict__ vals,
+                                                                 const int* __restrict__ item_ptr, int n_cols,
+                                                                 int n_items, const float4* __restrict__ U, int kp,
+                                                                 double* __restrict__ part) {
+  __shared__ double acc_s[WARPS][32 * 4];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int G = kp >> 2;             // lanes per strand
+  const int P = 32 / G;              // strands per warp
+  const int strand = lane / G, q = lane - strand * G;
+  double* acc_w = acc_s[warp];
+  for (int item = blockIdx.x * WARPS + warp; item < n_items; item += gridDim.x * WARPS) {
+    // column of the item: last c with item_ptr[c] <= item
+    int lo = 0, hi = n_cols;
+    while (hi - lo > 1) {
+      const int mid = (lo + hi) >> 1;
+      if (item_ptr[mid] <= item) lo = mid; else hi = mid;
+    }
+    const long long beg = col_ptr[lo] + (long long)(item - item_ptr[lo]) * CSC_CHUNK;
+    const long long end = min(beg + CSC_CHUNK, col_ptr[lo + 1]);
+    double a0 = 0.0, a1 = 0.0, a2 = 0.0, a3 = 0.0;
+    if (strand < P) {
+#pragma unroll 4
+      for (long long j = beg + strand; j < end; j += P) {
+        const double v = vals[j];
+        const float4 u = U[(long long)row_idx[j] * G + q];
+        // fp32 x fp32 is exact in fp64: the fma rounds once, like the separate add
+        a0 = fma((double)u.x, v, a0);
+        a1 = fma((double)u.y, v, a1);
+        a2 = fma((double)u.z, v, a2);
+        a3 = fma((double)u.w, v, a3);
+      }
+    }
+    // lane = strand * G + q holds components 4q..4q+3 of its strand: acc_w[strand * kp + c]
+    acc_w[lane * 4 + 0] = a0;
+    acc_w[lane * 4 + 1] = a1;
+    acc_w[lane * 4 + 2] = a2;
+    acc_w[lane * 4 + 3] = a3;
+    __syncwarp();
+    if (lane < kp) {
+      double t = 0.0;
+      for (int s = 0; s < P; ++s) t += acc_w[s * kp + lane];
+      part[(long long)item * kp + lane] = t;
+    }
+    __syncwarp();
+  }
+}
+
+// out[c][col] = sum of the column's chunk partials in chunk order, rounded to fp32 once
+__global__ void csc_project_reduce_kernel(const double* __restrict__ part, const int* __restrict__ item_ptr, int n_cols,
+                                          int k, int kp, float* __restrict__ out, int ld) {
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= (long long)k * n_cols) return;
+  const int c = (int)(i / n_cols), col = (int)(i % n_cols);
+  double t = 0.0;
+  for (int it = item_ptr[col]; it < item_ptr[col + 1]; ++it) t += part[(long long)it * kp + c];
+  out[(long long)c * ld + col] = (float)t;
+}
+
+// U (n x kp) <- F^T for F (k x ld, first n columns), zero beyond k
+__global__ void stage_rows_kernel(const float* __restrict__ F, int k, int n, int ld, int kp, float* __restrict__ U) {
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= (long long)n * kp) return;
+  const int r = (int)(i / kp), c = (int)(i % kp);
+  U[i] = c < k ? F[(long long)c * ld + r] : 0.f;
+}
+
+// one warp per column: sum(x), sum(x^2) in fp64 (lane strides, then the xor tree of warp_sum: a fixed order)
+__global__ void __launch_bounds__(WARPS * 32) csc_col_stats_kernel(const long long* __restrict__ col_ptr,
+                                                                   const float* __restrict__ vals, int n_cols,
+                                                                   double* __restrict__ col_sums) {
+  const int col = blockIdx.x * WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (col >= n_cols) return;
+  double s = 0.0, q = 0.0;
+  for (long long j = col_ptr[col] + lane; j < col_ptr[col + 1]; j += 32) {
+    const double v = vals[j];
+    s += v;
+    q = fma(v, v, q);
+  }
+  s = warp_sum(s);
+  q = warp_sum(q);
+  if (lane == 0) {
+    col_sums[col] = s;
+    col_sums[n_cols + col] = q;
+  }
+}
+
+// dataset totals from the column sums: one block, fixed strides, fixed tree
+__global__ void csc_totals_kernel(const double* __restrict__ col_sums, int n_cols, double* __restrict__ out) {
+  __shared__ double sh[2][256];
+  double s = 0.0, q = 0.0;
+  for (int c = threadIdx.x; c < n_cols; c += 256) {
+    s += col_sums[c];
+    q += col_sums[n_cols + c];
+  }
+  sh[0][threadIdx.x] = s;
+  sh[1][threadIdx.x] = q;
+  __syncthreads();
+  for (int o = 128; o > 0; o >>= 1) {
+    if (threadIdx.x < o) {
+      sh[0][threadIdx.x] += sh[0][threadIdx.x + o];
+      sh[1][threadIdx.x] += sh[1][threadIdx.x + o];
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    out[0] = sh[0][0];
+    out[1] = sh[1][0];
+  }
+}
+
+// smallest positive stored value per column and per row, as int bit patterns (positive floats order like them);
+// both arrays start at 0x7f7f7f7f.  Integer atomics: the result does not depend on the order.
+__global__ void csc_min_positive_kernel(const long long* __restrict__ col_ptr, const int* __restrict__ row_idx,
+                                        const float* __restrict__ vals, int n_cols, int* __restrict__ col_min,
+                                        int* __restrict__ row_min) {
+  const int col = blockIdx.x * WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (col >= n_cols) return;
+  int cm = 0x7f7f7f7f;
+  for (long long j = col_ptr[col] + lane; j < col_ptr[col + 1]; j += 32) {
+    const float v = vals[j];
+    if (v > 0.f) {
+      cm = min(cm, __float_as_int(v));
+      atomicMin(&row_min[row_idx[j]], __float_as_int(v));
+    }
+  }
+  for (int o = 16; o > 0; o >>= 1) cm = min(cm, __shfl_xor_sync(0xffffffffu, cm, o));
+  if (lane == 0) col_min[col] = cm;
+}
+
+// entries that are not an integer multiple of their column scale (n_bad[0]) / row scale (n_bad[1])
+__global__ void csc_check_scaled_int_kernel(const long long* __restrict__ col_ptr, const int* __restrict__ row_idx,
+                                            const float* __restrict__ vals, int n_cols, const float* __restrict__ cs,
+                                            const float* __restrict__ rs, int* __restrict__ n_bad) {
+  const int col = blockIdx.x * WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (col >= n_cols) return;
+  int bad_c = 0, bad_r = 0;
+  for (long long j = col_ptr[col] + lane; j < col_ptr[col + 1]; j += 32) {
+    const float v = vals[j];
+    if (v == 0.f) continue;
+    bad_c += !is_scaled_int(v, cs[col]);
+    bad_r += !is_scaled_int(v, rs[row_idx[j]]);
+  }
+  bad_c = warp_sum(bad_c);
+  bad_r = warp_sum(bad_r);
+  if (lane == 0 && bad_c) atomicAdd(&n_bad[0], bad_c);
+  if (lane == 0 && bad_r) atomicAdd(&n_bad[1], bad_r);
+}
+
+// one warp per selected column: dst[row][c] = X[row][cols[c]] * scale[c] (the product gather_cols_kernel forms)
+__global__ void __launch_bounds__(WARPS * 32) csc_gather_cols_kernel(const long long* __restrict__ col_ptr,
+                                                                     const int* __restrict__ row_idx,
+                                                                     const float* __restrict__ vals,
+                                                                     const int* __restrict__ cols,
+                                                                     const float* __restrict__ scale, int n_sel,
+                                                                     float* __restrict__ dst, int ld_dst) {
+  const int c = blockIdx.x * WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (c >= n_sel) return;
+  const int src = cols[c];
+  const float f = scale[c];
+  for (long long j = col_ptr[src] + lane; j < col_ptr[src + 1]; j += 32) dst[(long long)row_idx[j] * ld_dst + c] = vals[j] * f;
+}
+
+}  // namespace
+
+namespace cnmf {
+
+int require_dense(const cnmf_dataset_s* d, const char* what) {
+  if (d && d->sparse) {
+    set_last_error(std::string(what) + " is not implemented for sparse (CSC) datasets: they serve the consensus "
+                   "step only (col_stats, project_rows, from_columns, transposed Frobenius refit)");
+    return -3;
+  }
+  return 0;
+}
+
+int csc_project(const cnmf_dataset_s* d, const float* U, int k, int kp, float* out, int ld, cudaStream_t s) {
+  cnmf_handle_s* h = d->h;
+  double* part = static_cast<double*>(h->dev_buf("csc.part", sizeof(double) * std::max(1, d->n_items) * (size_t)kp));
+  if (!part) return -2;
+  h->launches += 2;
+  // algorithmic bytes: the entries (row index + value), col_ptr, U and the output
+  const double bytes = 8.0 * d->nnz + 8.0 * (d->n_cols + 1) + 4.0 * d->n_rows * kp + 4.0 * k * d->n_cols;
+  const int slot = h->prof_begin(s, bytes, 2);
+  if (d->n_items > 0) {
+    const int blocks = std::min((d->n_items + WARPS - 1) / WARPS, h->sm_count * 16);
+    csc_project_kernel<<<blocks, WARPS * 32, 0, s>>>(d->col_ptr, d->row_idx, d->vals, d->item_ptr, d->n_cols, d->n_items,
+                                                      reinterpret_cast<const float4*>(U), kp, part);
+  }
+  const long long n_out = (long long)k * d->n_cols;
+  csc_project_reduce_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, s>>>(part, d->item_ptr, d->n_cols, k, kp, out, ld);
+  h->prof_end(s, slot);
+  CNMF_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+int csc_col_stats(cnmf_dataset_s* d, cudaStream_t s) {
+  cnmf_handle_s* h = d->h;
+  double* tot = static_cast<double*>(h->dev_buf("csc.totals", sizeof(double) * 2));
+  if (!tot) return -2;
+  csc_col_stats_kernel<<<(d->n_cols + WARPS - 1) / WARPS, WARPS * 32, 0, s>>>(d->col_ptr, d->vals, d->n_cols, d->col_sums);
+  csc_totals_kernel<<<1, 256, 0, s>>>(d->col_sums, d->n_cols, tot);
+  h->launches += 2;
+  CNMF_CUDA_CHECK(cudaGetLastError());
+  double out2[2];
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(out2, tot, sizeof(out2), cudaMemcpyDeviceToHost, s));
+  CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
+  d->sum = out2[0];
+  d->sum_sq = out2[1];
+  return 0;
+}
+
+int csc_detect_exact(cnmf_dataset_s* d, cudaStream_t s) {
+  cnmf_handle_s* h = d->h;
+  float *cmin = nullptr, *rmin = nullptr;
+  CNMF_TRY(cnmf_dataset_alloc_internal(d, &cmin, (size_t)d->ld_c));
+  CNMF_TRY(cnmf_dataset_alloc_internal(d, &rmin, (size_t)d->ld_r));
+  int* n_bad = static_cast<int*>(h->dev_buf("dataset.nbad", sizeof(int) * 2));
+  if (!n_bad) return -2;
+  CNMF_CUDA_CHECK(cudaMemsetAsync(cmin, 0x7f, sizeof(float) * d->n_cols, s));   // 0x7f7f7f7f: a huge finite float
+  CNMF_CUDA_CHECK(cudaMemsetAsync(rmin, 0x7f, sizeof(float) * d->n_rows, s));
+  CNMF_CUDA_CHECK(cudaMemsetAsync(n_bad, 0, sizeof(int) * 2, s));
+  const int blocks = (d->n_cols + WARPS - 1) / WARPS;
+  csc_min_positive_kernel<<<blocks, WARPS * 32, 0, s>>>(d->col_ptr, d->row_idx, d->vals, d->n_cols,
+                                                        reinterpret_cast<int*>(cmin), reinterpret_cast<int*>(rmin));
+  CNMF_CUDA_CHECK(cudaGetLastError());
+  CNMF_TRY(launch_fix_scale(cmin, d->n_cols, d->ld_c, s));
+  CNMF_TRY(launch_fix_scale(rmin, d->n_rows, d->ld_r, s));
+  csc_check_scaled_int_kernel<<<blocks, WARPS * 32, 0, s>>>(d->col_ptr, d->row_idx, d->vals, d->n_cols, cmin, rmin, n_bad);
+  CNMF_CUDA_CHECK(cudaGetLastError());
+  h->launches += 4;
+  int bad[2] = {1, 1};
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(bad, n_bad, sizeof(int) * 2, cudaMemcpyDeviceToHost, s));
+  CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
+  if (bad[0] == 0) { d->exact = true; d->col_scale = cmin; }
+  else if (bad[1] == 0) { d->exact = true; d->row_scale = rmin; }
+  return 0;
+}
+
+int csc_gather_cols(const cnmf_dataset_s* d, const int* cols, const float* scale, int n_cols, float* dst, int ld_dst,
+                    cudaStream_t s) {
+  csc_gather_cols_kernel<<<(n_cols + WARPS - 1) / WARPS, WARPS * 32, 0, s>>>(d->col_ptr, d->row_idx, d->vals, cols, scale,
+                                                                              n_cols, dst, ld_dst);
+  d->h->launches += 1;
+  CNMF_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+int stage_rows(cnmf_handle_s* h, const float* F, int k, int n, int ld, int kp, float* U, cudaStream_t s) {
+  const long long total = (long long)n * kp;
+  stage_rows_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(F, k, n, ld, kp, U);
+  h->launches += 1;
+  CNMF_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+}  // namespace cnmf
+
+extern "C" {
+
+int cnmf_dataset_create_csc(cnmf_handle_t h, int n_rows, int n_cols, long long nnz, const int64_t* col_ptr,
+                            const int32_t* row_idx, const float* values, int precision, void* stream,
+                            cnmf_dataset_t* out) {
+  CNMF_REQUIRE(h && col_ptr && out && (nnz == 0 || (row_idx && values)), "dataset_create_csc: NULL argument");
+  CNMF_REQUIRE(n_rows > 0 && n_cols > 0 && nnz >= 0, "dataset_create_csc: bad shape");
+  CNMF_REQUIRE(precision == CNMF_PRECISION_FP32 || precision == CNMF_PRECISION_TF32X3 ||
+                   precision == CNMF_PRECISION_TF32X3_GENERAL || precision == CNMF_PRECISION_F16X2,
+               "dataset_create_csc: bad precision");
+  CNMF_REQUIRE(col_ptr[0] == 0 && col_ptr[n_cols] == nnz, "dataset_create_csc: col_ptr must start at 0 and end at nnz");
+  // chunk table of csc_project_kernel, built while col_ptr is checked
+  std::vector<int> item_ptr(n_cols + 1);
+  long long items = 0;
+  for (int c = 0; c < n_cols; ++c) {
+    CNMF_REQUIRE(col_ptr[c + 1] >= col_ptr[c], "dataset_create_csc: col_ptr is not monotone");
+    item_ptr[c] = (int)items;
+    items += (col_ptr[c + 1] - col_ptr[c] + CSC_CHUNK - 1) / CSC_CHUNK;
+    CNMF_REQUIRE(items < (1LL << 31), "dataset_create_csc: too many entries");
+  }
+  item_ptr[n_cols] = (int)items;
+  for (long long j = 0; j < nnz; ++j)
+    CNMF_REQUIRE(row_idx[j] >= 0 && row_idx[j] < n_rows, "dataset_create_csc: row index out of range");
+  cudaStream_t s = as_stream(stream);
+  CNMF_CUDA_CHECK(cudaSetDevice(h->device));
+  auto* d = new cnmf_dataset_s();
+  d->h = h;
+  d->sparse = true;
+  d->n_rows = n_rows;
+  d->n_cols = n_cols;
+  d->ld_c = pad_ld(n_cols);
+  d->ld_r = pad_ld(n_rows);
+  d->nnz = nnz;
+  d->n_items = (int)items;
+  d->allow_exact = precision != CNMF_PRECISION_TF32X3_GENERAL;
+  d->want_f16 = precision == CNMF_PRECISION_F16X2;
+  d->precision = (precision == CNMF_PRECISION_TF32X3_GENERAL || precision == CNMF_PRECISION_F16X2) ? CNMF_PRECISION_TF32X3
+                                                                                                : precision;
+  auto alloc = [&](auto** p, size_t bytes) {
+    float* q = nullptr;
+    const int rc = cnmf_dataset_alloc_internal(d, &q, (bytes + 3) / 4);
+    *p = reinterpret_cast<std::remove_pointer_t<decltype(p)>>(q);
+    return rc;
+  };
+  auto upload = [&](void* dst, const void* src, size_t bytes) {
+    if (bytes == 0) return 0;
+    const cudaError_t e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, s);
+    if (e != cudaSuccess) {
+      set_last_error(std::string("dataset_create_csc: upload failed: ") + cudaGetErrorString(e));
+      return -2;
+    }
+    return 0;
+  };
+  int rc = alloc(&d->col_ptr, sizeof(long long) * (n_cols + 1));
+  if (rc == 0) rc = alloc(&d->row_idx, sizeof(int) * (size_t)nnz);
+  if (rc == 0) rc = alloc(&d->vals, sizeof(float) * (size_t)nnz);
+  if (rc == 0) rc = alloc(&d->item_ptr, sizeof(int) * (n_cols + 1));
+  if (rc == 0) rc = alloc(&d->col_sums, sizeof(double) * 2 * (size_t)n_cols);
+  if (rc == 0) rc = upload(d->col_ptr, col_ptr, sizeof(long long) * (n_cols + 1));
+  if (rc == 0) rc = upload(d->row_idx, row_idx, sizeof(int) * (size_t)nnz);
+  if (rc == 0) rc = upload(d->vals, values, sizeof(float) * (size_t)nnz);
+  if (rc == 0) rc = upload(d->item_ptr, item_ptr.data(), sizeof(int) * (n_cols + 1));
+  if (rc == 0) rc = csc_col_stats(d, s);    // synchronises: item_ptr may go out of scope afterwards
+  static const bool allow_exact = [] { const char* e = std::getenv("CNMF_EXACT"); return !(e && e[0] == '0'); }();
+  // the condition under which dataset_finish tests the dense form
+  if (rc == 0 && d->precision == CNMF_PRECISION_TF32X3 && allow_exact && d->allow_exact && n_rows <= 65535 * 64)
+    rc = csc_detect_exact(d, s);
+  if (rc != 0) {
+    cudaStreamSynchronize(s);
+    cnmf_dataset_destroy(d);
+    return rc;
+  }
+  *out = d;
+  return 0;
+}
+
+}  // extern "C"

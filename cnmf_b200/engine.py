@@ -156,7 +156,8 @@ class Engine:
 
     def profile_get(self, kernel_class=0):
         """(total device ms, launches, algorithmic work) of a kernel class since profile(True):
-        0 = batched GEMM (work in FLOPs), 1 = fused update kernels (work in bytes)."""
+        0 = batched GEMM (work in FLOPs), 1 = fused update kernels (work in bytes), 2 = sparse-dataset products
+        (work in bytes)."""
         ms, n, fl = ctypes.c_double(), ctypes.c_longlong(), ctypes.c_double()
         check(self.lib.cnmf_profile_get_class(self._h, int(kernel_class), ctypes.byref(ms), ctypes.byref(n),
                                               ctypes.byref(fl)))
@@ -177,6 +178,31 @@ class Engine:
     def dataset(self, X, precision=_DEFAULT_PRECISION, stream=None):
         return Dataset(self, X, precision, stream)
 
+    def sparse_dataset(self, X, precision=_DEFAULT_PRECISION, stream=None):
+        """X (any scipy sparse matrix or an ndarray) resident on the GPU as canonical float32 CSC, 8 bytes per stored
+        entry; no dense copy is made on the host or the device.  Serves the consensus step's TPM uses: sums, col_stats,
+        project_rows, from_columns (returns a dense dataset) and refit(transposed=True) with the Frobenius loss;
+        everything else raises CnmfError."""
+        import scipy.sparse as sp
+        C = sp.csc_matrix(X, dtype=np.float32)
+        if not C.has_canonical_format:          # sorted row indices, no duplicates: the library does not sort
+            C = C.copy()
+            C.sum_duplicates()
+        n, g = C.shape
+        col_ptr = np.ascontiguousarray(C.indptr, dtype=np.int64)
+        row_idx = np.ascontiguousarray(C.indices, dtype=np.int32)
+        vals = np.ascontiguousarray(C.data, dtype=np.float32)
+        out = ctypes.c_void_p()
+        check(self.lib.cnmf_dataset_create_csc(self._h, n, g, int(col_ptr[-1]), ptr(col_ptr), ptr(row_idx), ptr(vals),
+                                               precision_code(precision), stream, ctypes.byref(out)))
+        return Dataset(self, None, precision, _handle=out, sparse=True)
+
+    def dense_dataset_bytes(self, n_rows, n_cols, precision=_DEFAULT_PRECISION):
+        """Worst-case device bytes dataset() of an n_rows x n_cols matrix needs while it is built."""
+        peak = ctypes.c_longlong()
+        check(self.lib.cnmf_dataset_dense_bytes(int(n_rows), int(n_cols), precision_code(precision), ctypes.byref(peak)))
+        return int(peak.value)
+
     def gemm_abt(self, A, B, precision=PRECISION_TF32X3, splits=1, reps=1):
         """C = A @ B.T through the solver's GEMM kernels (test / micro-benchmark hook)."""
         A, B = f32c(A), f32c(B)
@@ -195,10 +221,11 @@ class Engine:
 class Dataset:
     """A cells x genes matrix resident on the GPU (norm_counts.X / tpm.X of the reference)."""
 
-    def __init__(self, engine, X, precision=_DEFAULT_PRECISION, stream=None, _handle=None):
+    def __init__(self, engine, X, precision=_DEFAULT_PRECISION, stream=None, _handle=None, sparse=False):
         self.engine = engine
         self.lib = engine.lib
         self.precision = precision_code(precision)
+        self.sparse = sparse        # CSC-resident (Engine.sparse_dataset)
         self._d = ctypes.c_void_p()
         if _handle is not None:
             self._d = _handle

@@ -56,6 +56,27 @@ _PATH_SPECS = [
 ]
 
 
+# The TPM dataset of consensus is built dense (the tensor-core forms) when the library's worst case for creating it is
+# at most this fraction of the device memory that is free or cached by the engine -- the fraction max_rows_per_solve
+# sizes restart groups with -- and kept sparse (CSC, 8 bytes per stored entry) otherwise.
+TPM_DENSE_FRACTION = 0.8
+
+
+def tpm_dataset(eng, X, precision, beta_loss="frobenius"):
+    """The resident TPM matrix for consensus (refit_spectra, the OLS z-scores and the HVG refit, cnmf.py:950-969):
+    dense as everywhere else when it fits, else CSC (Engine.sparse_dataset).  A sparse TPM supports the Frobenius
+    refits only: a KL / IS run that would need it raises NotImplementedError before anything is built."""
+    from .engine import LOSS_FROBENIUS, loss_code
+    n, g = X.shape
+    free, _, cached = eng.mem_info()
+    if eng.dense_dataset_bytes(n, g, precision) <= TPM_DENSE_FRACTION * (free + cached):
+        return eng.dataset(X, precision=precision)
+    if loss_code(beta_loss) != LOSS_FROBENIUS:
+        raise NotImplementedError("cnmf_b200: the %d x %d TPM matrix does not fit on the device in dense form, and the "
+                                  "sparse KL / IS refit is not implemented (beta_loss=%r)" % (n, g, beta_loss))
+    return eng.sparse_dataset(X, precision=precision)
+
+
 def worker_filter(iterable, worker_index, total_workers):
     """cnmf.py:52-53."""
     return (p for i, p in enumerate(iterable) if (i - worker_index) % total_workers == 0)
@@ -412,7 +433,7 @@ class cNMF:
         if not stats_only:
             tpm = cio.read_matrix(self.paths["tpm"])                                # cnmf.py:950-953
             tpm_stats = load_df_from_npz(self.paths["tpm_stats"])
-            tpm_ds = self._dataset(tpm.X)
+            tpm_ds = tpm_dataset(eng, tpm.X, self.precision, kw.get("beta_loss", "frobenius"))
             if refit_usage:
                 hvgs = open(self.paths["nmf_genes_list"]).read().split("\n")
                 hv_idx = tpm.var_names.get_indexer(hvgs)

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define CNMF_B200_ABI_VERSION 7
+#define CNMF_B200_ABI_VERSION 8
 #define CNMF_MAX_COMPONENTS 32          /* largest n_components per restart on the CUDA path */
 
 typedef struct cnmf_handle_s* cnmf_handle_t;
@@ -82,7 +82,8 @@ long long cnmf_solve_bytes_per_row(cnmf_dataset_t d);
 int cnmf_profile_enable(cnmf_handle_t h, int on);
 int cnmf_profile_get(cnmf_handle_t h, double* gemm_ms, long long* gemm_launches, double* gemm_flops);
 /* same counters per kernel class: 0 = batched GEMM (work = algorithmic FLOPs), 1 = fused update kernels
- * (work = algorithmic bytes: factor read + product slices read + factor and tf32 pieces written) */
+ * (work = algorithmic bytes: factor read + product slices read + factor and tf32 pieces written), 2 = the product
+ * of a sparse dataset, both of its kernels (work = algorithmic bytes: 8 per entry, col_ptr, staged U, output) */
 int cnmf_profile_get_class(cnmf_handle_t h, int kernel_class, double* ms, long long* launches, double* work);
 
 /* host wall-clock phases (ms) of the last cnmf_factorize on this handle: host RNG, H2D of the initial
@@ -95,6 +96,20 @@ int cnmf_last_timing(cnmf_handle_t h, double* rng_ms, double* h2d_ms, double* so
  * sum(X), sum(X^2).  `src_is_device` = 0: X is host memory (copied H2D inside the call). */
 int cnmf_dataset_create(cnmf_handle_t h, const float* X, int n_rows, int n_cols, long long ld,
                         int src_is_device, int precision, void* stream, cnmf_dataset_t* out);
+/* A cells x genes matrix kept sparse on the device: canonical CSC from the host (col_ptr[n_cols + 1] int64, monotone,
+ * from 0 to nnz; row_idx int32 in [0, n_rows), increasing and unique within a column -- scipy.sparse tocsc() gives
+ * exactly that; the order is not checked; values fp32), 8 bytes per stored entry.  For the TPM matrix of the consensus
+ * step (cnmf.py:950-969) when its dense forms do not fit.  Supported on such a dataset: shape, ld, sums, col_stats,
+ * from_columns (the result is an ordinary dense dataset), destroy, project_rows and refit with transposed = 1 and
+ * beta_loss = frobenius (MU and CD; the one product X^T W is formed in fp64).  Every other entry point returns -3.
+ * cnmf_dataset_is_exact reports 0 (no tensor-core product runs on it). */
+int cnmf_dataset_create_csc(cnmf_handle_t h, int n_rows, int n_cols, long long nnz, const int64_t* col_ptr,
+                            const int32_t* row_idx, const float* values, int precision, void* stream,
+                            cnmf_dataset_t* out);
+/* worst-case device bytes cnmf_dataset_create of an n_rows x n_cols matrix at `precision` needs while the dataset is
+ * built, over the forms it can take (exact f16, exact tf32, general): what a caller compares with free memory to
+ * choose between the dense and the CSC dataset */
+int cnmf_dataset_dense_bytes(int n_rows, int n_cols, int precision, long long* peak);
 /* new dataset = src[:, cols] * col_scale (cnmf.py:965-969: tpm[:, hvgs] / std) */
 int cnmf_dataset_from_columns(cnmf_dataset_t src, const int32_t* cols_host, const float* col_scale_host,
                               int n_cols, void* stream, cnmf_dataset_t* out);
@@ -193,7 +208,8 @@ int cnmf_refit(cnmf_dataset_t d, int transposed, int k, const float* fixed_host,
                float* out_host, int32_t* n_iter_host, double* err_host, void* stream);
 
 /* out (k x n_cols) = Ut (k x n_rows) * X : the X^T Y accumulator of efficient_ols_all_cols
- * (cnmf.py:98-119) as one tensor-core GEMM; the caller centres U (see cnmf_b200/consensus.py). */
+ * (cnmf.py:98-119) as one tensor-core GEMM; the caller centres U (see cnmf_b200/consensus.py).
+ * On a sparse dataset (k <= 32): fp64 products and sums in a fixed order, bit-identical from call to call. */
 int cnmf_project_rows(cnmf_dataset_t d, int k, const float* Ut_host, float* out_host, void* stream);
 
 /* test / micro-benchmark hook: C (M x N) = A (M x Kd) * B (N x Kd)^T through the same GEMM kernels the
