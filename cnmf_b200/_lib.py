@@ -62,6 +62,7 @@ SIGNATURES = {
     "cnmf_dataset_row_sums": (_i, [_vp, _vp, _vp]),
     "cnmf_dataset_scaled_col_stats": (_i, [_vp, _vp, _vp, _vp, _vp]),
     "cnmf_dataset_scale_rows": (_i, [_vp, _vp, _vp, _pp(_vp)]),
+    "cnmf_dataset_tpm_stats": (_i, [_vp, _d, _vp, _vp, _vp, _vp]),
     "cnmf_random_init_host": (_i, [_c.c_uint32, _d, _i, _i, _i, _vp, _ll, _vp, _ll]),
     "cnmf_random_init_dev": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp]),
     "cnmf_factorize": (_i, [_vp, _i, _vp, _vp, _pp(NmfParams), _vp, _vp, _vp, _vp, _vp]),
@@ -90,7 +91,7 @@ SIGNATURES = {
 _lib = None
 
 
-ABI_VERSION = 8      # include/cnmf_b200.h CNMF_B200_ABI_VERSION
+ABI_VERSION = 9     # include/cnmf_b200.h CNMF_B200_ABI_VERSION
 
 
 def load():

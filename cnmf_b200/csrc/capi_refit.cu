@@ -102,6 +102,15 @@ __global__ void gather_cols_kernel(const float* __restrict__ src, int rows, int 
 
 extern "C" {
 
+// column sums (mean_host) and sums of squares (var_host) over n rows -> mean and population variance, in place
+static void finish_col_stats(double n, int n_cols, double* mean_host, double* var_host) {
+  for (int c = 0; c < n_cols; ++c) {
+    const double m = mean_host[c] / n;
+    mean_host[c] = m;
+    var_host[c] = std::max(var_host[c] / n - m * m, 0.0);
+  }
+}
+
 static int col_stats_impl(cnmf_dataset_t d, const double* row_scale_host, double* mean_host, double* var_host, void* stream) {
   CNMF_REQUIRE(d && mean_host && var_host, "col_stats: NULL argument");
   cnmf_handle_s* h = d->h;
@@ -129,12 +138,7 @@ static int col_stats_impl(cnmf_dataset_t d, const double* row_scale_host, double
   CNMF_CUDA_CHECK(cudaMemcpyAsync(mean_host, buf, sizeof(double) * d->n_cols, cudaMemcpyDeviceToHost, s));
   CNMF_CUDA_CHECK(cudaMemcpyAsync(var_host, buf + d->n_cols, sizeof(double) * d->n_cols, cudaMemcpyDeviceToHost, s));
   CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
-  const double n = d->n_rows;
-  for (int c = 0; c < d->n_cols; ++c) {
-    const double m = mean_host[c] / n;
-    mean_host[c] = m;
-    var_host[c] = std::max(var_host[c] / n - m * m, 0.0);
-  }
+  finish_col_stats(d->n_rows, d->n_cols, mean_host, var_host);
   return 0;
 }
 
@@ -161,6 +165,29 @@ int cnmf_dataset_row_sums(cnmf_dataset_t d, double* row_sums_host, void* stream)
   h->launches += 1;
   CNMF_CUDA_CHECK(cudaMemcpyAsync(row_sums_host, buf, sizeof(double) * d->n_rows, cudaMemcpyDeviceToHost, s));
   CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
+  return 0;
+}
+
+int cnmf_dataset_tpm_stats(cnmf_dataset_t d, double target_sum, double* totals_host, double* mean_host,
+                           double* var_host, void* stream) {
+  CNMF_REQUIRE(d && totals_host && mean_host && var_host, "tpm_stats: NULL argument");
+  if (!d->sparse) {
+    set_last_error("tpm_stats is implemented for sparse (CSC) datasets only: a dense dataset gives the same numbers "
+                   "through row_sums and scaled_col_stats");
+    return -3;
+  }
+  cnmf_handle_s* h = d->h;
+  cudaStream_t s = as_stream(stream);
+  CNMF_CUDA_CHECK(cudaSetDevice(h->device));
+  double* tot = static_cast<double*>(h->dev_buf("rowsums", sizeof(double) * d->n_rows));
+  double* sums = static_cast<double*>(h->dev_buf("colstats", sizeof(double) * 2 * d->n_cols));
+  if (!tot || !sums) return -2;
+  CNMF_TRY(csc_tpm_sums(d, target_sum, tot, sums, s));
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(totals_host, tot, sizeof(double) * d->n_rows, cudaMemcpyDeviceToHost, s));
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(mean_host, sums, sizeof(double) * d->n_cols, cudaMemcpyDeviceToHost, s));
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(var_host, sums + d->n_cols, sizeof(double) * d->n_cols, cudaMemcpyDeviceToHost, s));
+  CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
+  finish_col_stats(d->n_rows, d->n_cols, mean_host, var_host);
   return 0;
 }
 

@@ -159,5 +159,8 @@ int csc_detect_exact(cnmf_dataset_s* d, cudaStream_t s);
 // dst (n_rows x ld_dst, zeroed by the caller)[:, c] = X[:, cols[c]] * scale[c]
 int csc_gather_cols(const cnmf_dataset_s* d, const int* cols, const float* scale, int n_cols, float* dst, int ld_dst,
                     cudaStream_t s);
+// device totals (n_rows): fp64 row sums; col_sums (2 x n_cols): per column sum(v), sum(v^2) of v = x * target_sum /
+// (row total), 0 for a row without counts.  Fixed reduction order, no floating-point atomics.  Does not synchronise.
+int csc_tpm_sums(const cnmf_dataset_s* d, double target_sum, double* totals, double* col_sums, cudaStream_t s);
 
 }  // namespace cnmf

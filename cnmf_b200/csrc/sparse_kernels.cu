@@ -5,6 +5,9 @@
 //                          refit_spectra (cnmf.py:952), after which the refit iterates on K x K Grams only
 //   csc_col_stats_kernel   per-column sum(x), sum(x^2) in fp64: col_stats and the refit's ||X||^2 and mean(X)
 //   csc_gather_cols_kernel X[:, cols] * scale into a dense matrix: the HVG dataset of cnmf.py:965-969
+// The same CSC form holds raw counts for prepare (cnmf.py:245-251, 436-445) when their dense dataset does not fit:
+//   csc_row_partials_kernel + csc_row_totals_kernel   cell totals and the TPM row scale
+//   csc_scaled_col_sums_kernel                         per-column sums of the TPM, formed entry by entry
 // Products and sums run in fp64 in a fixed order, without floating-point atomics: two runs are bit-identical.
 #include <algorithm>
 #include <cstdlib>
@@ -28,6 +31,7 @@ extern "C" int cnmf_dataset_alloc_internal(cnmf_dataset_t d, float** p, size_t e
 namespace {
 
 constexpr int WARPS = 8;    // warps per block of the warp-per-column / warp-per-chunk kernels
+constexpr int TPM_SLABS = 128;   // most column slabs of the cell-total reduction (csc_row_partials_kernel)
 
 // One warp per chunk item (at most CSC_CHUNK entries of one column).  The kp / 4 lanes of a strand share one entry:
 // lane q of the strand gathers float4 number q of the entry's U row, so an entry costs one contiguous kp-float read.
@@ -182,6 +186,86 @@ __global__ void csc_check_scaled_int_kernel(const long long* __restrict__ col_pt
   if (lane == 0 && bad_r) atomicAdd(&n_bad[1], bad_r);
 }
 
+// Cell totals, pass 1 (prepare on sparse counts): slab s, one block, owns the columns whose entries start in
+// [nnz * s / S, nnz * (s + 1) / S) and adds them into its own fp64 row vector part[s], one column at a time.  The row
+// indices of a canonical CSC column are distinct, so the threads of one column never touch the same row, and the
+// barrier orders the columns: the result is a function of the matrix alone.  Four entries per thread are loaded
+// before their partials are written back (distinct rows: no aliasing), so each thread keeps four gathers in flight.
+constexpr int TPM_THREADS = 512;
+__global__ void __launch_bounds__(TPM_THREADS) csc_row_partials_kernel(const long long* __restrict__ col_ptr,
+                                                                      const int* __restrict__ row_idx,
+                                                                      const float* __restrict__ vals, int n_rows,
+                                                                      int n_cols, double* __restrict__ part) {
+  const int S = gridDim.x, s = blockIdx.x;
+  const long long nnz = col_ptr[n_cols];
+  // first column whose entries start at or after `target` (col_ptr is monotone)
+  auto first_col = [&](long long target) {
+    int lo = 0, hi = n_cols;
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (col_ptr[mid] < target) lo = mid + 1; else hi = mid;
+    }
+    return lo;
+  };
+  const int c0 = s == 0 ? 0 : first_col(nnz * s / S);
+  const int c1 = s == S - 1 ? n_cols : first_col(nnz * (s + 1) / S);
+  double* p = part + (long long)s * n_rows;
+  constexpr int B = TPM_THREADS;
+  for (int c = c0; c < c1; ++c) {
+    const long long end = col_ptr[c + 1];
+    long long j = col_ptr[c] + threadIdx.x;
+    for (; j + 3 * B < end; j += 4 * B) {
+      int r[4];
+      double v[4], a[4];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        r[u] = row_idx[j + u * B];
+        v[u] = vals[j + u * B];
+      }
+#pragma unroll
+      for (int u = 0; u < 4; ++u) a[u] = p[r[u]];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) p[r[u]] = a[u] + v[u];
+    }
+    for (; j < end; j += B) p[row_idx[j]] += (double)vals[j];
+    __syncthreads();
+  }
+}
+
+// Cell totals, pass 2: totals[r] = the slab partials added in slab order; row scale target / total, 0 for a row
+// without counts (scanpy's normalize_total leaves such a row at zero)
+__global__ void csc_row_totals_kernel(const double* __restrict__ part, int slabs, int n_rows, double target,
+                                      double* __restrict__ totals, double* __restrict__ scale) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n_rows) return;
+  double t = 0.0;
+  for (int s = 0; s < slabs; ++s) t += part[(long long)s * n_rows + r];
+  totals[r] = t;
+  scale[r] = t != 0.0 ? target / t : 0.0;
+}
+
+// csc_col_stats_kernel with every entry times its row scale: sum(x * rs), sum((x * rs)^2) per column in fp64
+__global__ void __launch_bounds__(WARPS * 32) csc_scaled_col_sums_kernel(const long long* __restrict__ col_ptr,
+                                                                         const int* __restrict__ row_idx,
+                                                                         const float* __restrict__ vals, int n_cols,
+                                                                         const double* __restrict__ rs,
+                                                                         double* __restrict__ col_sums) {
+  const int col = blockIdx.x * WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (col >= n_cols) return;
+  double s = 0.0, q = 0.0;
+  for (long long j = col_ptr[col] + lane; j < col_ptr[col + 1]; j += 32) {
+    const double v = (double)vals[j] * rs[row_idx[j]];
+    s += v;
+    q = fma(v, v, q);
+  }
+  s = warp_sum(s);
+  q = warp_sum(q);
+  if (lane == 0) {
+    col_sums[col] = s;
+    col_sums[n_cols + col] = q;
+  }
+}
+
 // one warp per selected column: dst[row][c] = X[row][cols[c]] * scale[c] (the product gather_cols_kernel forms)
 __global__ void __launch_bounds__(WARPS * 32) csc_gather_cols_kernel(const long long* __restrict__ col_ptr,
                                                                      const int* __restrict__ row_idx,
@@ -277,6 +361,24 @@ int csc_gather_cols(const cnmf_dataset_s* d, const int* cols, const float* scale
   csc_gather_cols_kernel<<<(n_cols + WARPS - 1) / WARPS, WARPS * 32, 0, s>>>(d->col_ptr, d->row_idx, d->vals, cols, scale,
                                                                               n_cols, dst, ld_dst);
   d->h->launches += 1;
+  CNMF_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+int csc_tpm_sums(const cnmf_dataset_s* d, double target_sum, double* totals, double* col_sums, cudaStream_t s) {
+  cnmf_handle_s* h = d->h;
+  // a function of the shape alone, so the reduction order is too; the partial vectors stay within 256 MB
+  const int slabs = (int)std::max(1LL, std::min({(long long)TPM_SLABS, (long long)d->n_cols, (1LL << 25) / d->n_rows}));
+  const size_t part_bytes = sizeof(double) * (size_t)slabs * d->n_rows;
+  double* part = static_cast<double*>(h->dev_buf("tpm.part", part_bytes));
+  double* scale = static_cast<double*>(h->dev_buf("tpm.scale", sizeof(double) * d->n_rows));
+  if (!part || !scale) return -2;
+  CNMF_CUDA_CHECK(cudaMemsetAsync(part, 0, part_bytes, s));
+  csc_row_partials_kernel<<<slabs, TPM_THREADS, 0, s>>>(d->col_ptr, d->row_idx, d->vals, d->n_rows, d->n_cols, part);
+  csc_row_totals_kernel<<<(d->n_rows + 255) / 256, 256, 0, s>>>(part, slabs, d->n_rows, target_sum, totals, scale);
+  csc_scaled_col_sums_kernel<<<(d->n_cols + WARPS - 1) / WARPS, WARPS * 32, 0, s>>>(d->col_ptr, d->row_idx, d->vals,
+                                                                                    d->n_cols, scale, col_sums);
+  h->launches += 3;
   CNMF_CUDA_CHECK(cudaGetLastError());
   return 0;
 }

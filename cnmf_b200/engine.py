@@ -181,8 +181,8 @@ class Engine:
     def sparse_dataset(self, X, precision=_DEFAULT_PRECISION, stream=None):
         """X (any scipy sparse matrix or an ndarray) resident on the GPU as canonical float32 CSC, 8 bytes per stored
         entry; no dense copy is made on the host or the device.  Serves the consensus step's TPM uses: sums, col_stats,
-        project_rows, from_columns (returns a dense dataset) and refit(transposed=True) with the Frobenius loss;
-        everything else raises CnmfError."""
+        project_rows, from_columns (returns a dense dataset) and refit(transposed=True) with the Frobenius loss; and
+        prepare's uses of raw counts: tpm_stats, col_stats, from_columns.  Everything else raises CnmfError."""
         import scipy.sparse as sp
         C = sp.csc_matrix(X, dtype=np.float32)
         if not C.has_canonical_format:          # sorted row indices, no duplicates: the library does not sort
@@ -348,6 +348,15 @@ class Dataset:
         out = np.empty(self.shape[0])
         check(self.lib.cnmf_dataset_row_sums(self._d, ptr(out), None))
         return out
+
+    def tpm_stats(self, target_sum=1e6):
+        """Sparse (CSC) counts only: (cell totals, mean, population variance) in float64, the statistics being those of
+        the TPM matrix diag(target_sum / total) @ X (a cell without counts stays at zero), computed on the device
+        without forming it (cnmf.py:245-251, 436-445).  A dense dataset has row_sums() and col_stats(row_scale=...)."""
+        n, g = self.shape
+        totals, mean, var = np.empty(n), np.empty(g), np.empty(g)
+        check(self.lib.cnmf_dataset_tpm_stats(self._d, float(target_sum), ptr(totals), ptr(mean), ptr(var), None))
+        return totals, mean, var
 
     def scale_rows(self, row_scale):
         """New resident dataset diag(row_scale) @ X (TPM from counts without a trip through the host)."""

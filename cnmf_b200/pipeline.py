@@ -56,10 +56,17 @@ _PATH_SPECS = [
 ]
 
 
-# The TPM dataset of consensus is built dense (the tensor-core forms) when the library's worst case for creating it is
-# at most this fraction of the device memory that is free or cached by the engine -- the fraction max_rows_per_solve
-# sizes restart groups with -- and kept sparse (CSC, 8 bytes per stored entry) otherwise.
+# A cells x all-genes matrix -- the TPM dataset of consensus, the raw counts of prepare(on_device=True) -- is built
+# dense (the tensor-core forms) when the library's worst case for creating it is at most this fraction of the device
+# memory that is free or cached by the engine -- the fraction max_rows_per_solve sizes restart groups with -- and kept
+# sparse (CSC, 8 bytes per stored entry) otherwise.
 TPM_DENSE_FRACTION = 0.8
+
+
+def fits_dense(eng, shape, precision):
+    """True when the dense dataset of a matrix of this shape fits on the device (TPM_DENSE_FRACTION)."""
+    free, _, cached = eng.mem_info()
+    return eng.dense_dataset_bytes(shape[0], shape[1], precision) <= TPM_DENSE_FRACTION * (free + cached)
 
 
 def tpm_dataset(eng, X, precision, beta_loss="frobenius"):
@@ -68,8 +75,7 @@ def tpm_dataset(eng, X, precision, beta_loss="frobenius"):
     refits only: a KL / IS run that would need it raises NotImplementedError before anything is built."""
     from .engine import LOSS_FROBENIUS, loss_code
     n, g = X.shape
-    free, _, cached = eng.mem_info()
-    if eng.dense_dataset_bytes(n, g, precision) <= TPM_DENSE_FRACTION * (free + cached):
+    if fits_dense(eng, X.shape, precision):
         return eng.dataset(X, precision=precision)
     if loss_code(beta_loss) != LOSS_FROBENIUS:
         raise NotImplementedError("cnmf_b200: the %d x %d TPM matrix does not fit on the device in dense form, and the "
@@ -168,7 +174,9 @@ class cNMF:
         on_device=True (cnmf_b200 extension, `--prepare-on-device`): the raw counts are made resident and the
         per-cell totals, the TPM gene statistics behind the over-dispersion ranking and `tpm_stats`, the per-gene
         scale of the HVG matrix and the HVG matrix itself are computed by CUDA kernels (float64 accumulation from the
-        exact integer counts); the normalised matrix stays in HBM for factorize().  Raises without a GPU."""
+        exact integer counts); the normalised matrix stays in HBM for factorize().  Raises without a GPU.  Counts
+        stored sparse (and densify=False) whose dense dataset would not fit (TPM_DENSE_FRACTION) stay CSC on the device
+        and CSR on the host, so an atlas needs no cells x all-genes dense matrix anywhere."""
         from .engine import check_supported
         check_supported(components, init, beta_loss)                  # fail here, not hours later in factorize
         counts = cio.read_counts(counts_fn)
@@ -177,11 +185,30 @@ class cNMF:
         # -- sc.pp.scale(zero_center=False) maps a zero standard deviation to 1 (cnmf.py:538, 967) where the dense
         # branch divides by it (cnmf.py:542) -- and the stored matrices stay CSR like the reference's
         sparse_sem = (not densify) and (counts.is_sparse or not counts_fn.endswith(".h5ad"))
-        C = counts.dense(np.float64)
+        if on_device and tpm_fn is not None:
+            raise ValueError("on_device=True derives TPM from the counts; it cannot be combined with tpm_fn")
+        # counts stored sparse whose dense dataset does not fit stay CSC on the device, and no cells x all-genes dense
+        # matrix is formed anywhere; with integer counts the files are bit-identical to the dense branch's (totals and
+        # raw column sums are exact in fp64), tpm_stats agree to the last bits (summation order)
+        stay_sparse = (on_device and counts.is_sparse and not densify
+                       and not fits_dense(self.engine(), counts.shape, self.precision))
+        if stay_sparse:
+            import scipy.sparse as sp
+            C = sp.csr_matrix(counts.X, dtype=np.float64)
+            C.sum_duplicates()                  # the entries sp.csr_matrix(dense) would hold, in the same order
+            C.eliminate_zeros()
+        else:
+            C = counts.dense(np.float64)
         dev = None
-        if on_device:
-            if tpm_fn is not None:
-                raise ValueError("on_device=True derives TPM from the counts; it cannot be combined with tpm_fn")
+        if stay_sparse:
+            dev = self.engine().sparse_dataset(C, precision=self.precision)     # raw counts resident as CSC
+            totals, t_mean, t_var = dev.tpm_stats(1e6)
+            tpm_X = C.copy()
+            tpm_X.data /= np.repeat(totals, np.diff(C.indptr))
+            tpm_X.data *= 1e6                                              # C / totals * 1e6, as below
+            tpm = cio.CellGeneMatrix(tpm_X, counts.obs_names, counts.var_names)
+            t_std = np.sqrt(t_var)
+        elif on_device:
             dev = self.engine().dataset(C, precision=self.precision)       # raw counts resident in HBM
             totals = dev.row_sums()
             tpm_X = C / totals[:, None] * 1e6                              # host copy only for the tpm file
@@ -216,7 +243,11 @@ class cNMF:
             std1 = np.sqrt(c_var[idx] * n / (n - 1.0))                 # std(ddof=1) of the selected count columns
             if sparse_sem:
                 std1[std1 == 0] = 1.0
-            X /= std1
+            if stay_sparse:
+                X.sort_indices()                                       # the column order sp.csr_matrix(dense) gives
+                X.data /= std1[X.indices]
+            else:
+                X /= std1
             with np.errstate(divide="ignore"):
                 self._resident_norm = dev.from_columns(idx, 1.0 / std1)   # counts[:, hvgs] / std, built on the device
             dev.close()
@@ -225,7 +256,7 @@ class cNMF:
             if sparse_sem:
                 std1[std1 == 0] = 1.0                                  # sc.pp.scale(zero_center=False), cnmf.py:538
             X /= std1                                                  # cnmf.py:542 (no centring)
-        if np.isnan(X).sum() > 0:
+        if np.isnan(X.data if stay_sparse else X).sum() > 0:
             print("Warning NaNs in normalized counts matrix")
         norm.X = _maybe_csr(X, sparse_sem)
         with open(self.paths["nmf_genes_list"], "w") as F:

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define CNMF_B200_ABI_VERSION 8
+#define CNMF_B200_ABI_VERSION 9
 #define CNMF_MAX_COMPONENTS 32          /* largest n_components per restart on the CUDA path */
 
 typedef struct cnmf_handle_s* cnmf_handle_t;
@@ -99,9 +99,10 @@ int cnmf_dataset_create(cnmf_handle_t h, const float* X, int n_rows, int n_cols,
 /* A cells x genes matrix kept sparse on the device: canonical CSC from the host (col_ptr[n_cols + 1] int64, monotone,
  * from 0 to nnz; row_idx int32 in [0, n_rows), increasing and unique within a column -- scipy.sparse tocsc() gives
  * exactly that; the order is not checked; values fp32), 8 bytes per stored entry.  For the TPM matrix of the consensus
- * step (cnmf.py:950-969) when its dense forms do not fit.  Supported on such a dataset: shape, ld, sums, col_stats,
- * from_columns (the result is an ordinary dense dataset), destroy, project_rows and refit with transposed = 1 and
- * beta_loss = frobenius (MU and CD; the one product X^T W is formed in fp64).  Every other entry point returns -3.
+ * step (cnmf.py:950-969), or the raw counts of prepare, when its dense forms do not fit.  Supported on such a dataset:
+ * shape, ld, sums, col_stats, tpm_stats, from_columns (the result is an ordinary dense dataset), destroy, project_rows
+ * and refit with transposed = 1 and beta_loss = frobenius (MU and CD; the one product X^T W is formed in fp64).  Every
+ * other entry point returns -3.
  * cnmf_dataset_is_exact reports 0 (no tensor-core product runs on it). */
 int cnmf_dataset_create_csc(cnmf_handle_t h, int n_rows, int n_cols, long long nnz, const int64_t* col_ptr,
                             const int32_t* row_idx, const float* values, int precision, void* stream,
@@ -138,6 +139,12 @@ int cnmf_dataset_row_sums(cnmf_dataset_t d, double* row_sums_host, void* stream)
  * materialising TPM */
 int cnmf_dataset_scaled_col_stats(cnmf_dataset_t d, const double* row_scale_host, double* mean_host, double* var_host,
                                   void* stream);
+/* sparse (CSC) counts datasets only -- a dense one gets -3 and has row_sums / scaled_col_stats instead: per-row totals
+ * (fp64 sums of the stored values) and the per-column mean and population variance of diag(target_sum / total) * X,
+ * the row scale being 0 for a row whose total is 0.  The TPM totals and gene statistics of prepare (cnmf.py:245-251,
+ * 436-445) for counts that stay sparse on the device; fixed reduction order, so two calls are bit-identical. */
+int cnmf_dataset_tpm_stats(cnmf_dataset_t d, double target_sum, double* totals_host, double* mean_host,
+                           double* var_host, void* stream);
 /* new dataset = diag(row_scale) * src (TPM from counts, cnmf.py:245-251); the exact-count detection runs again */
 int cnmf_dataset_scale_rows(cnmf_dataset_t src, const float* row_scale_host, void* stream, cnmf_dataset_t* out);
 
