@@ -15,6 +15,8 @@ LIB_PATH = os.path.join(_HERE, "libcnmf_b200.so")
 SOLVER_MU, SOLVER_CD = 0, 1
 PRECISION_FP32, PRECISION_TF32X3, PRECISION_TF32X3_GENERAL, PRECISION_F16X2 = 0, 1, 2, 3
 LOSS_FROBENIUS, LOSS_KULLBACK_LEIBLER, LOSS_ITAKURA_SAITO = 0, 1, 2
+INIT_RANDOM, INIT_NNDSVD, INIT_NNDSVDA, INIT_NNDSVDAR = 0, 1, 2, 3
+INIT_CODES = {"random": INIT_RANDOM, "nndsvd": INIT_NNDSVD, "nndsvda": INIT_NNDSVDA, "nndsvdar": INIT_NNDSVDAR}
 MAX_COMPONENTS = 32
 
 
@@ -65,6 +67,9 @@ SIGNATURES = {
     "cnmf_dataset_tpm_stats": (_i, [_vp, _d, _vp, _vp, _vp, _vp]),
     "cnmf_random_init_host": (_i, [_c.c_uint32, _d, _i, _i, _i, _vp, _ll, _vp, _ll]),
     "cnmf_random_init_dev": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp]),
+    "cnmf_nndsvd_init_dev": (_i, [_vp, _i, _vp, _vp, _i, _vp, _vp, _vp]),
+    "cnmf_nndsvd_chunk_limit": (_i, [_vp, _i]),
+    "cnmf_nndsvd_gemm_host": (_i, [_vp, _i, _i, _vp, _vp, _vp]),
     "cnmf_factorize": (_i, [_vp, _i, _vp, _vp, _pp(NmfParams), _vp, _vp, _vp, _vp, _vp]),
     "cnmf_factorize_seeds_dev": (_i, [_vp, _i, _vp, _vp, _pp(NmfParams), _vp, _ll, _vp, _vp, _vp]),
     "cnmf_allgather_spectra": (_i, [_vp, _vp, _ll, _ll, _vp, _vp]),
@@ -91,7 +96,7 @@ SIGNATURES = {
 _lib = None
 
 
-ABI_VERSION = 9     # include/cnmf_b200.h CNMF_B200_ABI_VERSION
+ABI_VERSION = 10     # include/cnmf_b200.h CNMF_B200_ABI_VERSION
 
 
 def load():

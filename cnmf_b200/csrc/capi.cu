@@ -584,6 +584,13 @@ static int factorize_impl(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in
   using clk = std::chrono::steady_clock;
   auto ms_since = [](clk::time_point t0) { return std::chrono::duration<double, std::milli>(clk::now() - t0).count(); };
   h->t_rng_ms = h->t_h2d_ms = h->t_solve_ms = h->t_d2h_ms = 0;
+  const int init = (p->reserved >> 1) & 3;
+  if (init != CNMF_INIT_RANDOM) {
+    auto t_init = clk::now();
+    CNMF_TRY(nndsvd_starts_dev(d, n_restarts, ks.data(), seeds, init, fb.Fr, fb.Fc, s));
+    h->t_rng_ms = ms_since(t_init);
+    return run_and_download(d, ks, SK, fb, *p, spectra_host, usages_host, n_iter_host, err_host, s, spectra_dev, ld_dev);
+  }
   if ((p->reserved & 1) == 0) {
     // ---- device RNG (default): the same legacy MT19937 / polar-gauss stream, generated in place on the GPU
     auto t_rng = clk::now();

@@ -29,10 +29,11 @@ struct cnmf_handle_s {
   std::vector<Pending> ev_pending;
   size_t ev_used = 0;
   // kernel classes: 0 = batched GEMM (work = algorithmic FLOPs), 1 = fused update kernels (work = algorithmic bytes),
-  // 2 = sparse products csc_project (work = algorithmic bytes)
-  static constexpr int PROF_CLASSES = 3;
-  double prof_ms[PROF_CLASSES] = {0.0, 0.0, 0.0}, prof_work[PROF_CLASSES] = {0.0, 0.0, 0.0};
-  long long prof_launches[PROF_CLASSES] = {0, 0, 0};
+  // 2 = sparse products csc_project (work = algorithmic bytes), 3 = fp64 GEMM of the NNDSVD starts (work = FLOPs)
+  static constexpr int PROF_CLASSES = 4;
+  double prof_ms[PROF_CLASSES] = {0.0, 0.0, 0.0, 0.0}, prof_work[PROF_CLASSES] = {0.0, 0.0, 0.0, 0.0};
+  long long prof_launches[PROF_CLASSES] = {0, 0, 0, 0};
+  int nndsvd_chunk_restarts = 0;                // > 0: at most this many restarts per chunk of the NNDSVD starts
   double t_rng_ms = 0, t_h2d_ms = 0, t_solve_ms = 0, t_d2h_ms = 0;   // host wall-clock phases of the last cnmf_factorize
   int prof_begin(cudaStream_t s, double work, int cls = 0);    // start event (recorded or shared); returns slot or -1
   void prof_end(cudaStream_t s, int slot);
@@ -162,5 +163,16 @@ int csc_gather_cols(const cnmf_dataset_s* d, const int* cols, const float* scale
 // device totals (n_rows): fp64 row sums; col_sums (2 x n_cols): per column sum(v), sum(v^2) of v = x * target_sum /
 // (row total), 0 for a row without counts.  Fixed reduction order, no floating-point atomics.  Does not synchronise.
 int csc_tpm_sums(const cnmf_dataset_s* d, double target_sum, double* totals, double* col_sums, cudaStream_t s);
+
+// ---- NNDSVD starts on the device: gemm_f64.cu, nndsvd.cu
+// C (M x n_out, row stride ldc) = A (M x K, row stride lda) * op(X) in fp64 for the dataset matrix X (n_rows x n_cols,
+// fp32, row stride ldx): to_genes = false -> C = A X^T (K = n_cols, n_out = n_rows); true -> C = A X (K = n_rows,
+// n_out = n_cols).  Reduction order depends on the shape only.  Does not synchronise.
+int launch_gemm_f64(const double* A, int lda, int M, const float* X, int n_rows, int n_cols, int ldx, bool to_genes,
+                    double* C, int ldc, cudaStream_t s);
+// scikit-learn's NNDSVD starting factors of every restart (ks[r], seeds[r]) for init = CNMF_INIT_NNDSVD / NNDSVDA /
+// NNDSVDAR into packed padded Wt (sum ks x ld_r) and H (sum ks x ld_c); synchronises
+int nndsvd_starts_dev(cnmf_dataset_s* d, int R, const int* ks, const uint32_t* seeds, int init, float* Wt, float* H,
+                      cudaStream_t s);
 
 }  // namespace cnmf

@@ -1,134 +1,45 @@
 // Device-side random NMF initialisation: numpy's legacy RandomState(seed).standard_normal stream
-// (MT19937 + polar "legacy gauss"), reproduced in parallel -- one thread block per restart.
+// (MT19937 + polar "legacy gauss", legacy_gauss.cuh), reproduced in parallel -- one thread block per restart.
 //
 // What sklearn draws (sklearn/decomposition/_nmf.py:296-307, via check_random_state(int)):
 //   H = |avg * N(0,1)|  (k x n_features, row-major)  FIRST, then  W = |avg * N(0,1)|  (n_samples x k).
-// The legacy gauss consumes the MT19937 stream four 32-bit words per candidate pair:
-//   d = ((u0 >> 5) * 2^26 + (u1 >> 6)) / 2^53          (random double from two words)
-//   x1 = 2 d1 - 1, x2 = 2 d2 - 1, r2 = x1^2 + x2^2;  reject unless 0 < r2 < 1
-//   f = sqrt(-2 log(r2) / r2);  returns f*x2 first, then the saved f*x1
-// so the q-th ACCEPTED pair yields normals 2q and 2q+1 regardless of how they are later split between H
-// and W.  624 = 4 * 156: every regenerated MT block holds exactly 156 candidate pairs, nothing straddles.
-// Parallel form: the block regenerates the 624-word state in four dependency phases, 156 threads evaluate
-// one candidate each, a block-wide exclusive scan of the accept flags gives each accepted pair its output
-// slot, and the values are written straight into the packed device layout (H rows, W^T rows).
+// The values are written straight into the packed device layout (H rows, W^T rows).
 //
-// Exactness: every operation is IEEE (contraction disabled through __dmul_rn/__dadd_rn; sqrt and division
-// are correctly rounded) except log(), where CUDA (<= 1 ulp) and glibc may differ in the last bit of the
-// fp64 result; after |avg*z| is rounded to fp32 this is visible in about one value per 10^8.  The host
-// generator (legacy_rng.cpp, bit-exact by construction) stays available (`rng="host"`) and is what the
-// parity fixtures use.
+// Exactness: see legacy_gauss.cuh -- only log() may differ from glibc in the last bit of the fp64 result; after
+// |avg*z| is rounded to fp32 this is visible in about one value per 10^8.  The host generator (legacy_rng.cpp,
+// bit-exact by construction) stays available (`rng="host"`) and is what the parity fixtures use.
 #include <cuda_runtime.h>
 
 #include "common.cuh"
 #include "engine.h"
+#include "legacy_gauss.cuh"
 
 namespace cnmf {
 
 namespace {
 
-constexpr int MT_N = 624, MT_M = 397;
-constexpr uint32_t MT_A = 0x9908b0dfu, MT_UPPER = 0x80000000u, MT_LOWER = 0x7fffffffu;
-
-__device__ __forceinline__ uint32_t mt_twist(uint32_t cur, uint32_t nxt, uint32_t far) {
-  const uint32_t y = (cur & MT_UPPER) | (nxt & MT_LOWER);
-  return far ^ (y >> 1) ^ ((0u - (y & 1u)) & MT_A);
-}
-__device__ __forceinline__ uint32_t mt_temper(uint32_t y) {
-  y ^= (y >> 11);
-  y ^= (y << 7) & 0x9d2c5680u;
-  y ^= (y << 15) & 0xefc60000u;
-  y ^= (y >> 18);
-  return y;
-}
-
-__global__ void __launch_bounds__(256)
+__global__ void __launch_bounds__(LEGACY_GAUSS_THREADS)
 rng_init_kernel(const uint32_t* __restrict__ seeds, const int* __restrict__ ks, const int* __restrict__ offs,
                 const double* __restrict__ avgs, int n_samples, int n_features, float* __restrict__ Wt, long long ldW,
                 float* __restrict__ H, long long ldH) {
-  __shared__ uint32_t st[2][MT_N];
-  __shared__ int warp_tot[8];
-  __shared__ long long s_base;
+  __shared__ LegacyGaussShared sh;
   const int r = blockIdx.x;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int k = ks[r];
   const long long row0 = offs[r];
   const double avg = avgs[r];
   const long long nH = (long long)k * n_features;
   const long long total = nH + (long long)n_samples * k;
-
-  if (tid == 0) {                                   // init_genrand (numpy mt19937_seed)
-    uint32_t s = seeds[r];
-    for (int pos = 0; pos < MT_N; ++pos) {
-      st[0][pos] = s;
-      s = 1812433253u * (s ^ (s >> 30)) + (uint32_t)pos + 1u;
+  legacy_gauss_block(seeds[r], total, sh, [&](long long t, double z) {
+    const float v = (float)fabs(__dmul_rn(avg, z));
+    if (t < nH) {
+      const long long c = t / n_features, g = t % n_features;
+      H[(row0 + c) * ldH + g] = v;
+    } else {
+      const long long tt = t - nH;
+      const long long j = tt / k, c = tt % k;
+      Wt[(row0 + c) * ldW + j] = v;
     }
-    s_base = 0;
-  }
-  __syncthreads();
-  int cur = 0;
-  for (;;) {
-    const long long base = s_base;                  // accepted pairs so far
-    if (2 * base >= total) break;
-    // ---- regenerate the state: new[i] = twist(old[i], old[i+1], x[i+397 mod]) in dependency order
-    uint32_t* o = st[cur];
-    uint32_t* nw = st[cur ^ 1];
-    for (int i = tid; i < MT_N - MT_M; i += 256) nw[i] = mt_twist(o[i], o[i + 1], o[i + MT_M]);            // 0..226
-    __syncthreads();
-    for (int i = MT_N - MT_M + tid; i < 2 * (MT_N - MT_M); i += 256) nw[i] = mt_twist(o[i], o[i + 1], nw[i - (MT_N - MT_M)]);   // 227..453
-    __syncthreads();
-    for (int i = 2 * (MT_N - MT_M) + tid; i < MT_N - 1; i += 256) nw[i] = mt_twist(o[i], o[i + 1], nw[i - (MT_N - MT_M)]);     // 454..622
-    __syncthreads();
-    if (tid == 0) nw[MT_N - 1] = mt_twist(o[MT_N - 1], nw[0], nw[MT_M - 1]);
-    __syncthreads();
-    cur ^= 1;
-    // ---- 156 candidate pairs
-    bool acc = false;
-    double x1 = 0.0, x2 = 0.0, r2 = 1.0;
-    if (tid < MT_N / 4) {
-      const uint32_t u0 = mt_temper(nw[4 * tid]), u1 = mt_temper(nw[4 * tid + 1]);
-      const uint32_t u2 = mt_temper(nw[4 * tid + 2]), u3 = mt_temper(nw[4 * tid + 3]);
-      const double d1 = ((double)(u0 >> 5) * 67108864.0 + (double)(u1 >> 6)) / 9007199254740992.0;
-      const double d2 = ((double)(u2 >> 5) * 67108864.0 + (double)(u3 >> 6)) / 9007199254740992.0;
-      x1 = __dadd_rn(__dmul_rn(2.0, d1), -1.0);
-      x2 = __dadd_rn(__dmul_rn(2.0, d2), -1.0);
-      r2 = __dadd_rn(__dmul_rn(x1, x1), __dmul_rn(x2, x2));
-      acc = (r2 < 1.0) && (r2 != 0.0);
-    }
-    const unsigned bal = __ballot_sync(0xffffffffu, acc);
-    const int before = __popc(bal & ((1u << lane) - 1u));
-    if (lane == 0) warp_tot[warp] = __popc(bal);
-    __syncthreads();
-    int wbase = 0, tot = 0;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) {
-      if (w < warp) wbase += warp_tot[w];
-      tot += warp_tot[w];
-    }
-    if (acc) {
-      const long long q = base + wbase + before;    // index of this accepted pair
-      const double f = sqrt(__ddiv_rn(__dmul_rn(-2.0, log(r2)), r2));
-      const double z[2] = {__dmul_rn(f, x2), __dmul_rn(f, x1)};
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const long long t = 2 * q + e;
-        if (t < total) {
-          const float v = (float)fabs(__dmul_rn(avg, z[e]));
-          if (t < nH) {
-            const long long c = t / n_features, g = t % n_features;
-            H[(row0 + c) * ldH + g] = v;
-          } else {
-            const long long tt = t - nH;
-            const long long j = tt / k, c = tt % k;
-            Wt[(row0 + c) * ldW + j] = v;
-          }
-        }
-      }
-    }
-    __syncthreads();
-    if (tid == 0) s_base = base + tot;
-    __syncthreads();
-  }
+  });
 }
 
 }  // namespace
@@ -156,7 +67,7 @@ int launch_rng_init(const uint32_t* seeds_host, const int* ks_host, const int* o
   const uint32_t* d_seed = reinterpret_cast<const uint32_t*>(d + sizeof(double) * R);
   const int* d_k = reinterpret_cast<const int*>(d + sizeof(double) * R + sizeof(int) * (size_t)R);
   const int* d_off = d_k + R;
-  rng_init_kernel<<<R, 256, 0, s>>>(d_seed, d_k, d_off, d_avg, n_samples, n_features, Wt, ldW, H, ldH);
+  rng_init_kernel<<<R, LEGACY_GAUSS_THREADS, 0, s>>>(d_seed, d_k, d_off, d_avg, n_samples, n_features, Wt, ldW, H, ldH);
   CNMF_CUDA_CHECK(cudaGetLastError());
   h->launches += 1;
   return 0;

@@ -32,9 +32,9 @@ def _params_precision(p):
 def check_supported(ks=None, init="random", beta_loss="frobenius"):
     """Options the CUDA path does not implement are refused where the user states them (prepare / the CLI), not
     hours later inside factorize: n_components > 32, an init scikit-learn does not know, beta_loss outside
-    {frobenius, kullback-leibler, itakura-saito}.  init: 'random' (the reference default, cnmf.py:335; generated on
-    the device) and the NNDSVD family ('nndsvd' is the CLI's other choice, cnmf.py:1252; starting factors computed on
-    the host by cnmf_b200.nndsvd, then the same batched solve)."""
+    {frobenius, kullback-leibler, itakura-saito}.  init: 'random' (the reference default, cnmf.py:335) and the NNDSVD
+    family ('nndsvd' is the CLI's other choice, cnmf.py:1252), both generated on the device before the same batched
+    solve (cnmf_b200.nndsvd restates the NNDSVD family on the host)."""
     from .nndsvd import INITS
     if ks is not None:
         bad = [int(k) for k in np.atleast_1d(ks) if int(k) < 1 or int(k) > _lib.MAX_COMPONENTS]
@@ -47,11 +47,22 @@ def check_supported(ks=None, init="random", beta_loss="frobenius"):
     loss_code(beta_loss)
 
 
+def init_code(init, ks, n_samples, n_features):
+    """CNMF_INIT_* of one call: init (None resolved as scikit-learn does, per n_components) must name the same
+    initialisation for every restart."""
+    from .nndsvd import resolve_init
+    which = {resolve_init(init, int(k), n_samples, n_features) for k in np.atleast_1d(ks)}
+    if len(which) > 1:
+        raise ValueError("init=%r resolves to %s for different n_components of one call; split the call by K"
+                         % (init, sorted(which)))
+    return _lib.INIT_CODES[which.pop()]
+
+
 def nndsvd_starts(X, ks, seeds, init):
     """Packed starting factors (W^T rows: sum ks x cells, H rows: sum ks x genes; fp32) of every restart (k, seed) for
     init in {'nndsvd', 'nndsvda', 'nndsvdar', None}: scikit-learn's `_initialize_nmf` as the reference's call reaches it
     (cnmf.py:672), restated in cnmf_b200/nndsvd.py.  One randomized SVD per restart on the host (threads: LAPACK / BLAS
-    release the GIL)."""
+    release the GIL).  Dataset.nndsvd_init_dev computes the same starts on the GPU."""
     import concurrent.futures
     import os
     from .nndsvd import nndsvd_init, resolve_init
@@ -157,7 +168,7 @@ class Engine:
     def profile_get(self, kernel_class=0):
         """(total device ms, launches, algorithmic work) of a kernel class since profile(True):
         0 = batched GEMM (work in FLOPs), 1 = fused update kernels (work in bytes), 2 = sparse-dataset products
-        (work in bytes)."""
+        (work in bytes), 3 = fp64 GEMM of the NNDSVD starts (work in FLOPs)."""
         ms, n, fl = ctypes.c_double(), ctypes.c_longlong(), ctypes.c_double()
         check(self.lib.cnmf_profile_get_class(self._h, int(kernel_class), ctypes.byref(ms), ctypes.byref(n),
                                               ctypes.byref(fl)))
@@ -174,6 +185,10 @@ class Engine:
         v = [ctypes.c_double() for _ in range(4)]
         check(self.lib.cnmf_last_timing(self._h, *[ctypes.byref(x) for x in v]))
         return dict(zip(("rng_ms", "h2d_ms", "solve_ms", "d2h_ms"), [x.value for x in v]))
+
+    def nndsvd_chunk_limit(self, max_restarts):
+        """Test hook: at most max_restarts restarts per chunk of the device NNDSVD starts (0 = sized from free memory)."""
+        check(self.lib.cnmf_nndsvd_chunk_limit(self._h, int(max_restarts)))
 
     def dataset(self, X, precision=_DEFAULT_PRECISION, stream=None):
         return Dataset(self, X, precision, stream)
@@ -274,16 +289,40 @@ class Dataset:
         check(self.lib.cnmf_random_init_dev(self._d, len(ks), ptr(ks), ptr(seeds), ctypes.c_void_p(Wt_ptr),
                                             ctypes.c_void_p(H_ptr), None))
 
+    def nndsvd_init_dev(self, ks, seeds, init, Wt_ptr, H_ptr):
+        """scikit-learn's NNDSVD starts (init 'nndsvd' | 'nndsvda' | 'nndsvdar' | None, resolved per n_components as
+        scikit-learn does) of every (k, seed), computed on the GPU in float64 into packed padded device buffers laid
+        out as for random_init_dev."""
+        ks = np.ascontiguousarray(ks, dtype=np.int32)
+        seeds = np.ascontiguousarray(seeds, dtype=np.uint32)
+        code = init_code(init, ks, *self.shape)
+        if code == _lib.INIT_RANDOM:
+            raise ValueError("nndsvd_init_dev: init=%r is the random init (random_init_dev)" % (init,))
+        check(self.lib.cnmf_nndsvd_init_dev(self._d, len(ks), ptr(ks), ptr(seeds), code, ctypes.c_void_p(Wt_ptr),
+                                            ctypes.c_void_p(H_ptr), None))
+
+    def nndsvd_gemm(self, A, to_genes):
+        """float64 product of the NNDSVD starts (test hook): A (M x genes) @ X.T, or with to_genes A (M x cells) @ X."""
+        A = np.ascontiguousarray(A, dtype=np.float64)
+        n, g = self.shape
+        assert A.shape[1] == (n if to_genes else g)
+        C = np.empty((A.shape[0], g if to_genes else n))
+        check(self.lib.cnmf_nndsvd_gemm_host(self._d, 1 if to_genes else 0, A.shape[0], ptr(A), ptr(C), None))
+        return C
+
+    def _init_params(self, ks, nmf_kwargs):
+        """params with the initialisation of the call in bits 1-2 of `reserved`"""
+        p = self.params(nmf_kwargs)
+        p.reserved |= init_code(nmf_kwargs.get("init", "random"), ks, *self.shape) << 1
+        return p
+
     def factorize_seeds_dev(self, ks, seeds, out_ptr, ld_out, nmf_kwargs):
-        """cnmf_factorize (same seeds, same device RNG) with the spectra left on the device: out_ptr is a
-        (sum ks) x ld_out fp32 device buffer.  Returns (n_iter, err)."""
+        """cnmf_factorize (same seeds, same device starts: random or NNDSVD) with the spectra left on the device:
+        out_ptr is a (sum ks) x ld_out fp32 device buffer.  Returns (n_iter, err)."""
         ks = np.ascontiguousarray(ks, dtype=np.int32)
         seeds = np.ascontiguousarray(seeds, dtype=np.uint32)
         R = len(ks)
-        if nmf_kwargs.get("init", "random") != "random":
-            raise ValueError("factorize_seeds_dev draws the seeded random init on the device; init=%r goes through "
-                             "Dataset.factorize(X_host=...)" % (nmf_kwargs.get("init"),))
-        p = self.params(nmf_kwargs)
+        p = self._init_params(ks, nmf_kwargs)
         self._check_loss(p)
         n_iter = np.zeros(R, np.int32)
         err = np.zeros(R, np.float64)
@@ -378,8 +417,9 @@ class Dataset:
 
     def factorize(self, ks, seeds, nmf_kwargs, return_usages=False, W0=None, H0=None, X_host=None):
         """All restarts (ks[r], seeds[r]) at once.  Returns (spectra_list, usages_list|None, n_iter, err).
-        W0 / H0: packed starting factors (sum ks x cells, sum ks x genes) instead of the seeded random init; X_host: the
-        host matrix, needed only when nmf_kwargs['init'] is one of the NNDSVD family (starts computed from it)."""
+        W0 / H0: packed starting factors (sum ks x cells, sum ks x genes) instead of the seeded init.  The NNDSVD family
+        of nmf_kwargs['init'] runs on the device, unless X_host (the host matrix the dataset was created from) is
+        given: then its starts come from cnmf_b200.nndsvd on the host."""
         ks = np.ascontiguousarray(ks, dtype=np.int32)
         R = len(ks)
         SK = int(ks.sum())
@@ -391,14 +431,12 @@ class Dataset:
         n_iter = np.zeros(R, np.int32)
         err = np.zeros(R, np.float64)
         init = nmf_kwargs.get("init", "random")
-        if W0 is None and init != "random":
-            # NNDSVD family (cnmf.py:1252 / SK _nmf.py:309-369): starting factors from cnmf_b200.nndsvd on the host, one
+        if W0 is None and init != "random" and X_host is not None:
+            # NNDSVD family (cnmf.py:1252 / SK _nmf.py:309-369) on the host: starting factors from cnmf_b200.nndsvd, one
             # randomized SVD per restart (the seed enters through its test matrix), then the ordinary batched solve
-            if X_host is None:
-                raise ValueError("init=%r: pass X_host (the matrix the dataset was created from) or W0 / H0; the "
-                                 "device generator only covers init='random'" % (init,))
             W0, H0 = nndsvd_starts(X_host, ks, seeds, init)
         if W0 is None:
+            p.reserved |= init_code(init, ks, n, g) << 1
             seeds = np.ascontiguousarray(seeds, dtype=np.uint32)
             check(self.lib.cnmf_factorize(self._d, R, ptr(ks), ptr(seeds), ctypes.byref(p), ptr(spectra), ptr(usages),
                                           ptr(n_iter), ptr(err), None))

@@ -191,8 +191,8 @@ class ShardedSpectra:
 
 def factorize_sharded(ds, ks_all, seeds_all, nmf_kwargs, comm=None, X_host=None):
     """The multi-GPU factorize: this rank's jobs (idx % world == rank, cnmf.py:52-53) in one batched solve whose
-    spectra stay in HBM, then ONE NCCL all-gather of the per-rank slabs (cnmf_allgather_spectra).  No host staging
-    (except for the NNDSVD family of initialisations, whose starting factors come from the host: pass X_host).
+    spectra stay in HBM, then ONE NCCL all-gather of the per-rank slabs (cnmf_allgather_spectra).  No host staging:
+    random and NNDSVD starts are computed on the device (X_host: take the NNDSVD starts from the host instead).
     Returns (ShardedSpectra, n_iter of the local jobs, local job indices)."""
     import torch
     rank, world, _ = dist_info()
@@ -203,7 +203,7 @@ def factorize_sharded(ds, ks_all, seeds_all, nmf_kwargs, comm=None, X_host=None)
     gathered = torch.zeros((world, max_rows, ld), dtype=torch.float32, device=dev)
     slab = gathered[rank] if world == 1 else torch.zeros((max_rows, ld), dtype=torch.float32, device=dev)
     n_iter = np.zeros(0, np.int32)
-    if jobs and nmf_kwargs.get("init", "random") != "random":
+    if jobs and nmf_kwargs.get("init", "random") != "random" and X_host is not None:
         sp, _, n_iter, _ = ds.factorize([ks_all[j] for j in jobs], [seeds_all[j] for j in jobs], nmf_kwargs, X_host=X_host)
         rows = np.vstack(sp)
         slab[:rows.shape[0], :rows.shape[1]].copy_(torch.from_numpy(rows))
@@ -244,7 +244,7 @@ def factorize_distributed(cnmf_obj, write_files=True):
     ks_all = [int(k) for k in run_params["n_components"]]
     seeds_all = [int(s) for s in run_params["nmf_seed"]]
     ds = cnmf_obj._dataset(norm.X)
-    sharded, _, _ = factorize_sharded(ds, ks_all, seeds_all, kw, X_host=norm.X)
+    sharded, _, _ = factorize_sharded(ds, ks_all, seeds_all, kw)
     cnmf_obj.last_sharded_spectra = sharded          # consensus can take its matrices from the device slab
     full = sharded.host()
     merged = {}

@@ -338,7 +338,7 @@ class cNMF:
 
     def _nmf_batched(self, X, ks, seeds, nmf_kwargs, X_host=None):
         """All restarts at once; returns list of spectra (float64) and per-restart iteration counts.  X_host: the host
-        matrix, used only for the NNDSVD family of initialisations (their SVD runs on the host)."""
+        matrix, to compute the NNDSVD family of initialisations on the host instead of the device."""
         ds = self._dataset(X)
         sp, _, n_iter, err = ds.factorize(ks, seeds, nmf_kwargs, X_host=X_host)
         return [s.astype(np.float64) for s in sp], n_iter, err
@@ -370,7 +370,7 @@ class cNMF:
                                                                         "" if len(groups) == 1 else "s"))
         hit_max = False
         for lo, hi in groups:
-            spectra, n_iter, _ = self._nmf_batched(ds, ks[lo:hi], seeds[lo:hi], kw, X_host=norm.X)
+            spectra, n_iter, _ = self._nmf_batched(ds, ks[lo:hi], seeds[lo:hi], kw)
             hit_max = hit_max or int(np.max(n_iter)) >= int(kw["max_iter"])
             for j, sp in zip(jobs[lo:hi], spectra):
                 p = run_params.iloc[j]

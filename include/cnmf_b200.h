@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define CNMF_B200_ABI_VERSION 9
+#define CNMF_B200_ABI_VERSION 10
 #define CNMF_MAX_COMPONENTS 32          /* largest n_components per restart on the CUDA path */
 
 typedef struct cnmf_handle_s* cnmf_handle_t;
@@ -48,13 +48,17 @@ enum { CNMF_PRECISION_FP32 = 0, CNMF_PRECISION_TF32X3 = 1, CNMF_PRECISION_TF32X3
  * _nmf.py:551-608, 637-694 as fused streaming kernels (solver must be CNMF_SOLVER_MU, as in sklearn). */
 enum { CNMF_LOSS_FROBENIUS = 0, CNMF_LOSS_KULLBACK_LEIBLER = 1, CNMF_LOSS_ITAKURA_SAITO = 2 };
 
+/* yaml 'init' (cnmf.py:335, CLI --init cnmf.py:1252): scikit-learn's seeded random init or one of its NNDSVD starts */
+enum { CNMF_INIT_RANDOM = 0, CNMF_INIT_NNDSVD = 1, CNMF_INIT_NNDSVDA = 2, CNMF_INIT_NNDSVDAR = 3 };
+
 /* Mirrors the nmf_kwargs dict of cnmf.py:618-627 after sklearn's own scaling of the
  * regularisation (sklearn/decomposition/_nmf.py:1249-1260): l1_reg_W = n_features*alpha_W*l1_ratio ... */
 typedef struct cnmf_nmf_params {
   int32_t solver;        /* CNMF_SOLVER_* */
   int32_t precision;     /* CNMF_PRECISION_* */
   int32_t max_iter;      /* 'max_iter' (cnmf.py:625) */
-  int32_t reserved;      /* flags: bit 0 = draw the random init on the host (bit-exact numpy stream) instead of the GPU */
+  int32_t reserved;      /* flags: bit 0 = draw the random init on the host (bit-exact numpy stream) instead of the GPU;
+                          * bits 1-2 = CNMF_INIT_* of cnmf_factorize / cnmf_factorize_seeds_dev (0 = random) */
   double tol;            /* 'tol' (cnmf.py:624) */
   double l1_reg_W, l2_reg_W, l1_reg_H, l2_reg_H;
   int32_t beta_loss;     /* CNMF_LOSS_* ('beta_loss', cnmf.py:622); 0 = frobenius */
@@ -83,7 +87,8 @@ int cnmf_profile_enable(cnmf_handle_t h, int on);
 int cnmf_profile_get(cnmf_handle_t h, double* gemm_ms, long long* gemm_launches, double* gemm_flops);
 /* same counters per kernel class: 0 = batched GEMM (work = algorithmic FLOPs), 1 = fused update kernels
  * (work = algorithmic bytes: factor read + product slices read + factor and tf32 pieces written), 2 = the product
- * of a sparse dataset, both of its kernels (work = algorithmic bytes: 8 per entry, col_ptr, staged U, output) */
+ * of a sparse dataset, both of its kernels (work = algorithmic bytes: 8 per entry, col_ptr, staged U, output),
+ * 3 = the fp64 GEMM of cnmf_nndsvd_init_dev (work = algorithmic FLOPs, 2*M*N*K per launch) */
 int cnmf_profile_get_class(cnmf_handle_t h, int kernel_class, double* ms, long long* launches, double* work);
 
 /* host wall-clock phases (ms) of the last cnmf_factorize on this handle: host RNG, H2D of the initial
@@ -161,9 +166,26 @@ int cnmf_random_init_host(uint32_t seed, double avg, int n_samples, int n_featur
 int cnmf_random_init_dev(cnmf_dataset_t d, int n_restarts, const int32_t* ks, const uint32_t* seeds, float* Wt_dev,
                          float* H_dev, void* stream);
 
+/* NNDSVD starting factors (sklearn _nmf.py:309-369 after randomized_svd(X, k, random_state=seed), SK/utils/extmath.py)
+ * of every restart, computed on the device from the dataset's fp32 X with float64 arithmetic (fp64 tensor-core
+ * products, CholeskyQR2 in place of the LU / QR normalisers, Jacobi SVD of the small factor) into the same packed,
+ * padded buffers as cnmf_random_init_dev.  init = CNMF_INIT_NNDSVD / _NNDSVDA / _NNDSVDAR; every ks[r] must be
+ * <= min(n_rows, n_cols) (sklearn's condition).  The work space (about 8 * sum(ks + 10) * (n_rows + n_cols) bytes)
+ * is allocated and freed inside the call, in chunks of restarts sized from the free device memory; a restart's
+ * result does not depend on the chunking or on the other restarts.  Sparse datasets: -3. */
+int cnmf_nndsvd_init_dev(cnmf_dataset_t d, int n_restarts, const int32_t* ks, const uint32_t* seeds, int init,
+                         float* Wt_dev, float* H_dev, void* stream);
+/* test hook: at most max_restarts restarts per chunk of cnmf_nndsvd_init_dev on this handle (0 = sized from the free
+ * device memory only, the default) -- chunkings can then be compared without starving the device */
+int cnmf_nndsvd_chunk_limit(cnmf_handle_t h, int max_restarts);
+/* test hook: the fp64 GEMM of cnmf_nndsvd_init_dev.  to_genes = 0: C_host (M x n_rows) = A_host (M x n_cols) X^T;
+ * 1: C_host (M x n_cols) = A_host (M x n_rows) X.  Host arrays dense row-major fp64. */
+int cnmf_nndsvd_gemm_host(cnmf_dataset_t d, int to_genes, int M, const double* A_host, double* C_host, void* stream);
+
 /* ---- batched factorize: replaces the restart loop of cNMF.factorize ---------------- */
 /* For r in [0, n_restarts): one NMF of the dataset with n_components = ks[r] and
- * random_state = seeds[r] (cnmf.py:738-741), all restarts advanced together on the GPU.
+ * random_state = seeds[r] (cnmf.py:738-741), all restarts advanced together on the GPU.  The starting factors are
+ * sklearn's random init, or its NNDSVD starts (cnmf_nndsvd_init_dev) when params.reserved bits 1-2 name one.
  *   spectra_host : packed (sum ks) x n_cols, row stride n_cols; restart r owns rows
  *                  [sum ks[0..r), +ks[r])  -- what factorize saves per restart (cnmf.py:742-745)
  *   usages_host  : optional (may be NULL; the reference discards W) packed (sum ks) x n_rows,
