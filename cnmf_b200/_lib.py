@@ -33,6 +33,23 @@ class NmfParams(ctypes.Structure):
                 ("beta_loss", ctypes.c_int32), ("reserved2", ctypes.c_int32)]
 
 
+UNIT_SOLVER_NONE = -1
+UNIT_PIECES_NONE, UNIT_PIECES_TF32, UNIT_PIECES_F16 = 0, 1, 2
+UNIT_GRAM_NONE, UNIT_GRAM_FUSED, UNIT_GRAM_STANDALONE = 0, 1, 2
+
+
+class UpdateStepArgs(ctypes.Structure):
+    """struct cnmf_update_step_args (include/cnmf_b200.h): arguments of the cnmf_update_step_host test hook."""
+    _fields_ = [("n_slots", ctypes.c_int32), ("n_rids", ctypes.c_int32),
+                ("ks", ctypes.c_void_p), ("rids", ctypes.c_void_p), ("done", ctypes.c_void_p),
+                ("n", ctypes.c_int32), ("cpb_tiles", ctypes.c_int32), ("solver", ctypes.c_int32),
+                ("pieces", ctypes.c_int32), ("gram", ctypes.c_int32), ("want_scalar", ctypes.c_int32),
+                ("nsplit", ctypes.c_int32), ("l1", ctypes.c_float), ("l2", ctypes.c_float),
+                ("F", ctypes.c_void_p), ("num", ctypes.c_void_p), ("gram_in", ctypes.c_void_p),
+                ("piece_scale", ctypes.c_void_p), ("pieces_hi", ctypes.c_void_p), ("pieces_lo", ctypes.c_void_p),
+                ("tile_scale", ctypes.c_void_p), ("gram_out", ctypes.c_void_p), ("scal_out", ctypes.c_void_p)]
+
+
 _c = ctypes
 _vp, _i, _ll, _d = _c.c_void_p, _c.c_int, _c.c_longlong, _c.c_double
 _pp = _c.POINTER
@@ -80,7 +97,8 @@ SIGNATURES = {
     "cnmf_factorize_dev": (_i, [_vp, _i, _vp, _vp, _vp, _pp(NmfParams), _vp, _vp, _vp, _vp]),
     "cnmf_refit": (_i, [_vp, _i, _i, _vp, _pp(NmfParams), _vp, _pp(_c.c_int32), _pp(_d), _vp]),
     "cnmf_project_rows": (_i, [_vp, _i, _vp, _vp, _vp]),
-    "cnmf_gemm_abt_host": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _vp, _i, _pp(_c.c_float), _vp]),
+    "cnmf_gemm_abt_host": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _pp(_c.c_float), _vp]),
+    "cnmf_update_step_host": (_i, [_vp, _pp(UpdateStepArgs), _vp]),
     "cnmf_l2_normalize_rows": (_i, [_vp, _vp, _i, _i, _i, _vp]),
     "cnmf_local_density": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     "cnmf_col_stats_dev": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
@@ -96,7 +114,7 @@ SIGNATURES = {
 _lib = None
 
 
-ABI_VERSION = 10     # include/cnmf_b200.h CNMF_B200_ABI_VERSION
+ABI_VERSION = 11     # include/cnmf_b200.h CNMF_B200_ABI_VERSION
 
 
 def load():

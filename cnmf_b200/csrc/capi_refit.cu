@@ -474,9 +474,15 @@ int cnmf_project_rows(cnmf_dataset_t d, int k, const float* Ut_host, float* out_
 // --------------------------------------------------------------------------------- raw GEMM hook
 // C (M x N) = A (M x Kd) * B (N x Kd)^T on host buffers; reps > 1 re-runs the kernel and reports the
 // mean device time per launch in *ms_out (CUDA events).  Used by tests and by the roofline micro-bench.
+// Exact forms (b_exact, f16x2): A diag(k_scale) goes into the A pieces and out_col_scale onto C, as in the solver.
 int cnmf_gemm_abt_host(cnmf_handle_t h, int precision, const float* A, const float* B, int M, int N, int Kd, int splits,
-                       float* C, int reps, float* ms_out, void* stream) {
+                       int b_exact, const float* k_scale, const float* out_col_scale, float* C, int reps, float* ms_out,
+                       void* stream) {
   CNMF_REQUIRE(h && A && B && C && M > 0 && N > 0 && Kd > 0, "gemm_abt_host: bad arguments");
+  const bool f16 = precision == CNMF_PRECISION_F16X2;    // B must hold integers <= 2048 (exact in fp16)
+  CNMF_REQUIRE(!b_exact || f16 || precision == CNMF_PRECISION_TF32X3, "gemm_abt_host: b_exact needs tf32x3 or f16x2");
+  const bool exact = f16 || b_exact;
+  CNMF_REQUIRE(exact || (!k_scale && !out_col_scale), "gemm_abt_host: k_scale / out_col_scale need an exact form");
   cudaStream_t s = as_stream(stream);
   CNMF_CUDA_CHECK(cudaSetDevice(h->device));
   const int lda = pad_ld(Kd), ldc = pad_ld(N);
@@ -494,22 +500,38 @@ int cnmf_gemm_abt_host(cnmf_handle_t h, int precision, const float* A, const flo
   CNMF_CUDA_CHECK(cudaMemsetAsync(dB, 0, nb * 4, s));
   CNMF_CUDA_CHECK(cudaMemcpy2DAsync(dA, (size_t)lda * 4, A, (size_t)Kd * 4, (size_t)Kd * 4, M, cudaMemcpyHostToDevice, s));
   CNMF_CUDA_CHECK(cudaMemcpy2DAsync(dB, (size_t)lda * 4, B, (size_t)Kd * 4, (size_t)Kd * 4, N, cudaMemcpyHostToDevice, s));
-  CNMF_TRY(launch_split_tf32(dA, dAh, dAl, (long long)na, s));
+  // the scales as the solver holds a dataset's: zero-padded to the row stride, 16-byte aligned (dev_buf)
+  float* dKs = nullptr;
+  float* dCs = nullptr;
+  if (k_scale) {
+    dKs = static_cast<float*>(h->dev_buf("gemmtest.kscale", (size_t)lda * 4));
+    if (!dKs) return -2;
+    CNMF_CUDA_CHECK(cudaMemsetAsync(dKs, 0, (size_t)lda * 4, s));
+    CNMF_CUDA_CHECK(cudaMemcpyAsync(dKs, k_scale, (size_t)Kd * 4, cudaMemcpyHostToDevice, s));
+  }
+  if (out_col_scale) {
+    dCs = static_cast<float*>(h->dev_buf("gemmtest.cscale", (size_t)ldc * 4));
+    if (!dCs) return -2;
+    CNMF_CUDA_CHECK(cudaMemsetAsync(dCs, 0, (size_t)ldc * 4, s));
+    CNMF_CUDA_CHECK(cudaMemcpyAsync(dCs, out_col_scale, (size_t)N * 4, cudaMemcpyHostToDevice, s));
+  }
+  CNMF_TRY(launch_split_scaled(dA, dAh, dAl, M, lda, dKs, s));
   CNMF_TRY(launch_split_tf32(dB, dBh, dBl, (long long)nb, s));
   CNMF_CUDA_CHECK(cudaMemsetAsync(dC, 0xff, (size_t)se * M * ldc * 4, s));   // NaN pattern: unwritten outputs show up
   GemmArgs g{};
   g.M = M; g.N = N; g.Kd = Kd; g.lda = lda; g.ldb = lda; g.ldc = ldc;
   g.C = dC; g.c_split_stride = (long long)M * ldc; g.splits = splits; g.splits_effective = se;
-  const bool f16 = precision == CNMF_PRECISION_F16X2;    // B must hold integers <= 2048 (exact in fp16)
+  g.out_col_scale = dCs;
   if (f16) {
     const int tiles = (lda + 511) / 512;
     float* dRs = static_cast<float*>(h->dev_buf("gemmtest.rs", sizeof(float) * (size_t)M * tiles));
     if (!dRs) return -2;
-    CNMF_TRY(launch_emit_f16(dA, M, Kd, lda, nullptr, dAh, dAl, dRs, tiles, s));
+    CNMF_TRY(launch_emit_f16(dA, M, Kd, lda, dKs, dAh, dAl, dRs, tiles, s));
     CNMF_TRY(launch_to_half(dB, dBh, (long long)nb, s));
     g.A_hi = dAh; g.A_lo = dAl; g.B_hi = dBh; g.b_exact = 1; g.f16 = 1; g.a_tile_scale = dRs; g.a_tiles = tiles;
-  } else if (precision == CNMF_PRECISION_TF32X3) { g.A_hi = dAh; g.A_lo = dAl; g.B_hi = dBh; g.B_lo = dBl; }
-  else { g.A_hi = dA; g.B_hi = dB; }
+  } else if (precision == CNMF_PRECISION_TF32X3) {
+    g.A_hi = dAh; g.A_lo = dAl; g.B_hi = dBh; g.B_lo = b_exact ? nullptr : dBl; g.b_exact = b_exact ? 1 : 0;
+  } else { g.A_hi = dA; g.B_hi = dB; }
   const bool tc = f16 || precision == CNMF_PRECISION_TF32X3;
   cudaEvent_t e0, e1;
   CNMF_CUDA_CHECK(cudaEventCreate(&e0));

@@ -1,0 +1,152 @@
+// Test hook of the C ABI: one launch of the batched solver's update / Gram / <NUM, F> / piece kernels on host data
+// (cnmf_update_step_host, include/cnmf_b200.h).  It builds the FactorView / BatchMeta / FusedOut the solver builds
+// (nmf_engine.cu) and calls the same launch_* functions; no kernel code of its own.
+#include <algorithm>
+#include <vector>
+
+#include "engine.h"
+#include "nmf_kernels.cuh"
+
+using namespace cnmf;
+
+#define CNMF_TRY(expr)            \
+  do {                            \
+    int _rc = (expr);             \
+    if (_rc != 0) return _rc;     \
+  } while (0)
+
+extern "C" int cnmf_update_step_host(cnmf_handle_t h, const cnmf_update_step_args* a, void* stream) {
+  CNMF_REQUIRE(h && a && a->ks && a->rids && a->done && a->F && a->gram_in, "update_step: NULL argument");
+  CNMF_REQUIRE(a->n_slots >= 1 && a->n_rids >= 1 && a->n >= 1 && a->nsplit >= 1, "update_step: bad sizes");
+  CNMF_REQUIRE(a->cpb_tiles == 1 || a->cpb_tiles == 2 || a->cpb_tiles == 4, "update_step: cpb_tiles must be 1, 2 or 4");
+  CNMF_REQUIRE(a->solver == CNMF_SOLVER_MU || a->solver == CNMF_SOLVER_CD || a->solver == CNMF_UNIT_SOLVER_NONE,
+               "update_step: unknown solver");
+  CNMF_REQUIRE(a->pieces >= CNMF_UNIT_PIECES_NONE && a->pieces <= CNMF_UNIT_PIECES_F16, "update_step: unknown pieces mode");
+  CNMF_REQUIRE(a->gram >= CNMF_UNIT_GRAM_NONE && a->gram <= CNMF_UNIT_GRAM_STANDALONE, "update_step: unknown Gram mode");
+  CNMF_REQUIRE(a->pieces == CNMF_UNIT_PIECES_NONE || (a->pieces_hi && a->pieces_lo), "update_step: pieces buffers missing");
+  CNMF_REQUIRE(a->pieces != CNMF_UNIT_PIECES_F16 || a->tile_scale, "update_step: tile_scale missing");
+  CNMF_REQUIRE(a->gram == CNMF_UNIT_GRAM_NONE || a->gram_out, "update_step: gram_out missing");
+  CNMF_REQUIRE(!a->want_scalar || a->scal_out, "update_step: scal_out missing");
+  const bool none = a->solver == CNMF_UNIT_SOLVER_NONE;
+  CNMF_REQUIRE(!none || a->gram != CNMF_UNIT_GRAM_FUSED, "update_step: no update launch to fuse the Gram into");
+  CNMF_REQUIRE(a->num || (none && !a->want_scalar), "update_step: num missing");
+  const int R = a->n_slots, NR = a->n_rids;
+  std::vector<int> meta(3 * R + NR, 0);         // off | k | rid per slot, done per rid
+  std::vector<char> seen(NR, 0);
+  int SK = 0, kmax = 0;
+  for (int s = 0; s < R; ++s) {
+    CNMF_REQUIRE(a->ks[s] >= 1 && a->ks[s] <= KMAX, "update_step: ks must be in [1, 32]");
+    CNMF_REQUIRE(a->rids[s] >= 0 && a->rids[s] < NR && !seen[a->rids[s]], "update_step: rids must be distinct and < n_rids");
+    seen[a->rids[s]] = 1;
+    meta[s] = SK;
+    meta[R + s] = a->ks[s];
+    meta[2 * R + s] = a->rids[s];
+    SK += a->ks[s];
+    kmax = std::max(kmax, a->ks[s]);
+  }
+  for (int r = 0; r < NR; ++r) meta[3 * R + r] = a->done[r];
+  const int kp = kmax <= 16 ? 16 : 32;
+  CNMF_REQUIRE(a->gram != CNMF_UNIT_GRAM_FUSED || kp == 16, "update_step: the fused Gram exists for kp == 16 batches only");
+
+  cudaStream_t s = as_stream(stream);
+  CNMF_CUDA_CHECK(cudaSetDevice(h->device));
+  const int n = a->n, ld = pad_ld(n), n_ktiles = (ld + 511) / 512;
+  const int tile = upd_tile_cols(kp);
+  const int cpb = a->cpb_tiles * tile;
+  const int gcpb = pick_cols_per_block(n, R, 8192, 1024, h->sm_count * 2);     // as solve_batched
+  const int chunks = (n + cpb - 1) / cpb, gchunks = (n + gcpb - 1) / gcpb;
+  const size_t nf = (size_t)SK * ld;
+  const int RR = std::max(R, NR);              // partials: slot-indexed (update launches) or rid-indexed (the others)
+  const size_t piece_bytes = a->pieces == CNMF_UNIT_PIECES_F16 ? 2 : 4;
+
+  int* d_meta = static_cast<int*>(h->dev_buf("unit.meta", sizeof(int) * meta.size()));
+  float* d_F = static_cast<float*>(h->dev_buf("unit.F", nf * 4));
+  float* d_num = static_cast<float*>(h->dev_buf("unit.num", (size_t)a->nsplit * nf * 4));
+  double* d_gin = static_cast<double*>(h->dev_buf("unit.gram_in", sizeof(double) * (size_t)NR * KMAX * KMAX));
+  double* d_gout = static_cast<double*>(h->dev_buf("unit.gram_out", sizeof(double) * (size_t)NR * KMAX * KMAX));
+  double* d_scal = static_cast<double*>(h->dev_buf("unit.scal", sizeof(double) * NR));
+  double* d_gpart = static_cast<double*>(h->dev_buf("unit.gram_part", sizeof(double) * (size_t)RR * std::max(chunks, gchunks) * kp * kp));
+  double* d_spart = static_cast<double*>(h->dev_buf("unit.scal_part", sizeof(double) * (size_t)RR * chunks));
+  float* d_ps = static_cast<float*>(h->dev_buf("unit.piece_scale", (size_t)ld * 4));
+  void* d_hi = h->dev_buf("unit.pieces_hi", nf * piece_bytes);
+  void* d_lo = h->dev_buf("unit.pieces_lo", nf * piece_bytes);
+  float* d_ts = static_cast<float*>(h->dev_buf("unit.tile_scale", sizeof(float) * (size_t)SK * n_ktiles));
+  if (!d_meta || !d_F || !d_num || !d_gin || !d_gout || !d_scal || !d_gpart || !d_spart || !d_ps || !d_hi || !d_lo || !d_ts)
+    return -2;
+  // tickets: zeroed when first allocated, never again (the fused launches leave them at zero themselves)
+  const size_t tbytes = sizeof(int) * (size_t)std::max(NR, 64);
+  auto tk = h->ws.find("unit.tickets");
+  const bool fresh = tk == h->ws.end() || !tk->second.first || tk->second.second < tbytes;
+  int* d_ticket = static_cast<int*>(h->dev_buf("unit.tickets", tbytes));
+  if (!d_ticket) return -2;
+  if (fresh) CNMF_CUDA_CHECK(cudaMemsetAsync(d_ticket, 0, tbytes, s));
+
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(d_meta, meta.data(), sizeof(int) * meta.size(), cudaMemcpyHostToDevice, s));
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(d_F, a->F, nf * 4, cudaMemcpyHostToDevice, s));
+  if (a->num) CNMF_CUDA_CHECK(cudaMemcpyAsync(d_num, a->num, (size_t)a->nsplit * nf * 4, cudaMemcpyHostToDevice, s));
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(d_gin, a->gram_in, sizeof(double) * (size_t)NR * KMAX * KMAX, cudaMemcpyHostToDevice, s));
+  if (a->gram_out)
+    CNMF_CUDA_CHECK(cudaMemcpyAsync(d_gout, a->gram_out, sizeof(double) * (size_t)NR * KMAX * KMAX, cudaMemcpyHostToDevice, s));
+  if (a->want_scalar) CNMF_CUDA_CHECK(cudaMemcpyAsync(d_scal, a->scal_out, sizeof(double) * NR, cudaMemcpyHostToDevice, s));
+  if (a->piece_scale) CNMF_CUDA_CHECK(cudaMemcpyAsync(d_ps, a->piece_scale, (size_t)ld * 4, cudaMemcpyHostToDevice, s));
+  if (a->pieces != CNMF_UNIT_PIECES_NONE) {
+    CNMF_CUDA_CHECK(cudaMemcpyAsync(d_hi, a->pieces_hi, nf * piece_bytes, cudaMemcpyHostToDevice, s));
+    CNMF_CUDA_CHECK(cudaMemcpyAsync(d_lo, a->pieces_lo, nf * piece_bytes, cudaMemcpyHostToDevice, s));
+  }
+  if (a->pieces == CNMF_UNIT_PIECES_F16)
+    CNMF_CUDA_CHECK(cudaMemcpyAsync(d_ts, a->tile_scale, sizeof(float) * (size_t)SK * n_ktiles, cudaMemcpyHostToDevice, s));
+
+  const BatchMeta b{d_meta, d_meta + R, d_meta + 2 * R, d_meta + 3 * R, R, kp};
+  const float* pscale = a->piece_scale ? d_ps : nullptr;
+  const bool fused = a->gram == CNMF_UNIT_GRAM_FUSED;
+  FactorView f{};
+  f.F = d_F;
+  f.n = n; f.ld = ld; f.piece_scale = pscale;
+  if (a->pieces == CNMF_UNIT_PIECES_TF32) { f.F_hi = static_cast<float*>(d_hi); f.F_lo = static_cast<float*>(d_lo); }
+  if (a->pieces == CNMF_UNIT_PIECES_F16 && fused) { f.P_hi = d_hi; f.P_mid = d_lo; f.tile_scale = d_ts; f.n_ktiles = n_ktiles; }
+  f.cpb = cpb; f.gcpb = gcpb;
+  const long long sstride = (long long)nf;
+
+  if (none) {
+    // start of a solve: pieces of the initial factors (run_and_download / emit_pieces), stand-alone Gram, <NUM, F>
+    if (a->pieces == CNMF_UNIT_PIECES_TF32) CNMF_TRY(launch_split_scaled(d_F, f.F_hi, f.F_lo, SK, ld, pscale, s));
+    if (a->pieces == CNMF_UNIT_PIECES_F16) CNMF_TRY(launch_emit_f16(d_F, SK, n, ld, pscale, d_hi, d_lo, d_ts, n_ktiles, s));
+    if (a->gram == CNMF_UNIT_GRAM_STANDALONE) {
+      CNMF_TRY(launch_gram_partial(f, b, d_gpart, s));
+      CNMF_TRY(launch_finalize(d_gpart, d_gout, nullptr, nullptr, gchunks, b, s));
+    }
+    if (a->want_scalar) {
+      CNMF_TRY(launch_cross(f, d_num, a->nsplit, sstride, b, d_spart, s));
+      CNMF_TRY(launch_finalize(nullptr, nullptr, d_spart, d_scal, chunks, b, s));
+    }
+  } else {
+    FusedOut o{};
+    if (fused) { o.gram_part = d_gpart; o.gram = d_gout; }
+    if (a->want_scalar) { o.scal_part = d_spart; o.scal = d_scal; }
+    o.counter = d_ticket;
+    const bool cd = a->solver == CNMF_SOLVER_CD;
+    CNMF_TRY(cd ? launch_cd_update(f, d_num, a->nsplit, sstride, d_gin, b, a->l1, a->l2, o, s)
+                : launch_mu_update(f, d_num, a->nsplit, sstride, d_gin, b, a->l1, a->l2, o, s));
+    if (a->gram == CNMF_UNIT_GRAM_STANDALONE) {          // gram_after() of the solver for batches without the fused Gram
+      CNMF_TRY(launch_gram_partial(f, b, d_gpart, s));
+      CNMF_TRY(launch_finalize(d_gpart, d_gout, nullptr, nullptr, gchunks, b, s));
+    }
+    // f16 pieces: emitted by the Gram-fused launch itself, else by the stand-alone kernel after it (update() of the solver)
+    if (a->pieces == CNMF_UNIT_PIECES_F16 && !fused)
+      CNMF_TRY(launch_emit_f16(d_F, SK, n, ld, pscale, d_hi, d_lo, d_ts, n_ktiles, s));
+  }
+  h->launches += 1;
+
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(a->F, d_F, nf * 4, cudaMemcpyDeviceToHost, s));
+  if (a->pieces != CNMF_UNIT_PIECES_NONE) {
+    CNMF_CUDA_CHECK(cudaMemcpyAsync(a->pieces_hi, d_hi, nf * piece_bytes, cudaMemcpyDeviceToHost, s));
+    CNMF_CUDA_CHECK(cudaMemcpyAsync(a->pieces_lo, d_lo, nf * piece_bytes, cudaMemcpyDeviceToHost, s));
+  }
+  if (a->pieces == CNMF_UNIT_PIECES_F16)
+    CNMF_CUDA_CHECK(cudaMemcpyAsync(a->tile_scale, d_ts, sizeof(float) * (size_t)SK * n_ktiles, cudaMemcpyDeviceToHost, s));
+  if (a->gram_out)
+    CNMF_CUDA_CHECK(cudaMemcpyAsync(a->gram_out, d_gout, sizeof(double) * (size_t)NR * KMAX * KMAX, cudaMemcpyDeviceToHost, s));
+  if (a->want_scalar) CNMF_CUDA_CHECK(cudaMemcpyAsync(a->scal_out, d_scal, sizeof(double) * NR, cudaMemcpyDeviceToHost, s));
+  CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
+  return 0;
+}

@@ -222,7 +222,8 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
   // emit_pieces() after the update (the hi / lo buffers then hold halves)
   const bool upd_pieces = tf32 && !f16;
   // f16: the Gram-fused update kernels (K <= 16, factor being iterated) emit the fp16 pieces themselves, per 512-column
-  // tile; everything else (initial factors, compaction, K > 16) goes through emit_pieces() with one scale per row
+  // tile; everything else (initial factors, compaction, K > 16) goes through emit_pieces(), which normalises the same
+  // 512-column groups and writes the same bits
   const int ktiles_r = (v.ld_r + 511) / 512, ktiles_c = (v.ld_c + 511) / 512;
   const bool emit_in_update = f16 && kp == 16 && io.update_cols;
   auto fr = [&]() {

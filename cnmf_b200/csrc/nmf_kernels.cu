@@ -838,12 +838,12 @@ __device__ __forceinline__ double mu_body(const FactorView& f, const float* __re
   return scal;
 }
 
-// MU: returns <NUM, F_new> over the thread's items (fp32 within a tile, fp64 across tiles).
-// CD: returns sum |projected gradient|.
-template <int KP, int VEC, bool CD, bool GRAM>
-__device__ __forceinline__ double update_body(const FactorView& f, const float* __restrict__ NUM, int nsplit,
-                                              long long sstride, const float* G, int K, int o, float l1, float l2,
-                                              int col_begin, int col_end, float* tile, double* gsum) {
+// One coordinate-descent sweep (the multiplicative update is mu_body): returns sum |projected gradient| over the
+// thread's items.
+template <int KP, int VEC, bool GRAM>
+__device__ __forceinline__ double cd_body(const FactorView& f, const float* __restrict__ NUM, int nsplit,
+                                          long long sstride, const float* G, int K, int o, float l1,
+                                          int col_begin, int col_end, float* tile, double* gsum) {
   constexpr int NP = VecIO<VEC>::NP;
   constexpr int TILE = UPD_THREADS * VEC;
   const volatile float4* Gv = reinterpret_cast<const volatile float4*>(G);
@@ -872,64 +872,38 @@ __device__ __forceinline__ double update_body(const FactorView& f, const float* 
       for (int c = 0; c < KP; ++c) {
         float2 out[NP];
         if (c < K) {
-          if constexpr (!CD) {
-            float2 den[NP];
+          // -(XHt - l1) + sum_r Gram[t, r] * F[r], summed in the order of the Cython loop (r = 0..K-1)
+          float2 g[NP];
 #pragma unroll
-            for (int i4 = 0; i4 < KP / 4; ++i4) {
-              const volatile float4& gq = Gv[c * (KP / 4) + i4];
-              const float g0 = gq.x, g1 = gq.y, g2 = gq.z, g3 = gq.w;
+          for (int p = 0; p < NP; ++p) g[p] = make_float2(l1 - nv[c][p].x, l1 - nv[c][p].y);
 #pragma unroll
-              for (int p = 0; p < NP; ++p) {
-                den[p] = i4 == 0 ? mul2(bcast2(g0), fv[0][p]) : fma2(bcast2(g0), fv[4 * i4 + 0][p], den[p]);
-                den[p] = fma2(bcast2(g1), fv[4 * i4 + 1][p], den[p]);
-                den[p] = fma2(bcast2(g2), fv[4 * i4 + 2][p], den[p]);
-                den[p] = fma2(bcast2(g3), fv[4 * i4 + 3][p], den[p]);
-              }
-            }
+          for (int i4 = 0; i4 < KP / 4; ++i4) {
+            const volatile float4& gq = Gv[c * (KP / 4) + i4];
+            const float g0 = gq.x, g1 = gq.y, g2 = gq.z, g3 = gq.w;
 #pragma unroll
             for (int p = 0; p < NP; ++p) {
-              if (l1 > 0.f) den[p] = add2(den[p], bcast2(l1));
-              if (l2 > 0.f) den[p] = fma2(bcast2(l2), fv[c][p], den[p]);
-              // zero denominators -> eps (sklearn _nmf.py:615,701); the Newton quotient needs a normal number
-              den[p].x = (den[p].x < FLT_MIN_NORMAL) ? EPSILON_F32 : den[p].x;
-              den[p].y = (den[p].y < FLT_MIN_NORMAL) ? EPSILON_F32 : den[p].y;
-              out[p] = mul2(fv[c][p], div_nr2(nv[c][p], den[p]));
-              sacc = fma2(nv[c][p], out[p], sacc);
+              g[p] = fma2(bcast2(g0), fv[4 * i4 + 0][p], g[p]);
+              g[p] = fma2(bcast2(g1), fv[4 * i4 + 1][p], g[p]);
+              g[p] = fma2(bcast2(g2), fv[4 * i4 + 2][p], g[p]);
+              g[p] = fma2(bcast2(g3), fv[4 * i4 + 3][p], g[p]);
             }
-          } else {
-            // -(XHt - l1) + sum_r Gram[t, r] * F[r], summed in the order of the Cython loop (r = 0..K-1)
-            float2 g[NP];
+          }
+          const float h = Gs[c * KP + c];
+          const float hinv = Gs[KP * KP + c];                    // refined 1 / h (0 when h == 0)
 #pragma unroll
-            for (int p = 0; p < NP; ++p) g[p] = make_float2(l1 - nv[c][p].x, l1 - nv[c][p].y);
-#pragma unroll
-            for (int i4 = 0; i4 < KP / 4; ++i4) {
-              const volatile float4& gq = Gv[c * (KP / 4) + i4];
-              const float g0 = gq.x, g1 = gq.y, g2 = gq.z, g3 = gq.w;
-#pragma unroll
-              for (int p = 0; p < NP; ++p) {
-                g[p] = fma2(bcast2(g0), fv[4 * i4 + 0][p], g[p]);
-                g[p] = fma2(bcast2(g1), fv[4 * i4 + 1][p], g[p]);
-                g[p] = fma2(bcast2(g2), fv[4 * i4 + 2][p], g[p]);
-                g[p] = fma2(bcast2(g3), fv[4 * i4 + 3][p], g[p]);
-              }
+          for (int p = 0; p < NP; ++p) {
+            const float pgx = (fv[c][p].x == 0.f) ? fminf(0.f, g[p].x) : g[p].x;
+            const float pgy = (fv[c][p].y == 0.f) ? fminf(0.f, g[p].y) : g[p].y;
+            sacc.x += fabsf(pgx);
+            sacc.y += fabsf(pgy);
+            if (h != 0.f) {                                      // block-uniform
+              float2 q = mul2(g[p], bcast2(hinv));               // g / h: quotient + residual correction
+              const float2 rem = fma2(bcast2(-h), q, g[p]);
+              q = fma2(bcast2(hinv), rem, q);
+              fv[c][p].x = fmaxf(fv[c][p].x - q.x, 0.f);
+              fv[c][p].y = fmaxf(fv[c][p].y - q.y, 0.f);
             }
-            const float h = Gs[c * KP + c];
-            const float hinv = Gs[KP * KP + c];                  // refined 1 / h (0 when h == 0)
-#pragma unroll
-            for (int p = 0; p < NP; ++p) {
-              const float pgx = (fv[c][p].x == 0.f) ? fminf(0.f, g[p].x) : g[p].x;
-              const float pgy = (fv[c][p].y == 0.f) ? fminf(0.f, g[p].y) : g[p].y;
-              sacc.x += fabsf(pgx);
-              sacc.y += fabsf(pgy);
-              if (h != 0.f) {                                    // block-uniform
-                float2 q = mul2(g[p], bcast2(hinv));             // g / h: quotient + residual correction
-                const float2 rem = fma2(bcast2(-h), q, g[p]);
-                q = fma2(bcast2(hinv), rem, q);
-                fv[c][p].x = fmaxf(fv[c][p].x - q.x, 0.f);
-                fv[c][p].y = fmaxf(fv[c][p].y - q.y, 0.f);
-              }
-              out[p] = fv[c][p];
-            }
+            out[p] = fv[c][p];
           }
           store_items<VEC>(pF, pH, pL, (unsigned)c * ld, out, pscale);
         } else {
@@ -1006,8 +980,8 @@ update_kernel(FactorView f, const float* __restrict__ NUM, int nsplit, long long
   const bool want_scal = out.scal_part != nullptr;
   double scal = 0.0;
   if constexpr (CD) {
-    CNMF_KP_SWITCH(K, KPMAX, (scal = update_body<KP, VEC, true, GRAM>(f, NUM, nsplit, sstride, G, K, o, l1, 0.f,
-                                                                       col_begin, col_end, tile, gsum)));
+    CNMF_KP_SWITCH(K, KPMAX, (scal = cd_body<KP, VEC, GRAM>(f, NUM, nsplit, sstride, G, K, o, l1, col_begin, col_end,
+                                                             tile, gsum)));
   } else {
     float* tileN = tile + UPD_TILE_F_FLOATS;
     CNMF_KP_SWITCH(K, KPMAX, (scal = mu_body<KP, VEC, GRAM, STREAMN>(f, NUM, nsplit, sstride, G, K, o, l1, l2, col_begin, col_end,

@@ -218,19 +218,72 @@ class Engine:
         check(self.lib.cnmf_dataset_dense_bytes(int(n_rows), int(n_cols), precision_code(precision), ctypes.byref(peak)))
         return int(peak.value)
 
-    def gemm_abt(self, A, B, precision=PRECISION_TF32X3, splits=1, reps=1):
-        """C = A @ B.T through the solver's GEMM kernels (test / micro-benchmark hook)."""
+    def gemm_abt(self, A, B, precision=PRECISION_TF32X3, splits=1, reps=1, b_exact=False, k_scale=None,
+                 out_col_scale=None):
+        """C = A @ B.T through the solver's GEMM kernels (test / micro-benchmark hook).  The exact-count forms:
+        b_exact (tf32x3; implied by f16x2) takes B as exact tf32 values, and then C = A diag(k_scale) B^T
+        diag(out_col_scale) with the scales applied where the solver applies a dataset's (either may be None)."""
         A, B = f32c(A), f32c(B)
         M, Kd = A.shape
         N = B.shape[0]
         assert B.shape[1] == Kd
+        ks = None if k_scale is None else f32c(k_scale)
+        cs = None if out_col_scale is None else f32c(out_col_scale)
+        assert ks is None or ks.shape == (Kd,)
+        assert cs is None or cs.shape == (N,)
         C = np.empty((M, N), np.float32)
         ms = ctypes.c_float(0)
         pc = precision_code(precision)
         pc = PRECISION_TF32X3 if pc == PRECISION_TF32X3_GENERAL else pc      # f16x2: B must hold integers <= 2048
-        check(self.lib.cnmf_gemm_abt_host(self._h, pc, ptr(A), ptr(B), M, N, Kd, splits,
-                                          ptr(C), reps, ctypes.byref(ms), None))
+        check(self.lib.cnmf_gemm_abt_host(self._h, pc, ptr(A), ptr(B), M, N, Kd, splits, 1 if b_exact else 0,
+                                          ptr(ks), ptr(cs), ptr(C), reps, ctypes.byref(ms), None))
         return C, float(ms.value)
+
+    def update_step(self, ks, rids, done, n, F, num, gram_in, solver="mu", pieces=None, gram=None, want_scalar=False,
+                    cpb_tiles=1, l1=0.0, l2=0.0, piece_scale=None, pieces_hi=None, pieces_lo=None, tile_scale=None,
+                    gram_out=None, scal_out=None):
+        """Test hook: one launch of the solver's update kernel (solver 'mu' / 'cd') or, with solver=None, the
+        stand-alone Gram / <NUM, F> / piece launches that start a solve, on packed host data (slot s holds restart
+        rids[s] with ks[s] components; F is (sum ks) x ld with ld = ceil(n / 32) * 32, num nsplit x (sum ks) x ld,
+        gram_in n_rids x 32 x 32 float64).  pieces: None | 'tf32' | 'f16'; gram: None | 'fused' | 'standalone'.
+        The optional in/out arrays (pieces, tile scales, Gram, scalar) are uploaded as given, so a caller can pre-fill
+        them with a sentinel; missing ones start as zeros.  Returns dict(F, hi, lo, tile_scale, gram, scal)."""
+        ks = np.ascontiguousarray(ks, np.int32)
+        rids = np.ascontiguousarray(rids, np.int32)
+        done = np.ascontiguousarray(done, np.int32)
+        F = f32c(F).copy()
+        SK, ld = F.shape
+        assert SK == int(ks.sum()) and ld == -(-int(n) // 32) * 32
+        num = f32c(num).reshape(-1, SK, ld) if num is not None else None
+        gram_in = np.ascontiguousarray(gram_in, np.float64)
+        n_rids = len(done)
+        assert gram_in.shape == (n_rids, 32, 32)
+        pmode = {None: _lib.UNIT_PIECES_NONE, "tf32": _lib.UNIT_PIECES_TF32, "f16": _lib.UNIT_PIECES_F16}[pieces]
+        gmode = {None: _lib.UNIT_GRAM_NONE, "fused": _lib.UNIT_GRAM_FUSED, "standalone": _lib.UNIT_GRAM_STANDALONE}[gram]
+        smode = {None: _lib.UNIT_SOLVER_NONE, "mu": SOLVER_MU, "cd": SOLVER_CD}[solver]
+        pdt = np.float16 if pieces == "f16" else np.float32
+        hi = lo = ts = None
+        if pieces is not None:
+            hi = np.zeros((SK, ld), pdt) if pieces_hi is None else np.ascontiguousarray(pieces_hi, pdt).copy()
+            lo = np.zeros((SK, ld), pdt) if pieces_lo is None else np.ascontiguousarray(pieces_lo, pdt).copy()
+        if pieces == "f16":
+            nt = (ld + 511) // 512
+            ts = np.zeros((SK, nt), np.float32) if tile_scale is None else f32c(tile_scale).copy()
+        g_out = np.zeros((n_rids, 32, 32)) if gram_out is None else np.ascontiguousarray(gram_out, np.float64).copy()
+        s_out = np.zeros(n_rids) if scal_out is None else np.ascontiguousarray(scal_out, np.float64).copy()
+        ps = None if piece_scale is None else f32c(piece_scale)
+        assert ps is None or ps.shape == (ld,)
+        a = _lib.UpdateStepArgs()
+        a.n_slots, a.n_rids, a.n, a.cpb_tiles = len(ks), n_rids, int(n), int(cpb_tiles)
+        a.ks, a.rids, a.done = ptr(ks), ptr(rids), ptr(done)
+        a.solver, a.pieces, a.gram, a.want_scalar = smode, pmode, gmode, 1 if want_scalar else 0
+        a.nsplit = 1 if num is None else num.shape[0]
+        a.l1, a.l2 = float(l1), float(l2)
+        a.F, a.num, a.gram_in, a.piece_scale = ptr(F), ptr(num), ptr(gram_in), ptr(ps)
+        a.pieces_hi, a.pieces_lo, a.tile_scale = ptr(hi), ptr(lo), ptr(ts)
+        a.gram_out, a.scal_out = ptr(g_out), ptr(s_out)
+        check(self.lib.cnmf_update_step_host(self._h, ctypes.byref(a), None))
+        return dict(F=F, hi=hi, lo=lo, tile_scale=ts, gram=g_out, scal=s_out)
 
 
 class Dataset:

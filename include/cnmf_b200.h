@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define CNMF_B200_ABI_VERSION 10
+#define CNMF_B200_ABI_VERSION 11
 #define CNMF_MAX_COMPONENTS 32          /* largest n_components per restart on the CUDA path */
 
 typedef struct cnmf_handle_s* cnmf_handle_t;
@@ -242,9 +242,52 @@ int cnmf_refit(cnmf_dataset_t d, int transposed, int k, const float* fixed_host,
 int cnmf_project_rows(cnmf_dataset_t d, int k, const float* Ut_host, float* out_host, void* stream);
 
 /* test / micro-benchmark hook: C (M x N) = A (M x Kd) * B (N x Kd)^T through the same GEMM kernels the
- * solver uses (precision selects FFMA or wgmma 3xTF32); reps > 1 reports mean device ms per launch. */
+ * solver uses (precision selects FFMA or wgmma 3xTF32); reps > 1 reports mean device ms per launch.
+ * The exact-count forms the solver runs on scaled-integer datasets: b_exact = 1 (tf32x3; implied by f16x2) takes B as
+ * exact tf32 values (2 passes, no lo piece of B); then k_scale (length Kd, or NULL) is folded into the A pieces as the
+ * solver folds the dataset's scale, A diag(k_scale), and out_col_scale (length N, or NULL) multiplies column n of C:
+ * C = A diag(k_scale) B^T diag(out_col_scale).  The scales are refused without the exact form. */
 int cnmf_gemm_abt_host(cnmf_handle_t h, int precision, const float* A, const float* B, int M, int N, int Kd,
-                       int splits, float* C, int reps, float* ms_out, void* stream);
+                       int splits, int b_exact, const float* k_scale, const float* out_col_scale, float* C, int reps,
+                       float* ms_out, void* stream);
+
+/* test hook: ONE update launch of the batched solver (or the stand-alone Gram / <NUM, F> / piece launches that start a
+ * solve) on host-supplied packed data, issued exactly as the solver issues it.  Slot s holds restart rids[s] with
+ * ks[s] components at packed rows [sum ks[0..s), +ks[s]); every per-restart output is indexed by rid.  Host arrays are
+ * dense row-major with the padded row stride ld = ceil(n / 32) * 32; every array marked in/out is uploaded before the
+ * launch and downloaded after it, so entries the launch must not touch can be pre-filled and checked. */
+enum { CNMF_UNIT_SOLVER_NONE = -1 };                               /* or CNMF_SOLVER_MU / CNMF_SOLVER_CD */
+enum { CNMF_UNIT_PIECES_NONE = 0, CNMF_UNIT_PIECES_TF32 = 1, CNMF_UNIT_PIECES_F16 = 2 };
+enum { CNMF_UNIT_GRAM_NONE = 0, CNMF_UNIT_GRAM_FUSED = 1, CNMF_UNIT_GRAM_STANDALONE = 2 };
+typedef struct cnmf_update_step_args {
+  int32_t n_slots;              /* restarts in the batch */
+  int32_t n_rids;               /* length of done / scal_out, and of gram_in / gram_out in 32 x 32 blocks */
+  const int32_t* ks;            /* [n_slots], 1..32; kp = 16 when every K <= 16, else 32 (as the solver decides) */
+  const int32_t* rids;          /* [n_slots], distinct, < n_rids */
+  const int32_t* done;          /* [n_rids] 1 = frozen restart: the launches skip it */
+  int32_t n;                    /* valid columns of the factor */
+  int32_t cpb_tiles;            /* columns per block of the update / cross launches, in update tiles: 1, 2 or 4 */
+  int32_t solver;               /* CNMF_SOLVER_MU / CNMF_SOLVER_CD: one update launch; CNMF_UNIT_SOLVER_NONE: no update
+                                 * (initial factors): stand-alone Gram, <NUM, F> and pieces of F as it stands */
+  int32_t pieces;               /* CNMF_UNIT_PIECES_*: tf32 hi / lo of F * piece_scale, or fp16 hi / mid + group scales */
+  int32_t gram;                 /* CNMF_UNIT_GRAM_*: Gram of the new F fused into the update (kp == 16 only), or the
+                                 * stand-alone gram_partial + finalize launches after it */
+  int32_t want_scalar;          /* MU: <NUM, F_new>; CD: sum |projected gradient|; NONE: <NUM, F> */
+  int32_t nsplit;               /* split-K slices of the product */
+  float l1, l2;
+  float* F;                     /* in/out: (sum ks) x ld */
+  const float* num;             /* nsplit x (sum ks) x ld */
+  const double* gram_in;        /* n_rids x 32 x 32: finalised Gram of the other factor */
+  const float* piece_scale;     /* ld, or NULL */
+  void* pieces_hi;              /* in/out (pieces != NONE): (sum ks) x ld floats (tf32) or fp16 halves (f16) */
+  void* pieces_lo;
+  float* tile_scale;            /* in/out (f16 pieces): (sum ks) x ceil(ld / 512) */
+  double* gram_out;             /* in/out (gram != NONE): n_rids x 32 x 32 */
+  double* scal_out;             /* in/out (want_scalar): n_rids */
+} cnmf_update_step_args;
+/* The last-block tickets of the fused launches are zeroed once per handle, when first allocated: a second call relies
+ * on the kernel's own reset. */
+int cnmf_update_step_host(cnmf_handle_t h, const cnmf_update_step_args* args, void* stream);
 
 /* ---- consensus kernels (cnmf.py:882-916) on a stacked-spectra matrix S (R x G, device, row stride ld) -- */
 /* rows / ||row||_2 in place (cnmf.py:882) */

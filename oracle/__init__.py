@@ -26,6 +26,8 @@ Modules
   make_golden.py    script that generated tests/golden/ (committed with the fixtures)
   nmf_ref.py        numpy restatement of sklearn's MU / CD NMF solvers + random init
   consensus_ref.py  numpy restatement of cNMF.consensus numerics
+  kernel_ref.py     float64 references of one update launch (MU half-step, CD sweep) and bit-exact
+                    restatements of the GEMM operand pieces (tf32 split, fp16 group scale and pieces)
   reference_path.py the reference's factorize/consensus call sequence on sklearn
                     (runs anywhere scikit-learn is installed)
 """

@@ -1,0 +1,106 @@
+"""ORACLE (test infrastructure) -- float64 references of ONE launch of the batched solver's kernels
+(cnmf_b200/csrc/nmf_kernels.cu) and bit-exact numpy restatements of the operand pieces the GEMM reads.
+
+Layout as in the kernels: a factor is K x n (components x items); `num` is the product the update divides by
+(X H^T for W, W^T X for H) summed over its split-K slices; `G` is the K x K Gram of the other factor.  The update
+references take the fp32 inputs the kernel takes: G already rounded to fp32 (load_gram_smem), everything else exact.
+Pinned to scikit-learn's own update functions by tests/test_oracle_golden.py.
+"""
+import numpy as np
+
+EPSILON = float(np.finfo(np.float32).eps)      # SK/decomposition/_nmf.py:32
+FLT_MIN = float(np.finfo(np.float32).tiny)
+
+
+def gram_fp32(gram_in, K, diag_add=0.0):
+    """The K x K Gram as the update kernel holds it in shared memory (load_gram_smem): each fp64 entry rounded to fp32,
+    then `diag_add` (CD: l2) added to the diagonal in fp32.  Returned as float64 holding those fp32 values."""
+    G = np.asarray(gram_in, np.float64)[:K, :K].astype(np.float32)
+    if diag_add:
+        idx = np.arange(K)
+        G[idx, idx] = G[idx, idx] + np.float32(diag_add)
+    return G.astype(np.float64)
+
+
+def mu_half_step(F, num, G, l1=0.0, l2=0.0):
+    """One multiplicative update of F (SK/decomposition/_nmf.py:535-549,610-624 for W; :633-635,696-721 for H), float64:
+        den = G F + l1 + l2 F;   den < FLT_MIN -> float32 eps;   F_new = F * num / den.
+    The floor is the kernel's rule (its Newton quotient needs a normal denominator); scikit-learn maps only exact
+    zeros to eps, which is the same for every denominator a test builds."""
+    F = np.asarray(F, np.float64)
+    den = G @ F + l1 + l2 * F
+    den = np.where(den < FLT_MIN, EPSILON, den)
+    return F * np.asarray(num, np.float64) / den
+
+
+def cd_sweep(F, num, G, l1=0.0, l2=0.0, jacobi=False):
+    """One coordinate-descent sweep over the K coordinates of every item (SK/decomposition/_cdnmf_fast.pyx:8-37 with
+    shuffle=False; l1 subtracted from the product and l2 added to the Gram diagonal, SK/decomposition/_nmf.py:
+    379-385), float64.  G must be the Gram WITHOUT l2 (gram_fp32(..., diag_add=l2) gives the kernel's form; pass
+    l2=0 then).  Returns (F_new, violation, magnitude): violation = sum |projected gradient| over items and
+    coordinates, magnitude[t, j] = |num - l1| + sum_r |G[t, r] F[r, j]| of each gradient (what its rounding error
+    scales with).  jacobi=True evaluates every gradient from the OLD F (a wrong order, for tests that must tell
+    Gauss-Seidel from it)."""
+    F = np.array(F, np.float64)
+    num = np.asarray(num, np.float64)
+    G = np.asarray(G, np.float64) + l2 * np.eye(len(G))
+    K = F.shape[0]
+    F0 = F.copy()
+    viol = 0.0
+    mag = np.zeros_like(F)
+    for t in range(K):
+        src = F0 if jacobi else F
+        grad = l1 - num[t] + G[t] @ src
+        mag[t] = np.abs(l1 - num[t]) + np.abs(G[t]) @ np.abs(src)
+        pg = np.where(src[t] == 0.0, np.minimum(0.0, grad), grad)
+        viol += float(np.abs(pg).sum())
+        h = G[t, t]
+        if h != 0.0:
+            F[t] = np.maximum(src[t] - grad / h, 0.0)
+    return F, viol, mag
+
+
+# ---------------------------------------------------------------------------------------- operand pieces
+def to_tf32(x):
+    """cvt.rna.tf32.f32 on finite fp32 values (to_tf32 of common.cuh): add half an ulp of tf32, clear 13 bits."""
+    u = np.ascontiguousarray(x, np.float32).view(np.uint32)
+    return ((u + np.uint32(0x1000)) & np.uint32(0xffffe000)).view(np.float32)
+
+
+def tf32_pieces(F, scale=None):
+    """(hi, lo) tf32 pieces of F * scale (fp32 product), as split_scaled_kernel and the update kernels' store_items
+    write them: hi = tf32(x), lo = tf32(x - hi)."""
+    x = np.ascontiguousarray(F, np.float32)
+    if scale is not None:
+        x = x * np.asarray(scale, np.float32)
+    hi = to_tf32(x)
+    lo = to_tf32(x - hi)
+    return hi, lo
+
+
+def f16_group_scale(m):
+    """f16_group_scale of common.cuh: the power of two 2^max(e - 15, -126) for a group maximum m = f 2^e (f in
+    [0.5, 1)), which puts m in [2^14, 2^15); 1 for m = 0 or m >= 3e38.  Maxima below 2^-111 get the floor 2^-126."""
+    m = np.ascontiguousarray(m, np.float32)
+    b = (m.view(np.uint32) >> np.uint32(23)).astype(np.int64)
+    sc = (np.maximum(b - 14, 1).astype(np.uint32) << np.uint32(23)).view(np.float32)
+    return np.where((m > 0) & (m < np.float32(3.0e38)), sc, np.float32(1.0)).astype(np.float32)
+
+
+def f16_pieces(F, scale=None, group=512):
+    """fp16 pieces of the rows of F * scale (fp32 product) as emit_f16_kernel / emit_tile_f16 write them: per row and
+    group of `group` columns sc = f16_group_scale(max |x|), hi = fp16(x / sc), mid = fp16(x / sc - hi) (division by a
+    power of two is exact).  F is rows x ld, ld the padded row stride.  Returns (hi, mid, tile_scale)."""
+    x = np.ascontiguousarray(F, np.float32)
+    if scale is not None:
+        x = x * np.asarray(scale, np.float32)
+    rows, ld = x.shape
+    nt = (ld + group - 1) // group
+    pad = np.zeros((rows, nt * group), np.float32)
+    pad[:, :ld] = x
+    m = np.abs(pad).reshape(rows, nt, group).max(axis=2)
+    ts = f16_group_scale(m)
+    y = (pad.reshape(rows, nt, group) / ts[:, :, None]).reshape(rows, nt * group)[:, :ld].astype(np.float32)
+    hi = y.astype(np.float16)
+    mid = (y - hi.astype(np.float32)).astype(np.float16)
+    return hi, mid, ts

@@ -234,26 +234,34 @@ def test_precision_names_and_hvg_ranking_from_stats():
 
 
 def test_fp16_two_piece_split_bounds():
-    """The operand representation of the default precision, restated in numpy (what emit_f16_kernel / emit_tile_f16
-    compute): a row divided by the power of two that puts its maximum in [2^14, 2^15), then hi = fp16(x),
-    mid = fp16(x - hi).  Entries down to 2^-18 of the row maximum keep >= 21 significant bits like a tf32 pair; smaller
-    ones are off by at most 2^-39 of the row maximum; integer counts <= 2048 are exact in fp16."""
+    """The operand representation of the default precision, restated in numpy (oracle/kernel_ref.f16_pieces, what
+    emit_f16_kernel / emit_tile_f16 compute): each 512-column group of a row divided by the power of two that puts the
+    group maximum in [2^14, 2^15), then hi = fp16(x), mid = fp16(x - hi).  Entries down to 2^-18 of the group maximum
+    keep >= 21 significant bits like a tf32 pair; smaller ones are off by at most 2^-39 of the group maximum; groups
+    below 2^-111 keep the floor scale 2^-126; integer counts <= 2048 are exact in fp16."""
+    from oracle.kernel_ref import f16_group_scale, f16_pieces
     rng = np.random.RandomState(0)
-    A = (np.abs(rng.standard_cauchy((64, 4096))) * 10.0 ** rng.uniform(-8, 8, size=(64, 1))).astype(np.float32).astype(np.float64)
-    A[:, ::11] = 0.0
-    rowmax = A.max(axis=1, keepdims=True)
-    mant, exp = np.frexp(rowmax)                       # rowmax = mant * 2^exp, mant in [0.5, 1)
-    sc = np.ldexp(1.0, exp - 15)
+    A32 = (np.abs(rng.standard_cauchy((64, 4096))) * 10.0 ** rng.uniform(-8, 8, size=(64, 1))).astype(np.float32)
+    A32[:, ::11] = 0.0
+    A32[:, 512:1024] *= np.float32(2.0 ** -40)         # neighbouring groups 2^40 apart: a scale per group, not per row
+    A = A32.astype(np.float64)
+    h16, m16, ts = f16_pieces(A32)
+    sc = np.repeat(ts, 512, axis=1).astype(np.float64)
+    gmax = np.repeat(A.reshape(64, 8, 512).max(axis=2), 512, axis=1)
     x = A / sc
-    assert x.max() < 2 ** 15 and (x.max(axis=1) >= 2 ** 14).all()
-    hi = x.astype(np.float16).astype(np.float64)
-    mid = (x - hi).astype(np.float16).astype(np.float64)
+    assert x.max() < 2 ** 15 and (x.reshape(64, 8, 512).max(axis=2) >= 2 ** 14).all()
+    hi = h16.astype(np.float64)
+    mid = m16.astype(np.float64)
+    assert np.array_equal(hi, x.astype(np.float16).astype(np.float64))      # the restatement is the plain formula
     assert np.isfinite(hi).all() and np.isfinite(mid).all()
     err = np.abs((hi + mid) * sc - A)
     big = x >= 2.0 ** -3                               # both pieces normal fp16 numbers
     assert (err[big] <= A[big] * 2.0 ** -21).all()     # two 11-bit pieces
     assert ((err / sc)[~big] <= 2.0 ** -25).all()      # subnormal `mid`: half an fp16 subnormal step, in scaled units ...
-    assert ((err / rowmax)[~big] <= 2.0 ** -39).all()  # ... which is 2^-39 of a row maximum >= 2^14
+    assert ((err / gmax)[~big] <= 2.0 ** -39).all()    # ... which is 2^-39 of a group maximum >= 2^14
+    # the floor: maxima at and below 2^-111 keep 2^-126 (1 / scale finite), above it the exponent follows the maximum
+    m = np.float32([2.0 ** -111, np.nextafter(np.float32(2.0 ** -111), np.float32(0)), 2.0 ** -130, 1e-45, 0.0, 1.0])
+    assert f16_group_scale(m).tolist() == [2.0 ** -125, 2.0 ** -126, 2.0 ** -126, 2.0 ** -126, 1.0, 2.0 ** -14]
     C = np.arange(0, 2049, dtype=np.float64)
     assert np.array_equal(C.astype(np.float16).astype(np.float64), C)
     # a product against integer counts: same error class as the tf32 pair

@@ -114,3 +114,33 @@ def test_stats_branch_matches_reference(golden):
         # (init='nndsvd': intra-cluster distances are ~1e-8 cancellation noise, so the silhouette is 1 - noise)
         assert abs(consensus_ref.silhouette(l2, labels) - stats[2]) < (1e-9 if golden["init"] == "random" else 1e-7)
         assert abs(err - stats[3]) / stats[3] < 1e-9
+
+
+@pytest.mark.parametrize("l1,l2", [(0.0, 0.0), (0.3, 0.0), (0.0, 0.7), (0.25, 1.5)])
+def test_kernel_step_references_match_sklearn(l1, l2):
+    """oracle/kernel_ref.py's one-launch references -- what tests/test_kernel_units.py holds the update kernels to --
+    against scikit-learn's own update functions in float64 (MU: _multiplicative_update_w; CD:
+    _update_coordinate_descent with shuffle=False), in the kernels' layout F = W^T, num = (X H^T)^T, G = H H^T."""
+    from sklearn.decomposition import _nmf
+    from oracle import kernel_ref
+    rng = np.random.RandomState(int(10 * l1 + 100 * l2))
+    n, g, K = 60, 45, 7
+    X = np.abs(rng.randn(n, g))
+    W = np.abs(rng.randn(n, K))
+    W[::5, 2] = 0.0                     # zero coordinates: the projected gradient's min(0, g) branch
+    H = np.abs(rng.randn(K, g))
+    num, G = (X @ H.T).T, H @ H.T
+    Wm, *_ = _nmf._multiplicative_update_w(X, W.copy(), H, 2, l1, l2, 1.0)
+    assert np.allclose(kernel_ref.mu_half_step(W.T, num, G, l1, l2), Wm.T, rtol=1e-13, atol=0)
+    Wc = W.copy()
+    viol = _nmf._update_coordinate_descent(X, Wc, H.T, l1, l2, False, None)
+    Fc, v, mag = kernel_ref.cd_sweep(W.T, num, G, l1, l2)
+    assert np.allclose(Fc, Wc.T, rtol=1e-12, atol=1e-13) and abs(v - viol) <= 1e-12 * viol
+    assert (mag >= 0).all()
+    Fj, _, _ = kernel_ref.cd_sweep(W.T, num, G, l1, l2, jacobi=True)
+    assert np.abs(Fj - Fc).max() > 1e-3                 # the coupling is strong enough to tell the orders apart
+    # the kernel's denominator floor: below FLT_MIN -> eps, exactly as sklearn's den == 0 -> eps on a zero row
+    G0 = G.copy()
+    G0[3] = 0.0
+    ref = kernel_ref.mu_half_step(W.T, num, G0, 0.0, 0.0)
+    assert np.allclose(ref[3], W.T[3] * num[3] / kernel_ref.EPSILON, rtol=1e-15)
