@@ -27,12 +27,6 @@ void set_last_error(const std::string& msg) { g_last_error = msg; }
 
 using namespace cnmf;
 
-#define CNMF_TRY(expr)            \
-  do {                            \
-    int _rc = (expr);             \
-    if (_rc != 0) return _rc;     \
-  } while (0)
-
 // ----------------------------------------------------------------------------- handle
 void* cnmf_handle_s::dev_buf(const std::string& name, size_t bytes) {
   auto& e = ws[name];
@@ -171,13 +165,6 @@ int cnmf_create(cnmf_handle_t* out, int device) {
   auto* h = new cnmf_handle_s();
   h->device = device;
   h->sm_count = prop.multiProcessorCount;
-  {
-    int lo = 0, hi = 0;
-    cudaDeviceGetStreamPriorityRange(&lo, &hi);      // lo = lowest priority (numerically largest)
-    if (cudaStreamCreateWithPriority(&h->aux, cudaStreamNonBlocking, lo) != cudaSuccess) h->aux = nullptr;
-    if (cudaEventCreateWithFlags(&h->ev_upd, cudaEventDisableTiming) != cudaSuccess) h->ev_upd = nullptr;
-    if (cudaEventCreateWithFlags(&h->ev_gram, cudaEventDisableTiming) != cudaSuccess) h->ev_gram = nullptr;
-  }
   *out = h;
   return 0;
 }
@@ -185,9 +172,6 @@ int cnmf_create(cnmf_handle_t* out, int device) {
 int cnmf_destroy(cnmf_handle_t h) {
   if (!h) return 0;
   cudaSetDevice(h->device);
-  if (h->aux) cudaStreamDestroy(h->aux);
-  if (h->ev_upd) cudaEventDestroy(h->ev_upd);
-  if (h->ev_gram) cudaEventDestroy(h->ev_gram);
   h->release_all();
   delete h;
   return 0;
@@ -210,7 +194,7 @@ int cnmf_mem_info(cnmf_handle_t h, long long* free_bytes, long long* total_bytes
 
 long long cnmf_solve_bytes_per_row(cnmf_dataset_t d) {
   if (!d) return 0;
-  // nmf_engine.cu / alloc_factors: Fr + 2 piece buffers, their 3 compaction alternates, the result slab and the
+  // factorize / solve_batched: Fr + 2 piece buffers, their 3 compaction alternates, the result slab and the
   // product NUM_r along the cells; the same along the genes with one product slice per split-K slice
   const long long splits_c = gemm_fixed_splits(d->n_rows, d->f16 ? 1 : 0);
   const long long splits_r = gemm_fixed_splits(d->n_cols, d->f16 ? 1 : 0);
@@ -469,22 +453,25 @@ int cnmf_random_init_host(uint32_t seed, double avg, int n_samples, int n_featur
 // ----------------------------------------------------------------------------- factorize
 namespace {
 
-struct FactorBuffers {
-  float *Fr, *Fr_hi, *Fr_lo, *Fc, *Fc_hi, *Fc_lo;
+using clk = std::chrono::steady_clock;
+double ms_since(clk::time_point t0) { return std::chrono::duration<double, std::milli>(clk::now() - t0).count(); }
+
+// the restarts of one batched solve: n_components and first packed row of each, and the packed factors
+// (Fr = W^T rows, SK x ld_r; Fc = H rows, SK x ld_c)
+struct Batch {
+  std::vector<int> ks, off;
+  int SK = 0;
+  float *Fr = nullptr, *Fc = nullptr;
 };
 
-int alloc_factors(cnmf_handle_s* h, int SK, int ld_r, int ld_c, bool tf32, FactorBuffers* fb) {
-  const size_t nr = (size_t)SK * ld_r, nc = (size_t)SK * ld_c;
-  fb->Fr = static_cast<float*>(h->dev_buf("fac.Fr", nr * 4));
-  fb->Fc = static_cast<float*>(h->dev_buf("fac.Fc", nc * 4));
-  fb->Fr_hi = fb->Fr_lo = fb->Fc_hi = fb->Fc_lo = nullptr;
-  if (!fb->Fr || !fb->Fc) return -2;
-  if (tf32) {
-    fb->Fr_hi = static_cast<float*>(h->dev_buf("fac.Fr_hi", nr * 4));
-    fb->Fr_lo = static_cast<float*>(h->dev_buf("fac.Fr_lo", nr * 4));
-    fb->Fc_hi = static_cast<float*>(h->dev_buf("fac.Fc_hi", nc * 4));
-    fb->Fc_lo = static_cast<float*>(h->dev_buf("fac.Fc_lo", nc * 4));
-    if (!fb->Fr_hi || !fb->Fr_lo || !fb->Fc_hi || !fb->Fc_lo) return -2;
+int pack_restarts(int n_restarts, const int32_t* ks_in, const std::string& what, Batch* b) {
+  b->ks.assign(ks_in, ks_in + n_restarts);
+  b->off.resize(n_restarts);
+  b->SK = 0;
+  for (int r = 0; r < n_restarts; ++r) {
+    CNMF_REQUIRE(b->ks[r] >= 1 && b->ks[r] <= KMAX, what + ": n_components must be in [1, 32] on the CUDA path");
+    b->off[r] = b->SK;
+    b->SK += b->ks[r];
   }
   return 0;
 }
@@ -511,46 +498,6 @@ void parallel_for(int n, const std::function<void(int)>& fn) {
   for (auto& t : th) t.join();
 }
 
-// shared tail of cnmf_factorize / cnmf_factorize_init: factors already in fb.Fr / fb.Fc (full fp32)
-int run_and_download(cnmf_dataset_s* d, const std::vector<int>& ks, int SK, FactorBuffers& fb,
-                     const cnmf_nmf_params& p, float* spectra_host, float* usages_host, int32_t* n_iter_host,
-                     double* err_host, cudaStream_t s, float* spectra_dev = nullptr, long long ld_dev = 0) {
-  cnmf_handle_s* h = d->h;
-  const bool tf32 = p.precision == CNMF_PRECISION_TF32X3;
-  DataView v = make_view(d, false);
-  if (tf32 && !v.f16) {      // f16 datasets: the solver emits fp16 pieces itself; tf32 pieces would be dead work
-    CNMF_TRY(launch_split_scaled(fb.Fr, fb.Fr_hi, fb.Fr_lo, SK, d->ld_r, v.exact ? v.scale_r : nullptr, s));
-    CNMF_TRY(launch_split_scaled(fb.Fc, fb.Fc_hi, fb.Fc_lo, SK, d->ld_c, v.exact ? v.scale_c : nullptr, s));
-    h->launches += 2;
-  }
-  SolveIO io;
-  io.R = (int)ks.size();
-  io.ks = ks;
-  io.Fr = fb.Fr; io.Fr_hi = fb.Fr_hi; io.Fr_lo = fb.Fr_lo;
-  io.Fc = fb.Fc; io.Fc_hi = fb.Fc_hi; io.Fc_lo = fb.Fc_lo;
-  io.update_cols = true;
-  auto t_solve = std::chrono::steady_clock::now();
-  CNMF_TRY(solve_batched(h, v, io, p, s));
-  h->t_solve_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_solve).count();
-  auto t_d2h = std::chrono::steady_clock::now();
-  if (spectra_dev)      // result stays in HBM (multi-GPU path: the slab goes straight into the NCCL all-gather)
-    CNMF_CUDA_CHECK(cudaMemcpy2DAsync(spectra_dev, (size_t)ld_dev * 4, fb.Fc, (size_t)d->ld_c * 4,
-                                      (size_t)d->n_cols * 4, SK, cudaMemcpyDeviceToDevice, s));
-  if (spectra_host)
-    CNMF_CUDA_CHECK(cudaMemcpy2DAsync(spectra_host, (size_t)d->n_cols * 4, fb.Fc, (size_t)d->ld_c * 4,
-                                      (size_t)d->n_cols * 4, SK, cudaMemcpyDeviceToHost, s));
-  if (usages_host)
-    CNMF_CUDA_CHECK(cudaMemcpy2DAsync(usages_host, (size_t)d->n_rows * 4, fb.Fr, (size_t)d->ld_r * 4,
-                                      (size_t)d->n_rows * 4, SK, cudaMemcpyDeviceToHost, s));
-  CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
-  h->t_d2h_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_d2h).count();
-  for (size_t r = 0; r < ks.size(); ++r) {
-    if (n_iter_host) n_iter_host[r] = io.n_iter[r];
-    if (err_host) err_host[r] = io.err[r];
-  }
-  return 0;
-}
-
 int check_params(cnmf_dataset_s* d, const cnmf_nmf_params* p) {
   CNMF_REQUIRE(d && p, "NULL dataset or params");
   CNMF_REQUIRE(p->precision == d->precision, "params.precision must match the precision the dataset was created with");
@@ -560,53 +507,42 @@ int check_params(cnmf_dataset_s* d, const cnmf_nmf_params* p) {
   return 0;
 }
 
-}  // namespace
-
-static int factorize_impl(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, const uint32_t* seeds,
-                          const cnmf_nmf_params* p, float* spectra_host, float* usages_host, int32_t* n_iter_host,
-                          double* err_host, void* stream, float* spectra_dev, long long ld_dev) {
+// start of every factorize entry point: parameters and arguments checked (args_ok: the entry point's own pointers),
+// restarts packed, factor buffers allocated on the handle's device, phase timings reset
+int begin_factorize(cnmf_dataset_s* d, const cnmf_nmf_params* p, int n_restarts, const int32_t* ks_in, bool args_ok,
+                    const std::string& what, Batch* b) {
   CNMF_TRY(check_params(d, p));
-  CNMF_REQUIRE(n_restarts > 0 && ks_in && seeds && (spectra_host || spectra_dev), "factorize: bad arguments");
-  CNMF_REQUIRE(!spectra_dev || ld_dev >= d->n_cols, "factorize: device output row stride too small");
+  CNMF_REQUIRE(args_ok && n_restarts > 0 && ks_in, what + ": bad arguments");
+  CNMF_TRY(pack_restarts(n_restarts, ks_in, what, b));
   cnmf_handle_s* h = d->h;
-  cudaStream_t s = as_stream(stream);
   CNMF_CUDA_CHECK(cudaSetDevice(h->device));
-  std::vector<int> ks(ks_in, ks_in + n_restarts), off(n_restarts);
-  int SK = 0;
-  for (int r = 0; r < n_restarts; ++r) {
-    CNMF_REQUIRE(ks[r] >= 1 && ks[r] <= KMAX, "factorize: n_components must be in [1, 32] on the CUDA path");
-    off[r] = SK;
-    SK += ks[r];
-  }
-  FactorBuffers fb;
-  CNMF_TRY(alloc_factors(h, SK, d->ld_r, d->ld_c, p->precision == CNMF_PRECISION_TF32X3, &fb));
-
-  using clk = std::chrono::steady_clock;
-  auto ms_since = [](clk::time_point t0) { return std::chrono::duration<double, std::milli>(clk::now() - t0).count(); };
+  b->Fr = static_cast<float*>(h->dev_buf("fac.Fr", (size_t)b->SK * d->ld_r * 4));
+  b->Fc = static_cast<float*>(h->dev_buf("fac.Fc", (size_t)b->SK * d->ld_c * 4));
+  if (!b->Fr || !b->Fc) return -2;
   h->t_rng_ms = h->t_h2d_ms = h->t_solve_ms = h->t_d2h_ms = 0;
-  const int init = (p->reserved >> 1) & 3;
-  if (init != CNMF_INIT_RANDOM) {
-    auto t_init = clk::now();
-    CNMF_TRY(nndsvd_starts_dev(d, n_restarts, ks.data(), seeds, init, fb.Fr, fb.Fc, s));
-    h->t_rng_ms = ms_since(t_init);
-    return run_and_download(d, ks, SK, fb, *p, spectra_host, usages_host, n_iter_host, err_host, s, spectra_dev, ld_dev);
-  }
-  if ((p->reserved & 1) == 0) {
-    // ---- device RNG (default): the same legacy MT19937 / polar-gauss stream, generated in place on the GPU
-    auto t_rng = clk::now();
-    const double mean_d = d->sum / ((double)d->n_rows * (double)d->n_cols);
-    std::vector<double> avgs(n_restarts);
-    for (int r = 0; r < n_restarts; ++r) avgs[r] = std::sqrt(mean_d / ks[r]);
-    CNMF_CUDA_CHECK(cudaMemsetAsync(fb.Fr, 0, (size_t)SK * d->ld_r * 4, s));
-    CNMF_CUDA_CHECK(cudaMemsetAsync(fb.Fc, 0, (size_t)SK * d->ld_c * 4, s));
-    CNMF_TRY(launch_rng_init(seeds, ks.data(), off.data(), avgs.data(), n_restarts, d->n_rows, d->n_cols, fb.Fr, d->ld_r,
-                             fb.Fc, d->ld_c, h, s));
-    // no host synchronisation here: launch_rng_init stages its arguments itself, and the solve is enqueued behind
-    // the generator on the same stream (t_rng_ms = enqueue time; the kernel's time is part of t_solve_ms)
-    h->t_rng_ms = ms_since(t_rng);
-    return run_and_download(d, ks, SK, fb, *p, spectra_host, usages_host, n_iter_host, err_host, s, spectra_dev, ld_dev);
-  }
-  // host RNG (bit-exact numpy legacy stream) in groups through a pinned staging buffer
+  return 0;
+}
+
+// sklearn's random starts of every restart (the legacy MT19937 / polar-gauss stream), generated in place on the device
+// into packed, padded Wt / H.  No host synchronisation: launch_rng_init stages its arguments itself.
+int rng_starts_dev(cnmf_dataset_s* d, const Batch& b, const uint32_t* seeds, float* Wt, float* H, cudaStream_t s) {
+  const int R = (int)b.ks.size();
+  const double mean = d->sum / ((double)d->n_rows * (double)d->n_cols);
+  std::vector<double> avgs(R);
+  for (int r = 0; r < R; ++r) avgs[r] = std::sqrt(mean / b.ks[r]);
+  CNMF_CUDA_CHECK(cudaMemsetAsync(Wt, 0, (size_t)b.SK * d->ld_r * 4, s));
+  CNMF_CUDA_CHECK(cudaMemsetAsync(H, 0, (size_t)b.SK * d->ld_c * 4, s));
+  return launch_rng_init(seeds, b.ks.data(), b.off.data(), avgs.data(), R, d->n_rows, d->n_cols, Wt, d->ld_r, H, d->ld_c,
+                         d->h, s);
+}
+
+// the same starts drawn on the host (bit-exact numpy legacy stream) into b.Fr / b.Fc, in groups through a pinned
+// staging buffer
+int rng_starts_host(cnmf_dataset_s* d, const Batch& b, const uint32_t* seeds, cudaStream_t s) {
+  cnmf_handle_s* h = d->h;
+  const std::vector<int>& ks = b.ks;
+  const std::vector<int>& off = b.off;
+  const int n_restarts = (int)ks.size();
   const double mean = d->sum / ((double)d->n_rows * (double)d->n_cols);
   const size_t group_budget = (size_t)256 << 20;   // bytes of W^T staged per group
   int r0 = 0;
@@ -635,15 +571,75 @@ static int factorize_impl(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in
     });
     h->t_rng_ms += ms_since(t_rng);
     auto t_h2d = clk::now();
-    CNMF_CUDA_CHECK(cudaMemcpyAsync(fb.Fr + (size_t)off[r0] * d->ld_r, stW, (size_t)rows * d->ld_r * 4,
+    CNMF_CUDA_CHECK(cudaMemcpyAsync(b.Fr + (size_t)off[r0] * d->ld_r, stW, (size_t)rows * d->ld_r * 4,
                                     cudaMemcpyHostToDevice, s));
-    CNMF_CUDA_CHECK(cudaMemcpyAsync(fb.Fc + (size_t)off[r0] * d->ld_c, stH, (size_t)rows * d->ld_c * 4,
+    CNMF_CUDA_CHECK(cudaMemcpyAsync(b.Fc + (size_t)off[r0] * d->ld_c, stH, (size_t)rows * d->ld_c * 4,
                                     cudaMemcpyHostToDevice, s));
     CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
     h->t_h2d_ms += ms_since(t_h2d);
     r0 = r1;
   }
-  return run_and_download(d, ks, SK, fb, *p, spectra_host, usages_host, n_iter_host, err_host, s, spectra_dev, ld_dev);
+  return 0;
+}
+
+// end of every factorize entry point: the solve from the starts in b.Fr / b.Fc (full fp32), then its results out.
+// Null outputs are skipped; spectra_dev gets SK rows of dev_cols floats at row stride ld_dev.
+int solve_and_copy_out(cnmf_dataset_s* d, const Batch& b, const cnmf_nmf_params& p, float* spectra_host,
+                       float* usages_host, float* spectra_dev, long long ld_dev, int dev_cols, int32_t* n_iter_host,
+                       double* err_host, cudaStream_t s) {
+  cnmf_handle_s* h = d->h;
+  SolveIO io;
+  io.R = (int)b.ks.size();
+  io.ks = b.ks;
+  io.Fr = b.Fr;
+  io.Fc = b.Fc;
+  io.update_cols = true;
+  auto t_solve = clk::now();
+  CNMF_TRY(solve_batched(h, make_view(d, false), io, p, s));
+  h->t_solve_ms = ms_since(t_solve);
+  auto t_d2h = clk::now();
+  if (spectra_dev)      // result stays in HBM (multi-GPU path: the slab goes straight into the NCCL all-gather)
+    CNMF_CUDA_CHECK(cudaMemcpy2DAsync(spectra_dev, (size_t)ld_dev * 4, b.Fc, (size_t)d->ld_c * 4, (size_t)dev_cols * 4,
+                                      b.SK, cudaMemcpyDeviceToDevice, s));
+  if (spectra_host)
+    CNMF_CUDA_CHECK(cudaMemcpy2DAsync(spectra_host, (size_t)d->n_cols * 4, b.Fc, (size_t)d->ld_c * 4,
+                                      (size_t)d->n_cols * 4, b.SK, cudaMemcpyDeviceToHost, s));
+  if (usages_host)
+    CNMF_CUDA_CHECK(cudaMemcpy2DAsync(usages_host, (size_t)d->n_rows * 4, b.Fr, (size_t)d->ld_r * 4,
+                                      (size_t)d->n_rows * 4, b.SK, cudaMemcpyDeviceToHost, s));
+  CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
+  h->t_d2h_ms = ms_since(t_d2h);
+  for (int r = 0; r < io.R; ++r) {
+    if (n_iter_host) n_iter_host[r] = io.n_iter[r];
+    if (err_host) err_host[r] = io.err[r];
+  }
+  return 0;
+}
+
+}  // namespace
+
+static int factorize_impl(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, const uint32_t* seeds,
+                          const cnmf_nmf_params* p, float* spectra_host, float* usages_host, int32_t* n_iter_host,
+                          double* err_host, void* stream, float* spectra_dev, long long ld_dev) {
+  Batch b;
+  CNMF_TRY(begin_factorize(d, p, n_restarts, ks_in, seeds && (spectra_host || spectra_dev), "factorize", &b));
+  CNMF_REQUIRE(!spectra_dev || ld_dev >= d->n_cols, "factorize: device output row stride too small");
+  cudaStream_t s = as_stream(stream);
+  const int init = (p->reserved >> 1) & 3;
+  auto t_init = clk::now();
+  if (init != CNMF_INIT_RANDOM) {
+    CNMF_TRY(nndsvd_starts_dev(d, n_restarts, b.ks.data(), seeds, init, b.Fr, b.Fc, s));
+    d->h->t_rng_ms = ms_since(t_init);
+  } else if ((p->reserved & 1) == 0) {
+    // device RNG (default): the solve is enqueued behind the generator on the same stream (t_rng_ms = enqueue time;
+    // the kernel's time is part of t_solve_ms)
+    CNMF_TRY(rng_starts_dev(d, b, seeds, b.Fr, b.Fc, s));
+    d->h->t_rng_ms = ms_since(t_init);
+  } else {
+    CNMF_TRY(rng_starts_host(d, b, seeds, s));
+  }
+  return solve_and_copy_out(d, b, *p, spectra_host, usages_host, spectra_dev, ld_dev, d->n_cols, n_iter_host, err_host,
+                            s);
 }
 
 int cnmf_factorize(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, const uint32_t* seeds,
@@ -672,90 +668,42 @@ int cnmf_last_timing(cnmf_handle_t h, double* rng_ms, double* h2d_ms, double* so
 int cnmf_factorize_init(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, const float* Wt0_host,
                         const float* H0_host, const cnmf_nmf_params* p, float* spectra_host, float* usages_host,
                         int32_t* n_iter_host, double* err_host, void* stream) {
-  CNMF_TRY(check_params(d, p));
-  CNMF_REQUIRE(n_restarts > 0 && ks_in && Wt0_host && H0_host && spectra_host, "factorize_init: bad arguments");
-  cnmf_handle_s* h = d->h;
+  Batch b;
+  CNMF_TRY(begin_factorize(d, p, n_restarts, ks_in, Wt0_host && H0_host && spectra_host, "factorize_init", &b));
   cudaStream_t s = as_stream(stream);
-  CNMF_CUDA_CHECK(cudaSetDevice(h->device));
-  std::vector<int> ks(ks_in, ks_in + n_restarts);
-  int SK = 0;
-  for (int r = 0; r < n_restarts; ++r) {
-    CNMF_REQUIRE(ks[r] >= 1 && ks[r] <= KMAX, "factorize_init: n_components must be in [1, 32] on the CUDA path");
-    SK += ks[r];
-  }
-  FactorBuffers fb;
-  CNMF_TRY(alloc_factors(h, SK, d->ld_r, d->ld_c, p->precision == CNMF_PRECISION_TF32X3, &fb));
-  CNMF_CUDA_CHECK(cudaMemsetAsync(fb.Fr, 0, (size_t)SK * d->ld_r * 4, s));
-  CNMF_CUDA_CHECK(cudaMemsetAsync(fb.Fc, 0, (size_t)SK * d->ld_c * 4, s));
-  CNMF_CUDA_CHECK(cudaMemcpy2DAsync(fb.Fr, (size_t)d->ld_r * 4, Wt0_host, (size_t)d->n_rows * 4, (size_t)d->n_rows * 4,
-                                    SK, cudaMemcpyHostToDevice, s));
-  CNMF_CUDA_CHECK(cudaMemcpy2DAsync(fb.Fc, (size_t)d->ld_c * 4, H0_host, (size_t)d->n_cols * 4, (size_t)d->n_cols * 4,
-                                    SK, cudaMemcpyHostToDevice, s));
-  return run_and_download(d, ks, SK, fb, *p, spectra_host, usages_host, n_iter_host, err_host, s);
+  auto t_h2d = clk::now();
+  CNMF_CUDA_CHECK(cudaMemsetAsync(b.Fr, 0, (size_t)b.SK * d->ld_r * 4, s));
+  CNMF_CUDA_CHECK(cudaMemsetAsync(b.Fc, 0, (size_t)b.SK * d->ld_c * 4, s));
+  CNMF_CUDA_CHECK(cudaMemcpy2DAsync(b.Fr, (size_t)d->ld_r * 4, Wt0_host, (size_t)d->n_rows * 4, (size_t)d->n_rows * 4,
+                                    b.SK, cudaMemcpyHostToDevice, s));
+  CNMF_CUDA_CHECK(cudaMemcpy2DAsync(b.Fc, (size_t)d->ld_c * 4, H0_host, (size_t)d->n_cols * 4, (size_t)d->n_cols * 4,
+                                    b.SK, cudaMemcpyHostToDevice, s));
+  CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
+  d->h->t_h2d_ms = ms_since(t_h2d);
+  return solve_and_copy_out(d, b, *p, spectra_host, usages_host, nullptr, 0, 0, n_iter_host, err_host, s);
 }
 
 int cnmf_factorize_dev(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, const float* Wt0_dev,
                        const float* H0_dev, const cnmf_nmf_params* p, float* spectra_dev, int32_t* n_iter_host,
                        double* err_host, void* stream) {
-  CNMF_TRY(check_params(d, p));
-  CNMF_REQUIRE(n_restarts > 0 && ks_in && Wt0_dev && H0_dev && spectra_dev, "factorize_dev: bad arguments");
-  cnmf_handle_s* h = d->h;
+  Batch b;
+  CNMF_TRY(begin_factorize(d, p, n_restarts, ks_in, Wt0_dev && H0_dev && spectra_dev, "factorize_dev", &b));
   cudaStream_t s = as_stream(stream);
-  CNMF_CUDA_CHECK(cudaSetDevice(h->device));
-  std::vector<int> ks(ks_in, ks_in + n_restarts);
-  int SK = 0;
-  for (int r = 0; r < n_restarts; ++r) {
-    CNMF_REQUIRE(ks[r] >= 1 && ks[r] <= KMAX, "factorize_dev: n_components must be in [1, 32] on the CUDA path");
-    SK += ks[r];
-  }
-  const bool tf32 = p->precision == CNMF_PRECISION_TF32X3;
-  FactorBuffers fb;
-  CNMF_TRY(alloc_factors(h, SK, d->ld_r, d->ld_c, tf32, &fb));
-  CNMF_CUDA_CHECK(cudaMemcpyAsync(fb.Fr, Wt0_dev, (size_t)SK * d->ld_r * 4, cudaMemcpyDeviceToDevice, s));
-  CNMF_CUDA_CHECK(cudaMemcpyAsync(fb.Fc, H0_dev, (size_t)SK * d->ld_c * 4, cudaMemcpyDeviceToDevice, s));
-  DataView v = make_view(d, false);
-  if (tf32 && !v.f16) {      // f16 datasets: the solver emits fp16 pieces itself; tf32 pieces would be dead work
-    CNMF_TRY(launch_split_scaled(fb.Fr, fb.Fr_hi, fb.Fr_lo, SK, d->ld_r, v.exact ? v.scale_r : nullptr, s));
-    CNMF_TRY(launch_split_scaled(fb.Fc, fb.Fc_hi, fb.Fc_lo, SK, d->ld_c, v.exact ? v.scale_c : nullptr, s));
-    h->launches += 2;
-  }
-  SolveIO io;
-  io.R = n_restarts;
-  io.ks = ks;
-  io.Fr = fb.Fr; io.Fr_hi = fb.Fr_hi; io.Fr_lo = fb.Fr_lo;
-  io.Fc = fb.Fc; io.Fc_hi = fb.Fc_hi; io.Fc_lo = fb.Fc_lo;
-  io.update_cols = true;
-  CNMF_TRY(solve_batched(h, v, io, *p, s));
-  CNMF_CUDA_CHECK(cudaMemcpyAsync(spectra_dev, fb.Fc, (size_t)SK * d->ld_c * 4, cudaMemcpyDeviceToDevice, s));
-  CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
-  for (int r = 0; r < n_restarts; ++r) {
-    if (n_iter_host) n_iter_host[r] = io.n_iter[r];
-    if (err_host) err_host[r] = io.err[r];
-  }
-  return 0;
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(b.Fr, Wt0_dev, (size_t)b.SK * d->ld_r * 4, cudaMemcpyDeviceToDevice, s));
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(b.Fc, H0_dev, (size_t)b.SK * d->ld_c * 4, cudaMemcpyDeviceToDevice, s));
+  // spectra_dev has the layout of H0_dev: whole padded rows, the zero padding included
+  return solve_and_copy_out(d, b, *p, nullptr, nullptr, spectra_dev, d->ld_c, d->ld_c, n_iter_host, err_host, s);
 }
 
 int cnmf_random_init_dev(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, const uint32_t* seeds, float* Wt_dev,
                          float* H_dev, void* stream) {
   CNMF_REQUIRE(d && n_restarts > 0 && ks_in && seeds && Wt_dev && H_dev, "random_init_dev: bad arguments");
   CNMF_TRY(require_dense(d, "random_init_dev"));
-  cnmf_handle_s* h = d->h;
   cudaStream_t s = as_stream(stream);
-  CNMF_CUDA_CHECK(cudaSetDevice(h->device));
-  std::vector<int> ks(ks_in, ks_in + n_restarts), off(n_restarts);
-  std::vector<double> avgs(n_restarts);
-  const double mean_d = d->sum / ((double)d->n_rows * (double)d->n_cols);
-  int SK = 0;
-  for (int r = 0; r < n_restarts; ++r) {
-    CNMF_REQUIRE(ks[r] >= 1 && ks[r] <= KMAX, "random_init_dev: n_components must be in [1, 32]");
-    off[r] = SK;
-    SK += ks[r];
-    avgs[r] = std::sqrt(mean_d / ks[r]);
-  }
-  CNMF_CUDA_CHECK(cudaMemsetAsync(Wt_dev, 0, (size_t)SK * d->ld_r * 4, s));
-  CNMF_CUDA_CHECK(cudaMemsetAsync(H_dev, 0, (size_t)SK * d->ld_c * 4, s));
-  CNMF_TRY(launch_rng_init(seeds, ks.data(), off.data(), avgs.data(), n_restarts, d->n_rows, d->n_cols, Wt_dev, d->ld_r,
-                           H_dev, d->ld_c, h, s));
+  CNMF_CUDA_CHECK(cudaSetDevice(d->h->device));
+  Batch b;
+  CNMF_TRY(pack_restarts(n_restarts, ks_in, "random_init_dev", &b));
+  CNMF_TRY(rng_starts_dev(d, b, seeds, Wt_dev, H_dev, s));
   CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
   return 0;
 }

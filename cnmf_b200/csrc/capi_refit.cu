@@ -13,12 +13,6 @@
 
 using namespace cnmf;
 
-#define CNMF_TRY(expr)            \
-  do {                            \
-    int _rc = (expr);             \
-    if (_rc != 0) return _rc;     \
-  } while (0)
-
 namespace {
 
 __global__ void fill_kernel(float* p, float v, int rows, int n, int ld) {
@@ -305,7 +299,6 @@ int cnmf_refit(cnmf_dataset_t d, int transposed, int k, const float* fixed_host,
   // iterates on K x K Grams only -- no GEMM runs, so no operand pieces are made (fp32 solver code)
   cnmf_nmf_params pp = *p;
   if (d->sparse) pp.precision = CNMF_PRECISION_FP32;
-  const bool tf32 = pp.precision == CNMF_PRECISION_TF32X3;
   if (p->beta_loss != CNMF_LOSS_FROBENIUS) CNMF_TRY(dataset_ensure_full_transpose(d, s));
   DataView v = make_view(d, transposed != 0);
   if (d->sparse) {
@@ -316,15 +309,7 @@ int cnmf_refit(cnmf_dataset_t d, int transposed, int k, const float* fixed_host,
   const size_t nr = (size_t)k * v.ld_r, nc = (size_t)k * v.ld_c;
   float* Fr = static_cast<float*>(h->dev_buf("refit.Fr", nr * 4));
   float* Fc = static_cast<float*>(h->dev_buf("refit.Fc", nc * 4));
-  float *Fr_hi = nullptr, *Fr_lo = nullptr, *Fc_hi = nullptr, *Fc_lo = nullptr;
   if (!Fr || !Fc) return -2;
-  if (tf32) {
-    Fr_hi = static_cast<float*>(h->dev_buf("refit.Fr_hi", nr * 4));
-    Fr_lo = static_cast<float*>(h->dev_buf("refit.Fr_lo", nr * 4));
-    Fc_hi = static_cast<float*>(h->dev_buf("refit.Fc_hi", nc * 4));
-    Fc_lo = static_cast<float*>(h->dev_buf("refit.Fc_lo", nc * 4));
-    if (!Fr_hi || !Fr_lo || !Fc_hi || !Fc_lo) return -2;
-  }
   CNMF_CUDA_CHECK(cudaMemsetAsync(Fr, 0, nr * 4, s));
   CNMF_CUDA_CHECK(cudaMemsetAsync(Fc, 0, nc * 4, s));
   CNMF_CUDA_CHECK(cudaMemcpy2DAsync(Fc, (size_t)v.ld_c * 4, fixed_host, (size_t)v.n_c * 4, (size_t)v.n_c * 4, k,
@@ -336,16 +321,11 @@ int cnmf_refit(cnmf_dataset_t d, int transposed, int k, const float* fixed_host,
     CNMF_CUDA_CHECK(cudaGetLastError());
     h->launches += 1;
   }  // 'cd': zeros (sklearn _nmf.py:1227-1228)
-  if (tf32 && !v.f16) {
-    CNMF_TRY(launch_split_scaled(Fr, Fr_hi, Fr_lo, k, v.ld_r, v.exact ? v.scale_r : nullptr, s));
-    CNMF_TRY(launch_split_scaled(Fc, Fc_hi, Fc_lo, k, v.ld_c, v.exact ? v.scale_c : nullptr, s));
-    h->launches += 2;
-  }
   SolveIO io;
   io.R = 1;
   io.ks = {k};
-  io.Fr = Fr; io.Fr_hi = Fr_hi; io.Fr_lo = Fr_lo;
-  io.Fc = Fc; io.Fc_hi = Fc_hi; io.Fc_lo = Fc_lo;
+  io.Fr = Fr;
+  io.Fc = Fc;
   io.update_cols = false;
   if (d->sparse) {
     const int kp = round_up(k, 4);

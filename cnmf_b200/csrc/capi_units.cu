@@ -9,12 +9,6 @@
 
 using namespace cnmf;
 
-#define CNMF_TRY(expr)            \
-  do {                            \
-    int _rc = (expr);             \
-    if (_rc != 0) return _rc;     \
-  } while (0)
-
 extern "C" int cnmf_update_step_host(cnmf_handle_t h, const cnmf_update_step_args* a, void* stream) {
   CNMF_REQUIRE(h && a && a->ks && a->rids && a->done && a->F && a->gram_in, "update_step: NULL argument");
   CNMF_REQUIRE(a->n_slots >= 1 && a->n_rids >= 1 && a->n >= 1 && a->nsplit >= 1, "update_step: bad sizes");
@@ -108,7 +102,7 @@ extern "C" int cnmf_update_step_host(cnmf_handle_t h, const cnmf_update_step_arg
   const long long sstride = (long long)nf;
 
   if (none) {
-    // start of a solve: pieces of the initial factors (run_and_download / emit_pieces), stand-alone Gram, <NUM, F>
+    // start of a solve: pieces of the initial factors (solve_batched: split or emit_pieces), stand-alone Gram, <NUM, F>
     if (a->pieces == CNMF_UNIT_PIECES_TF32) CNMF_TRY(launch_split_scaled(d_F, f.F_hi, f.F_lo, SK, ld, pscale, s));
     if (a->pieces == CNMF_UNIT_PIECES_F16) CNMF_TRY(launch_emit_f16(d_F, SK, n, ld, pscale, d_hi, d_lo, d_ts, n_ktiles, s));
     if (a->gram == CNMF_UNIT_GRAM_STANDALONE) {

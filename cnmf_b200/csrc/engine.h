@@ -15,9 +15,6 @@ struct cnmf_handle_s {
   long long launches = 0;                       // kernels launched by this library (bench: gpu_launches)
   // optional per-launch timing of the hot kernels (batched GEMM, fused update) with CUDA events on the
   // launching stream; read back by bench.py for the roofline lines
-  // auxiliary stream + events (kept for experiments that co-schedule streaming kernels under a GEMM)
-  cudaStream_t aux = nullptr;
-  cudaEvent_t ev_upd = nullptr, ev_gram = nullptr;
   bool profile = false;
   std::vector<cudaEvent_t> ev_pool;
   struct Pending { int begin; int end; int cls; double work; };   // indices of the start / end events in ev_pool
@@ -34,7 +31,7 @@ struct cnmf_handle_s {
   double prof_ms[PROF_CLASSES] = {0.0, 0.0, 0.0, 0.0}, prof_work[PROF_CLASSES] = {0.0, 0.0, 0.0, 0.0};
   long long prof_launches[PROF_CLASSES] = {0, 0, 0, 0};
   int nndsvd_chunk_restarts = 0;                // > 0: at most this many restarts per chunk of the NNDSVD starts
-  double t_rng_ms = 0, t_h2d_ms = 0, t_solve_ms = 0, t_d2h_ms = 0;   // host wall-clock phases of the last cnmf_factorize
+  double t_rng_ms = 0, t_h2d_ms = 0, t_solve_ms = 0, t_d2h_ms = 0;   // host wall-clock phases of the last factorize
   int prof_begin(cudaStream_t s, double work, int cls = 0);    // start event (recorded or shared); returns slot or -1
   void prof_end(cudaStream_t s, int slot);
   void prof_collect();                              // after a stream sync: fold pending pairs into the totals
@@ -123,9 +120,9 @@ DataView make_view(const cnmf_dataset_s* d, bool transposed);
 struct SolveIO {
   int R = 0;
   std::vector<int> ks;      // per restart
-  // packed device factors (SK x ld): row factor Fr (e.g. W^T), column factor Fc (e.g. H)
-  float *Fr = nullptr, *Fr_hi = nullptr, *Fr_lo = nullptr;
-  float *Fc = nullptr, *Fc_hi = nullptr, *Fc_lo = nullptr;
+  // packed device factors (SK x ld), full fp32: row factor Fr (e.g. W^T), column factor Fc (e.g. H).  The solver
+  // makes their operand pieces itself.
+  float *Fr = nullptr, *Fc = nullptr;
   bool update_cols = true;  // false: Fc fixed (refit)
   // the row product, computed by the caller (refits of sparse datasets: NUM_r = Fc * X^T, SK x ld_r, one split).
   // Requires update_cols = false; the solver then runs no GEMM and reads no B operand.

@@ -79,12 +79,6 @@ int run_gemm(cnmf_handle_s* h, int precision, const float* A, const float* A_hi,
   return rc;
 }
 
-#define CNMF_TRY(expr)            \
-  do {                            \
-    int _rc = (expr);             \
-    if (_rc != 0) return _rc;     \
-  } while (0)
-
 }  // namespace
 
 int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_nmf_params& p, cudaStream_t s) {
@@ -204,8 +198,17 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
   double* d_gpartR = d_gram_part;                      // partials of Gram(Fr)
   double* d_gpartC = d_gram_part + gpart_elems;        // partials of Gram(Fc)
 
-  // working factor arrays (start in the caller's buffers; compaction ping-pongs to "solve.alt.*")
-  float *wFr = io.Fr, *wFr_hi = io.Fr_hi, *wFr_lo = io.Fr_lo, *wFc = io.Fc, *wFc_hi = io.Fc_hi, *wFc_lo = io.Fc_lo;
+  // working factor arrays (start in the caller's buffers; compaction ping-pongs to "solve.alt.*") and their operand
+  // pieces: tf32 hi / lo, or on f16 datasets the two fp16 pieces in the same buffers
+  float *wFr = io.Fr, *wFr_hi = nullptr, *wFr_lo = nullptr, *wFc = io.Fc, *wFc_hi = nullptr, *wFc_lo = nullptr;
+  if (tf32) {
+    const size_t nr = (size_t)SK0 * v.ld_r, nc = (size_t)SK0 * v.ld_c;
+    wFr_hi = static_cast<float*>(h->dev_buf("solve.Fr_hi", nr * 4));
+    wFr_lo = static_cast<float*>(h->dev_buf("solve.Fr_lo", nr * 4));
+    wFc_hi = static_cast<float*>(h->dev_buf("solve.Fc_hi", nc * 4));
+    wFc_lo = static_cast<float*>(h->dev_buf("solve.Fc_lo", nc * 4));
+    if (!wFr_hi || !wFr_lo || !wFc_hi || !wFc_lo) return -2;
+  }
   float *aFr = nullptr, *aFr_hi = nullptr, *aFr_lo = nullptr, *aFc = nullptr, *aFc_hi = nullptr, *aFc_lo = nullptr;
   float *resFr = nullptr, *resFc = nullptr;   // final factors of restarts that were compacted away (original offsets)
   bool compacted = false;
@@ -435,7 +438,12 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
 
   const float l1W = (float)p.l1_reg_W, l2W = (float)p.l2_reg_W, l1H = (float)p.l1_reg_H, l2H = (float)p.l2_reg_H;
   int it = 0;
-  CNMF_TRY(emit_pieces(0));        // f16: the callers' tf32 pieces are replaced by fp16 pieces of the initial factors
+  if (upd_pieces) {                // pieces of the starting factors; afterwards the update kernels write them
+    CNMF_TRY(launch_split_scaled(wFr, wFr_hi, wFr_lo, SK, v.ld_r, v.exact ? v.scale_r : nullptr, s));
+    CNMF_TRY(launch_split_scaled(wFc, wFc_hi, wFc_lo, SK, v.ld_c, v.exact ? v.scale_c : nullptr, s));
+    h->launches += 2;
+  }
+  CNMF_TRY(emit_pieces(0));        // f16: fp16 pieces of the starting factors
   CNMF_TRY(emit_pieces(1));
 
   if (mu) {

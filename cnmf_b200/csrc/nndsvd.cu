@@ -41,12 +41,6 @@
 #include "engine.h"
 #include "legacy_gauss.cuh"
 
-#define CNMF_TRY(expr)            \
-  do {                            \
-    int _rc = (expr);             \
-    if (_rc != 0) return _rc;     \
-  } while (0)
-
 namespace cnmf {
 
 namespace {

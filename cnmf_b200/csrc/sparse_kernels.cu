@@ -22,12 +22,6 @@ using namespace cnmf;
 
 extern "C" int cnmf_dataset_alloc_internal(cnmf_dataset_t d, float** p, size_t elems);   // capi.cu
 
-#define CNMF_TRY(expr)            \
-  do {                            \
-    int _rc = (expr);             \
-    if (_rc != 0) return _rc;     \
-  } while (0)
-
 namespace {
 
 constexpr int WARPS = 8;    // warps per block of the warp-per-column / warp-per-chunk kernels

@@ -91,8 +91,9 @@ int cnmf_profile_get(cnmf_handle_t h, double* gemm_ms, long long* gemm_launches,
  * 3 = the fp64 GEMM of cnmf_nndsvd_init_dev (work = algorithmic FLOPs, 2*M*N*K per launch) */
 int cnmf_profile_get_class(cnmf_handle_t h, int kernel_class, double* ms, long long* launches, double* work);
 
-/* host wall-clock phases (ms) of the last cnmf_factorize on this handle: host RNG, H2D of the initial
- * factors, batched solve, D2H of the results */
+/* host wall-clock phases (ms) of the last cnmf_factorize, cnmf_factorize_seeds_dev, cnmf_factorize_init or
+ * cnmf_factorize_dev on this handle: starting factors (host RNG, device RNG enqueue or NNDSVD), H2D of host initial
+ * factors, batched solve, copy-out of the results.  A phase the call does not have reads 0. */
 int cnmf_last_timing(cnmf_handle_t h, double* rng_ms, double* h2d_ms, double* solve_ms, double* d2h_ms);
 
 /* ---- dataset: a cells x genes matrix made resident on the device ------------------- */
