@@ -196,8 +196,9 @@ long long cnmf_solve_bytes_per_row(cnmf_dataset_t d) {
   if (!d) return 0;
   // factorize / solve_batched: Fr + 2 piece buffers, their 3 compaction alternates, the result slab and the
   // product NUM_r along the cells; the same along the genes with one product slice per split-K slice
-  const long long splits_c = gemm_fixed_splits(d->n_rows, d->f16 ? 1 : 0);
-  const long long splits_r = gemm_fixed_splits(d->n_cols, d->f16 ? 1 : 0);
+  const int f16 = make_view(d, false).form == Form::F16_EXACT ? 1 : 0;
+  const long long splits_c = gemm_fixed_splits(d->n_rows, f16);
+  const long long splits_r = gemm_fixed_splits(d->n_cols, f16);
   return 4LL * ((7 + splits_r) * (long long)d->ld_r + (7 + splits_c) * (long long)d->ld_c);
 }
 
@@ -237,8 +238,12 @@ int cnmf_profile_get_class(cnmf_handle_t h, int cls, double* ms, long long* laun
   return 0;
 }
 
+}  // extern "C"
+
 // ----------------------------------------------------------------------------- dataset
-static int dataset_alloc(cnmf_dataset_s* d, float** p, size_t elems) {
+namespace cnmf {
+
+int dataset_alloc(cnmf_dataset_s* d, float** p, size_t elems) {
   const size_t bytes = std::max<size_t>(elems, 64) * sizeof(float);
   void* q = d->h->pool_take(bytes);
   if (!q) {
@@ -253,17 +258,15 @@ static int dataset_alloc(cnmf_dataset_s* d, float** p, size_t elems) {
   return 0;
 }
 
-int cnmf_dataset_alloc_internal(cnmf_dataset_t d, float** p, size_t elems) { return dataset_alloc(d, p, elems); }
-
-// builds Xt / tf32 pieces / sums from d->X (already resident, padding zeroed)
-static int dataset_finish(cnmf_dataset_s* d, cudaStream_t s) {
-  cnmf_handle_s* h = d->h;
-  const size_t nx = (size_t)d->n_rows * d->ld_c, nxt = (size_t)d->n_cols * d->ld_r;
-  if (d->precision == CNMF_PRECISION_TF32X3) {
-    // ---- exact-count detection: is X = diag(r) C diag(s) with C integer <= 2048 ?  (column scale first,
-    //      then row scale; datasets derived by cnmf_dataset_from_columns arrive with `exact` already decided)
-    static const bool allow_exact = [] { const char* e = std::getenv("CNMF_EXACT"); return !(e && e[0] == '0'); }();
-    if (allow_exact && d->allow_exact && !d->exact && d->n_rows <= 65535 * 64) {
+int dataset_resolve_form(cnmf_dataset_s* d, bool exact, cudaStream_t s) {
+  // exact-count detection: is X = diag(r) C diag(s) with C integer <= 2048 ?  (column scale first, then row scale).
+  // The same condition for dense and CSC matrices, so that both give the same dataset.
+  const bool may_be_exact = d->precision == CNMF_PRECISION_TF32X3 || d->precision == CNMF_PRECISION_F16X2;
+  if (may_be_exact && !exact && d->n_rows <= 65535 * 64) {
+    if (d->sparse) {
+      CNMF_TRY(csc_detect_exact(d, s, &exact));
+    } else {
+      cnmf_handle_s* h = d->h;
       float* cmin = nullptr;
       float* rmin = nullptr;
       CNMF_TRY(dataset_alloc(d, &cmin, (size_t)d->ld_c));
@@ -280,33 +283,26 @@ static int dataset_finish(cnmf_dataset_s* d, cudaStream_t s) {
       int bad[2] = {1, 1};
       CNMF_CUDA_CHECK(cudaMemcpyAsync(bad, n_bad, sizeof(int) * 2, cudaMemcpyDeviceToHost, s));
       CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
-      if (bad[0] == 0) { d->exact = true; d->col_scale = cmin; d->row_scale = nullptr; }
-      else if (bad[1] == 0) { d->exact = true; d->row_scale = rmin; d->col_scale = nullptr; }
+      if (bad[0] == 0) { exact = true; d->col_scale = cmin; d->row_scale = nullptr; }
+      else if (bad[1] == 0) { exact = true; d->row_scale = rmin; d->col_scale = nullptr; }
     }
-    if (d->exact) {
-      CNMF_TRY(dataset_alloc(d, &d->X_hi, nx));
-      CNMF_TRY(dataset_alloc(d, &d->Xt_hi, nxt));
-      CNMF_CUDA_CHECK(cudaMemsetAsync(d->X_hi, 0, nx * sizeof(float), s));
-      CNMF_CUDA_CHECK(cudaMemsetAsync(d->Xt_hi, 0, nxt * sizeof(float), s));
-      CNMF_TRY(launch_build_counts(d->X, d->n_rows, d->n_cols, d->ld_c, d->row_scale, d->col_scale, d->X_hi, s));
-      CNMF_TRY(launch_transpose(d->X_hi, d->n_rows, d->n_cols, d->ld_c, d->Xt_hi, nullptr, nullptr, d->ld_r, s));
-      h->launches += 2;
-      if (d->want_f16) {       // counts <= 2048 are exact in fp16: the B operands of the f16 products
-        float *xh = nullptr, *xth = nullptr;
-        CNMF_TRY(dataset_alloc(d, &xh, (nx + 1) / 2));
-        CNMF_TRY(dataset_alloc(d, &xth, (nxt + 1) / 2));
-        d->X_h16 = xh;
-        d->Xt_h16 = xth;
-        CNMF_TRY(launch_to_half(d->X_hi, d->X_h16, (long long)nx, s));
-        CNMF_TRY(launch_to_half(d->Xt_hi, d->Xt_h16, (long long)nxt, s));
-        h->launches += 2;
-        d->f16 = true;
-        // every product of an f16 dataset reads the fp16 count matrices: the fp32 copies of C / C^T were scaffolding.
-        // Resident forms are then X (fp32, column operations and derived datasets) + C and C^T as fp16: 2 x the
-        // bytes of X instead of 4 x.  (Released after the stream has drained, below.)
-        d->drop_tf32 = true;
-      }
-    } else {
+  }
+  if (d->precision == CNMF_PRECISION_FP32) d->form = Form::FP32;
+  else if (!exact) d->form = Form::TF32;
+  else d->form = d->precision == CNMF_PRECISION_F16X2 ? Form::F16_EXACT : Form::TF32_EXACT;
+  return 0;
+}
+
+int dataset_finish(cnmf_dataset_s* d, cudaStream_t s, bool exact) {
+  cnmf_handle_s* h = d->h;
+  const size_t nx = (size_t)d->n_rows * d->ld_c, nxt = (size_t)d->n_cols * d->ld_r;
+  CNMF_TRY(dataset_resolve_form(d, exact, s));
+  if (d->form == Form::FP32) {
+    CNMF_TRY(dataset_alloc(d, &d->Xt, nxt));
+    CNMF_CUDA_CHECK(cudaMemsetAsync(d->Xt, 0, nxt * sizeof(float), s));
+    CNMF_TRY(launch_transpose(d->X, d->n_rows, d->n_cols, d->ld_c, d->Xt, nullptr, nullptr, d->ld_r, s));
+    h->launches += 1;
+  } else if (d->form == Form::TF32) {
     CNMF_TRY(dataset_alloc(d, &d->X_hi, nx));
     CNMF_TRY(dataset_alloc(d, &d->X_lo, nx));
     CNMF_TRY(dataset_alloc(d, &d->Xt_hi, nxt));
@@ -316,12 +312,24 @@ static int dataset_finish(cnmf_dataset_s* d, cudaStream_t s) {
     CNMF_TRY(launch_split_tf32(d->X, d->X_hi, d->X_lo, (long long)nx, s));
     CNMF_TRY(launch_transpose(d->X, d->n_rows, d->n_cols, d->ld_c, nullptr, d->Xt_hi, d->Xt_lo, d->ld_r, s));
     h->launches += 2;
-    }
   } else {
-    CNMF_TRY(dataset_alloc(d, &d->Xt, nxt));
-    CNMF_CUDA_CHECK(cudaMemsetAsync(d->Xt, 0, nxt * sizeof(float), s));
-    CNMF_TRY(launch_transpose(d->X, d->n_rows, d->n_cols, d->ld_c, d->Xt, nullptr, nullptr, d->ld_r, s));
-    h->launches += 1;
+    CNMF_TRY(dataset_alloc(d, &d->X_hi, nx));
+    CNMF_TRY(dataset_alloc(d, &d->Xt_hi, nxt));
+    CNMF_CUDA_CHECK(cudaMemsetAsync(d->X_hi, 0, nx * sizeof(float), s));
+    CNMF_CUDA_CHECK(cudaMemsetAsync(d->Xt_hi, 0, nxt * sizeof(float), s));
+    CNMF_TRY(launch_build_counts(d->X, d->n_rows, d->n_cols, d->ld_c, d->row_scale, d->col_scale, d->X_hi, s));
+    CNMF_TRY(launch_transpose(d->X_hi, d->n_rows, d->n_cols, d->ld_c, d->Xt_hi, nullptr, nullptr, d->ld_r, s));
+    h->launches += 2;
+    if (d->form == Form::F16_EXACT) {       // counts <= 2048 are exact in fp16: the B operands of the f16 products
+      float *xh = nullptr, *xth = nullptr;
+      CNMF_TRY(dataset_alloc(d, &xh, (nx + 1) / 2));
+      CNMF_TRY(dataset_alloc(d, &xth, (nxt + 1) / 2));
+      d->X_h16 = xh;
+      d->Xt_h16 = xth;
+      CNMF_TRY(launch_to_half(d->X_hi, d->X_h16, (long long)nx, s));
+      CNMF_TRY(launch_to_half(d->Xt_hi, d->Xt_h16, (long long)nxt, s));
+      h->launches += 2;
+    }
   }
   const int scratch_len = 2 * cnmf::NUM_SMS * 8 + 2;
   double* scratch = static_cast<double*>(h->dev_buf("dataset.sums", sizeof(double) * (scratch_len + 2)));
@@ -333,7 +341,10 @@ static int dataset_finish(cnmf_dataset_s* d, cudaStream_t s) {
   CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
   d->sum = out2[0];
   d->sum_sq = out2[1];
-  if (d->drop_tf32) {          // the conversions above have completed: hand the fp32 count matrices back
+  // every product of an f16 dataset reads the fp16 count matrices: the fp32 copies of C / C^T were scaffolding.
+  // Resident forms are then X (fp32, column operations and derived datasets) + C and C^T as fp16: 2 x the bytes of X
+  // instead of 4 x.  Released only now, after the synchronisation above: the conversions have completed.
+  if (d->form == Form::F16_EXACT) {
     for (float** pp : {&d->X_hi, &d->Xt_hi}) {
       for (auto it = d->owned.begin(); it != d->owned.end(); ++it)
         if (it->first == *pp) {
@@ -343,10 +354,19 @@ static int dataset_finish(cnmf_dataset_s* d, cudaStream_t s) {
         }
       *pp = nullptr;
     }
-    d->drop_tf32 = false;
   }
   return 0;
 }
+
+int check_params_precision(const cnmf_dataset_s* d, const cnmf_nmf_params* p) {
+  const int want = d->precision == CNMF_PRECISION_FP32 ? CNMF_PRECISION_FP32 : CNMF_PRECISION_TF32X3;
+  CNMF_REQUIRE(p->precision == want, "params.precision must match the precision the dataset was created with");
+  return 0;
+}
+
+}  // namespace cnmf
+
+extern "C" {
 
 int cnmf_dataset_create(cnmf_handle_t h, const float* X, int n_rows, int n_cols, long long ld, int src_is_device,
                         int precision, void* stream, cnmf_dataset_t* out) {
@@ -357,16 +377,7 @@ int cnmf_dataset_create(cnmf_handle_t h, const float* X, int n_rows, int n_cols,
                "dataset_create: bad precision");
   cudaStream_t s = as_stream(stream);
   CNMF_CUDA_CHECK(cudaSetDevice(h->device));
-  auto* d = new cnmf_dataset_s();
-  d->h = h;
-  d->n_rows = n_rows;
-  d->n_cols = n_cols;
-  d->ld_c = pad_ld(n_cols);
-  d->ld_r = pad_ld(n_rows);
-  d->allow_exact = precision != CNMF_PRECISION_TF32X3_GENERAL;
-  d->want_f16 = precision == CNMF_PRECISION_F16X2;
-  d->precision = (precision == CNMF_PRECISION_TF32X3_GENERAL || precision == CNMF_PRECISION_F16X2) ? CNMF_PRECISION_TF32X3
-                                                                                                : precision;
+  auto* d = new cnmf_dataset_s(h, n_rows, n_cols, precision);
   int rc = dataset_alloc(d, &d->X, (size_t)n_rows * d->ld_c);
   if (rc == 0) {
     cudaError_t e = cudaMemsetAsync(d->X, 0, (size_t)n_rows * d->ld_c * sizeof(float), s);
@@ -387,8 +398,6 @@ int cnmf_dataset_create(cnmf_handle_t h, const float* X, int n_rows, int n_cols,
   *out = d;
   return 0;
 }
-
-int cnmf_dataset_finish_internal(cnmf_dataset_t d, void* stream) { return dataset_finish(d, as_stream(stream)); }
 
 int cnmf_dataset_dense_bytes(int n_rows, int n_cols, int precision, long long* peak) {
   CNMF_REQUIRE(peak && n_rows > 0 && n_cols > 0, "dataset_dense_bytes: bad arguments");
@@ -432,7 +441,9 @@ int cnmf_dataset_shape(cnmf_dataset_t d, int* n_rows, int* n_cols) {
   return 0;
 }
 
-int cnmf_dataset_is_exact(cnmf_dataset_t d) { return (d && d->exact && !d->sparse) ? (d->f16 ? 2 : 1) : 0; }
+int cnmf_dataset_is_exact(cnmf_dataset_t d) {
+  return (d && !d->sparse && form_exact(d->form)) ? (d->form == Form::F16_EXACT ? 2 : 1) : 0;
+}
 
 int cnmf_dataset_sums(cnmf_dataset_t d, double* sum, double* sum_sq) {
   CNMF_REQUIRE(d, "dataset_sums: NULL dataset");
@@ -500,7 +511,7 @@ void parallel_for(int n, const std::function<void(int)>& fn) {
 
 int check_params(cnmf_dataset_s* d, const cnmf_nmf_params* p) {
   CNMF_REQUIRE(d && p, "NULL dataset or params");
-  CNMF_REQUIRE(p->precision == d->precision, "params.precision must match the precision the dataset was created with");
+  CNMF_TRY(check_params_precision(d, p));
   CNMF_REQUIRE(p->reserved2 == 0, "params.reserved2 must be 0");
   CNMF_TRY(require_dense(d, "factorize"));
   if (p->beta_loss != CNMF_LOSS_FROBENIUS) CNMF_TRY(cnmf::dataset_ensure_full_transpose(d, nullptr));
@@ -723,7 +734,7 @@ int dataset_ensure_full_transpose(cnmf_dataset_s* d, cudaStream_t s) {
   if (d->Xt) return 0;
   CNMF_CUDA_CHECK(cudaSetDevice(d->h->device));
   const size_t nxt = (size_t)d->n_cols * d->ld_r;
-  CNMF_TRY(cnmf_dataset_alloc_internal(d, &d->Xt, nxt));
+  CNMF_TRY(dataset_alloc(d, &d->Xt, nxt));
   CNMF_CUDA_CHECK(cudaMemsetAsync(d->Xt, 0, nxt * sizeof(float), s));
   CNMF_TRY(launch_transpose(d->X, d->n_rows, d->n_cols, d->ld_c, d->Xt, nullptr, nullptr, d->ld_r, s));
   d->h->launches += 1;

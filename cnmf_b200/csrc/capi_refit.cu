@@ -185,10 +185,6 @@ int cnmf_dataset_tpm_stats(cnmf_dataset_t d, double target_sum, double* totals_h
   return 0;
 }
 
-// defined in capi.cu (internal; not in the public header)
-int cnmf_dataset_finish_internal(cnmf_dataset_t d, void* stream);
-int cnmf_dataset_alloc_internal(cnmf_dataset_t d, float** p, size_t elems);
-
 int cnmf_dataset_from_columns(cnmf_dataset_t src, const int32_t* cols_host, const float* col_scale_host, int n_cols,
                               void* stream, cnmf_dataset_t* out) {
   CNMF_REQUIRE(src && cols_host && col_scale_host && out && n_cols > 0, "dataset_from_columns: bad arguments");
@@ -202,16 +198,8 @@ int cnmf_dataset_from_columns(cnmf_dataset_t src, const int32_t* cols_host, cons
   if (!d_cols || !d_scale) return -2;
   CNMF_CUDA_CHECK(cudaMemcpyAsync(d_cols, cols_host, sizeof(int) * n_cols, cudaMemcpyHostToDevice, s));
   CNMF_CUDA_CHECK(cudaMemcpyAsync(d_scale, col_scale_host, sizeof(float) * n_cols, cudaMemcpyHostToDevice, s));
-  auto* d = new cnmf_dataset_s();
-  d->h = h;
-  d->n_rows = src->n_rows;
-  d->n_cols = n_cols;
-  d->ld_c = pad_ld(n_cols);
-  d->ld_r = pad_ld(src->n_rows);
-  d->precision = src->precision;
-  d->allow_exact = src->allow_exact;
-  d->want_f16 = src->want_f16;
-  int rc = cnmf_dataset_alloc_internal(d, &d->X, (size_t)d->n_rows * d->ld_c);
+  auto* d = new cnmf_dataset_s(h, src->n_rows, n_cols, src->precision);
+  int rc = dataset_alloc(d, &d->X, (size_t)d->n_rows * d->ld_c);
   if (rc == 0) {
     cudaError_t e = cudaMemsetAsync(d->X, 0, (size_t)d->n_rows * d->ld_c * sizeof(float), s);
     if (e != cudaSuccess) rc = -2;
@@ -224,23 +212,23 @@ int cnmf_dataset_from_columns(cnmf_dataset_t src, const int32_t* cols_host, cons
     h->launches += 1;
     if (cudaGetLastError() != cudaSuccess) rc = -2;
   }
-  if (rc == 0 && src->exact) {
+  const bool exact = form_exact(src->form);
+  if (rc == 0 && exact) {
     // an exact-count source stays exact: same integer matrix (the selected columns), same row scale, and the
     // column scale becomes scale[c] * src.col_scale[cols[c]]; finish() rebuilds C from the scaled values
-    d->exact = true;
-    rc = cnmf_dataset_alloc_internal(d, &d->col_scale, (size_t)d->ld_c);
+    rc = dataset_alloc(d, &d->col_scale, (size_t)d->ld_c);
     if (rc == 0) {
       combine_scale_kernel<<<(d->ld_c + 255) / 256, 256, 0, s>>>(d_scale, src->col_scale, d_cols, n_cols, d->ld_c, d->col_scale);
       h->launches += 1;
       if (cudaGetLastError() != cudaSuccess) rc = -2;
     }
     if (rc == 0 && src->row_scale) {
-      rc = cnmf_dataset_alloc_internal(d, &d->row_scale, (size_t)d->ld_r);
+      rc = dataset_alloc(d, &d->row_scale, (size_t)d->ld_r);
       if (rc == 0 && cudaMemcpyAsync(d->row_scale, src->row_scale, sizeof(float) * d->ld_r, cudaMemcpyDeviceToDevice, s) != cudaSuccess)
         rc = -2;
     }
   }
-  if (rc == 0) rc = cnmf_dataset_finish_internal(d, stream);
+  if (rc == 0) rc = dataset_finish(d, s, exact);
   if (rc != 0) {
     cnmf_dataset_destroy(d);
     return rc;
@@ -258,23 +246,15 @@ int cnmf_dataset_scale_rows(cnmf_dataset_t src, const float* row_scale_host, voi
   float* d_rs = static_cast<float*>(h->dev_buf("scalerows.rs", sizeof(float) * src->n_rows));
   if (!d_rs) return -2;
   CNMF_CUDA_CHECK(cudaMemcpyAsync(d_rs, row_scale_host, sizeof(float) * src->n_rows, cudaMemcpyHostToDevice, s));
-  auto* d = new cnmf_dataset_s();
-  d->h = h;
-  d->n_rows = src->n_rows;
-  d->n_cols = src->n_cols;
-  d->ld_c = src->ld_c;
-  d->ld_r = src->ld_r;
-  d->precision = src->precision;
-  d->allow_exact = src->allow_exact;
-  d->want_f16 = src->want_f16;
-  int rc = cnmf_dataset_alloc_internal(d, &d->X, (size_t)d->n_rows * d->ld_c);
+  auto* d = new cnmf_dataset_s(h, src->n_rows, src->n_cols, src->precision);
+  int rc = dataset_alloc(d, &d->X, (size_t)d->n_rows * d->ld_c);
   if (rc == 0) {
     scale_rows_kernel<<<NUM_SMS * 8, 256, 0, s>>>(src->X, d->n_rows, d->n_cols, d->ld_c, d_rs, d->X);
     h->launches += 1;
     if (cudaGetLastError() != cudaSuccess) rc = -2;
   }
   // exact-count detection runs from scratch in finish(): counts x (1e6 / cell total) is again scaled integers
-  if (rc == 0) rc = cnmf_dataset_finish_internal(d, stream);
+  if (rc == 0) rc = dataset_finish(d, s);
   if (rc != 0) {
     cnmf_dataset_destroy(d);
     return rc;
@@ -287,7 +267,7 @@ int cnmf_dataset_scale_rows(cnmf_dataset_t src, const float* row_scale_host, voi
 int cnmf_refit(cnmf_dataset_t d, int transposed, int k, const float* fixed_host, const cnmf_nmf_params* p,
                float* out_host, int32_t* n_iter_host, double* err_host, void* stream) {
   CNMF_REQUIRE(d && fixed_host && p && out_host, "refit: NULL argument");
-  CNMF_REQUIRE(p->precision == d->precision, "params.precision must match the precision the dataset was created with");
+  CNMF_TRY(check_params_precision(d, p));
   CNMF_REQUIRE(k >= 1 && k <= KMAX, "refit: n_components must be in [1, 32] on the CUDA path");
   if (d->sparse && !transposed) CNMF_TRY(require_dense(d, "refit with transposed = 0"));
   if (d->sparse && p->beta_loss != CNMF_LOSS_FROBENIUS) CNMF_TRY(require_dense(d, "refit with a KL / IS beta_loss"));
@@ -296,15 +276,9 @@ int cnmf_refit(cnmf_dataset_t d, int transposed, int k, const float* fixed_host,
   cudaStream_t s = as_stream(stream);
   CNMF_CUDA_CHECK(cudaSetDevice(h->device));
   // sparse datasets: the one product X^T W is formed by csc_project_kernel in fp64 before the solve, which then
-  // iterates on K x K Grams only -- no GEMM runs, so no operand pieces are made (fp32 solver code)
-  cnmf_nmf_params pp = *p;
-  if (d->sparse) pp.precision = CNMF_PRECISION_FP32;
+  // iterates on K x K Grams only -- no GEMM runs, so no operand pieces are made (make_view: FP32 form)
   if (p->beta_loss != CNMF_LOSS_FROBENIUS) CNMF_TRY(dataset_ensure_full_transpose(d, s));
-  DataView v = make_view(d, transposed != 0);
-  if (d->sparse) {
-    v.exact = v.f16 = false;
-    v.scale_r = v.scale_c = nullptr;
-  }
+  const DataView v = make_view(d, transposed != 0);
 
   const size_t nr = (size_t)k * v.ld_r, nc = (size_t)k * v.ld_c;
   float* Fr = static_cast<float*>(h->dev_buf("refit.Fr", nr * 4));
@@ -343,7 +317,7 @@ int cnmf_refit(cnmf_dataset_t d, int transposed, int k, const float* fixed_host,
     h->t_h2d_ms = std::chrono::duration<double, std::milli>(t_solve - t_enter).count();
     t_solve = std::chrono::steady_clock::now();
   }
-  CNMF_TRY(solve_batched(h, v, io, pp, s));
+  CNMF_TRY(solve_batched(h, v, io, *p, s));
   if (h->profile) h->t_solve_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_solve).count();
 
   // Fr is k x n_r; the caller wants n_r x k (row-major).  Transposed on the device into a COMPACT n_r x k array and
@@ -384,27 +358,23 @@ int cnmf_project_rows(cnmf_dataset_t d, int k, const float* Ut_host, float* out_
     CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
     return 0;
   }
-  const bool tf32 = d->precision == CNMF_PRECISION_TF32X3;
+  const DataView v = make_view(d, false);     // out = the solver's NUM_c product of the rows Ut
   const size_t nr = (size_t)k * d->ld_r;
   float* A = static_cast<float*>(h->dev_buf("proj.A", nr * 4));
-  float *A_hi = nullptr, *A_lo = nullptr;
+  float *A_hi = nullptr, *A_lo = nullptr, *A_rs = nullptr;
   if (!A) return -2;
   CNMF_CUDA_CHECK(cudaMemsetAsync(A, 0, nr * 4, s));
   CNMF_CUDA_CHECK(cudaMemcpy2DAsync(A, (size_t)d->ld_r * 4, Ut_host, (size_t)d->n_rows * 4, (size_t)d->n_rows * 4, k,
                                     cudaMemcpyHostToDevice, s));
-  float* A_rs = nullptr;
-  const int a_tiles = (d->ld_r + 511) / 512;
-  if (tf32) {
+  if (v.form != Form::FP32) {     // pieces of the (signed) rows; on f16 datasets two fp16 pieces with group scales
     A_hi = static_cast<float*>(h->dev_buf("proj.A_hi", nr * 4));
     A_lo = static_cast<float*>(h->dev_buf("proj.A_lo", nr * 4));
     if (!A_hi || !A_lo) return -2;
-    if (d->f16) {            // f16 datasets keep C^T as fp16 only: two fp16 pieces of the (signed) rows, group scales
-      A_rs = static_cast<float*>(h->dev_buf("proj.A_rs", sizeof(float) * (size_t)k * a_tiles));
+    if (v.form == Form::F16_EXACT) {
+      A_rs = static_cast<float*>(h->dev_buf("proj.A_rs", sizeof(float) * (size_t)k * ((d->ld_r + 511) / 512)));
       if (!A_rs) return -2;
-      CNMF_TRY(launch_emit_f16(A, k, d->n_rows, d->ld_r, d->exact ? d->row_scale : nullptr, A_hi, A_lo, A_rs, a_tiles, s));
-    } else {
-      CNMF_TRY(launch_split_scaled(A, A_hi, A_lo, k, d->ld_r, d->exact ? d->row_scale : nullptr, s));
     }
+    CNMF_TRY(make_pieces(v.form, A, k, d->n_rows, d->ld_r, v.scale_r, A_hi, A_lo, A_rs, s));
     h->launches += 1;
   }
   GemmArgs g{};
@@ -416,28 +386,14 @@ int cnmf_project_rows(cnmf_dataset_t d, int k, const float* Ut_host, float* out_
     if (tiles < 2 * h->sm_count) splits = (2 * h->sm_count + tiles - 1) / tiles;
     splits = std::min(splits, std::max(1, ((d->n_rows + 31) / 32) / 8));
     splits = std::min(splits, 32);
-    splits = gemm_effective_splits(d->n_rows, splits, d->f16 ? 1 : 0);
+    splits = gemm_effective_splits(d->n_rows, splits, v.form == Form::F16_EXACT ? 1 : 0);
   }
   g.splits = g.splits_effective = splits;
   g.c_split_stride = (long long)k * d->ld_c;
   float* C = static_cast<float*>(h->dev_buf("proj.C", (size_t)splits * k * d->ld_c * 4));
   if (!C) return -2;
   g.C = C;
-  if (tf32) {
-    g.A_hi = A_hi; g.A_lo = A_lo; g.B_hi = d->Xt_hi; g.B_lo = d->Xt_lo;
-    g.b_exact = d->exact ? 1 : 0;
-    g.out_col_scale = d->exact ? d->col_scale : nullptr;
-    if (d->f16) {
-      g.f16 = 1;
-      g.B_hi = static_cast<const float*>(d->Xt_h16);
-      g.a_tile_scale = A_rs;
-      g.a_tiles = a_tiles;
-    }
-    CNMF_TRY(gemm_tf32x3(g, s));
-  } else {
-    g.A_hi = A; g.B_hi = d->Xt;
-    CNMF_TRY(gemm_fp32_simt(g, s));
-  }
+  CNMF_TRY(form_gemm(v.form, g, A, A_hi, A_lo, A_rs, v.B_cols, v.scale_c, s));
   h->launches += 1;
   std::vector<float> tmp((size_t)splits * k * d->ld_c);
   CNMF_CUDA_CHECK(cudaMemcpyAsync(tmp.data(), C, tmp.size() * 4, cudaMemcpyDeviceToHost, s));
@@ -463,6 +419,10 @@ int cnmf_gemm_abt_host(cnmf_handle_t h, int precision, const float* A, const flo
   CNMF_REQUIRE(!b_exact || f16 || precision == CNMF_PRECISION_TF32X3, "gemm_abt_host: b_exact needs tf32x3 or f16x2");
   const bool exact = f16 || b_exact;
   CNMF_REQUIRE(exact || (!k_scale && !out_col_scale), "gemm_abt_host: k_scale / out_col_scale need an exact form");
+  // the dataset form whose GEMM this runs; precisions other than tf32x3 and f16x2 run the fp32 path
+  const Form form = f16 ? Form::F16_EXACT
+                  : precision != CNMF_PRECISION_TF32X3 ? Form::FP32
+                  : b_exact ? Form::TF32_EXACT : Form::TF32;
   cudaStream_t s = as_stream(stream);
   CNMF_CUDA_CHECK(cudaSetDevice(h->device));
   const int lda = pad_ld(Kd), ldc = pad_ld(N);
@@ -473,9 +433,10 @@ int cnmf_gemm_abt_host(cnmf_handle_t h, int precision, const float* A, const flo
   float* dAl = static_cast<float*>(h->dev_buf("gemmtest.Al", na * 4));
   float* dBh = static_cast<float*>(h->dev_buf("gemmtest.Bh", nb * 4));
   float* dBl = static_cast<float*>(h->dev_buf("gemmtest.Bl", nb * 4));
-  const int se = gemm_effective_splits(Kd, splits, precision == CNMF_PRECISION_F16X2 ? 1 : 0);
+  const int se = gemm_effective_splits(Kd, splits, f16 ? 1 : 0);
   float* dC = static_cast<float*>(h->dev_buf("gemmtest.C", (size_t)se * M * ldc * 4));
-  if (!dA || !dB || !dAh || !dAl || !dBh || !dBl || !dC) return -2;
+  float* dRs = static_cast<float*>(h->dev_buf("gemmtest.rs", sizeof(float) * (size_t)M * ((lda + 511) / 512)));
+  if (!dA || !dB || !dAh || !dAl || !dBh || !dBl || !dC || !dRs) return -2;
   CNMF_CUDA_CHECK(cudaMemsetAsync(dA, 0, na * 4, s));
   CNMF_CUDA_CHECK(cudaMemsetAsync(dB, 0, nb * 4, s));
   CNMF_CUDA_CHECK(cudaMemcpy2DAsync(dA, (size_t)lda * 4, A, (size_t)Kd * 4, (size_t)Kd * 4, M, cudaMemcpyHostToDevice, s));
@@ -495,32 +456,23 @@ int cnmf_gemm_abt_host(cnmf_handle_t h, int precision, const float* A, const flo
     CNMF_CUDA_CHECK(cudaMemsetAsync(dCs, 0, (size_t)ldc * 4, s));
     CNMF_CUDA_CHECK(cudaMemcpyAsync(dCs, out_col_scale, (size_t)N * 4, cudaMemcpyHostToDevice, s));
   }
-  CNMF_TRY(launch_split_scaled(dA, dAh, dAl, M, lda, dKs, s));
-  CNMF_TRY(launch_split_tf32(dB, dBh, dBl, (long long)nb, s));
+  // B as a dataset of that form holds it: fp16 (integers <= 2048), tf32 pieces (exact forms read only hi), or as is
+  if (f16) CNMF_TRY(launch_to_half(dB, dBh, (long long)nb, s));
+  else if (form != Form::FP32) CNMF_TRY(launch_split_tf32(dB, dBh, dBl, (long long)nb, s));
+  CNMF_TRY(make_pieces(form, dA, M, Kd, lda, dKs, dAh, dAl, dRs, s));
   CNMF_CUDA_CHECK(cudaMemsetAsync(dC, 0xff, (size_t)se * M * ldc * 4, s));   // NaN pattern: unwritten outputs show up
   GemmArgs g{};
   g.M = M; g.N = N; g.Kd = Kd; g.lda = lda; g.ldb = lda; g.ldc = ldc;
   g.C = dC; g.c_split_stride = (long long)M * ldc; g.splits = splits; g.splits_effective = se;
-  g.out_col_scale = dCs;
-  if (f16) {
-    const int tiles = (lda + 511) / 512;
-    float* dRs = static_cast<float*>(h->dev_buf("gemmtest.rs", sizeof(float) * (size_t)M * tiles));
-    if (!dRs) return -2;
-    CNMF_TRY(launch_emit_f16(dA, M, Kd, lda, dKs, dAh, dAl, dRs, tiles, s));
-    CNMF_TRY(launch_to_half(dB, dBh, (long long)nb, s));
-    g.A_hi = dAh; g.A_lo = dAl; g.B_hi = dBh; g.b_exact = 1; g.f16 = 1; g.a_tile_scale = dRs; g.a_tiles = tiles;
-  } else if (precision == CNMF_PRECISION_TF32X3) {
-    g.A_hi = dAh; g.A_lo = dAl; g.B_hi = dBh; g.B_lo = b_exact ? nullptr : dBl; g.b_exact = b_exact ? 1 : 0;
-  } else { g.A_hi = dA; g.B_hi = dB; }
-  const bool tc = f16 || precision == CNMF_PRECISION_TF32X3;
+  const Operand Bop{dB, dBh, dBl, N, Kd, lda};
   cudaEvent_t e0, e1;
   CNMF_CUDA_CHECK(cudaEventCreate(&e0));
   CNMF_CUDA_CHECK(cudaEventCreate(&e1));
   if (reps < 1) reps = 1;
-  int rc = tc ? gemm_tf32x3(g, s) : gemm_fp32_simt(g, s);   // warm-up + result
+  int rc = form_gemm(form, g, dA, dAh, dAl, dRs, Bop, dCs, s);   // warm-up + result
   if (rc == 0 && reps > 1) {
     cudaEventRecord(e0, s);
-    for (int i = 0; i < reps && rc == 0; ++i) rc = tc ? gemm_tf32x3(g, s) : gemm_fp32_simt(g, s);
+    for (int i = 0; i < reps && rc == 0; ++i) rc = form_gemm(form, g, dA, dAh, dAl, dRs, Bop, dCs, s);
     cudaEventRecord(e1, s);
   }
   h->launches += reps;

@@ -62,8 +62,8 @@ extern "C" int cnmf_update_step_host(cnmf_handle_t h, const cnmf_update_step_arg
   double* d_gpart = static_cast<double*>(h->dev_buf("unit.gram_part", sizeof(double) * (size_t)RR * std::max(chunks, gchunks) * kp * kp));
   double* d_spart = static_cast<double*>(h->dev_buf("unit.scal_part", sizeof(double) * (size_t)RR * chunks));
   float* d_ps = static_cast<float*>(h->dev_buf("unit.piece_scale", (size_t)ld * 4));
-  void* d_hi = h->dev_buf("unit.pieces_hi", nf * piece_bytes);
-  void* d_lo = h->dev_buf("unit.pieces_lo", nf * piece_bytes);
+  float* d_hi = static_cast<float*>(h->dev_buf("unit.pieces_hi", nf * piece_bytes));
+  float* d_lo = static_cast<float*>(h->dev_buf("unit.pieces_lo", nf * piece_bytes));
   float* d_ts = static_cast<float*>(h->dev_buf("unit.tile_scale", sizeof(float) * (size_t)SK * n_ktiles));
   if (!d_meta || !d_F || !d_num || !d_gin || !d_gout || !d_scal || !d_gpart || !d_spart || !d_ps || !d_hi || !d_lo || !d_ts)
     return -2;
@@ -93,18 +93,20 @@ extern "C" int cnmf_update_step_host(cnmf_handle_t h, const cnmf_update_step_arg
   const BatchMeta b{d_meta, d_meta + R, d_meta + 2 * R, d_meta + 3 * R, R, kp};
   const float* pscale = a->piece_scale ? d_ps : nullptr;
   const bool fused = a->gram == CNMF_UNIT_GRAM_FUSED;
+  // the dataset form whose pieces the mode names
+  const Form form = a->pieces == CNMF_UNIT_PIECES_TF32 ? Form::TF32
+                  : a->pieces == CNMF_UNIT_PIECES_F16 ? Form::F16_EXACT : Form::FP32;
   FactorView f{};
   f.F = d_F;
   f.n = n; f.ld = ld; f.piece_scale = pscale;
-  if (a->pieces == CNMF_UNIT_PIECES_TF32) { f.F_hi = static_cast<float*>(d_hi); f.F_lo = static_cast<float*>(d_lo); }
+  if (a->pieces == CNMF_UNIT_PIECES_TF32) { f.F_hi = d_hi; f.F_lo = d_lo; }
   if (a->pieces == CNMF_UNIT_PIECES_F16 && fused) { f.P_hi = d_hi; f.P_mid = d_lo; f.tile_scale = d_ts; f.n_ktiles = n_ktiles; }
   f.cpb = cpb; f.gcpb = gcpb;
   const long long sstride = (long long)nf;
 
   if (none) {
     // start of a solve: pieces of the initial factors (solve_batched: split or emit_pieces), stand-alone Gram, <NUM, F>
-    if (a->pieces == CNMF_UNIT_PIECES_TF32) CNMF_TRY(launch_split_scaled(d_F, f.F_hi, f.F_lo, SK, ld, pscale, s));
-    if (a->pieces == CNMF_UNIT_PIECES_F16) CNMF_TRY(launch_emit_f16(d_F, SK, n, ld, pscale, d_hi, d_lo, d_ts, n_ktiles, s));
+    CNMF_TRY(make_pieces(form, d_F, SK, n, ld, pscale, d_hi, d_lo, d_ts, s));
     if (a->gram == CNMF_UNIT_GRAM_STANDALONE) {
       CNMF_TRY(launch_gram_partial(f, b, d_gpart, s));
       CNMF_TRY(launch_finalize(d_gpart, d_gout, nullptr, nullptr, gchunks, b, s));
@@ -127,7 +129,7 @@ extern "C" int cnmf_update_step_host(cnmf_handle_t h, const cnmf_update_step_arg
     }
     // f16 pieces: emitted by the Gram-fused launch itself, else by the stand-alone kernel after it (update() of the solver)
     if (a->pieces == CNMF_UNIT_PIECES_F16 && !fused)
-      CNMF_TRY(launch_emit_f16(d_F, SK, n, ld, pscale, d_hi, d_lo, d_ts, n_ktiles, s));
+      CNMF_TRY(make_pieces(form, d_F, SK, n, ld, pscale, d_hi, d_lo, d_ts, s));
   }
   h->launches += 1;
 

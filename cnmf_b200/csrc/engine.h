@@ -8,6 +8,20 @@
 
 #include "../../include/cnmf_b200.h"
 #include "common.cuh"
+#include "gemm.h"
+
+namespace cnmf {
+
+// How a dense dataset feeds the tensor cores, decided once per dataset (dataset_resolve_form):
+//   FP32        X, Xt                        factor used as is        gemm_fp32_simt
+//   TF32        X, X_hi / X_lo, Xt_hi / lo   tf32 hi / lo pieces      gemm_tf32x3, 3 passes
+//   TF32_EXACT  X, C = X_hi, C^T = Xt_hi     tf32 pieces of F * scale gemm_tf32x3, exact B, 2 passes
+//   F16_EXACT   X, C, C^T as fp16            fp16 pieces of F * scale gemm_tf32x3, f16 = 1
+// The exact forms hold X = diag(row_scale) C diag(col_scale) with C small non-negative integers.
+enum class Form { FP32, TF32, TF32_EXACT, F16_EXACT };
+inline bool form_exact(Form f) { return f == Form::TF32_EXACT || f == Form::F16_EXACT; }
+
+}  // namespace cnmf
 
 struct cnmf_handle_s {
   int device = 0;
@@ -52,30 +66,25 @@ struct cnmf_handle_s {
 // A cells x genes matrix resident on the device in the forms the two GEMM orientations need.
 //   X   (n_rows x ld_c)  : K-major over columns  -> B operand of  NUM_rows = F_cols * X^T
 //   Xt  (n_cols x ld_r)  : K-major over rows     -> B operand of  NUM_cols = F_rows * X
-// fp32 mode keeps X and Xt; tf32x3 mode keeps X (full, for column ops) + the hi/lo pieces of both.
+// The resident operands follow the dataset's form (cnmf::Form); X is always kept (column operations, derived datasets).
 struct cnmf_dataset_s {
   cnmf_handle_s* h = nullptr;
   int n_rows = 0, n_cols = 0;
   int ld_c = 0;   // row stride of X  (>= n_cols)
   int ld_r = 0;   // row stride of Xt (>= n_rows)
-  int precision = 0;
+  int precision = 0;                        // CNMF_PRECISION_* the dataset was created with
+  cnmf::Form form = cnmf::Form::FP32;
   float *X = nullptr, *Xt = nullptr;
   float *X_hi = nullptr, *X_lo = nullptr, *Xt_hi = nullptr, *Xt_lo = nullptr;
-  // "exact" datasets (tf32x3 only): X = diag(row_scale) * C * diag(col_scale) with C small non-negative integers
-  // (what HVG-normalised counts and TPM are).  Then X_hi / Xt_hi hold C / C^T -- exactly representable in tf32,
-  // no lo piece -- the scales are folded into the factor pieces / applied to the GEMM output, and every big
-  // product needs 2 tensor-core passes instead of 3.  Either scale may be nullptr (= 1).
-  bool exact = false;
-  bool allow_exact = true;
-  // f16x2 precision: requested at creation (want_f16); active (f16) once the dataset turned out exact.  X_h16 / Xt_h16
-  // hold the integer matrices C / C^T as fp16 (same shapes and element strides as X_hi / Xt_hi)
-  bool want_f16 = false, f16 = false;
-  bool drop_tf32 = false;       // f16 datasets: X_hi / Xt_hi are released once the fp16 matrices exist
+  // exact forms (what HVG-normalised counts and TPM are): X_hi / Xt_hi hold C / C^T -- exactly representable in tf32, no
+  // lo piece -- and the scales are folded into the factor pieces / applied to the GEMM output.  On F16_EXACT, X_h16 /
+  // Xt_h16 hold C / C^T as fp16 (same shapes and element strides) and the fp32 copies are released.  Either scale may
+  // be nullptr (= 1); both are nullptr on the other forms.
   void *X_h16 = nullptr, *Xt_h16 = nullptr;
   float *row_scale = nullptr, *col_scale = nullptr;    // lengths ld_r / ld_c, zero padded
   double sum = 0.0, sum_sq = 0.0;
   // sparse datasets (cnmf_dataset_create_csc): X stays canonical CSC and none of the dense forms above exist
-  // (X == nullptr).  `exact` and the scales are still detected, so that cnmf_dataset_from_columns builds the same
+  // (X == nullptr).  The form and the scales are still detected, so that cnmf_dataset_from_columns builds the same
   // dense dataset from it as from the dense form of the matrix.  col_sums: per column sum(x) then sum(x^2), fp64.
   // Columns are cut into chunks of at most CSC_CHUNK entries (item_ptr: first chunk of each column, n_cols + 1):
   // csc_project_kernel gives one warp to a chunk.
@@ -88,6 +97,10 @@ struct cnmf_dataset_s {
   int* item_ptr = nullptr;
   int n_items = 0;
   std::vector<std::pair<void*, size_t>> owned;
+
+  // every creator starts here: shape, padded strides and the creation precision
+  cnmf_dataset_s(cnmf_handle_s* h_, int rows, int cols, int precision_)
+      : h(h_), n_rows(rows), n_cols(cols), ld_c(cnmf::pad_ld(cols)), ld_r(cnmf::pad_ld(rows)), precision(precision_) {}
 };
 
 namespace cnmf {
@@ -96,9 +109,8 @@ inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s
 
 struct Operand {     // a K-major matrix as the GEMM sees it
   const float* full;
-  const float* hi;     // tf32 hi piece, or the exact integer matrix when `exact`
+  const float* hi;     // tf32 hi piece, or the exact integer matrix C (as fp16 on F16_EXACT)
   const float* lo;
-  const void* h16;     // the exact integer matrix as fp16 (f16x2 datasets), else nullptr
   int rows, cols, ld;
 };
 
@@ -109,13 +121,31 @@ struct DataView {
   Operand B_cols;   // n_c x n_r : B operand when updating Fc (reduction over n_r)
   int n_r, n_c, ld_r, ld_c;
   double sum, sum_sq;
-  bool exact;               // both operands hold exact integers; scales below complete X
-  bool f16;                 // fp16 operand path active (exact datasets created with CNMF_PRECISION_F16X2)
+  Form form;                // FP32 on sparse datasets: their solves run no GEMM and make no pieces
   const float* scale_r;     // per row-item scale (length ld_r) or nullptr
   const float* scale_c;     // per column-item scale (length ld_c) or nullptr
 };
 
 DataView make_view(const cnmf_dataset_s* d, bool transposed);
+
+// C = A * B^T in the given form: g holds the shape, C and split-K; this fills the operands (factor A in fp32, its pieces
+// and tile scales from make_pieces; out_scale on the output columns of the exact forms) and launches the GEMM
+int form_gemm(Form form, GemmArgs g, const float* A, const float* A_hi, const float* A_lo, const float* a_tile_scale,
+              const Operand& B, const float* out_scale, cudaStream_t s);
+// operand pieces of F diag(scale) (rows x ld, n valid columns) for the form: none, tf32 split, or two fp16 pieces with
+// tile scales (rows x ceil(ld / 512)); at most one launch
+int make_pieces(Form form, const float* F, int rows, int n, int ld, const float* scale, float* hi, float* lo,
+                float* tile_scale, cudaStream_t s);
+
+// ---- datasets: capi.cu
+int dataset_alloc(cnmf_dataset_s* d, float** p, size_t elems);   // owned by d, from the handle's pool if one fits
+// form, operands and sums from d->X (resident, padding zeroed); exact: inherited (scales set), no detection
+int dataset_finish(cnmf_dataset_s* d, cudaStream_t s, bool exact = false);
+// d->form from the creation precision and, where it allows an exact form and `exact` is not yet known, exact-count
+// detection on the dense or CSC matrix (synchronises)
+int dataset_resolve_form(cnmf_dataset_s* d, bool exact, cudaStream_t s);
+// params.precision must be FP32 or, for every tensor-core precision, TF32X3
+int check_params_precision(const cnmf_dataset_s* d, const cnmf_nmf_params* p);
 
 struct SolveIO {
   int R = 0;
@@ -152,8 +182,9 @@ int csc_project(const cnmf_dataset_s* d, const float* U, int k, int kp, float* o
 int stage_rows(cnmf_handle_s* h, const float* F, int k, int n, int ld, int kp, float* U, cudaStream_t s);
 // per column sum(x), sum(x^2) into d->col_sums and the dataset totals into d->sum / d->sum_sq (synchronises)
 int csc_col_stats(cnmf_dataset_s* d, cudaStream_t s);
-// exact-count detection on the stored entries: the test dataset_finish runs on the dense form (synchronises)
-int csc_detect_exact(cnmf_dataset_s* d, cudaStream_t s);
+// exact-count detection on the stored entries: the test dataset_resolve_form runs on the dense form; sets the scale of
+// an exact matrix (synchronises)
+int csc_detect_exact(cnmf_dataset_s* d, cudaStream_t s, bool* exact);
 // dst (n_rows x ld_dst, zeroed by the caller)[:, c] = X[:, cols[c]] * scale[c]
 int csc_gather_cols(const cnmf_dataset_s* d, const int* cols, const float* scale, int n_cols, float* dst, int ld_dst,
                     cudaStream_t s);

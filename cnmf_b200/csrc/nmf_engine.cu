@@ -20,8 +20,9 @@
 namespace cnmf {
 
 DataView make_view(const cnmf_dataset_s* d, bool transposed) {
-  Operand X{d->X, d->X_hi, d->X_lo, d->f16 ? d->X_h16 : nullptr, d->n_rows, d->n_cols, d->ld_c};
-  Operand Xt{d->Xt, d->Xt_hi, d->Xt_lo, d->f16 ? d->Xt_h16 : nullptr, d->n_cols, d->n_rows, d->ld_r};
+  const bool f16 = d->form == Form::F16_EXACT;
+  Operand X{d->X, f16 ? static_cast<const float*>(d->X_h16) : d->X_hi, d->X_lo, d->n_rows, d->n_cols, d->ld_c};
+  Operand Xt{d->Xt, f16 ? static_cast<const float*>(d->Xt_h16) : d->Xt_hi, d->Xt_lo, d->n_cols, d->n_rows, d->ld_r};
   DataView v;
   if (!transposed) {
     v.B_rows = X; v.B_cols = Xt;
@@ -32,11 +33,41 @@ DataView make_view(const cnmf_dataset_s* d, bool transposed) {
   }
   v.sum = d->sum;
   v.sum_sq = d->sum_sq;
-  v.exact = d->exact;
-  v.f16 = d->f16;
-  v.scale_r = transposed ? d->col_scale : d->row_scale;
-  v.scale_c = transposed ? d->row_scale : d->col_scale;
+  // a sparse dataset keeps its detected form and scales for cnmf_dataset_from_columns; its solves (refits) take the
+  // one product from csc_project and run the fp32 solver code: no GEMM, no pieces, no scales
+  v.form = d->sparse ? Form::FP32 : d->form;
+  v.scale_r = d->sparse ? nullptr : transposed ? d->col_scale : d->row_scale;
+  v.scale_c = d->sparse ? nullptr : transposed ? d->row_scale : d->col_scale;
   return v;
+}
+
+int form_gemm(Form form, GemmArgs g, const float* A, const float* A_hi, const float* A_lo, const float* a_tile_scale,
+              const Operand& B, const float* out_scale, cudaStream_t s) {
+  switch (form) {
+    case Form::FP32:
+      g.A_hi = A; g.B_hi = B.full;
+      return gemm_fp32_simt(g, s);
+    case Form::TF32:
+      g.B_lo = B.lo;
+      break;
+    case Form::F16_EXACT:      // A_hi / A_lo hold the two fp16 pieces of the row-normalised factor, B.hi fp16 C
+      g.f16 = 1; g.a_tile_scale = a_tile_scale; g.a_tiles = (g.lda + 511) / 512;
+      [[fallthrough]];
+    case Form::TF32_EXACT:
+      g.b_exact = 1; g.out_col_scale = out_scale;
+      break;
+  }
+  g.A_hi = A_hi; g.A_lo = A_lo; g.B_hi = B.hi;
+  return gemm_tf32x3(g, s);
+}
+
+int make_pieces(Form form, const float* F, int rows, int n, int ld, const float* scale, float* hi, float* lo,
+                float* tile_scale, cudaStream_t s) {
+  switch (form) {
+    case Form::FP32: return 0;
+    case Form::F16_EXACT: return launch_emit_f16(F, rows, n, ld, scale, hi, lo, tile_scale, (ld + 511) / 512, s);
+    default: return launch_split_scaled(F, hi, lo, rows, ld, scale, s);
+  }
 }
 
 namespace {
@@ -46,10 +77,10 @@ struct GemmPlan {
   long long split_stride;   // elements
 };
 
-// C[z] (SK x N) = A (SK x Kd) * B (N x Kd)^T
-int run_gemm(cnmf_handle_s* h, int precision, const float* A, const float* A_hi, const float* A_lo, int SK, int lda,
-             const Operand& B, float* C, int ldc, const GemmPlan& plan, bool exact, const float* out_scale,
-             bool f16, const float* a_tile_scale, cudaStream_t s) {
+// C[z] (SK x N) = A (SK x Kd) * B (N x Kd)^T, counted and profiled as a batched GEMM
+int run_gemm(cnmf_handle_s* h, Form form, const float* A, const float* A_hi, const float* A_lo, const float* a_tile_scale,
+             int SK, int lda, const Operand& B, const float* out_scale, float* C, int ldc, const GemmPlan& plan,
+             cudaStream_t s) {
   GemmArgs g{};
   g.M = SK; g.N = B.rows; g.Kd = B.cols;
   g.lda = lda; g.ldb = B.ld; g.ldc = ldc;
@@ -59,22 +90,7 @@ int run_gemm(cnmf_handle_s* h, int precision, const float* A, const float* A_hi,
   g.splits_effective = plan.splits;
   h->launches += 1;
   const int slot = h->prof_begin(s, 2.0 * (double)g.M * (double)g.N * (double)g.Kd);
-  int rc;
-  if (precision == CNMF_PRECISION_TF32X3) {
-    g.A_hi = A_hi; g.A_lo = A_lo; g.B_hi = B.hi; g.B_lo = B.lo;
-    g.b_exact = exact ? 1 : 0;
-    g.out_col_scale = exact ? out_scale : nullptr;
-    if (f16) {       // A_hi / A_lo hold the two fp16 pieces of the row-normalised factor, B its fp16 integer matrix
-      g.f16 = 1;
-      g.B_hi = static_cast<const float*>(B.h16);
-      g.a_tile_scale = a_tile_scale;
-      g.a_tiles = (lda + 511) / 512;
-    }
-    rc = gemm_tf32x3(g, s);
-  } else {
-    g.A_hi = A; g.A_lo = nullptr; g.B_hi = B.full; g.B_lo = nullptr;
-    rc = gemm_fp32_simt(g, s);
-  }
+  const int rc = form_gemm(form, g, A, A_hi, A_lo, a_tile_scale, B, out_scale, s);
   h->prof_end(s, slot);
   return rc;
 }
@@ -88,8 +104,8 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
   CNMF_REQUIRE(p.solver == CNMF_SOLVER_MU || p.solver == CNMF_SOLVER_CD, "solve: unknown solver");
   CNMF_REQUIRE(p.max_iter >= 1, "solve: max_iter must be >= 1");
   CNMF_REQUIRE(!io.num_rows || !io.update_cols, "solve: a caller-computed row product needs update_cols = false");
-  const bool tf32 = p.precision == CNMF_PRECISION_TF32X3;
-  const bool f16 = tf32 && v.f16;       // exact-count dataset created with CNMF_PRECISION_F16X2: f16 products
+  const bool tf32 = v.form != Form::FP32;        // the factors have operand pieces
+  const bool f16 = v.form == Form::F16_EXACT;
   const bool mu = p.solver == CNMF_SOLVER_MU;
 
   // ---- slot tables (host mirrors); slot s holds restart rid[s] at packed rows [off[s], off[s]+k[s])
@@ -232,7 +248,7 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
   auto fr = [&]() {
     FactorView f{};
     f.F = wFr; f.F_hi = upd_pieces ? wFr_hi : nullptr; f.F_lo = upd_pieces ? wFr_lo : nullptr;
-    f.n = v.n_r; f.ld = v.ld_r; f.piece_scale = v.exact ? v.scale_r : nullptr;
+    f.n = v.n_r; f.ld = v.ld_r; f.piece_scale = v.scale_r;
     if (emit_in_update) { f.P_hi = wFr_hi; f.P_mid = wFr_lo; f.tile_scale = d_rs_r; f.n_ktiles = ktiles_r; }
     f.cpb = cpb_r; f.gcpb = gcpb_r;
     return f;
@@ -240,7 +256,7 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
   auto fc = [&]() {
     FactorView f{};
     f.F = wFc; f.F_hi = upd_pieces ? wFc_hi : nullptr; f.F_lo = upd_pieces ? wFc_lo : nullptr;
-    f.n = v.n_c; f.ld = v.ld_c; f.piece_scale = v.exact ? v.scale_c : nullptr;
+    f.n = v.n_c; f.ld = v.ld_c; f.piece_scale = v.scale_c;
     if (emit_in_update) { f.P_hi = wFc_hi; f.P_mid = wFc_lo; f.tile_scale = d_rs_c; f.n_ktiles = ktiles_c; }
     f.cpb = cpb_c; f.gcpb = gcpb_c;
     if (!io.update_cols) { f.F_hi = nullptr; f.F_lo = nullptr; }   // never rewritten
@@ -257,14 +273,16 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
   auto gram_after = [&](const FactorView& f, int side_is_c) -> int {   // Gram of a factor the update kernel just wrote
     return fuse ? 0 : gram_full(f, side_is_c);
   };
+  auto pieces = [&](int side_is_c) -> int {
+    return side_is_c ? make_pieces(v.form, wFc, SK, v.n_c, v.ld_c, v.scale_c, wFc_hi, wFc_lo, d_rs_c, s)
+                     : make_pieces(v.form, wFr, SK, v.n_r, v.ld_r, v.scale_r, wFr_hi, wFr_lo, d_rs_r, s);
+  };
   auto emit_pieces = [&](int side_is_c) -> int {   // fp16 pieces + row scales of a factor that was just (re)written
     if (!f16) return 0;
     h->launches += 1;
     const int n = side_is_c ? v.n_c : v.n_r;
     const int slot = h->prof_begin(s, 8.0 * (double)SK * (double)n, 1);   // fp32 in, two fp16 pieces out
-    const int rc = side_is_c
-        ? launch_emit_f16(wFc, SK, v.n_c, v.ld_c, v.exact ? v.scale_c : nullptr, wFc_hi, wFc_lo, d_rs_c, ktiles_c, s)
-        : launch_emit_f16(wFr, SK, v.n_r, v.ld_r, v.exact ? v.scale_r : nullptr, wFr_hi, wFr_lo, d_rs_r, ktiles_r, s);
+    const int rc = pieces(side_is_c);
     h->prof_end(s, slot);
     return rc;
   };
@@ -301,12 +319,10 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
   };
   auto gemm_rows = [&]() -> int {   // NUM_r = Fc * B_rows^T
     if (io.num_rows) return 0;      // computed by the caller
-    return run_gemm(h, p.precision, wFc, wFc_hi, wFc_lo, SK, v.ld_c, v.B_rows, NUMr, v.ld_r, plan_r, v.exact, v.scale_r,
-                    f16, d_rs_c, s);
+    return run_gemm(h, v.form, wFc, wFc_hi, wFc_lo, d_rs_c, SK, v.ld_c, v.B_rows, v.scale_r, NUMr, v.ld_r, plan_r, s);
   };
   auto gemm_cols = [&]() -> int {   // NUM_c = Fr * B_cols^T
-    return run_gemm(h, p.precision, wFr, wFr_hi, wFr_lo, SK, v.ld_r, v.B_cols, NUMc, v.ld_c, plan_c, v.exact, v.scale_c,
-                    f16, d_rs_r, s);
+    return run_gemm(h, v.form, wFr, wFr_hi, wFr_lo, d_rs_r, SK, v.ld_r, v.B_cols, v.scale_c, NUMc, v.ld_c, plan_c, s);
   };
 
   // gathers `cnt` restarts' rows: dst[dst_off[i] ..] <- src[src_off[i] ..].  Index triples go through a pinned
@@ -405,7 +421,7 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
     CNMF_TRY(gather(wFc, resFc, f_src, f_dst, f_k, v.ld_c));
     CNMF_TRY(gather(wFr, aFr, l_src, l_dst, l_k, v.ld_r));          // live restarts -> packed front of the alt buffers
     CNMF_TRY(gather(wFc, aFc, l_src, l_dst, l_k, v.ld_c));
-    if (tf32 && !f16) {
+    if (upd_pieces) {
       CNMF_TRY(gather(wFr_hi, aFr_hi, l_src, l_dst, l_k, v.ld_r));
       CNMF_TRY(gather(wFr_lo, aFr_lo, l_src, l_dst, l_k, v.ld_r));
       CNMF_TRY(gather(wFc_hi, aFc_hi, l_src, l_dst, l_k, v.ld_c));
@@ -438,9 +454,9 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
 
   const float l1W = (float)p.l1_reg_W, l2W = (float)p.l2_reg_W, l1H = (float)p.l1_reg_H, l2H = (float)p.l2_reg_H;
   int it = 0;
-  if (upd_pieces) {                // pieces of the starting factors; afterwards the update kernels write them
-    CNMF_TRY(launch_split_scaled(wFr, wFr_hi, wFr_lo, SK, v.ld_r, v.exact ? v.scale_r : nullptr, s));
-    CNMF_TRY(launch_split_scaled(wFc, wFc_hi, wFc_lo, SK, v.ld_c, v.exact ? v.scale_c : nullptr, s));
+  if (upd_pieces) {                // tf32 pieces of the starting factors; afterwards the update kernels write them
+    CNMF_TRY(pieces(0));
+    CNMF_TRY(pieces(1));
     h->launches += 2;
   }
   CNMF_TRY(emit_pieces(0));        // f16: fp16 pieces of the starting factors

@@ -10,7 +10,6 @@
 //   csc_scaled_col_sums_kernel                         per-column sums of the TPM, formed entry by entry
 // Products and sums run in fp64 in a fixed order, without floating-point atomics: two runs are bit-identical.
 #include <algorithm>
-#include <cstdlib>
 #include <string>
 #include <type_traits>
 #include <vector>
@@ -19,8 +18,6 @@
 #include "nmf_kernels.cuh"
 
 using namespace cnmf;
-
-extern "C" int cnmf_dataset_alloc_internal(cnmf_dataset_t d, float** p, size_t elems);   // capi.cu
 
 namespace {
 
@@ -323,11 +320,11 @@ int csc_col_stats(cnmf_dataset_s* d, cudaStream_t s) {
   return 0;
 }
 
-int csc_detect_exact(cnmf_dataset_s* d, cudaStream_t s) {
+int csc_detect_exact(cnmf_dataset_s* d, cudaStream_t s, bool* exact) {
   cnmf_handle_s* h = d->h;
   float *cmin = nullptr, *rmin = nullptr;
-  CNMF_TRY(cnmf_dataset_alloc_internal(d, &cmin, (size_t)d->ld_c));
-  CNMF_TRY(cnmf_dataset_alloc_internal(d, &rmin, (size_t)d->ld_r));
+  CNMF_TRY(dataset_alloc(d, &cmin, (size_t)d->ld_c));
+  CNMF_TRY(dataset_alloc(d, &rmin, (size_t)d->ld_r));
   int* n_bad = static_cast<int*>(h->dev_buf("dataset.nbad", sizeof(int) * 2));
   if (!n_bad) return -2;
   CNMF_CUDA_CHECK(cudaMemsetAsync(cmin, 0x7f, sizeof(float) * d->n_cols, s));   // 0x7f7f7f7f: a huge finite float
@@ -345,8 +342,8 @@ int csc_detect_exact(cnmf_dataset_s* d, cudaStream_t s) {
   int bad[2] = {1, 1};
   CNMF_CUDA_CHECK(cudaMemcpyAsync(bad, n_bad, sizeof(int) * 2, cudaMemcpyDeviceToHost, s));
   CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
-  if (bad[0] == 0) { d->exact = true; d->col_scale = cmin; }
-  else if (bad[1] == 0) { d->exact = true; d->row_scale = rmin; }
+  if (bad[0] == 0) { *exact = true; d->col_scale = cmin; }
+  else if (bad[1] == 0) { *exact = true; d->row_scale = rmin; }
   return 0;
 }
 
@@ -412,22 +409,13 @@ int cnmf_dataset_create_csc(cnmf_handle_t h, int n_rows, int n_cols, long long n
     CNMF_REQUIRE(row_idx[j] >= 0 && row_idx[j] < n_rows, "dataset_create_csc: row index out of range");
   cudaStream_t s = as_stream(stream);
   CNMF_CUDA_CHECK(cudaSetDevice(h->device));
-  auto* d = new cnmf_dataset_s();
-  d->h = h;
+  auto* d = new cnmf_dataset_s(h, n_rows, n_cols, precision);
   d->sparse = true;
-  d->n_rows = n_rows;
-  d->n_cols = n_cols;
-  d->ld_c = pad_ld(n_cols);
-  d->ld_r = pad_ld(n_rows);
   d->nnz = nnz;
   d->n_items = (int)items;
-  d->allow_exact = precision != CNMF_PRECISION_TF32X3_GENERAL;
-  d->want_f16 = precision == CNMF_PRECISION_F16X2;
-  d->precision = (precision == CNMF_PRECISION_TF32X3_GENERAL || precision == CNMF_PRECISION_F16X2) ? CNMF_PRECISION_TF32X3
-                                                                                                : precision;
   auto alloc = [&](auto** p, size_t bytes) {
     float* q = nullptr;
-    const int rc = cnmf_dataset_alloc_internal(d, &q, (bytes + 3) / 4);
+    const int rc = dataset_alloc(d, &q, (bytes + 3) / 4);
     *p = reinterpret_cast<std::remove_pointer_t<decltype(p)>>(q);
     return rc;
   };
@@ -450,10 +438,7 @@ int cnmf_dataset_create_csc(cnmf_handle_t h, int n_rows, int n_cols, long long n
   if (rc == 0) rc = upload(d->vals, values, sizeof(float) * (size_t)nnz);
   if (rc == 0) rc = upload(d->item_ptr, item_ptr.data(), sizeof(int) * (n_cols + 1));
   if (rc == 0) rc = csc_col_stats(d, s);    // synchronises: item_ptr may go out of scope afterwards
-  static const bool allow_exact = [] { const char* e = std::getenv("CNMF_EXACT"); return !(e && e[0] == '0'); }();
-  // the condition under which dataset_finish tests the dense form
-  if (rc == 0 && d->precision == CNMF_PRECISION_TF32X3 && allow_exact && d->allow_exact && n_rows <= 65535 * 64)
-    rc = csc_detect_exact(d, s);
+  if (rc == 0) rc = dataset_resolve_form(d, false, s);
   if (rc != 0) {
     cudaStreamSynchronize(s);
     cnmf_dataset_destroy(d);
