@@ -15,14 +15,17 @@
 //   X H^T   (sklearn _nmf.py:538, :380)  ->  A = H_batch (SK x G),   B = X   (cells x G)
 //   W^T X   (sklearn _nmf.py:634, :380)  ->  A = W^T_batch (SK x N), B = X^T (G x cells), split-K
 //
-// Structure (one CTA per SM, persistent over a static tile schedule, 384 threads = 3 warpgroups; the CTAs run in
-// clusters of 2 whose tiles share an m-tile, and each CTA loads half of the shared A panel and multicasts it to both):
+// Structure (one CTA per SM, persistent over a static tile schedule of BM x 128 tiles, BM = 128 or 192; 128 + 2 BM
+// threads = 1 + BM / 64 warpgroups; the CTAs run in clusters of 2 whose tiles share an m-tile, and each CTA loads half
+// of the shared A panel and multicasts it to both):
 //   warpgroup 0     TMA producer (one thread): cp.async.bulk.tensor 2D, 128B-swizzled tiles, mbarrier full/empty ring,
 //                   a stage refilled only once both CTAs of the pair have released it
-//   warpgroups 1-2  consumers: rows [0, 64) / [64, 128) of the 128 x 128 tile, wgmma.mma_async m64n128 from shared
-//                   memory descriptors, fp32 fragment in registers, float2 stores.  Two named barriers make them take
-//                   turns issuing one k-block of MMAs each (ping-pong), so one warpgroup's chain drain and tile stores
-//                   run while the other's MMAs keep the tensor pipe busy.
+//   warpgroups 1-   consumers: rows [64 (w - 1), 64 w) of the tile, wgmma.mma_async m64n128 from shared memory
+//                   descriptors, fp32 fragment in registers, float2 stores.  Named barriers make them take turns in a
+//                   ring issuing one k-block of MMAs each (ping-pong), so one warpgroup's chain drain and tile stores
+//                   run while the others' MMAs keep the tensor pipe busy.
+//   At BM = 192 (512 threads) setmaxnreg moves the producer to 32 registers and the consumers to 160.  The launcher
+//   picks BM by shape (gemm_tf32x3 below); measured on one H100 SXM (700 W), DESIGN.md section 4.1.
 //
 // Accumulation accuracy.  The tensor core does not round its running sum to nearest: a long chain of MMAs on
 // non-negative data is biased low by about 3e-8 relative per MMA (2.3e-5 at K = 2048), far outside the 1e-4 parity
@@ -46,17 +49,20 @@ namespace cnmf {
 
 namespace {
 
-constexpr int BM = 128;          // rows of A per tile: two consumer warpgroups of 64
+// BM (rows of A per tile) is a template parameter: one consumer warpgroup per 64 rows, plus the producer warpgroup.
 constexpr int BN = 128;          // rows of B per tile (wgmma N)
 constexpr int BK = 32;           // fp32 elements per k-block = 128 B = one swizzle row
-constexpr int NUM_THREADS = 384;
 constexpr long long WAIT_TIMEOUT_CYCLES = 4000000000LL;   // ~2 s: a dead pipeline traps instead of hanging
 
+template <int BM>
+constexpr int num_threads() { return 128 * (1 + BM / 64); }
+
 // BEXACT: the B operand is exactly representable in tf32 / fp16 (e.g. integer counts), so it needs no "lo" piece:
-// 2 MMAs per k-step instead of 3, 48 KB stages (4 of them) instead of 64 KB (3).
-template <int STAGES, bool BEXACT>
+// 2 MMAs per k-step instead of 3.  Stages: 4 of 48 KB for the exact-B forms at BM = 128, 3 of 64 KB for them at
+// BM = 192 (24 KB per A piece), 3 of 64 KB for the general form (BM = 128 only).
+template <int BM, int STAGES, bool BEXACT>
 struct SmemLayout {
-  static constexpr int A_BYTES = BM * BK * 4;              // 16 KB
+  static constexpr int A_BYTES = BM * BK * 4;              // 16 KB (BM = 128) or 24 KB (BM = 192)
   static constexpr int B_BYTES = BN * BK * 4;              // 16 KB
   static constexpr int STAGE_BYTES = 2 * A_BYTES + (BEXACT ? 1 : 2) * B_BYTES;
   static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;  // full[STAGES], empty[STAGES], peer_free[STAGES]
@@ -86,12 +92,16 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// No printf on timeout: any call in the kernel makes ptxas serialise the wgmma pipeline.
+// No printf on timeout: any call in the kernel makes ptxas serialise the wgmma pipeline.  Only the producer's waits
+// trap: a trap in code after setmaxnreg.inc makes ptxas allocate that code at the launch-wide register count (and
+// spill).  A stalled consumer still ends in a trap, because the producer waits (with the timeout) for every stage to be
+// released before it leaves, and a consumer that stops releasing stages stalls it.
+template <bool TRAP>
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > WAIT_TIMEOUT_CYCLES) __trap();
+    if (TRAP && clock64() - t0 > WAIT_TIMEOUT_CYCLES) __trap();
   }
 }
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
@@ -149,6 +159,13 @@ __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
 __device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t count) {
   asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
+
+// Hand registers between warpgroups (all threads of the warpgroup, converged): the producer gives up what it never
+// uses so that the consumers can hold more than the launch-wide share.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -231,16 +248,18 @@ __host__ __device__ __forceinline__ void decode_item(int w, const TileOrder& o, 
 //
 // Fragment of consumer thread (warp w of its warpgroup, lane l): d[4j + e] is row 16w + l/4 (+8 for e >= 2),
 // column 8j + 2(l%4) + (e & 1) of the warpgroup's 64 x 128 block.
-template <int STAGES, bool BEXACT, bool F16>
+template <int BM, int STAGES, bool BEXACT, bool F16>
 __device__ __forceinline__ void
 gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMap& tmB_hi, const CUtensorMap& tmB_lo,
           float* __restrict__ C, int M, int ldc, long long c_split_stride,
           const TileOrder& ord, int n_tiles, int splits, int total_kb, int kb_per_split, int chain_kb,
           const float* __restrict__ out_scale, const float* __restrict__ a_tile_scale, int a_tiles, int a_gshift) {
   static_assert(!F16 || BEXACT, "the fp16 path exists for exact integer B operands only");
+  static_assert(BM == 128 || BM == 192, "two or three consumer warpgroups");
+  constexpr int NC = BM / 64;                                   // consumer warpgroups
   constexpr int BKE = F16 ? 2 * BK : BK;                        // elements per k-block
   constexpr int KSTEP_BYTES = 32;                               // wgmma K: 8 tf32 or 16 fp16 elements
-  using L = SmemLayout<STAGES, BEXACT>;
+  using L = SmemLayout<BM, STAGES, BEXACT>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;     // SWIZZLE_128B needs 1024 B alignment
 
@@ -249,7 +268,7 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
   auto peer_free_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + s); };
 
-  const int wg = threadIdx.x >> 7;
+  const int wg = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 7), 0);   // warp-uniform, as setmaxnreg needs
   const int warp = (threadIdx.x >> 5) & 3;                      // warp inside its warpgroup
   const int lane = threadIdx.x & 31;
   // __cluster_dims__(2, 1, 1): blocks 2c and 2c + 1 form cluster c, with ranks 0 and 1.
@@ -258,7 +277,7 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 8);                               // one arrival per consumer warp
+      mbar_init(empty_bar(s), 4 * NC);                          // one arrival per consumer warp
       mbar_init(peer_free_bar(s), 1);                           // the peer's producer
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -267,9 +286,13 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
 
   const int items = ord.m_tiles * ord.n_pairs * splits;
 
+  // 512 threads (BM = 192) get 128 registers each at launch; the producer drops to 32 and the consumers rise to 160
+  // (128 * 32 + 384 * 160 = 65 536).  At 384 threads (BM = 128) everyone keeps the launch-wide 168.
+  constexpr bool REBALANCE = NC == 3;
   if (wg == 0) {
+    if constexpr (REBALANCE) setmaxnreg_dec<32>();
     // ===================== TMA producer =====================
-    // Both CTAs of the pair need the whole 128-row A panel of the m-tile: each loads its 64-row half of A_hi and A_lo
+    // Both CTAs of the pair need the whole BM-row A panel of the m-tile: each loads its BM/2-row half of A_hi and A_lo
     // once from L2 and multicasts it to the same stage offset in both CTAs; B is the CTA's own n-tile, a local load.
     // So a stage of this CTA is written by both producers, and may be refilled only once the consumers of BOTH CTAs
     // have released it: after its local `empty` wait, the producer tells the peer (remote arrival on the peer's
@@ -287,9 +310,9 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
         const int kb0 = z * kb_per_split;
         const int kb1 = min(total_kb, kb0 + kb_per_split);
         for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(empty_bar(stage), phase ^ 1u);
+          mbar_wait<true>(empty_bar(stage), phase ^ 1u);
           mbar_arrive_remote(peer_free_bar(stage), rank ^ 1);
-          mbar_wait(peer_free_bar(stage), phase);
+          mbar_wait<true>(peer_free_bar(stage), phase);
           const uint32_t st = smem_base + stage * L::STAGE_BYTES;
           mbar_arrive_expect_tx(full_bar(stage), stage_tx);
           tma_load_2d_multicast(st + rank * HALF_A, &tmA_hi, full_bar(stage), kb * BKE, mt * BM + rank * (BM / 2), 0x3);
@@ -300,18 +323,25 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
           if (++stage == STAGES) { stage = 0; phase ^= 1u; }
         }
       }
+      for (int s = 0; s < STAGES; ++s) {                        // every stage released: the consumers are through
+        mbar_wait<true>(empty_bar(stage), phase ^ 1u);
+        if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+      }
     }
   } else {
     // ===================== consumers: MMA chains + drain + epilogue =====================
-    // The two warpgroups take turns issuing one k-block of MMAs each (warpgroup 1 first): barrier TURN_BAR + cw is this
-    // warpgroup's turn, and it hands the turn over right after its commit.  Each chain's drain, sums and tile stores
-    // then run while the other warpgroup's k-block is still in the tensor pipe.  Both walk the same items, so they take
-    // the same number of turns; warpgroup 2's hand-off before the first turn and warpgroup 1's sync after the last one
-    // pair the ends.  Only the issue time changes, not which MMAs form a chain or the order of the sums.
+    // The NC warpgroups take turns issuing one k-block of MMAs each, in a ring (warpgroup 1 first, then 2, ..., then 1
+    // again): barrier TURN_BAR + cw is this warpgroup's turn, and it hands the turn to the next one right after its
+    // commit.  Each chain's drain, sums and tile stores then run while the other warpgroups' k-blocks are still in the
+    // tensor pipe.  All walk the same items, so they take the same number of turns; the last warpgroup's hand-off
+    // before the first turn and warpgroup 1's sync after the last one pair the ends.  Only the issue time changes, not
+    // which MMAs form a chain or the order of the sums.
+    if constexpr (REBALANCE) setmaxnreg_inc<160>();
     constexpr uint32_t TURN_BAR = 1, TURN_THREADS = 256;
     const int cw = wg - 1;                                      // rows [64 cw, 64 cw + 64) of the tile
     const uint32_t a_off = static_cast<uint32_t>(cw * 64 * 128);
-    if (cw == 1) named_bar_arrive(TURN_BAR, TURN_THREADS);
+    const uint32_t next_bar = TURN_BAR + (cw + 1 == NC ? 0 : cw + 1);
+    if (cw == NC - 1) named_bar_arrive(TURN_BAR, TURN_THREADS);
     int stage = 0;
     uint32_t phase = 0;
     for (int w = cluster; w < items; w += clusters) {
@@ -332,7 +362,7 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
         float d[64];
         int prev = -1;
         for (int kb = c0; kb < c1; ++kb) {
-          mbar_wait(full_bar(stage), phase);
+          mbar_wait<false>(full_bar(stage), phase);
           named_bar_sync(TURN_BAR + cw, TURN_THREADS);
           const uint32_t st = smem_base + stage * L::STAGE_BYTES;
           const uint64_t a_hi = make_smem_desc(st + a_off);
@@ -349,7 +379,7 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
             wgmma_m64n128<F16>(d, a_hi + koff, b_hi + koff, 1u);
           }
           wgmma_commit();
-          named_bar_arrive(TURN_BAR + (cw ^ 1), TURN_THREADS);
+          named_bar_arrive(next_bar, TURN_THREADS);
           if (prev >= 0) {                                      // the previous k-block's MMAs have read their slot
             wgmma_wait<1>();
             if (lane == 0) mbar_arrive(empty_bar(prev));
@@ -409,15 +439,15 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
   cluster_sync();                 // neither CTA exits while the peer may still write its shared memory or barriers
 }
 
-template <int STAGES, bool BEXACT, bool F16>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NUM_THREADS, 1)
+template <int BM, int STAGES, bool BEXACT, bool F16>
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(num_threads<BM>(), 1)
 gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                    const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
                    float* __restrict__ C, int M, int ldc, long long c_split_stride,
                    const TileOrder ord, int n_tiles, int splits, int total_kb, int kb_per_split, int chain_kb,
                    const float* __restrict__ out_scale, const float* __restrict__ a_tile_scale, int a_tiles, int a_gshift) {
-  gemm_body<STAGES, BEXACT, F16>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, C, M, ldc, c_split_stride, ord, n_tiles, splits,
-                                 total_kb, kb_per_split, chain_kb, out_scale, a_tile_scale, a_tiles, a_gshift);
+  gemm_body<BM, STAGES, BEXACT, F16>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, C, M, ldc, c_split_stride, ord, n_tiles, splits,
+                                     total_kb, kb_per_split, chain_kb, out_scale, a_tile_scale, a_tiles, a_gshift);
 }
 
 // ------------------------------------------------------------------ host side
@@ -511,9 +541,10 @@ static TileOrder pick_tile_order(int m_tiles, int n_pairs, double a_panel, doubl
   return best;
 }
 
-template <int STAGES, bool BEXACT, bool F16>
+template <int BM, int STAGES, bool BEXACT, bool F16>
 int launch(const GemmArgs& g, cudaStream_t stream) {
-  using L = SmemLayout<STAGES, BEXACT>;
+  using L = SmemLayout<BM, STAGES, BEXACT>;
+  constexpr int NUM_THREADS = num_threads<BM>();
   constexpr int BKE = F16 ? 2 * BK : BK;
   CUtensorMap mAh, mAl, mBh, mBl;
   int rc;
@@ -535,7 +566,7 @@ int launch(const GemmArgs& g, cudaStream_t stream) {
   splits = (total_kb + kb_per_split - 1) / kb_per_split;      // no empty slices
   if (splits != g.splits_effective) { set_last_error("gemm: splits_effective mismatch (use gemm_effective_splits)"); return -1; }
 
-  auto kern = gemm_tf32x3_kernel<STAGES, BEXACT, F16>;
+  auto kern = gemm_tf32x3_kernel<BM, STAGES, BEXACT, F16>;
   // Per device (a second GPU in the same process needs its own calls): the shared-memory attribute, then how many
   // pairs fit at once (66 on a 132-SM H100 SXM).
   static int max_clusters[64] = {};
@@ -595,14 +626,19 @@ int gemm_tf32x3(const GemmArgs& g, cudaStream_t stream) {
                 reinterpret_cast<uintptr_t>(g.B_hi) | reinterpret_cast<uintptr_t>(g.B_lo) |
                 reinterpret_cast<uintptr_t>(g.C) | reinterpret_cast<uintptr_t>(g.out_col_scale)) % 16 == 0,
                "gemm: pointers must be 16-byte aligned");
+  // Tile height, a shape rule: 192-row tiles (three consumer warpgroups; 17 % less L2 -> shared-memory operand feed
+  // per FLOP) for split-K products of at least 2 048 rows, where they measured 3-6 % faster; 128-row tiles elsewhere,
+  // where the 192-row form measured no faster (one slice) or lost to padding (fewer rows).  Results do not depend on
+  // the choice: every element is formed by the same chains in the same order.
+  const bool tall = g.splits_effective > 1 && g.M >= 2048;
   if (g.f16) {
     CNMF_REQUIRE(g.b_exact, "gemm: the fp16 path needs an exact B operand");
     CNMF_REQUIRE(g.lda % 8 == 0 && g.ldb % 8 == 0, "gemm: fp16 leading dimensions must be multiples of 8 halves");
     CNMF_REQUIRE(!g.a_tile_scale || g.a_tiles * 512 >= g.Kd, "gemm: a_tiles does not cover the reduction length");
-    return launch<4, true, true>(g, stream);
+    return tall ? launch<192, 3, true, true>(g, stream) : launch<128, 4, true, true>(g, stream);
   }
-  if (g.b_exact) return launch<4, true, false>(g, stream);
-  return launch<3, false, false>(g, stream);
+  if (g.b_exact) return tall ? launch<192, 3, true, false>(g, stream) : launch<128, 4, true, false>(g, stream);
+  return launch<128, 3, false, false>(g, stream);
 }
 
 }  // namespace cnmf

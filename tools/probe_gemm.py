@@ -2,7 +2,10 @@
 """GPU probe: the batched GEMM alone, mean device time per launch, accuracy, the modelled HBM operand traffic of two
 tile orders: the m-tile-fastest order of the first kernel versions and the grouped order the launcher picks now (the
 same rule as pick_tile_order in csrc/gemm_tf32x3.cu, restated here), and the operand bytes the launch moves from the L2
-into shared memory, with and without the A multicast of the CTA pairs, with the rate the measured time gives.
+into shared memory, with and without the A multicast of the CTA pairs, with the rate the measured time gives.  The
+paired feed is also given for 192-row tiles (three consumer warpgroups, each CTA multicasting a 96-row half of A),
+which the launcher uses for split-K products of at least 2 048 rows in the exact-B forms (DESIGN.md section 4.1; the
+f16x2 cases mid_H_half and c3_H_half_full run them).
 
 The kernel runs in clusters of 2 CTAs: a pair's work item is an m-tile and two adjacent n-tiles (an n-pair), so the
 tile order is over m-tiles x n-pairs, a B panel is 256 rows, and the grid of the order is the number of pairs that
@@ -84,10 +87,19 @@ def model(M, N, Kd, splits, l2, sms, f16):
     piece = BM * KB_BYTES
     kb_total = sum(kbs)
     unpaired = m_tiles * n_tiles * kb_total * piece * (2 + b_pieces)
-    paired = m_tiles * kb_total * piece * (2 * n_pairs + b_pieces * n_tiles)
+    paired = paired_feed(M, n_tiles, kb_total, BM, b_pieces)
     return {"m_fastest_GB": round(flat / 1e9, 3), "grouped_GB": round(grouped / 1e9, 3), "min_GB": round(minimum / 1e9, 3),
             "grouped_order": "%d %s per group" % (g, "n-pairs" if gn else "m-tiles"), "slices": len(kbs),
-            "l2_to_smem_unpaired_GB": round(unpaired / 1e9, 2), "l2_to_smem_paired_GB": round(paired / 1e9, 2)}
+            "l2_to_smem_unpaired_GB": round(unpaired / 1e9, 2), "l2_to_smem_paired_GB": round(paired / 1e9, 2),
+            "l2_to_smem_paired_GB_192_rows": round(paired_feed(M, n_tiles, kb_total, 192, b_pieces) / 1e9, 2)}
+
+
+def paired_feed(M, n_tiles, kb_total, bm, b_pieces):
+    """L2 -> shared memory operand bytes of a paired launch with bm-row tiles: per m-tile and k-block, the bm rows of
+    both A pieces once per pair (each CTA loads half and multicasts it) and every CTA's own 128-row B pieces.  Per FLOP
+    that is 32 KB per 128 x 128 tile and 40 KB per 192 x 128 tile (f16x2): 17 % less at 192 rows, before padding."""
+    m_tiles, n_pairs = -(-M // bm), -(-n_tiles // 2)
+    return m_tiles * kb_total * KB_BYTES * (2 * bm * n_pairs + b_pieces * BN * n_tiles)
 
 
 def main():
