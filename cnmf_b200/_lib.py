@@ -50,6 +50,20 @@ class UpdateStepArgs(ctypes.Structure):
                 ("tile_scale", ctypes.c_void_p), ("gram_out", ctypes.c_void_p), ("scal_out", ctypes.c_void_p)]
 
 
+UNIT_BETA_UPDATE, UNIT_BETA_DIVERGENCE = 0, 1
+UNIT_SIDE_W, UNIT_SIDE_H = 0, 1
+
+
+class BetaStepArgs(ctypes.Structure):
+    """struct cnmf_beta_step_args (include/cnmf_b200.h): arguments of the cnmf_beta_step_host test hook."""
+    _fields_ = [("n_slots", ctypes.c_int32), ("n_rids", ctypes.c_int32),
+                ("ks", ctypes.c_void_p), ("rids", ctypes.c_void_p), ("done", ctypes.c_void_p),
+                ("op", ctypes.c_int32), ("side", ctypes.c_int32), ("loss", ctypes.c_int32),
+                ("n_items", ctypes.c_int32), ("n_contract", ctypes.c_int32), ("l1", ctypes.c_float), ("l2", ctypes.c_float),
+                ("D", ctypes.c_void_p), ("F_own", ctypes.c_void_p), ("F_other", ctypes.c_void_p),
+                ("oth_sum", ctypes.c_void_p), ("last", ctypes.c_void_p), ("totals", ctypes.c_void_p)]
+
+
 _c = ctypes
 _vp, _i, _ll, _d = _c.c_void_p, _c.c_int, _c.c_longlong, _c.c_double
 _pp = _c.POINTER
@@ -99,6 +113,7 @@ SIGNATURES = {
     "cnmf_project_rows": (_i, [_vp, _i, _vp, _vp, _vp]),
     "cnmf_gemm_abt_host": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _pp(_c.c_float), _vp]),
     "cnmf_update_step_host": (_i, [_vp, _pp(UpdateStepArgs), _vp]),
+    "cnmf_beta_step_host": (_i, [_vp, _pp(BetaStepArgs), _vp]),
     "cnmf_l2_normalize_rows": (_i, [_vp, _vp, _i, _i, _i, _vp]),
     "cnmf_local_density": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     "cnmf_col_stats_dev": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
@@ -114,7 +129,7 @@ SIGNATURES = {
 _lib = None
 
 
-ABI_VERSION = 11     # include/cnmf_b200.h CNMF_B200_ABI_VERSION
+ABI_VERSION = 12     # include/cnmf_b200.h CNMF_B200_ABI_VERSION
 
 
 def load():

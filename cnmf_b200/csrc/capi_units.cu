@@ -1,10 +1,12 @@
-// Test hook of the C ABI: one launch of the batched solver's update / Gram / <NUM, F> / piece kernels on host data
+// Test hooks of the C ABI: one launch of the batched solver's update / Gram / <NUM, F> / piece kernels on host data
 // (cnmf_update_step_host, include/cnmf_b200.h).  It builds the FactorView / BatchMeta / FusedOut the solver builds
-// (nmf_engine.cu) and calls the same launch_* functions; no kernel code of its own.
+// (nmf_engine.cu) and calls the same launch_* functions; no kernel code of its own.  cnmf_beta_step_host does the same
+// for the KL / IS solver (nmf_beta.cu).
 #include <algorithm>
 #include <vector>
 
 #include "engine.h"
+#include "nmf_beta.h"
 #include "nmf_kernels.cuh"
 
 using namespace cnmf;
@@ -144,5 +146,105 @@ extern "C" int cnmf_update_step_host(cnmf_handle_t h, const cnmf_update_step_arg
     CNMF_CUDA_CHECK(cudaMemcpyAsync(a->gram_out, d_gout, sizeof(double) * (size_t)NR * KMAX * KMAX, cudaMemcpyDeviceToHost, s));
   if (a->want_scalar) CNMF_CUDA_CHECK(cudaMemcpyAsync(a->scal_out, d_scal, sizeof(double) * NR, cudaMemcpyDeviceToHost, s));
   CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
+  return 0;
+}
+
+// cnmf_beta_step_host: one half-step or one divergence evaluation of the KL / IS solver.  The BetaSide comes from
+// beta_side on a view whose data operand is D, so the half's flags are the solver's; the launches are the solver's
+// beta_row_sums / beta_update / beta_check.
+extern "C" int cnmf_beta_step_host(cnmf_handle_t h, const cnmf_beta_step_args* a, void* stream) {
+  CNMF_REQUIRE(h && a && a->ks && a->rids && a->done && a->D && a->F_own && a->F_other, "beta_step: NULL argument");
+  CNMF_REQUIRE(a->n_slots >= 1 && a->n_rids >= 1 && a->n_items >= 1 && a->n_contract >= 1, "beta_step: bad sizes");
+  CNMF_REQUIRE(a->op == CNMF_UNIT_BETA_UPDATE || a->op == CNMF_UNIT_BETA_DIVERGENCE, "beta_step: unknown op");
+  CNMF_REQUIRE(a->side == CNMF_UNIT_SIDE_W || a->side == CNMF_UNIT_SIDE_H, "beta_step: unknown side");
+  const bool update = a->op == CNMF_UNIT_BETA_UPDATE;
+  CNMF_REQUIRE(a->loss == CNMF_LOSS_KULLBACK_LEIBLER || a->loss == CNMF_LOSS_ITAKURA_SAITO ||
+                   (!update && a->loss == CNMF_LOSS_FROBENIUS), "beta_step: unknown loss");
+  CNMF_REQUIRE(!update || a->loss != CNMF_LOSS_KULLBACK_LEIBLER || a->oth_sum, "beta_step: oth_sum missing");
+  CNMF_REQUIRE(update || (a->last && a->totals), "beta_step: last / totals missing");
+  const int R = a->n_slots, NR = a->n_rids;
+  std::vector<int> meta(3 * R + NR, 0);         // off | k | rid per slot, done per rid
+  std::vector<char> seen(NR, 0);
+  int SK = 0, kmax = 0;
+  for (int s = 0; s < R; ++s) {
+    CNMF_REQUIRE(a->ks[s] >= 1 && a->ks[s] <= KMAX, "beta_step: ks must be in [1, 32]");
+    CNMF_REQUIRE(a->rids[s] >= 0 && a->rids[s] < NR && !seen[a->rids[s]], "beta_step: rids must be distinct and < n_rids");
+    seen[a->rids[s]] = 1;
+    meta[s] = SK;
+    meta[R + s] = a->ks[s];
+    meta[2 * R + s] = a->rids[s];
+    SK += a->ks[s];
+    kmax = std::max(kmax, a->ks[s]);
+  }
+  for (int r = 0; r < NR; ++r) meta[3 * R + r] = a->done[r];
+
+  cudaStream_t s = as_stream(stream);
+  CNMF_CUDA_CHECK(cudaSetDevice(h->device));
+  const int ld_i = pad_ld(a->n_items), ld_k = pad_ld(a->n_contract);
+  const size_t n_d = (size_t)a->n_contract * ld_i, n_own = (size_t)SK * ld_i, n_oth = (size_t)SK * ld_k;
+  int* d_meta = static_cast<int*>(h->dev_buf("unit.meta", sizeof(int) * meta.size()));
+  float* d_D = static_cast<float*>(h->dev_buf("unit.beta_D", n_d * 4));
+  float* d_own = static_cast<float*>(h->dev_buf("unit.F", n_own * 4));
+  float* d_oth = static_cast<float*>(h->dev_buf("unit.beta_F_other", n_oth * 4));
+  double* d_sums = static_cast<double*>(h->dev_buf("unit.beta_sums", sizeof(double) * 2 * SK));
+  double* d_state = static_cast<double*>(h->dev_buf("unit.beta_state", sizeof(double) * 3 * NR));
+  int* d_niter = static_cast<int*>(h->dev_buf("unit.beta_niter", sizeof(int) * NR));
+  if (!d_meta || !d_D || !d_own || !d_oth || !d_sums || !d_state || !d_niter) return -2;
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(d_meta, meta.data(), sizeof(int) * meta.size(), cudaMemcpyHostToDevice, s));
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(d_D, a->D, n_d * 4, cudaMemcpyHostToDevice, s));
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(d_own, a->F_own, n_own * 4, cudaMemcpyHostToDevice, s));
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(d_oth, a->F_other, n_oth * 4, cudaMemcpyHostToDevice, s));
+  CNMF_CUDA_CHECK(cudaMemsetAsync(d_sums, 0, sizeof(double) * 2 * SK, s));
+  if (!update) CNMF_CUDA_CHECK(cudaMemcpyAsync(d_state + 2 * NR, a->last, sizeof(double) * NR, cudaMemcpyHostToDevice, s));
+
+  // the view the solver would hold: the data operand of the half is D, the factors are F_own and F_other
+  const bool w = a->side == CNMF_UNIT_SIDE_W;
+  DataView v{};
+  v.n_r = w ? a->n_items : a->n_contract;
+  v.n_c = w ? a->n_contract : a->n_items;
+  v.ld_r = pad_ld(v.n_r);
+  v.ld_c = pad_ld(v.n_c);
+  (w ? v.B_cols : v.B_rows) = Operand{d_D, nullptr, nullptr, a->n_contract, a->n_items, ld_i};
+  cnmf_nmf_params p{};
+  p.solver = CNMF_SOLVER_MU;
+  p.beta_loss = a->loss;
+  p.l1_reg_W = p.l1_reg_H = a->l1;
+  p.l2_reg_W = p.l2_reg_H = a->l2;
+  float* Fr = w ? d_own : d_oth;
+  float* Fc = w ? d_oth : d_own;
+  const BetaSide sd = beta_side(v, p, w ? BetaHalf::W : BetaHalf::H, Fr, Fc, d_sums + SK);
+  const BatchMeta b{d_meta, d_meta + R, d_meta + 2 * R, d_meta + 3 * R, R, 32};
+  const BetaLaunch L{h, s, SK, kmax};
+  const int chunks = beta_chunks(sd);
+  double* d_part = static_cast<double*>(h->dev_buf("unit.beta_part", sizeof(double) * 2 * (size_t)NR * chunks));
+  if (!d_part) return -2;
+
+  if (update) {
+    const bool is = a->loss == CNMF_LOSS_ITAKURA_SAITO;
+    if (!is) CNMF_TRY(beta_row_sums(L, sd.Foth, sd.n_contract, sd.ld_oth, d_sums + SK));
+    CNMF_TRY(beta_update(L, is, sd, b));
+    CNMF_CUDA_CHECK(cudaMemcpyAsync(a->F_own, d_own, n_own * 4, cudaMemcpyDeviceToHost, s));
+    if (!is) CNMF_CUDA_CHECK(cudaMemcpyAsync(a->oth_sum, d_sums + SK, sizeof(double) * SK, cudaMemcpyDeviceToHost, s));
+    CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
+    return 0;
+  }
+  const int mode = a->loss == CNMF_LOSS_KULLBACK_LEIBLER ? ERR_KL : a->loss == CNMF_LOSS_ITAKURA_SAITO ? ERR_IS : ERR_FROB;
+  const ConvState st{d_state, d_state + NR, d_state + 2 * NR, d_meta + 3 * R, d_niter};
+  CNMF_TRY(beta_check(L, mode, sd, b, st, d_part, 0, 0.0, 1));
+  std::vector<double> part(2 * (size_t)NR * chunks);
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(part.data(), d_part, sizeof(double) * part.size(), cudaMemcpyDeviceToHost, s));
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(a->last, d_state + 2 * NR, sizeof(double) * NR, cudaMemcpyDeviceToHost, s));
+  CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
+  for (int sl = 0; sl < R; ++sl) {
+    const int r = a->rids[sl];
+    if (a->done[r]) continue;
+    double t = 0.0, sx = 0.0;                    // beta_check_kernel's order
+    for (int c = 0; c < chunks; ++c) {
+      t += part[((size_t)r * chunks + c) * 2];
+      sx += part[((size_t)r * chunks + c) * 2 + 1];
+    }
+    a->totals[2 * r] = t;
+    a->totals[2 * r + 1] = sx;
+  }
   return 0;
 }

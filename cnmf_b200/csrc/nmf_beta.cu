@@ -22,8 +22,7 @@
 #include <cstring>
 #include <vector>
 
-#include "engine.h"
-#include "nmf_kernels.cuh"
+#include "nmf_beta.h"
 
 namespace cnmf {
 
@@ -35,20 +34,6 @@ constexpr int CC = 128;     // contraction rows staged per shared-memory tile
 constexpr int UJ = 4;       // rows per unrolled group (loads of a group are issued together)
 constexpr float EPS32 = 1.1920929e-07f;          // sklearn EPSILON = float32 eps (_nmf.py:32)
 constexpr float EPS64F = 2.220446049250313e-16f;  // np.finfo(float64).eps, the clipping threshold
-
-struct BetaSide {
-  const float* D;        // data, n_contract x ldD, item index contiguous
-  long long ldD;
-  int n_items, n_contract;
-  float* Fown;           // SK x ld_own, updated in place
-  int ld_own;
-  const float* Foth;     // SK x ld_oth
-  int ld_oth;
-  const double* oth_sum; // [SK] row sums of Foth (KL denominators)
-  float l1, l2;
-  int zero_sum_to_one;   // H half of KL: W_sum == 0 -> 1
-  int clip;              // flush values < float64 eps to zero after the update
-};
 
 // rcp_nr / div_nr (branch-free fp32 reciprocal / quotient) live in common.cuh
 
@@ -207,10 +192,17 @@ __global__ void __launch_bounds__(BT) beta_update_kernel(BetaSide sd, BatchMeta 
   CNMF_BETA_SWITCH(beta_update_body, (IS ? 1 : 2), IS, sd, row0, k, chunk * IPB, sm)
 }
 
-// ---- divergence (_nmf.py:77-175, dense branch): per block, fp64 partials {sum of terms, sum of X over X > EPS}
-// MODE 0: Kullback-Leibler, 1: Itakura-Saito, 2: plain squared residual sum (x - wh)^2 over every entry (the
-// Frobenius prediction error the consensus statistics report whatever the fitted loss, cnmf.py:926-930)
-enum { ERR_KL = 0, ERR_IS = 1, ERR_FROB = 2 };
+// ---- divergence (_nmf.py:77-175, dense branch): per block, fp64 partials {t, s} with res = t + s (KL), res = t - (N G -
+// s) (IS).  MODE 0: Kullback-Leibler, 1: Itakura-Saito, 2: plain squared residual sum (x - wh)^2 over every entry (the
+// Frobenius prediction error the consensus statistics report whatever the fitted loss, cnmf.py:926-930).
+// sklearn's formulas subtract sum X - sum WH (KL) or N G (IS) from sums of terms of the size of X (KL) or 1 (IS); near
+// convergence the divergence is a small remainder of that subtraction, below the resolution of an fp32 per-tile sum.
+// So each entry contributes its share of the divergence itself, which vanishes as WH -> X instead of cancelling:
+//   KL, x > eps:  wh' (div log div - div + 1) = x log(x / wh') - x + wh'      (wh' = max(wh, eps), div = x / wh')
+//                 s += wh - wh' (non-zero only where the floor applies);   x <= eps:  s += wh
+//   IS, x > eps:  (div - 1) - log div,  s += 1 (an exact count: N G - s entries are dropped, each owing -1)
+// Summed over the entries this is exactly sklearn's res, and both forms are insensitive to first order to the
+// rounding of wh and div (their derivatives in wh and div vanish at div = 1).
 template <int KP, int CT, int MODE>
 __device__ __forceinline__ void beta_error_body(const BetaSide& sd, int row0, int k, int item_base, float* sm,
                                                 double& t_out, double& sx_out) {
@@ -257,17 +249,23 @@ __device__ __forceinline__ void beta_error_body(const BetaSide& sd, int row0, in
               for (int c = 0; c < KP; ++c) wh = fmaf(w[ct][c], h[c], wh);
               const float d = xv - wh;                     // padded rows / items: x = 0 and w or h = 0 -> d = 0
               t = fmaf(d, d, t);
-            } else if (xv > EPS32) {                       // zeros of X are dropped (:140-142)
+            } else {
               float wh = 0.0f;
 #pragma unroll
               for (int c = 0; c < KP; ++c) wh = fmaf(w[ct][c], h[c], wh);
-              wh = fmaxf(wh, EPS32);                       // :145
-              const float div = div_nr(xv, wh);
-              if (MODE == ERR_KL) {
-                t = fmaf(xv, logf(div), t);                // sum X log(X / WH)          (:152-153)
-                sx += xv;
-              } else {
-                t += div - logf(div);                      // sum div - sum log div      (:160-161)
+              if (xv > EPS32) {                            // zeros of X are dropped (:140-142)
+                const float whf = fmaxf(wh, EPS32);        // :145
+                const float div = div_nr(xv, whf);
+                const float lg = logf(div);
+                if (MODE == ERR_KL) {
+                  t = fmaf(whf, fmaf(div, lg, 1.0f - div), t);   // X log(X / WH) - X + WH       (:150-155)
+                  sx += wh - whf;
+                } else {
+                  t += (div - 1.0f) - lg;                  // div - log div - 1                (:160-161)
+                  sx += 1.0f;
+                }
+              } else if (MODE == ERR_KL) {
+                sx += wh;                                  // sum(WH) over the dropped entries (padding: wh = 0)
               }
             }
           }
@@ -321,9 +319,8 @@ __global__ void __launch_bounds__(256) row_sum_kernel(const float* __restrict__ 
 }
 
 // err = sqrt(2 max(res, 0)) (_nmf.py:170-175); stopping rule of _fit_multiplicative_update (:867-879)
-__global__ void beta_check_kernel(ConvState st, const double* __restrict__ part, int chunks, const double* __restrict__ sumR,
-                                  const double* __restrict__ sumC, double n_elems, int is, BatchMeta b, int it, double tol,
-                                  int max_iter) {
+__global__ void beta_check_kernel(ConvState st, const double* __restrict__ part, int chunks, double n_elems, int is,
+                                  BatchMeta b, int it, double tol, int max_iter) {
   const int slot = blockIdx.x * blockDim.x + threadIdx.x;
   if (slot >= b.R) return;
   const int r = b.rid[slot];
@@ -337,14 +334,8 @@ __global__ void beta_check_kernel(ConvState st, const double* __restrict__ part,
     st.last[r] = sqrt(fmax(t, 0.0));
     return;
   }
-  double res;
-  if (is == ERR_KL) {
-    double swh = 0.0;                                      // sum(WH) = <sum_i W, sum_j H>          (:150)
-    for (int c = 0; c < b.k[slot]; ++c) swh += sumR[b.off[slot] + c] * sumC[b.off[slot] + c];
-    res = t + swh - sx;                                    // (:153-155)
-  } else {
-    res = t - n_elems;                                     // (:161)
-  }
+  // KL: t + sum(WH) over the dropped entries;  IS: t - one per dropped entry (n_elems - sx is an exact integer)
+  const double res = is == ERR_KL ? t + sx : t - (n_elems - sx);
   const double err = sqrt(2.0 * fmax(res, 0.0));
   st.last[r] = err;
   if (it == 0) {
@@ -396,6 +387,57 @@ int matrix_min(cnmf_handle_s* h, const float* X, int rows, int cols, int ld, flo
   return 0;
 }
 
+BetaSide beta_side(const DataView& v, const cnmf_nmf_params& p, BetaHalf half, float* Fr, float* Fc,
+                   const double* oth_sum) {
+  const bool is = p.beta_loss == CNMF_LOSS_ITAKURA_SAITO;
+  if (half == BetaHalf::W)   // items = rows of the view (cells), contraction over its columns; data read as X^T (n_c x ld_r)
+    return BetaSide{v.B_cols.full, v.B_cols.ld, v.n_r, v.n_c, Fr, v.ld_r, Fc, v.ld_c, oth_sum,
+                    (float)p.l1_reg_W, (float)p.l2_reg_W, 0, is ? 1 : 0};
+  // items = columns (genes), contraction over rows; data read as X (n_r x ld_c)
+  return BetaSide{v.B_rows.full, v.B_rows.ld, v.n_c, v.n_r, Fc, v.ld_c, Fr, v.ld_r, oth_sum,
+                  (float)p.l1_reg_H, (float)p.l2_reg_H, 1, 1};
+}
+
+int beta_chunks(const BetaSide& sd) { return (sd.n_items + IPB - 1) / IPB; }
+
+int beta_row_sums(const BetaLaunch& L, const float* F, int n, int ld, double* out) {
+  row_sum_kernel<<<L.SK, 256, 0, L.s>>>(F, n, ld, out);
+  CNMF_CUDA_CHECK(cudaGetLastError());
+  L.h->launches += 1;
+  return 0;
+}
+
+int beta_update(const BetaLaunch& L, bool is, const BetaSide& sd, const BatchMeta& b) {
+  const int grid = b.R * beta_chunks(sd);
+#define CNMF_LAUNCH_UPD(ISV, KPM) beta_update_kernel<ISV, KPM><<<grid, BT, 0, L.s>>>(sd, b)
+  if (is) { if (L.kpmax <= 8) CNMF_LAUNCH_UPD(true, 8); else if (L.kpmax <= 16) CNMF_LAUNCH_UPD(true, 16); else CNMF_LAUNCH_UPD(true, 32); }
+  else { if (L.kpmax <= 8) CNMF_LAUNCH_UPD(false, 8); else if (L.kpmax <= 16) CNMF_LAUNCH_UPD(false, 16); else CNMF_LAUNCH_UPD(false, 32); }
+#undef CNMF_LAUNCH_UPD
+  CNMF_CUDA_CHECK(cudaGetLastError());
+  L.h->launches += 1;
+  return 0;
+}
+
+int beta_check(const BetaLaunch& L, int mode, const BetaSide& sd, const BatchMeta& b, const ConvState& st, double* part,
+               int it, double tol, int max_iter) {
+  const int chunks = beta_chunks(sd);
+  const int grid = b.R * chunks;
+#define CNMF_LAUNCH_ERR(MD, KPM) beta_error_kernel<MD, KPM><<<grid, BT, 0, L.s>>>(sd, b, part, chunks)
+#define CNMF_LAUNCH_ERR_K(MD) { if (L.kpmax <= 8) CNMF_LAUNCH_ERR(MD, 8); else if (L.kpmax <= 16) CNMF_LAUNCH_ERR(MD, 16); else CNMF_LAUNCH_ERR(MD, 32); }
+  if (mode == ERR_KL) CNMF_LAUNCH_ERR_K(ERR_KL)
+  else if (mode == ERR_IS) CNMF_LAUNCH_ERR_K(ERR_IS)
+  else CNMF_LAUNCH_ERR_K(ERR_FROB)
+#undef CNMF_LAUNCH_ERR_K
+#undef CNMF_LAUNCH_ERR
+  CNMF_CUDA_CHECK(cudaGetLastError());
+  L.h->launches += 1;
+  beta_check_kernel<<<(b.R + 127) / 128, 128, 0, L.s>>>(st, part, chunks, (double)sd.n_items * (double)sd.n_contract,
+                                                       mode, b, it, tol, max_iter);
+  CNMF_CUDA_CHECK(cudaGetLastError());
+  L.h->launches += 1;
+  return 0;
+}
+
 int solve_batched_beta(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_nmf_params& p, cudaStream_t s) {
   const int R = io.R;
   CNMF_REQUIRE(R > 0 && (int)io.ks.size() == R, "solve: bad restart list");
@@ -404,6 +446,7 @@ int solve_batched_beta(cnmf_handle_s* h, const DataView& v, SolveIO& io, const c
   CNMF_REQUIRE(p.max_iter >= 1, "solve: max_iter must be >= 1");
   CNMF_REQUIRE(v.B_rows.full && v.B_cols.full, "solve: the beta-divergence kernels need X and X^T in full fp32");
   const bool is = p.beta_loss == CNMF_LOSS_ITAKURA_SAITO;
+  const int mode = is ? ERR_IS : ERR_KL;
 
   std::vector<int> hm(3 * R);
   int SK = 0, kpmax = 0;
@@ -415,7 +458,7 @@ int solve_batched_beta(cnmf_handle_s* h, const DataView& v, SolveIO& io, const c
     hm[2 * R + r] = r;
     SK += io.ks[r];
   }
-  const int chunks_r = (v.n_r + IPB - 1) / IPB, chunks_c = (v.n_c + IPB - 1) / IPB;
+  const int chunks_r = (v.n_r + IPB - 1) / IPB;
   int* d_meta = static_cast<int*>(h->dev_buf("solve.meta", sizeof(int) * 8 * R));
   double* d_state = static_cast<double*>(h->dev_buf("solve.state", sizeof(double) * 8 * R));
   double* d_sums = static_cast<double*>(h->dev_buf("beta.sums", sizeof(double) * 2 * SK));
@@ -431,67 +474,24 @@ int solve_batched_beta(cnmf_handle_s* h, const DataView& v, SolveIO& io, const c
   BatchMeta bm{d_meta, d_meta + R, d_meta + 2 * R, d_done, R, 32};
   double* d_sumR = d_sums;
   double* d_sumC = d_sums + SK;
+  const BetaLaunch L{h, s, SK, kpmax};
+  const BetaSide sideR = beta_side(v, p, BetaHalf::W, io.Fr, io.Fc, d_sumC);
+  const BetaSide sideC = beta_side(v, p, BetaHalf::H, io.Fr, io.Fc, d_sumR);
 
-  // W half: items = rows of the view (cells), contraction over its columns; data read as X^T (n_c x ld_r)
-  BetaSide sideR{v.B_cols.full, v.B_cols.ld, v.n_r, v.n_c, io.Fr, v.ld_r, io.Fc, v.ld_c, d_sumC,
-                 (float)p.l1_reg_W, (float)p.l2_reg_W, 0, is ? 1 : 0};
-  // H half: items = columns (genes), contraction over rows; data read as X (n_r x ld_c)
-  BetaSide sideC{v.B_rows.full, v.B_rows.ld, v.n_c, v.n_r, io.Fc, v.ld_c, io.Fr, v.ld_r, d_sumR,
-                 (float)p.l1_reg_H, (float)p.l2_reg_H, 1, 1};
-
-  auto row_sums = [&](const float* F, int n, int ld, double* out) -> int {
-    row_sum_kernel<<<SK, 256, 0, s>>>(F, n, ld, out);
-    CNMF_CUDA_CHECK(cudaGetLastError());
-    h->launches += 1;
-    return 0;
-  };
-  auto update = [&](const BetaSide& sd, int chunks) -> int {
-#define CNMF_LAUNCH_UPD(ISV, KPM) beta_update_kernel<ISV, KPM><<<R * chunks, BT, 0, s>>>(sd, bm)
-    if (is) { if (kpmax <= 8) CNMF_LAUNCH_UPD(true, 8); else if (kpmax <= 16) CNMF_LAUNCH_UPD(true, 16); else CNMF_LAUNCH_UPD(true, 32); }
-    else { if (kpmax <= 8) CNMF_LAUNCH_UPD(false, 8); else if (kpmax <= 16) CNMF_LAUNCH_UPD(false, 16); else CNMF_LAUNCH_UPD(false, 32); }
-#undef CNMF_LAUNCH_UPD
-    CNMF_CUDA_CHECK(cudaGetLastError());
-    h->launches += 1;
-    return 0;
-  };
-  auto error_pass = [&](int mode, const BatchMeta& m) -> int {
-#define CNMF_LAUNCH_ERR(MD, KPM) beta_error_kernel<MD, KPM><<<R * chunks_r, BT, 0, s>>>(sideR, m, d_part, chunks_r)
-#define CNMF_LAUNCH_ERR_K(MD) { if (kpmax <= 8) CNMF_LAUNCH_ERR(MD, 8); else if (kpmax <= 16) CNMF_LAUNCH_ERR(MD, 16); else CNMF_LAUNCH_ERR(MD, 32); }
-    if (mode == ERR_KL) CNMF_LAUNCH_ERR_K(ERR_KL)
-    else if (mode == ERR_IS) CNMF_LAUNCH_ERR_K(ERR_IS)
-    else CNMF_LAUNCH_ERR_K(ERR_FROB)
-#undef CNMF_LAUNCH_ERR_K
-#undef CNMF_LAUNCH_ERR
-    CNMF_CUDA_CHECK(cudaGetLastError());
-    h->launches += 1;
-    return 0;
-  };
-  auto check = [&](int it, double tol_eff) -> int {
-    if (!is) {
-      CNMF_TRY(row_sums(io.Fr, v.n_r, v.ld_r, d_sumR));
-      if (it == 0 || !io.update_cols) CNMF_TRY(row_sums(io.Fc, v.n_c, v.ld_c, d_sumC));
-    }
-    CNMF_TRY(error_pass(is ? ERR_IS : ERR_KL, bm));
-    beta_check_kernel<<<(R + 127) / 128, 128, 0, s>>>(st, d_part, chunks_r, d_sumR, d_sumC, (double)v.n_r * (double)v.n_c,
-                                                     is ? ERR_IS : ERR_KL, bm, it, tol_eff, p.max_iter);
-    CNMF_CUDA_CHECK(cudaGetLastError());
-    h->launches += 1;
-    return 0;
-  };
-
-  CNMF_TRY(check(0, p.tol));                       // error_at_init (:822); also leaves sum(H) rows for the first W half
+  if (!is) CNMF_TRY(beta_row_sums(L, io.Fc, v.n_c, v.ld_c, d_sumC));   // sum(H) rows for the first W half
+  CNMF_TRY(beta_check(L, mode, sideR, bm, st, d_part, 0, p.tol, p.max_iter));   // error_at_init (:822)
   std::vector<int> h_done(R, 0);
   for (int it = 1; it <= p.max_iter; ++it) {
-    CNMF_TRY(update(sideR, chunks_r));
+    CNMF_TRY(beta_update(L, is, sideR, bm));
     if (io.update_cols) {
-      if (!is) CNMF_TRY(row_sums(io.Fr, v.n_r, v.ld_r, d_sumR));
-      CNMF_TRY(update(sideC, chunks_c));
-      if (!is) CNMF_TRY(row_sums(io.Fc, v.n_c, v.ld_c, d_sumC));
+      if (!is) CNMF_TRY(beta_row_sums(L, io.Fr, v.n_r, v.ld_r, d_sumR));
+      CNMF_TRY(beta_update(L, is, sideC, bm));
+      if (!is) CNMF_TRY(beta_row_sums(L, io.Fc, v.n_c, v.ld_c, d_sumC));
     }
     const bool chk = (p.tol > 0 && it % 10 == 0) || it == p.max_iter;
     if (chk) {
       const double tol_eff = (p.tol > 0 && it % 10 == 0) ? p.tol : -1.0;
-      CNMF_TRY(check(it, tol_eff));
+      CNMF_TRY(beta_check(L, mode, sideR, bm, st, d_part, it, tol_eff, p.max_iter));
       CNMF_CUDA_CHECK(cudaMemcpyAsync(h_done.data(), d_done, sizeof(int) * R, cudaMemcpyDeviceToHost, s));
       CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
       bool all = true;
@@ -510,10 +510,7 @@ int solve_batched_beta(cnmf_handle_s* h, const DataView& v, SolveIO& io, const c
   CNMF_CUDA_CHECK(cudaMemsetAsync(d_zero, 0, sizeof(int) * 2 * R, s));
   BatchMeta bm0{d_meta, d_meta + R, d_meta + 2 * R, d_zero, R, 32};
   ConvState st0{d_state + 3 * R, d_state + 4 * R, d_state + 5 * R, d_zero, d_zero + R};
-  CNMF_TRY(error_pass(ERR_FROB, bm0));
-  beta_check_kernel<<<(R + 127) / 128, 128, 0, s>>>(st0, d_part, chunks_r, d_sumR, d_sumC, 0.0, ERR_FROB, bm0, 0, 0.0, p.max_iter);
-  CNMF_CUDA_CHECK(cudaGetLastError());
-  h->launches += 1;
+  CNMF_TRY(beta_check(L, ERR_FROB, sideR, bm0, st0, d_part, 0, 0.0, p.max_iter));
   CNMF_CUDA_CHECK(cudaMemcpyAsync(io.err.data(), st0.last, sizeof(double) * R, cudaMemcpyDeviceToHost, s));
   CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
   return 0;

@@ -285,6 +285,44 @@ class Engine:
         check(self.lib.cnmf_update_step_host(self._h, ctypes.byref(a), None))
         return dict(F=F, hi=hi, lo=lo, tile_scale=ts, gram=g_out, scal=s_out)
 
+    def beta_step(self, ks, rids, done, side, loss, D, F_own, F_other, n_items, n_contract, op="update", l1=0.0, l2=0.0,
+                  last=None, totals=None):
+        """Test hook: one launch of the KL / IS solver's update kernel (op 'update', loss 'kullback-leibler' /
+        'itakura-saito') or one divergence evaluation (op 'divergence', those losses or 'frobenius'), on packed host data
+        (slot s holds restart rids[s] with ks[s] components; done has one entry per rid).  side 'W' or 'H' names the
+        half whose flags the solver would use (only H maps a zero KL sum to 1; W clips only for IS).  D is n_contract x
+        ld_items with the item index contiguous, F_own (sum ks) x ld_items, F_other (sum ks) x ld_contract, ld_* =
+        ceil(n / 32) * 32; their padding is passed as given.  last (n_rids) and totals (n_rids x 2) are uploaded as given,
+        so a caller can pre-fill them with a sentinel; missing ones start as zeros.  Returns dict(F, oth_sum, last,
+        totals): the updated F_own and, for KL updates, the fp64 row sums of F_other; for divergences the statistic
+        sqrt(2 max(res, 0)) (||X - WH||_F for frobenius) and the fp64 (sum of terms, sum of x over x > eps) per rid."""
+        ks = np.ascontiguousarray(ks, np.int32)
+        rids = np.ascontiguousarray(rids, np.int32)
+        done = np.ascontiguousarray(done, np.int32)
+        SK, n_rids = int(ks.sum()), len(done)
+        ld_i, ld_k = -(-int(n_items) // 32) * 32, -(-int(n_contract) // 32) * 32
+        D = f32c(D)
+        F = f32c(F_own).copy()
+        Fo = f32c(F_other)
+        assert D.shape == (n_contract, ld_i) and F.shape == (SK, ld_i) and Fo.shape == (SK, ld_k)
+        lcode = {"kullback-leibler": LOSS_KULLBACK_LEIBLER, "itakura-saito": LOSS_ITAKURA_SAITO,
+                 "frobenius": LOSS_FROBENIUS}[loss]
+        oth = np.zeros(SK)
+        lo = np.zeros(n_rids) if last is None else np.ascontiguousarray(last, np.float64).copy()
+        tt = np.zeros((n_rids, 2)) if totals is None else np.ascontiguousarray(totals, np.float64).copy()
+        assert lo.shape == (n_rids,) and tt.shape == (n_rids, 2)
+        a = _lib.BetaStepArgs()
+        a.n_slots, a.n_rids = len(ks), n_rids
+        a.ks, a.rids, a.done = ptr(ks), ptr(rids), ptr(done)
+        a.op = {"update": _lib.UNIT_BETA_UPDATE, "divergence": _lib.UNIT_BETA_DIVERGENCE}[op]
+        a.side = {"W": _lib.UNIT_SIDE_W, "H": _lib.UNIT_SIDE_H}[side]
+        a.loss, a.n_items, a.n_contract = lcode, int(n_items), int(n_contract)
+        a.l1, a.l2 = float(l1), float(l2)
+        a.D, a.F_own, a.F_other = ptr(D), ptr(F), ptr(Fo)
+        a.oth_sum, a.last, a.totals = ptr(oth), ptr(lo), ptr(tt)
+        check(self.lib.cnmf_beta_step_host(self._h, ctypes.byref(a), None))
+        return dict(F=F, oth_sum=oth, last=lo, totals=tt)
+
 
 class Dataset:
     """A cells x genes matrix resident on the GPU (norm_counts.X / tpm.X of the reference)."""

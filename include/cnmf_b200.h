@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define CNMF_B200_ABI_VERSION 11
+#define CNMF_B200_ABI_VERSION 12
 #define CNMF_MAX_COMPONENTS 32          /* largest n_components per restart on the CUDA path */
 
 typedef struct cnmf_handle_s* cnmf_handle_t;
@@ -289,6 +289,41 @@ typedef struct cnmf_update_step_args {
 /* The last-block tickets of the fused launches are zeroed once per handle, when first allocated: a second call relies
  * on the kernel's own reset. */
 int cnmf_update_step_host(cnmf_handle_t h, const cnmf_update_step_args* args, void* stream);
+
+/* test hook: ONE half-step or ONE divergence evaluation of the KL / IS solver on host-supplied packed data, issued
+ * through the launch functions the solver uses (batch layout, rids and done as for cnmf_update_step_host).  side names
+ * the half whose BetaSide the solver would build: W (items = cells, D = X^T) or H (items = genes, D = X); the half
+ * decides the KL zero-sum rule and the clip.  Strides are the dataset's: ld_items = ceil(n_items / 32) * 32,
+ * ld_contract = ceil(n_contract / 32) * 32.
+ *   op UPDATE (loss KL or IS): KL first computes the fp64 row sums of F_other (row_sum_kernel) into oth_sum, then one
+ *     beta_update_kernel launch updates F_own in place with l1 / l2.
+ *   op DIVERGENCE (loss KL, IS or FROBENIUS): one beta_error_kernel pass, then beta_check_kernel at iteration 0.
+ *     last[rid] = sqrt(2 max(res, 0)), or ||D - F_own^T F_other||_F for FROBENIUS; totals[2 rid + {0, 1}] = the fp64
+ *     sums (t, s) of the per-block partials, in the order beta_check_kernel adds them: KL t = sum over x > eps of
+ *     x log(x / WH') - x + WH' (WH' = max(WH, eps)), s = sum(WH) over x <= eps plus sum(WH - WH') over x > eps,
+ *     res = t + s;  IS t = sum over x > eps of (x / WH' - 1) - log(x / WH'), s = number of entries x > eps,
+ *     res = t - (entries - s);  FROBENIUS t = sum (x - WH)^2, s = 0. */
+enum { CNMF_UNIT_BETA_UPDATE = 0, CNMF_UNIT_BETA_DIVERGENCE = 1 };
+enum { CNMF_UNIT_SIDE_W = 0, CNMF_UNIT_SIDE_H = 1 };
+typedef struct cnmf_beta_step_args {
+  int32_t n_slots;              /* restarts in the batch */
+  int32_t n_rids;               /* length of done / last, and of totals in pairs */
+  const int32_t* ks;            /* [n_slots], 1..32 */
+  const int32_t* rids;          /* [n_slots], distinct, < n_rids */
+  const int32_t* done;          /* [n_rids] 1 = frozen restart: the launches skip it */
+  int32_t op;                   /* CNMF_UNIT_BETA_* */
+  int32_t side;                 /* CNMF_UNIT_SIDE_* */
+  int32_t loss;                 /* CNMF_LOSS_* */
+  int32_t n_items, n_contract;
+  float l1, l2;                 /* regularisation of the updated half */
+  const float* D;               /* n_contract x ld_items: the data, item index contiguous */
+  float* F_own;                 /* in/out: (sum ks) x ld_items */
+  const float* F_other;         /* (sum ks) x ld_contract */
+  double* oth_sum;              /* out (update, KL): sum ks */
+  double* last;                 /* in/out (divergence): n_rids */
+  double* totals;               /* in/out (divergence): n_rids x 2 */
+} cnmf_beta_step_args;
+int cnmf_beta_step_host(cnmf_handle_t h, const cnmf_beta_step_args* args, void* stream);
 
 /* ---- consensus kernels (cnmf.py:882-916) on a stacked-spectra matrix S (R x G, device, row stride ld) -- */
 /* rows / ||row||_2 in place (cnmf.py:882) */

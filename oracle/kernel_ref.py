@@ -104,3 +104,78 @@ def f16_pieces(F, scale=None, group=512):
     hi = y.astype(np.float16)
     mid = (y - hi.astype(np.float32)).astype(np.float16)
     return hi, mid, ts
+
+
+# ---------------------------------------------------------------------------------------- KL / IS (nmf_beta.cu)
+EPS64 = float(np.finfo(np.float64).eps)
+
+
+def beta_half_step(F, D, Foth, beta, half, l1=0.0, l2=0.0):
+    """One multiplicative half-step of the KL (beta = 1) or IS (beta = 0) loss in the kernels' layout, float64:
+    F (K x items) is updated, Foth (K x n_contract) is the other factor, D (n_contract x items) the data with the item
+    index contiguous (X^T for the W half, X for the H half), so WH = Foth^T F in D's layout.  scikit-learn's rules
+    (SK/decomposition/_nmf.py:551-624 for W, :637-721 for H, :845-865 for the flush):
+        WH floored at float32 eps;  KL: num = Foth (D / WH), den = row sums of Foth (a zero sum -> 1 in the H half only);
+        IS: num = Foth (D WH^-2), den = Foth WH^-1;  den += l1, + l2 F;  den == 0 -> float32 eps;
+        F_new = F (num / den)^gamma, gamma = 1/2 for IS;  values below float64 eps -> 0 after the H half for beta <= 1
+        and after the W half for beta < 1."""
+    F = np.asarray(F, np.float64)
+    Foth = np.asarray(Foth, np.float64)
+    D = np.asarray(D, np.float64)
+    WH = np.maximum(Foth.T @ F, EPSILON)
+    if beta == 1:
+        num = Foth @ (D / WH)
+        den = np.repeat(Foth.sum(axis=1)[:, None], F.shape[1], axis=1)
+        if half == "H":
+            den[den == 0] = 1.0
+    elif beta == 0:
+        num = Foth @ (D / WH ** 2)
+        den = Foth @ (1.0 / WH)
+    else:
+        raise ValueError("beta must be 0 or 1")
+    if l1 > 0:
+        den = den + l1
+    if l2 > 0:
+        den = den + l2 * F
+    den = np.where(den == 0, EPSILON, den)
+    delta = num / den
+    if beta == 0:
+        delta = np.sqrt(delta)
+    out = F * delta
+    if half == "H" or beta < 1:
+        out[out < EPS64] = 0.0
+    return out
+
+
+def beta_terms(D, F, Foth, beta):
+    """(t, s, res, err) of SK/decomposition/_nmf.py:_beta_divergence (dense branch, square_root=True) for X = D,
+    WH = Foth^T F (either orientation: the divergence is the same for X^T), split as beta_error_kernel splits it: each
+    entry's share of the divergence, which vanishes as WH -> X, so nothing large cancels.  Entries with x <= float32 eps
+    are dropped; WH' = max(WH, eps) on the rest, div = x / WH'.
+      KL: t = sum x log div - x + WH',  s = sum(WH) over the dropped entries + sum(WH - WH') over the rest,  res = t + s
+          (= sum x log div + sum(WH) - sum x, scikit-learn's form);
+      IS: t = sum (div - 1) - log div,  s = number of entries kept,  res = t - (entries - s)
+          (= sum div - sum log div - entries);
+      beta = 2: t = res = sum (x - WH)^2 over every entry, s = 0.
+    err = sqrt(2 max(res, 0)), or sqrt(res) for beta = 2 (the kernel's ||X - WH||_F, which scikit-learn's formula
+    sqrt(2 * res / 2) equals)."""
+    D = np.asarray(D, np.float64)
+    WHr = np.asarray(Foth, np.float64).T @ np.asarray(F, np.float64)
+    if beta == 2:
+        t = float(((D - WHr) ** 2).sum())
+        return t, 0.0, t, float(np.sqrt(max(t, 0.0)))
+    keep = D > EPSILON
+    x = D[keep]
+    whf = np.maximum(WHr[keep], EPSILON)
+    div = x / whf
+    if beta == 1:
+        t = float(np.sum(x * np.log(div) - x + whf))
+        s = float(WHr[~keep].sum() + (WHr[keep] - whf).sum())
+        res = t + s
+    elif beta == 0:
+        t = float(np.sum((div - 1.0) - np.log(div)))
+        s = float(keep.sum())
+        res = t - (D.size - s)
+    else:
+        raise ValueError("beta must be 0, 1 or 2")
+    return t, s, res, float(np.sqrt(2.0 * max(res, 0.0)))

@@ -285,6 +285,14 @@ def test_binding_table_matches_header_prototypes():
     ver = int(re.search(r"#define CNMF_B200_ABI_VERSION (\d+)", header).group(1))
     assert ver == _lib.ABI_VERSION == ctypes.CDLL(_lib.LIB_PATH).cnmf_abi_version()
     assert ctypes.sizeof(_lib.NmfParams) == 4 * 4 + 5 * 8 + 2 * 4
+    # the test hooks' argument structs: the ctypes mirrors name the header's fields in the header's order
+    for cname, mirror in (("cnmf_update_step_args", _lib.UpdateStepArgs), ("cnmf_beta_step_args", _lib.BetaStepArgs)):
+        body = re.search(r"typedef struct %s \{(.*?)\}" % cname, header, flags=re.S).group(1)
+        names = []
+        for decl in (d.strip() for d in body.split(";") if d.strip()):
+            first, *rest = decl.split(",")
+            names += [re.findall(r"\w+", first)[-1]] + [r.strip() for r in rest]
+        assert names == [f[0] for f in mirror._fields_], cname
 
 
 # ------------------------------------------------------------------------------------ round-2 host logic

@@ -144,3 +144,56 @@ def test_kernel_step_references_match_sklearn(l1, l2):
     G0[3] = 0.0
     ref = kernel_ref.mu_half_step(W.T, num, G0, 0.0, 0.0)
     assert np.allclose(ref[3], W.T[3] * num[3] / kernel_ref.EPSILON, rtol=1e-15)
+
+
+@pytest.mark.parametrize("l1,l2", [(0.0, 0.0), (0.3, 0.0), (0.0, 0.7), (0.25, 1.5)])
+@pytest.mark.parametrize("beta", [1, 0])
+def test_beta_step_references_match_sklearn(beta, l1, l2):
+    """oracle/kernel_ref.py's KL / IS references -- what tests/test_beta_units.py holds the beta kernels to -- against
+    scikit-learn in float64: _multiplicative_update_w / _h (gamma = 1 / (2 - beta) for beta < 1, else 1) plus the flush
+    of _fit_multiplicative_update, and _beta_divergence.  Layout: W half F = W^T, Foth = H, D = X^T; H half F = H,
+    Foth = W^T, D = X.  The data has a zero component (zero KL sums, zero IS numerators and denominators), entries of
+    WH below eps, exact zeros and values at float32 eps in X, and values that the update drives below float64 eps."""
+    from sklearn.decomposition import _nmf
+    from oracle import kernel_ref
+    rng = np.random.RandomState(int(10 * l1 + 100 * l2) + beta)
+    n, g, K = 50, 40, 6
+    X = rng.uniform(0.2, 3.0, (n, g))
+    X[3, :5] = 0.0
+    X[4, :3] = kernel_ref.EPSILON
+    X[5, :3] = 2 * kernel_ref.EPSILON
+    W = rng.uniform(0.1, 1.5, (n, K))
+    H = rng.uniform(0.1, 1.5, (K, g))
+    W[:, 2] = 0.0                        # dead component: zero W sum (KL), zero numerator and denominator of H row 2
+    H[4, :] = 0.0                        # dead component for the W half
+    W[7, :] = 0.0                        # WH = 0 on a whole row: floored at eps
+    W[9, 1] = 1e-20                      # driven towards 0: below float64 eps after the update
+    H[1, 8] = 1e-20
+    gamma = 0.5 if beta == 0 else 1.0
+    Wn, *_ = _nmf._multiplicative_update_w(X, W.copy(), H, beta, l1, l2, gamma)
+    Wc = Wn.copy()
+    if beta < 1:
+        Wc[Wc < np.finfo(np.float64).eps] = 0.0
+    Fw = kernel_ref.beta_half_step(W.T, X.T, H, beta, "W", l1, l2)
+    assert np.allclose(Fw, Wc.T, rtol=1e-13, atol=0)
+    assert (Fw.T[9, 1] == 0.0) == (beta < 1) and (Fw.T[9, 1] > 0) == (beta == 1)
+    Hn = _nmf._multiplicative_update_h(X, W, H.copy(), beta, l1, l2, gamma)
+    Hn[Hn < np.finfo(np.float64).eps] = 0.0
+    Fh = kernel_ref.beta_half_step(H, X, W.T, beta, "H", l1, l2)
+    assert np.allclose(Fh, Hn, rtol=1e-13, atol=0)
+    assert Fh[1, 8] == 0.0 and np.isfinite(Fh).all() and np.isfinite(Fw).all()
+    for b in (beta, 2):
+        ref = _nmf._beta_divergence(X, W, H, b, square_root=True)
+        t, sx, res, err = kernel_ref.beta_terms(X.T, W.T, H, b)
+        assert abs(err - ref) <= 1e-12 * ref, (b, err, ref)
+        half = 2.0 if b == 2 else 1.0              # scikit-learn's Frobenius res is half the squared norm
+        assert res == pytest.approx(half * _nmf._beta_divergence(X, W, H, b, square_root=False), rel=1e-12)
+        assert kernel_ref.beta_terms(X, H, W.T, b)[3] == pytest.approx(err, rel=1e-13)
+        WH = W @ H
+        keep = X > kernel_ref.EPSILON
+        if b == 1:         # the kernel's split: sum(WH) over the dropped entries, plus the floor's share on the rest
+            assert sx == pytest.approx(WH[~keep].sum() + (WH[keep] - np.maximum(WH[keep], kernel_ref.EPSILON)).sum(),
+                                       rel=1e-13)
+            assert (WH[keep] < kernel_ref.EPSILON).any()
+        elif b == 0:
+            assert sx == keep.sum() and t >= 0
