@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libcnmf_b200.so")
 
 SOLVER_MU, SOLVER_CD = 0, 1
-PRECISION_FP32, PRECISION_TF32X3, PRECISION_TF32X3_GENERAL, PRECISION_F16X2 = 0, 1, 2, 3
+PRECISION_FP32, PRECISION_TF32X3, PRECISION_TF32X3_GENERAL, PRECISION_F16X2, PRECISION_FP64 = 0, 1, 2, 3, 4
 LOSS_FROBENIUS, LOSS_KULLBACK_LEIBLER, LOSS_ITAKURA_SAITO = 0, 1, 2
 INIT_RANDOM, INIT_NNDSVD, INIT_NNDSVDA, INIT_NNDSVDAR = 0, 1, 2, 3
 INIT_CODES = {"random": INIT_RANDOM, "nndsvd": INIT_NNDSVD, "nndsvda": INIT_NNDSVDA, "nndsvdar": INIT_NNDSVDAR}
@@ -101,6 +101,12 @@ SIGNATURES = {
     "cnmf_nndsvd_init_dev": (_i, [_vp, _i, _vp, _vp, _i, _vp, _vp, _vp]),
     "cnmf_nndsvd_chunk_limit": (_i, [_vp, _i]),
     "cnmf_nndsvd_gemm_host": (_i, [_vp, _i, _i, _vp, _vp, _vp]),
+    "cnmf_dataset_create_f64": (_i, [_vp, _vp, _i, _i, _ll, _i, _vp, _pp(_vp)]),
+    "cnmf_dataset_from_columns_f64": (_i, [_vp, _vp, _vp, _i, _vp, _pp(_vp)]),
+    "cnmf_factorize_f64": (_i, [_vp, _i, _vp, _vp, _pp(NmfParams), _vp, _vp, _vp, _vp, _vp]),
+    "cnmf_factorize_init_f64": (_i, [_vp, _i, _vp, _vp, _vp, _pp(NmfParams), _vp, _vp, _vp, _vp, _vp]),
+    "cnmf_refit_f64": (_i, [_vp, _i, _i, _vp, _pp(NmfParams), _vp, _pp(_c.c_int32), _pp(_d), _vp]),
+    "cnmf_project_rows_f64": (_i, [_vp, _i, _vp, _vp, _vp]),
     "cnmf_factorize": (_i, [_vp, _i, _vp, _vp, _pp(NmfParams), _vp, _vp, _vp, _vp, _vp]),
     "cnmf_factorize_seeds_dev": (_i, [_vp, _i, _vp, _vp, _pp(NmfParams), _vp, _ll, _vp, _vp, _vp]),
     "cnmf_allgather_spectra": (_i, [_vp, _vp, _ll, _ll, _vp, _vp]),
@@ -129,7 +135,7 @@ SIGNATURES = {
 _lib = None
 
 
-ABI_VERSION = 12     # include/cnmf_b200.h CNMF_B200_ABI_VERSION
+ABI_VERSION = 13     # include/cnmf_b200.h CNMF_B200_ABI_VERSION
 
 
 def load():
@@ -168,3 +174,7 @@ def ptr(a):
 
 def f32c(a):
     return np.ascontiguousarray(a, dtype=np.float32)
+
+
+def f64c(a):
+    return np.ascontiguousarray(a, dtype=np.float64)

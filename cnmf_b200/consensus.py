@@ -314,7 +314,8 @@ def ols_zscore(usages, tpm_ds):
     var[var < 1e-12] = 1e-12
     std = np.sqrt(var)
     Uc = U - U.mean(axis=0)
-    UtZ = tpm_ds.project_rows(np.ascontiguousarray(Uc.T, dtype=np.float32)).astype(np.float64) / std
+    dt = np.float64 if getattr(tpm_ds, "fp64", False) else np.float32     # a float64 dataset projects in float64
+    UtZ = tpm_ds.project_rows(np.ascontiguousarray(Uc.T, dtype=dt)).astype(np.float64) / std
     UtU = U.T @ U
     beta, *_ = np.linalg.lstsq(UtU, UtZ, rcond=None)
     return beta
@@ -406,7 +407,10 @@ def _consensus_numerics(eng, merged, k, norm_ds, kw, density_threshold=0.5, n_ne
         std1 = np.sqrt(var[hvg_idx] * n / (n - 1.0))                              # std(ddof=1)
         if tpm_sparse:
             std1[std1 == 0] = 1.0                                                 # sc.pp.scale, cnmf.py:967
-        norm_tpm_ds = tpm_ds.from_columns(hvg_idx, 1.0 / std1)
+        if getattr(tpm_ds, "fp64", False):      # X /= std as the host divides (cnmf.py:967-969), bit for bit
+            norm_tpm_ds = tpm_ds.from_columns_div(hvg_idx, std1)
+        else:
+            norm_tpm_ds = tpm_ds.from_columns(hvg_idx, 1.0 / std1)
         sp_rf = spectra_tpm[:, hvg_idx] / np.asarray(tpm_std_hvg, dtype=np.float64)[None, :]
         rf2, it_c, _ = norm_tpm_ds.refit(sp_rf, kw)
         STATS.setdefault("refits", []).append((norm_tpm_ds.shape[0], norm_tpm_ds.shape[1], it_c))

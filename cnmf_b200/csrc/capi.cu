@@ -19,6 +19,9 @@ namespace cnmf {
 int launch_rng_init(const uint32_t* seeds_host, const int* ks_host, const int* offs_host, const double* avgs_host, int R,
                     int n_samples, int n_features, float* Wt, long long ldW, float* H, long long ldH, cnmf_handle_s* h,
                     cudaStream_t s);
+int launch_rng_init(const uint32_t* seeds_host, const int* ks_host, const int* offs_host, const double* avgs_host, int R,
+                    int n_samples, int n_features, double* Wt, long long ldW, double* H, long long ldH, cnmf_handle_s* h,
+                    cudaStream_t s);
 
 static thread_local std::string g_last_error;
 void set_last_error(const std::string& msg) { g_last_error = msg; }
@@ -194,6 +197,8 @@ int cnmf_mem_info(cnmf_handle_t h, long long* free_bytes, long long* total_bytes
 
 long long cnmf_solve_bytes_per_row(cnmf_dataset_t d) {
   if (!d) return 0;
+  // float64 solve: the factor, its compaction alternate and result slab and one product, each side, 8 bytes an entry
+  if (d->precision == CNMF_PRECISION_FP64) return 8LL * 4 * ((long long)d->ld_r + d->ld_c);
   // factorize / solve_batched: Fr + 2 piece buffers, their 3 compaction alternates, the result slab and the
   // product NUM_r along the cells; the same along the genes with one product slice per split-K slice
   const int f16 = make_view(d, false).form == Form::F16_EXACT ? 1 : 0;
@@ -359,8 +364,26 @@ int dataset_finish(cnmf_dataset_s* d, cudaStream_t s, bool exact) {
 }
 
 int check_params_precision(const cnmf_dataset_s* d, const cnmf_nmf_params* p) {
-  const int want = d->precision == CNMF_PRECISION_FP32 ? CNMF_PRECISION_FP32 : CNMF_PRECISION_TF32X3;
+  const int want = d->precision == CNMF_PRECISION_FP32 || d->precision == CNMF_PRECISION_FP64 ? d->precision
+                                                                                                : CNMF_PRECISION_TF32X3;
   CNMF_REQUIRE(p->precision == want, "params.precision must match the precision the dataset was created with");
+  return 0;
+}
+
+int require_f32(const cnmf_dataset_s* d, const char* what) {
+  if (d && d->precision == CNMF_PRECISION_FP64) {
+    set_last_error(std::string("cnmf_") + what + " takes float data; this dataset is float64: call cnmf_" + what + "_f64");
+    return -3;
+  }
+  return 0;
+}
+
+int require_f64(const cnmf_dataset_s* d, const char* what) {
+  if (d && d->precision != CNMF_PRECISION_FP64) {
+    set_last_error(std::string("cnmf_") + what + "_f64 needs a float64 dataset (cnmf_dataset_create_f64); this one "
+                   "holds float data: call cnmf_" + what);
+    return -3;
+  }
   return 0;
 }
 
@@ -404,6 +427,10 @@ int cnmf_dataset_dense_bytes(int n_rows, int n_cols, int precision, long long* p
   // what dataset_alloc hands out for one array of `elems` floats
   auto bytes = [](size_t elems) { return (long long)(std::max<size_t>(elems, 64) * sizeof(float)); };
   const size_t nx = (size_t)n_rows * pad_ld(n_cols), nxt = (size_t)n_cols * pad_ld(n_rows);
+  if (precision == CNMF_PRECISION_FP64) {
+    *peak = bytes(2 * nx);                                                 // X64
+    return 0;
+  }
   if (precision == CNMF_PRECISION_FP32) {
     *peak = bytes(nx) + bytes(nxt);                                        // X, Xt
     return 0;
@@ -417,6 +444,41 @@ int cnmf_dataset_dense_bytes(int n_rows, int n_cols, int precision, long long* p
   const long long exact_tf32 = bytes(nx) * 2 + bytes(nxt) + scales;
   const long long exact_f16 = exact_tf32 + bytes((nx + 1) / 2) + bytes((nxt + 1) / 2);
   *peak = std::max(general, std::max(exact_tf32, exact_f16));
+  return 0;
+}
+
+int cnmf_dataset_create_f64(cnmf_handle_t h, const double* X, int n_rows, int n_cols, long long ld, int src_is_device,
+                            void* stream, cnmf_dataset_t* out) {
+  CNMF_REQUIRE(h && X && out, "dataset_create_f64: NULL argument");
+  CNMF_REQUIRE(n_rows > 0 && n_cols > 0 && ld >= n_cols, "dataset_create_f64: bad shape");
+  cudaStream_t s = as_stream(stream);
+  CNMF_CUDA_CHECK(cudaSetDevice(h->device));
+  auto* d = new cnmf_dataset_s(h, n_rows, n_cols, CNMF_PRECISION_FP64);
+  d->form = Form::FP64;
+  const size_t nx = (size_t)n_rows * d->ld_c;
+  float* buf = nullptr;
+  int rc = dataset_alloc(d, &buf, 2 * nx);
+  if (rc == 0) {
+    d->X64 = reinterpret_cast<double*>(buf);
+    cudaError_t e = cudaMemsetAsync(d->X64, 0, nx * sizeof(double), s);
+    if (e == cudaSuccess)
+      e = cudaMemcpy2DAsync(d->X64, (size_t)d->ld_c * sizeof(double), X, (size_t)ld * sizeof(double),
+                            (size_t)n_cols * sizeof(double), n_rows,
+                            src_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s);
+    if (e != cudaSuccess) {
+      set_last_error(std::string("dataset upload failed: ") + cudaGetErrorString(e));
+      rc = -2;
+    }
+  }
+  double sums[2] = {0.0, 0.0};
+  if (rc == 0) rc = matrix_sums_f64(h, d->X64, n_rows, n_cols, d->ld_c, sums, s);
+  if (rc != 0) {
+    cnmf_dataset_destroy(d);
+    return rc;
+  }
+  d->sum = sums[0];
+  d->sum_sq = sums[1];
+  *out = d;
   return 0;
 }
 
@@ -627,6 +689,58 @@ int solve_and_copy_out(cnmf_dataset_s* d, const Batch& b, const cnmf_nmf_params&
   return 0;
 }
 
+// start of the float64 factorize entry points: as begin_factorize, with fp64 factor buffers
+int begin_factorize_f64(cnmf_dataset_s* d, const cnmf_nmf_params* p, int n_restarts, const int32_t* ks_in, bool args_ok,
+                        const std::string& what, Batch* b, double** Fr, double** Fc) {
+  CNMF_REQUIRE(d && p, "NULL dataset or params");
+  CNMF_TRY(require_f64(d, what.c_str()));
+  CNMF_TRY(check_params_precision(d, p));
+  CNMF_REQUIRE(p->reserved2 == 0, "params.reserved2 must be 0");
+  if (p->beta_loss != CNMF_LOSS_FROBENIUS) {
+    set_last_error("cnmf_" + what + "_f64: float64 datasets support beta_loss = frobenius only");
+    return -3;
+  }
+  CNMF_REQUIRE(args_ok && n_restarts > 0 && ks_in, what + "_f64: bad arguments");
+  CNMF_TRY(pack_restarts(n_restarts, ks_in, what, b));
+  cnmf_handle_s* h = d->h;
+  CNMF_CUDA_CHECK(cudaSetDevice(h->device));
+  *Fr = static_cast<double*>(h->dev_buf("fac.Fr64", (size_t)b->SK * d->ld_r * 8));
+  *Fc = static_cast<double*>(h->dev_buf("fac.Fc64", (size_t)b->SK * d->ld_c * 8));
+  if (!*Fr || !*Fc) return -2;
+  h->t_rng_ms = h->t_h2d_ms = h->t_solve_ms = h->t_d2h_ms = 0;
+  return 0;
+}
+
+// the float64 solve from the starts in Fr / Fc, then its results out (null outputs skipped)
+int solve_and_copy_out_f64(cnmf_dataset_s* d, const Batch& b, double* Fr, double* Fc, const cnmf_nmf_params& p,
+                           double* spectra_host, double* usages_host, int32_t* n_iter_host, double* err_host,
+                           cudaStream_t s) {
+  cnmf_handle_s* h = d->h;
+  SolveIO io;
+  io.R = (int)b.ks.size();
+  io.ks = b.ks;
+  io.Fr64 = Fr;
+  io.Fc64 = Fc;
+  io.update_cols = true;
+  auto t_solve = clk::now();
+  CNMF_TRY(solve_batched(h, make_view(d, false), io, p, s));
+  h->t_solve_ms = ms_since(t_solve);
+  auto t_d2h = clk::now();
+  if (spectra_host)
+    CNMF_CUDA_CHECK(cudaMemcpy2DAsync(spectra_host, (size_t)d->n_cols * 8, Fc, (size_t)d->ld_c * 8,
+                                      (size_t)d->n_cols * 8, b.SK, cudaMemcpyDeviceToHost, s));
+  if (usages_host)
+    CNMF_CUDA_CHECK(cudaMemcpy2DAsync(usages_host, (size_t)d->n_rows * 8, Fr, (size_t)d->ld_r * 8,
+                                      (size_t)d->n_rows * 8, b.SK, cudaMemcpyDeviceToHost, s));
+  CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
+  h->t_d2h_ms = ms_since(t_d2h);
+  for (int r = 0; r < io.R; ++r) {
+    if (n_iter_host) n_iter_host[r] = io.n_iter[r];
+    if (err_host) err_host[r] = io.err[r];
+  }
+  return 0;
+}
+
 }  // namespace
 
 static int factorize_impl(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, const uint32_t* seeds,
@@ -656,6 +770,7 @@ static int factorize_impl(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in
 int cnmf_factorize(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, const uint32_t* seeds,
                    const cnmf_nmf_params* p, float* spectra_host, float* usages_host, int32_t* n_iter_host,
                    double* err_host, void* stream) {
+  CNMF_TRY(require_f32(d, "factorize"));
   CNMF_REQUIRE(spectra_host, "factorize: spectra_host is NULL");
   return factorize_impl(d, n_restarts, ks_in, seeds, p, spectra_host, usages_host, n_iter_host, err_host, stream, nullptr, 0);
 }
@@ -663,6 +778,7 @@ int cnmf_factorize(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, const
 int cnmf_factorize_seeds_dev(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, const uint32_t* seeds,
                              const cnmf_nmf_params* p, float* spectra_dev, long long ld_out, int32_t* n_iter_host,
                              double* err_host, void* stream) {
+  CNMF_TRY(require_dense(d, "factorize_seeds_dev"));
   CNMF_REQUIRE(spectra_dev, "factorize_seeds_dev: spectra_dev is NULL");
   return factorize_impl(d, n_restarts, ks_in, seeds, p, nullptr, nullptr, n_iter_host, err_host, stream, spectra_dev, ld_out);
 }
@@ -679,6 +795,7 @@ int cnmf_last_timing(cnmf_handle_t h, double* rng_ms, double* h2d_ms, double* so
 int cnmf_factorize_init(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, const float* Wt0_host,
                         const float* H0_host, const cnmf_nmf_params* p, float* spectra_host, float* usages_host,
                         int32_t* n_iter_host, double* err_host, void* stream) {
+  CNMF_TRY(require_f32(d, "factorize_init"));
   Batch b;
   CNMF_TRY(begin_factorize(d, p, n_restarts, ks_in, Wt0_host && H0_host && spectra_host, "factorize_init", &b));
   cudaStream_t s = as_stream(stream);
@@ -704,6 +821,54 @@ int cnmf_factorize_dev(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, c
   CNMF_CUDA_CHECK(cudaMemcpyAsync(b.Fc, H0_dev, (size_t)b.SK * d->ld_c * 4, cudaMemcpyDeviceToDevice, s));
   // spectra_dev has the layout of H0_dev: whole padded rows, the zero padding included
   return solve_and_copy_out(d, b, *p, nullptr, nullptr, spectra_dev, d->ld_c, d->ld_c, n_iter_host, err_host, s);
+}
+
+int cnmf_factorize_f64(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, const uint32_t* seeds,
+                       const cnmf_nmf_params* p, double* spectra_host, double* usages_host, int32_t* n_iter_host,
+                       double* err_host, void* stream) {
+  Batch b;
+  double *Fr = nullptr, *Fc = nullptr;
+  CNMF_TRY(begin_factorize_f64(d, p, n_restarts, ks_in, seeds && spectra_host, "factorize", &b, &Fr, &Fc));
+  cudaStream_t s = as_stream(stream);
+  const int init = (p->reserved >> 1) & 3;
+  auto t_init = clk::now();
+  if (init != CNMF_INIT_RANDOM) {
+    CNMF_TRY(nndsvd_starts_dev(d, n_restarts, b.ks.data(), seeds, init, Fr, Fc, s));
+  } else {
+    if (p->reserved & 1) {
+      set_last_error("cnmf_factorize_f64: the host random generator (params.reserved bit 0) serves float datasets only");
+      return -3;
+    }
+    const double mean = d->sum / ((double)d->n_rows * (double)d->n_cols);
+    std::vector<double> avgs(n_restarts);
+    for (int r = 0; r < n_restarts; ++r) avgs[r] = std::sqrt(mean / b.ks[r]);
+    CNMF_CUDA_CHECK(cudaMemsetAsync(Fr, 0, (size_t)b.SK * d->ld_r * 8, s));
+    CNMF_CUDA_CHECK(cudaMemsetAsync(Fc, 0, (size_t)b.SK * d->ld_c * 8, s));
+    CNMF_TRY(launch_rng_init(seeds, b.ks.data(), b.off.data(), avgs.data(), n_restarts, d->n_rows, d->n_cols, Fr, d->ld_r,
+                             Fc, d->ld_c, d->h, s));
+  }
+  d->h->t_rng_ms = ms_since(t_init);
+  return solve_and_copy_out_f64(d, b, Fr, Fc, *p, spectra_host, usages_host, n_iter_host, err_host, s);
+}
+
+int cnmf_factorize_init_f64(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, const double* Wt0_host,
+                            const double* H0_host, const cnmf_nmf_params* p, double* spectra_host, double* usages_host,
+                            int32_t* n_iter_host, double* err_host, void* stream) {
+  Batch b;
+  double *Fr = nullptr, *Fc = nullptr;
+  CNMF_TRY(begin_factorize_f64(d, p, n_restarts, ks_in, Wt0_host && H0_host && spectra_host, "factorize_init", &b, &Fr,
+                               &Fc));
+  cudaStream_t s = as_stream(stream);
+  auto t_h2d = clk::now();
+  CNMF_CUDA_CHECK(cudaMemsetAsync(Fr, 0, (size_t)b.SK * d->ld_r * 8, s));
+  CNMF_CUDA_CHECK(cudaMemsetAsync(Fc, 0, (size_t)b.SK * d->ld_c * 8, s));
+  CNMF_CUDA_CHECK(cudaMemcpy2DAsync(Fr, (size_t)d->ld_r * 8, Wt0_host, (size_t)d->n_rows * 8, (size_t)d->n_rows * 8, b.SK,
+                                    cudaMemcpyHostToDevice, s));
+  CNMF_CUDA_CHECK(cudaMemcpy2DAsync(Fc, (size_t)d->ld_c * 8, H0_host, (size_t)d->n_cols * 8, (size_t)d->n_cols * 8, b.SK,
+                                    cudaMemcpyHostToDevice, s));
+  CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
+  d->h->t_h2d_ms = ms_since(t_h2d);
+  return solve_and_copy_out_f64(d, b, Fr, Fc, *p, spectra_host, usages_host, n_iter_host, err_host, s);
 }
 
 int cnmf_random_init_dev(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, const uint32_t* seeds, float* Wt_dev,

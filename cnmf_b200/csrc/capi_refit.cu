@@ -24,7 +24,8 @@ __global__ void fill_kernel(float* p, float v, int rows, int n, int ld) {
 // column sums of v and v^2 with v = X[r, c] * (row_scale ? row_scale[r] : 1), fp64.  Threads own columns (coalesced),
 // blockIdx.y owns a fixed strip of rows: partial[y][c], reduced in strip order by col_stats_reduce_kernel
 // (deterministic: the HVG ranking of prepare() is a sort of these numbers).
-__global__ void col_stats_kernel(const float* __restrict__ X, int rows, int cols, int ld,
+template <typename T>
+__global__ void col_stats_kernel(const T* __restrict__ X, int rows, int cols, int ld,
                                  const double* __restrict__ row_scale, double* __restrict__ part) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= cols) return;
@@ -39,6 +40,25 @@ __global__ void col_stats_kernel(const float* __restrict__ X, int rows, int cols
   }
   part[((long long)blockIdx.y * 2) * cols + c] = s;
   part[((long long)blockIdx.y * 2 + 1) * cols + c] = q;
+}
+
+// float64 datasets: dst[r, c] = src[r, cols[c]] / divisor[c] (one IEEE division, as numpy's X /= std)
+__global__ void gather_cols_div_kernel(const double* __restrict__ src, int rows, int ld_src, const int* __restrict__ cols,
+                                       const double* __restrict__ divisor, int n_cols, double* __restrict__ dst,
+                                       int ld_dst) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= n_cols) return;
+  const int sc = cols[c];
+  const double f = divisor[c];
+  for (int r = blockIdx.y; r < rows; r += gridDim.y)
+    dst[(long long)r * ld_dst + c] = __ddiv_rn(src[(long long)r * ld_src + sc], f);
+}
+
+// out (n x k, dense) = F^T for F (k x ld, n valid columns)
+__global__ void transpose64_kernel(const double* __restrict__ F, int k, int n, int ld, double* __restrict__ out) {
+  const long long total = (long long)n * k;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x)
+    out[i] = F[(i % k) * ld + i / k];
 }
 
 __global__ void col_stats_reduce_kernel(const double* __restrict__ part, int strips, int cols, double* __restrict__ out) {
@@ -111,6 +131,7 @@ static int col_stats_impl(cnmf_dataset_t d, const double* row_scale_host, double
   cudaStream_t s = as_stream(stream);
   CNMF_CUDA_CHECK(cudaSetDevice(h->device));
   if (row_scale_host) CNMF_TRY(require_dense(d, "scaled_col_stats"));
+  const bool f64 = d->precision == CNMF_PRECISION_FP64;
   double* buf = d->col_sums;        // sparse datasets: csc_col_stats_kernel ran at creation
   if (!d->sparse) {
     const int strips = std::max(1, std::min(64, d->n_rows / 64));
@@ -124,7 +145,8 @@ static int col_stats_impl(cnmf_dataset_t d, const double* row_scale_host, double
     }
     if (!part || !buf) return -2;
     dim3 grid((d->n_cols + 127) / 128, strips);
-    col_stats_kernel<<<grid, 128, 0, s>>>(d->X, d->n_rows, d->n_cols, d->ld_c, d_rs, part);
+    if (f64) col_stats_kernel<<<grid, 128, 0, s>>>(d->X64, d->n_rows, d->n_cols, d->ld_c, d_rs, part);
+    else col_stats_kernel<<<grid, 128, 0, s>>>(d->X, d->n_rows, d->n_cols, d->ld_c, d_rs, part);
     col_stats_reduce_kernel<<<(d->n_cols + 127) / 128, 128, 0, s>>>(part, strips, d->n_cols, buf);
     CNMF_CUDA_CHECK(cudaGetLastError());
     h->launches += 2;
@@ -188,6 +210,7 @@ int cnmf_dataset_tpm_stats(cnmf_dataset_t d, double target_sum, double* totals_h
 int cnmf_dataset_from_columns(cnmf_dataset_t src, const int32_t* cols_host, const float* col_scale_host, int n_cols,
                               void* stream, cnmf_dataset_t* out) {
   CNMF_REQUIRE(src && cols_host && col_scale_host && out && n_cols > 0, "dataset_from_columns: bad arguments");
+  CNMF_TRY(require_f32(src, "dataset_from_columns"));
   for (int c = 0; c < n_cols; ++c)
     CNMF_REQUIRE(cols_host[c] >= 0 && cols_host[c] < src->n_cols, "dataset_from_columns: column index out of range");
   cnmf_handle_s* h = src->h;
@@ -267,6 +290,7 @@ int cnmf_dataset_scale_rows(cnmf_dataset_t src, const float* row_scale_host, voi
 int cnmf_refit(cnmf_dataset_t d, int transposed, int k, const float* fixed_host, const cnmf_nmf_params* p,
                float* out_host, int32_t* n_iter_host, double* err_host, void* stream) {
   CNMF_REQUIRE(d && fixed_host && p && out_host, "refit: NULL argument");
+  CNMF_TRY(require_f32(d, "refit"));
   CNMF_TRY(check_params_precision(d, p));
   CNMF_REQUIRE(k >= 1 && k <= KMAX, "refit: n_components must be in [1, 32] on the CUDA path");
   if (d->sparse && !transposed) CNMF_TRY(require_dense(d, "refit with transposed = 0"));
@@ -340,6 +364,7 @@ int cnmf_refit(cnmf_dataset_t d, int transposed, int k, const float* fixed_host,
 // out (k x n_cols) = Ut (k x n_rows) * X  -- the X^T Y accumulator of efficient_ols_all_cols (cnmf.py:119)
 int cnmf_project_rows(cnmf_dataset_t d, int k, const float* Ut_host, float* out_host, void* stream) {
   CNMF_REQUIRE(d && Ut_host && out_host && k >= 1, "project_rows: bad arguments");
+  CNMF_TRY(require_f32(d, "project_rows"));
   cnmf_handle_s* h = d->h;
   cudaStream_t s = as_stream(stream);
   CNMF_CUDA_CHECK(cudaSetDevice(h->device));
@@ -404,6 +429,115 @@ int cnmf_project_rows(cnmf_dataset_t d, int k, const float* Ut_host, float* out_
       for (int z = 0; z < splits; ++z) a += tmp[(size_t)z * k * d->ld_c + (size_t)c * d->ld_c + j];
       out_host[(size_t)c * d->n_cols + j] = (float)a;
     }
+  return 0;
+}
+
+// --------------------------------------------------------------------------------- float64 datasets
+int cnmf_dataset_from_columns_f64(cnmf_dataset_t src, const int32_t* cols_host, const double* divisor_host, int n_cols,
+                                  void* stream, cnmf_dataset_t* out) {
+  CNMF_REQUIRE(src && cols_host && divisor_host && out && n_cols > 0, "dataset_from_columns_f64: bad arguments");
+  CNMF_TRY(require_f64(src, "dataset_from_columns"));
+  for (int c = 0; c < n_cols; ++c)
+    CNMF_REQUIRE(cols_host[c] >= 0 && cols_host[c] < src->n_cols, "dataset_from_columns_f64: column index out of range");
+  cnmf_handle_s* h = src->h;
+  cudaStream_t s = as_stream(stream);
+  CNMF_CUDA_CHECK(cudaSetDevice(h->device));
+  int* d_cols = static_cast<int*>(h->dev_buf("fromcols.idx", sizeof(int) * n_cols));
+  double* d_div = static_cast<double*>(h->dev_buf("fromcols.div64", sizeof(double) * n_cols));
+  if (!d_cols || !d_div) return -2;
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(d_cols, cols_host, sizeof(int) * n_cols, cudaMemcpyHostToDevice, s));
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(d_div, divisor_host, sizeof(double) * n_cols, cudaMemcpyHostToDevice, s));
+  auto* d = new cnmf_dataset_s(h, src->n_rows, n_cols, CNMF_PRECISION_FP64);
+  d->form = Form::FP64;
+  const size_t nx = (size_t)d->n_rows * d->ld_c;
+  float* buf = nullptr;
+  int rc = dataset_alloc(d, &buf, 2 * nx);
+  if (rc == 0) {
+    d->X64 = reinterpret_cast<double*>(buf);
+    if (cudaMemsetAsync(d->X64, 0, nx * sizeof(double), s) != cudaSuccess) rc = -2;
+  }
+  if (rc == 0) {
+    dim3 grid((n_cols + 127) / 128, std::min(d->n_rows, 16384));
+    gather_cols_div_kernel<<<grid, 128, 0, s>>>(src->X64, d->n_rows, src->ld_c, d_cols, d_div, n_cols, d->X64, d->ld_c);
+    h->launches += 1;
+    if (cudaGetLastError() != cudaSuccess) rc = -2;
+  }
+  double sums[2] = {0.0, 0.0};
+  if (rc == 0) rc = matrix_sums_f64(h, d->X64, d->n_rows, d->n_cols, d->ld_c, sums, s);
+  if (rc != 0) {
+    cnmf_dataset_destroy(d);
+    return rc;
+  }
+  d->sum = sums[0];
+  d->sum_sq = sums[1];
+  *out = d;
+  return 0;
+}
+
+int cnmf_refit_f64(cnmf_dataset_t d, int transposed, int k, const double* fixed_host, const cnmf_nmf_params* p,
+                   double* out_host, int32_t* n_iter_host, double* err_host, void* stream) {
+  CNMF_REQUIRE(d && fixed_host && p && out_host, "refit_f64: NULL argument");
+  CNMF_TRY(require_f64(d, "refit"));
+  CNMF_TRY(check_params_precision(d, p));
+  CNMF_REQUIRE(k >= 1 && k <= KMAX, "refit_f64: n_components must be in [1, 32] on the CUDA path");
+  if (p->beta_loss != CNMF_LOSS_FROBENIUS) {
+    set_last_error("cnmf_refit_f64: float64 datasets support beta_loss = frobenius only");
+    return -3;
+  }
+  cnmf_handle_s* h = d->h;
+  cudaStream_t s = as_stream(stream);
+  CNMF_CUDA_CHECK(cudaSetDevice(h->device));
+  const DataView v = make_view(d, transposed != 0);
+  const size_t nr = (size_t)k * v.ld_r, nc = (size_t)k * v.ld_c;
+  double* Fr = static_cast<double*>(h->dev_buf("refit.Fr64", nr * 8));
+  double* Fc = static_cast<double*>(h->dev_buf("refit.Fc64", nc * 8));
+  double* T = static_cast<double*>(h->dev_buf("refit.T64", (size_t)v.n_r * k * 8));
+  if (!Fr || !Fc || !T) return -2;
+  CNMF_CUDA_CHECK(cudaMemsetAsync(Fr, 0, nr * 8, s));
+  CNMF_CUDA_CHECK(cudaMemsetAsync(Fc, 0, nc * 8, s));
+  CNMF_CUDA_CHECK(cudaMemcpy2DAsync(Fc, (size_t)v.ld_c * 8, fixed_host, (size_t)v.n_c * 8, (size_t)v.n_c * 8, k,
+                                    cudaMemcpyHostToDevice, s));
+  if (p->solver == CNMF_SOLVER_MU) {
+    // sklearn _nmf.py:1223-1226: W = full(sqrt(X.mean() / k))
+    const double mean = v.sum / ((double)v.n_r * (double)v.n_c);
+    CNMF_TRY(fill_f64(Fr, std::sqrt(mean / k), k, v.n_r, v.ld_r, s));
+    h->launches += 1;
+  }  // 'cd': zeros (sklearn _nmf.py:1227-1228)
+  SolveIO io;
+  io.R = 1;
+  io.ks = {k};
+  io.Fr64 = Fr;
+  io.Fc64 = Fc;
+  io.update_cols = false;
+  CNMF_TRY(solve_batched(h, v, io, *p, s));
+  transpose64_kernel<<<NUM_SMS * 4, 256, 0, s>>>(Fr, k, v.n_r, v.ld_r, T);
+  CNMF_CUDA_CHECK(cudaGetLastError());
+  h->launches += 1;
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(out_host, T, (size_t)v.n_r * k * 8, cudaMemcpyDeviceToHost, s));
+  CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
+  if (n_iter_host) *n_iter_host = io.n_iter[0];
+  if (err_host) *err_host = io.err[0];
+  return 0;
+}
+
+int cnmf_project_rows_f64(cnmf_dataset_t d, int k, const double* Ut_host, double* out_host, void* stream) {
+  CNMF_REQUIRE(d && Ut_host && out_host && k >= 1, "project_rows_f64: bad arguments");
+  CNMF_TRY(require_f64(d, "project_rows"));
+  cnmf_handle_s* h = d->h;
+  cudaStream_t s = as_stream(stream);
+  CNMF_CUDA_CHECK(cudaSetDevice(h->device));
+  const size_t na = (size_t)k * d->ld_r, nc = (size_t)k * d->ld_c;
+  double* A = static_cast<double*>(h->dev_buf("proj.A64", na * 8));
+  double* C = static_cast<double*>(h->dev_buf("proj.C64", nc * 8));
+  if (!A || !C) return -2;
+  CNMF_CUDA_CHECK(cudaMemsetAsync(A, 0, na * 8, s));
+  CNMF_CUDA_CHECK(cudaMemcpy2DAsync(A, (size_t)d->ld_r * 8, Ut_host, (size_t)d->n_rows * 8, (size_t)d->n_rows * 8, k,
+                                    cudaMemcpyHostToDevice, s));
+  h->launches += 1;
+  CNMF_TRY(launch_gemm_f64(A, d->ld_r, k, d->X64, d->n_rows, d->n_cols, d->ld_c, true, C, d->ld_c, s));
+  CNMF_CUDA_CHECK(cudaMemcpy2DAsync(out_host, (size_t)d->n_cols * 8, C, (size_t)d->ld_c * 8, (size_t)d->n_cols * 8, k,
+                                    cudaMemcpyDeviceToHost, s));
+  CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
   return 0;
 }
 

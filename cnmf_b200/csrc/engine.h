@@ -17,8 +17,9 @@ namespace cnmf {
 //   TF32        X, X_hi / X_lo, Xt_hi / lo   tf32 hi / lo pieces      gemm_tf32x3, 3 passes
 //   TF32_EXACT  X, C = X_hi, C^T = Xt_hi     tf32 pieces of F * scale gemm_tf32x3, exact B, 2 passes
 //   F16_EXACT   X, C, C^T as fp16            fp16 pieces of F * scale gemm_tf32x3, f16 = 1
+//   FP64        X64 only (fp64, row-major)    factor in fp64            gemm_f64 (DMMA), both orientations
 // The exact forms hold X = diag(row_scale) C diag(col_scale) with C small non-negative integers.
-enum class Form { FP32, TF32, TF32_EXACT, F16_EXACT };
+enum class Form { FP32, TF32, TF32_EXACT, F16_EXACT, FP64 };
 inline bool form_exact(Form f) { return f == Form::TF32_EXACT || f == Form::F16_EXACT; }
 
 }  // namespace cnmf
@@ -40,10 +41,11 @@ struct cnmf_handle_s {
   std::vector<Pending> ev_pending;
   size_t ev_used = 0;
   // kernel classes: 0 = batched GEMM (work = algorithmic FLOPs), 1 = fused update kernels (work = algorithmic bytes),
-  // 2 = sparse products csc_project (work = algorithmic bytes), 3 = fp64 GEMM of the NNDSVD starts (work = FLOPs)
-  static constexpr int PROF_CLASSES = 4;
-  double prof_ms[PROF_CLASSES] = {0.0, 0.0, 0.0, 0.0}, prof_work[PROF_CLASSES] = {0.0, 0.0, 0.0, 0.0};
-  long long prof_launches[PROF_CLASSES] = {0, 0, 0, 0};
+  // 2 = sparse products csc_project (work = algorithmic bytes), 3 = fp64 GEMM of the NNDSVD starts (work = FLOPs),
+  // 4 = fp64 GEMM of the float64 solver (work = FLOPs)
+  static constexpr int PROF_CLASSES = 5;
+  double prof_ms[PROF_CLASSES] = {0.0, 0.0, 0.0, 0.0, 0.0}, prof_work[PROF_CLASSES] = {0.0, 0.0, 0.0, 0.0, 0.0};
+  long long prof_launches[PROF_CLASSES] = {0, 0, 0, 0, 0};
   int nndsvd_chunk_restarts = 0;                // > 0: at most this many restarts per chunk of the NNDSVD starts
   double t_rng_ms = 0, t_h2d_ms = 0, t_solve_ms = 0, t_d2h_ms = 0;   // host wall-clock phases of the last factorize
   int prof_begin(cudaStream_t s, double work, int cls = 0);    // start event (recorded or shared); returns slot or -1
@@ -96,6 +98,9 @@ struct cnmf_dataset_s {
   double* col_sums = nullptr;
   int* item_ptr = nullptr;
   int n_items = 0;
+  // float64 datasets (precision CNMF_PRECISION_FP64, form FP64): X64 is the only resident form, n_rows x ld_c, padding
+  // zeroed; X and every other array above stay nullptr
+  double* X64 = nullptr;
   std::vector<std::pair<void*, size_t>> owned;
 
   // every creator starts here: shape, padded strides and the creation precision
@@ -124,6 +129,8 @@ struct DataView {
   Form form;                // FP32 on sparse datasets: their solves run no GEMM and make no pieces
   const float* scale_r;     // per row-item scale (length ld_r) or nullptr
   const float* scale_c;     // per column-item scale (length ld_c) or nullptr
+  const double* X64;        // FP64: the dataset's fp64 X (n_rows x ld_c); both products read it through gemm_f64
+  bool transposed;          // rows are the dataset's columns
 };
 
 DataView make_view(const cnmf_dataset_s* d, bool transposed);
@@ -144,8 +151,12 @@ int dataset_finish(cnmf_dataset_s* d, cudaStream_t s, bool exact = false);
 // d->form from the creation precision and, where it allows an exact form and `exact` is not yet known, exact-count
 // detection on the dense or CSC matrix (synchronises)
 int dataset_resolve_form(cnmf_dataset_s* d, bool exact, cudaStream_t s);
-// params.precision must be FP32 or, for every tensor-core precision, TF32X3
+// params.precision must be FP32, FP64 on a float64 dataset or, for every tensor-core precision, TF32X3
 int check_params_precision(const cnmf_dataset_s* d, const cnmf_nmf_params* p);
+// -3 with a message naming the float64 entry point `what`_f64 when d is a float64 dataset (float entry points)
+int require_f32(const cnmf_dataset_s* d, const char* what);
+// -3 with a message naming the float entry point `what` when d is not a float64 dataset (_f64 entry points)
+int require_f64(const cnmf_dataset_s* d, const char* what);
 
 struct SolveIO {
   int R = 0;
@@ -157,6 +168,8 @@ struct SolveIO {
   // the row product, computed by the caller (refits of sparse datasets: NUM_r = Fc * X^T, SK x ld_r, one split).
   // Requires update_cols = false; the solver then runs no GEMM and reads no B operand.
   const float* num_rows = nullptr;
+  // FP64 datasets: the packed factors in fp64 (same slot layout); Fr / Fc and num_rows are unused
+  double *Fr64 = nullptr, *Fc64 = nullptr;
   std::vector<int> n_iter;  // out
   std::vector<double> last; // out: last convergence statistic (mu: error, cd: violation)
   std::vector<double> err;  // out: final ||X - Fr^T Fc||_F
@@ -166,6 +179,12 @@ struct SolveIO {
 int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_nmf_params& p, cudaStream_t s);
 // beta_loss = kullback-leibler / itakura-saito (nmf_beta.cu); reached through solve_batched
 int solve_batched_beta(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_nmf_params& p, cudaStream_t s);
+// float64 datasets (form FP64, Frobenius loss, MU and CD; nmf_f64.cu): io.Fr64 / io.Fc64; reached through solve_batched
+int solve_batched_f64(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_nmf_params& p, cudaStream_t s);
+// out[0] = sum(X), out[1] = sum(X^2) of a float64 dataset matrix, fp64 in an order fixed by the shape (synchronises)
+int matrix_sums_f64(cnmf_handle_s* h, const double* X, int rows, int cols, int ld, double* out_host, cudaStream_t s);
+// p[r, j] = v for r < rows, j < n (row stride ld); does not synchronise
+int fill_f64(double* p, double v, int rows, int n, int ld, cudaStream_t s);
 int matrix_min(cnmf_handle_s* h, const float* X, int rows, int cols, int ld, float* out_host, cudaStream_t s);
 // the streaming beta-divergence kernels read X in both orientations in full fp32: builds d->Xt if the dataset
 // (tf32x3 mode) only holds the pieces
@@ -173,7 +192,7 @@ int dataset_ensure_full_transpose(cnmf_dataset_s* d, cudaStream_t s);
 
 // ---- sparse (CSC) datasets: sparse_kernels.cu
 constexpr int CSC_CHUNK = 4096;     // most entries of a column one warp of csc_project_kernel reduces
-// -3 with a message naming the entry point when d is sparse
+// -3 with a message naming the entry point when d is sparse or float64
 int require_dense(const cnmf_dataset_s* d, const char* what);
 // out (k x ld, first n_cols columns written) = U^T * X with U staged on the device as n_rows x kp floats
 // (kp = k rounded up to 4, zero padded); fp64 products and sums in a fixed order, rounded to fp32 once
@@ -198,9 +217,16 @@ int csc_tpm_sums(const cnmf_dataset_s* d, double target_sum, double* totals, dou
 // n_out = n_cols).  Reduction order depends on the shape only.  Does not synchronise.
 int launch_gemm_f64(const double* A, int lda, int M, const float* X, int n_rows, int n_cols, int ldx, bool to_genes,
                     double* C, int ldc, cudaStream_t s);
+// the same product for a float64 dataset matrix X (the float64 solver's NUM_r / NUM_c and the NNDSVD starts of a
+// float64 dataset): same tiles, same reduction order
+int launch_gemm_f64(const double* A, int lda, int M, const double* X, int n_rows, int n_cols, int ldx, bool to_genes,
+                    double* C, int ldc, cudaStream_t s);
 // scikit-learn's NNDSVD starting factors of every restart (ks[r], seeds[r]) for init = CNMF_INIT_NNDSVD / NNDSVDA /
 // NNDSVDAR into packed padded Wt (sum ks x ld_r) and H (sum ks x ld_c); synchronises
 int nndsvd_starts_dev(cnmf_dataset_s* d, int R, const int* ks, const uint32_t* seeds, int init, float* Wt, float* H,
+                      cudaStream_t s);
+// the same starts of a float64 dataset into fp64 Wt / H: no rounding to fp32
+int nndsvd_starts_dev(cnmf_dataset_s* d, int R, const int* ks, const uint32_t* seeds, int init, double* Wt, double* H,
                       cudaStream_t s);
 
 }  // namespace cnmf

@@ -1,10 +1,12 @@
-// float64 tensor-core GEMM of the NNDSVD range finder (nndsvd.cu): packed fp64 rows times the dataset's fp32 X, in
-// either orientation, on the fp64 MMA (mma.sync m16n8k16 .f64 -> DMMA.16x8x16; Hopper has no fp64 wgmma).
+// float64 tensor-core GEMM: packed fp64 rows times the dataset's X, in either orientation, on the fp64 MMA
+// (mma.sync m16n8k16 .f64 -> DMMA.16x8x16; Hopper has no fp64 wgmma).  X is the fp32 matrix of an ordinary dataset
+// (the NNDSVD range finder, nndsvd.cu) or the fp64 matrix of a float64 dataset (its NNDSVD starts and the float64
+// solver's two products, nmf_f64.cu); the element type only changes how a tile is loaded.
 //
 //   to_genes = false:  C[m, i] = sum_g A[m, g] X[i, g]     (A over genes, output over cells; X read K-major)
 //   to_genes = true:   C[m, g] = sum_i A[m, i] X[i, g]     (A over cells, output over genes; X read MN-major)
 //
-// X is converted to fp64 on its way into shared memory: no fp64 or transposed copy of it exists.  Every output
+// An fp32 X is converted to fp64 on its way into shared memory: no fp64 or transposed copy of it exists.  Every output
 // element accumulates its K tiles in ascending order, one MMA per 16-deep tile, whatever M is and wherever its row
 // sits in the tile: a restart's products do not depend on the other restarts of the call.
 #include <cuda_runtime.h>
@@ -29,9 +31,25 @@ __device__ __forceinline__ void mma_f64_16816(double (&d)[4], const double (&a)[
         "d"(b[2]), "d"(b[3]));
 }
 
-template <bool TO_GENES>
+// 8 consecutive elements of X (16-byte aligned for float, 64-byte for double) into registers
+__device__ __forceinline__ void load8(const float* p, float (&r)[8]) {
+  const float4* src = reinterpret_cast<const float4*>(p);
+  const float4 v0 = src[0], v1 = src[1];
+  r[0] = v0.x; r[1] = v0.y; r[2] = v0.z; r[3] = v0.w;
+  r[4] = v1.x; r[5] = v1.y; r[6] = v1.z; r[7] = v1.w;
+}
+__device__ __forceinline__ void load8(const double* p, double (&r)[8]) {
+  const double2* src = reinterpret_cast<const double2*>(p);
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    const double2 v = src[e];
+    r[2 * e] = v.x; r[2 * e + 1] = v.y;
+  }
+}
+
+template <bool TO_GENES, typename TX>
 __global__ void __launch_bounds__(F64_THREADS)
-gemm_f64_kernel(const double* __restrict__ A, int lda, int M, int K, const float* __restrict__ X, int ldx, int n_rows,
+gemm_f64_kernel(const double* __restrict__ A, int lda, int M, int K, const TX* __restrict__ X, int ldx, int n_rows,
                 double* __restrict__ C, int ldc, int n_out) {
   __shared__ double As[F64_BM][F64_PAD];
   __shared__ double Bs[F64_BN][F64_PAD];      // [output item][k]
@@ -43,7 +61,7 @@ gemm_f64_kernel(const double* __restrict__ A, int lda, int M, int K, const float
   // global -> register staging of one K tile
   const int a_row = tid >> 2, a_k = (tid & 3) * 4;
   double ra[4];
-  float rb[8];
+  TX rb[8];
   auto load_tile = [&](int k0) {
     const long long am = m0 + a_row;
 #pragma unroll
@@ -55,25 +73,19 @@ gemm_f64_kernel(const double* __restrict__ A, int lda, int M, int K, const float
       const int n = tid >> 1, kh = (tid & 1) * 8;
       const long long i = n0 + n;
       if (i < n_rows) {
-        const float4* src = reinterpret_cast<const float4*>(X + i * ldx + k0 + kh);
-        const float4 v0 = src[0], v1 = src[1];
-        rb[0] = v0.x; rb[1] = v0.y; rb[2] = v0.z; rb[3] = v0.w;
-        rb[4] = v1.x; rb[5] = v1.y; rb[6] = v1.z; rb[7] = v1.w;
+        load8(X + i * ldx + k0 + kh, rb);
       } else {
 #pragma unroll
-        for (int e = 0; e < 8; ++e) rb[e] = 0.f;
+        for (int e = 0; e < 8; ++e) rb[e] = TX(0);
       }
     } else {                // Bs[n][k] = X[k0 + k][n0 + n]: 8 consecutive genes of one cell
       const int k = tid >> 4, nq = (tid & 15) * 8;
       const long long i = k0 + k;
       if (i < n_rows && n0 + nq + 8 <= ldx) {
-        const float4* src = reinterpret_cast<const float4*>(X + i * ldx + n0 + nq);
-        const float4 v0 = src[0], v1 = src[1];
-        rb[0] = v0.x; rb[1] = v0.y; rb[2] = v0.z; rb[3] = v0.w;
-        rb[4] = v1.x; rb[5] = v1.y; rb[6] = v1.z; rb[7] = v1.w;
+        load8(X + i * ldx + n0 + nq, rb);
       } else {
 #pragma unroll
-        for (int e = 0; e < 8; ++e) rb[e] = 0.f;
+        for (int e = 0; e < 8; ++e) rb[e] = TX(0);
       }
     }
   };
@@ -138,9 +150,8 @@ gemm_f64_kernel(const double* __restrict__ A, int lda, int M, int K, const float
       }
 }
 
-}  // namespace
-
-int launch_gemm_f64(const double* A, int lda, int M, const float* X, int n_rows, int n_cols, int ldx, bool to_genes,
+template <typename TX>
+int gemm_f64_launch(const double* A, int lda, int M, const TX* X, int n_rows, int n_cols, int ldx, bool to_genes,
                     double* C, int ldc, cudaStream_t s) {
   if (M <= 0) return 0;
   const int n_out = to_genes ? n_cols : n_rows;
@@ -148,11 +159,23 @@ int launch_gemm_f64(const double* A, int lda, int M, const float* X, int n_rows,
   dim3 grid((n_out + F64_BN - 1) / F64_BN, (M + F64_BM - 1) / F64_BM);
   CNMF_REQUIRE(grid.y <= 65535, "fp64 GEMM: too many rows");
   if (to_genes)
-    gemm_f64_kernel<true><<<grid, F64_THREADS, 0, s>>>(A, lda, M, K, X, ldx, n_rows, C, ldc, n_out);
+    gemm_f64_kernel<true, TX><<<grid, F64_THREADS, 0, s>>>(A, lda, M, K, X, ldx, n_rows, C, ldc, n_out);
   else
-    gemm_f64_kernel<false><<<grid, F64_THREADS, 0, s>>>(A, lda, M, K, X, ldx, n_rows, C, ldc, n_out);
+    gemm_f64_kernel<false, TX><<<grid, F64_THREADS, 0, s>>>(A, lda, M, K, X, ldx, n_rows, C, ldc, n_out);
   CNMF_CUDA_CHECK(cudaGetLastError());
   return 0;
+}
+
+}  // namespace
+
+int launch_gemm_f64(const double* A, int lda, int M, const float* X, int n_rows, int n_cols, int ldx, bool to_genes,
+                    double* C, int ldc, cudaStream_t s) {
+  return gemm_f64_launch(A, lda, M, X, n_rows, n_cols, ldx, to_genes, C, ldc, s);
+}
+
+int launch_gemm_f64(const double* A, int lda, int M, const double* X, int n_rows, int n_cols, int ldx, bool to_genes,
+                    double* C, int ldc, cudaStream_t s) {
+  return gemm_f64_launch(A, lda, M, X, n_rows, n_cols, ldx, to_genes, C, ldc, s);
 }
 
 }  // namespace cnmf

@@ -38,6 +38,8 @@ DataView make_view(const cnmf_dataset_s* d, bool transposed) {
   v.form = d->sparse ? Form::FP32 : d->form;
   v.scale_r = d->sparse ? nullptr : transposed ? d->col_scale : d->row_scale;
   v.scale_c = d->sparse ? nullptr : transposed ? d->row_scale : d->col_scale;
+  v.X64 = d->X64;
+  v.transposed = transposed;
   return v;
 }
 
@@ -56,6 +58,9 @@ int form_gemm(Form form, GemmArgs g, const float* A, const float* A_hi, const fl
     case Form::TF32_EXACT:
       g.b_exact = 1; g.out_col_scale = out_scale;
       break;
+    case Form::FP64:
+      set_last_error("float64 datasets run their products through gemm_f64");
+      return -3;
   }
   g.A_hi = A_hi; g.A_lo = A_lo; g.B_hi = B.hi;
   return gemm_tf32x3(g, s);
@@ -64,7 +69,8 @@ int form_gemm(Form form, GemmArgs g, const float* A, const float* A_hi, const fl
 int make_pieces(Form form, const float* F, int rows, int n, int ld, const float* scale, float* hi, float* lo,
                 float* tile_scale, cudaStream_t s) {
   switch (form) {
-    case Form::FP32: return 0;
+    case Form::FP32:
+    case Form::FP64: return 0;
     case Form::F16_EXACT: return launch_emit_f16(F, rows, n, ld, scale, hi, lo, tile_scale, (ld + 511) / 512, s);
     default: return launch_split_scaled(F, hi, lo, rows, ld, scale, s);
   }
@@ -99,6 +105,7 @@ int run_gemm(cnmf_handle_s* h, Form form, const float* A, const float* A_hi, con
 
 int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_nmf_params& p, cudaStream_t s) {
   const int R0 = io.R;
+  if (v.form == Form::FP64) return solve_batched_f64(h, v, io, p, s);
   if (p.beta_loss != CNMF_LOSS_FROBENIUS) return solve_batched_beta(h, v, io, p, s);
   CNMF_REQUIRE(R0 > 0 && (int)io.ks.size() == R0, "solve: bad restart list");
   CNMF_REQUIRE(p.solver == CNMF_SOLVER_MU || p.solver == CNMF_SOLVER_CD, "solve: unknown solver");

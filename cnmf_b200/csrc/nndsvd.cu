@@ -345,10 +345,12 @@ stats_kernel(Meta m, const double* __restrict__ Qcell, int ldc, int n_cells, con
 }
 
 // W^T rows (cells = true) or H rows of restart r, component j: sklearn's NNDSVD composition, eps zeroing and the
-// 'nndsvda' fill (the 'nndsvdar' fill follows in ar_fill_kernel), rounded to fp32 once.
+// 'nndsvda' fill (the 'nndsvdar' fill follows in ar_fill_kernel), rounded to fp32 once (T = float) or kept in fp64
+// (T = double, float64 datasets).
+template <typename T>
 __global__ void __launch_bounds__(256)
 compose_kernel(Meta m, const double* __restrict__ Qv, int ldq, int n, bool cells, const double* __restrict__ stats,
-               const double* __restrict__ Sv, float* __restrict__ out, int ldo, double fill) {
+               const double* __restrict__ Sv, T* __restrict__ out, int ldo, double fill) {
   const int r = m.comp_r[blockIdx.y], j = m.comp_j[blockIdx.y];
   const int item = blockIdx.x * 256 + threadIdx.x;
   if (item >= n) return;
@@ -374,7 +376,7 @@ compose_kernel(Meta m, const double* __restrict__ Qv, int ldq, int n, bool cells
     w = lbd * u;
   }
   if (w < NNDSVD_EPS) w = fill;
-  out[(long long)(m.koff[r] + j) * ldo + item] = (float)w;
+  out[(long long)(m.koff[r] + j) * ldo + item] = (T)w;
 }
 
 // block-wide exclusive scan of one flag per thread; returns this thread's slot, *total = number of set flags
@@ -397,8 +399,9 @@ __device__ __forceinline__ int block_rank(bool flag, int* warp_tot, int* total) 
 // 'nndsvdar': the zeros of W (n x k, row-major) then of H (k x g) take |avg * z / 100| for the normals z of a fresh
 // RandomState(seed), in that order.  The zeros' positions are listed in the restart's (no longer needed) rows of
 // Qc / Qg first.
+template <typename T>
 __global__ void __launch_bounds__(LEGACY_GAUSS_THREADS)
-ar_fill_kernel(Meta m, float* __restrict__ Wt, int ldw, int n_cells, float* __restrict__ H, int ldh, int n_genes,
+ar_fill_kernel(Meta m, T* __restrict__ Wt, int ldw, int n_cells, T* __restrict__ H, int ldh, int n_genes,
                double* Qc, int ld_r, double* Qg, int ld_c, double avg) {
   __shared__ LegacyGaussShared sh;
   __shared__ int warp_tot[8];
@@ -410,7 +413,7 @@ ar_fill_kernel(Meta m, float* __restrict__ Wt, int ldw, int n_cells, float* __re
   long long zW = 0, zH = 0;
   for (long long b = 0; b < nW; b += LEGACY_GAUSS_THREADS) {
     const long long t = b + tid;
-    const bool z = t < nW && Wt[(long long)(koff + t % k) * ldw + t / k] == 0.f;
+    const bool z = t < nW && Wt[(long long)(koff + t % k) * ldw + t / k] == T(0);
     int tot;
     const int slot = block_rank(z, warp_tot, &tot);
     if (z) posW[zW + slot] = t;
@@ -418,7 +421,7 @@ ar_fill_kernel(Meta m, float* __restrict__ Wt, int ldw, int n_cells, float* __re
   }
   for (long long b = 0; b < nH; b += LEGACY_GAUSS_THREADS) {
     const long long t = b + tid;
-    const bool z = t < nH && H[(long long)(koff + t / n_genes) * ldh + t % n_genes] == 0.f;
+    const bool z = t < nH && H[(long long)(koff + t / n_genes) * ldh + t % n_genes] == T(0);
     int tot;
     const int slot = block_rank(z, warp_tot, &tot);
     if (z) posH[zH + slot] = t;
@@ -426,7 +429,7 @@ ar_fill_kernel(Meta m, float* __restrict__ Wt, int ldw, int n_cells, float* __re
   }
   __syncthreads();
   legacy_gauss_block(m.seed[r], zW + zH, sh, [&](long long t, double z) {
-    const float v = (float)fabs(__ddiv_rn(__dmul_rn(avg, z), 100.0));
+    const T v = (T)fabs(__ddiv_rn(__dmul_rn(avg, z), 100.0));
     if (t < zW) {
       const long long p = posW[t];
       Wt[(long long)(koff + p % k) * ldw + p / k] = v;
@@ -442,12 +445,11 @@ struct DevBuf {          // cudaMalloc'd for one call: the solve that follows ge
   ~DevBuf() { if (p) cudaFree(p); }
 };
 
-}  // namespace
-
-int nndsvd_starts_dev(cnmf_dataset_s* d, int R, const int* ks, const uint32_t* seeds, int init, float* Wt, float* H,
-                      cudaStream_t s) {
-  CNMF_TRY(require_dense(d, "nndsvd_init_dev"));
-  CNMF_REQUIRE(R > 0 && ks && seeds && Wt && H, "nndsvd_init_dev: bad arguments");
+// TX: element type of the dataset's X (float, or double on float64 datasets); T: element type of the starts
+template <typename TX, typename T>
+int nndsvd_starts(cnmf_dataset_s* d, const TX* X, int R, const int* ks, const uint32_t* seeds, int init, T* Wt, T* H,
+                  cudaStream_t s) {
+  CNMF_REQUIRE(R > 0 && ks && seeds && Wt && H && X, "nndsvd_init_dev: bad arguments");
   CNMF_REQUIRE(init == CNMF_INIT_NNDSVD || init == CNMF_INIT_NNDSVDA || init == CNMF_INIT_NNDSVDAR,
                "nndsvd_init_dev: init must be CNMF_INIT_NNDSVD, _NNDSVDA or _NNDSVDAR");
   cnmf_handle_s* h = d->h;
@@ -465,8 +467,8 @@ int nndsvd_starts_dev(cnmf_dataset_s* d, int R, const int* ks, const uint32_t* s
     koff[r] = SK;
     SK += ks[r];
   }
-  CNMF_CUDA_CHECK(cudaMemsetAsync(Wt, 0, (size_t)SK * ld_r * 4, s));
-  CNMF_CUDA_CHECK(cudaMemsetAsync(H, 0, (size_t)SK * ld_c * 4, s));
+  CNMF_CUDA_CHECK(cudaMemsetAsync(Wt, 0, (size_t)SK * ld_r * sizeof(T), s));
+  CNMF_CUDA_CHECK(cudaMemsetAsync(H, 0, (size_t)SK * ld_c * sizeof(T), s));
   const double avg = d->sum / ((double)N * (double)G);
 
   // ---- chunk capacity from the free device memory: rows of Qc + Qg and the per-restart small matrices
@@ -544,7 +546,7 @@ int nndsvd_starts_dev(cnmf_dataset_s* d, int R, const int* ks, const uint32_t* s
         double* C = to_genes ? Qg : Qc;
         h->launches += 1;
         const int slot = h->prof_begin(s, 2.0 * rows * (double)N * G, 3);
-        CNMF_TRY(launch_gemm_f64(A, to_genes ? ld_r : ld_c, rows, d->X, N, G, ld_c, to_genes, C, to_genes ? ld_c : ld_r, s));
+        CNMF_TRY(launch_gemm_f64(A, to_genes ? ld_r : ld_c, rows, X, N, G, ld_c, to_genes, C, to_genes ? ld_c : ld_r, s));
         h->prof_end(s, slot);
         return 0;
       };
@@ -581,11 +583,11 @@ int nndsvd_starts_dev(cnmf_dataset_s* d, int R, const int* ks, const uint32_t* s
       apply_kernel<true><<<dim3((n_a + TILE - 1) / TILE, Rc), TILE, 0, s>>>(m, Qa, ld_a, n_a, Vs);
       stats_kernel<<<Kc, 256, 0, s>>>(m, Qc, ld_r, N, Qg, ld_c, G, stats);
       const double fill = init == CNMF_INIT_NNDSVDA ? avg : 0.0;
-      compose_kernel<<<dim3((N + 255) / 256, Kc), 256, 0, s>>>(m, Qc, ld_r, N, true, stats, Sv, Wt, ld_r, fill);
-      compose_kernel<<<dim3((G + 255) / 256, Kc), 256, 0, s>>>(m, Qg, ld_c, G, false, stats, Sv, H, ld_c, fill);
+      compose_kernel<T><<<dim3((N + 255) / 256, Kc), 256, 0, s>>>(m, Qc, ld_r, N, true, stats, Sv, Wt, ld_r, fill);
+      compose_kernel<T><<<dim3((G + 255) / 256, Kc), 256, 0, s>>>(m, Qg, ld_c, G, false, stats, Sv, H, ld_c, fill);
       h->launches += 6;
       if (init == CNMF_INIT_NNDSVDAR) {
-        ar_fill_kernel<<<Rc, LEGACY_GAUSS_THREADS, 0, s>>>(m, Wt, ld_r, N, H, ld_c, G, Qc, ld_r, Qg, ld_c, avg);
+        ar_fill_kernel<T><<<Rc, LEGACY_GAUSS_THREADS, 0, s>>>(m, Wt, ld_r, N, H, ld_c, G, Qc, ld_r, Qg, ld_c, avg);
         h->launches += 1;
       }
       CNMF_CUDA_CHECK(cudaGetLastError());
@@ -594,6 +596,20 @@ int nndsvd_starts_dev(cnmf_dataset_s* d, int R, const int* ks, const uint32_t* s
     }
   }
   return 0;
+}
+
+}  // namespace
+
+int nndsvd_starts_dev(cnmf_dataset_s* d, int R, const int* ks, const uint32_t* seeds, int init, float* Wt, float* H,
+                      cudaStream_t s) {
+  CNMF_TRY(require_dense(d, "nndsvd_init_dev"));
+  return nndsvd_starts(d, d->X, R, ks, seeds, init, Wt, H, s);
+}
+
+int nndsvd_starts_dev(cnmf_dataset_s* d, int R, const int* ks, const uint32_t* seeds, int init, double* Wt, double* H,
+                      cudaStream_t s) {
+  CNMF_TRY(require_f64(d, "nndsvd_init_dev"));
+  return nndsvd_starts(d, d->X64, R, ks, seeds, init, Wt, H, s);
 }
 
 }  // namespace cnmf

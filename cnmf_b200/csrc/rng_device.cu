@@ -18,10 +18,12 @@ namespace cnmf {
 
 namespace {
 
+// T = float: |avg*z| rounded to fp32 (the float datasets); T = double: kept in fp64 (float64 datasets)
+template <typename T>
 __global__ void __launch_bounds__(LEGACY_GAUSS_THREADS)
 rng_init_kernel(const uint32_t* __restrict__ seeds, const int* __restrict__ ks, const int* __restrict__ offs,
-                const double* __restrict__ avgs, int n_samples, int n_features, float* __restrict__ Wt, long long ldW,
-                float* __restrict__ H, long long ldH) {
+                const double* __restrict__ avgs, int n_samples, int n_features, T* __restrict__ Wt, long long ldW,
+                T* __restrict__ H, long long ldH) {
   __shared__ LegacyGaussShared sh;
   const int r = blockIdx.x;
   const int k = ks[r];
@@ -30,7 +32,7 @@ rng_init_kernel(const uint32_t* __restrict__ seeds, const int* __restrict__ ks, 
   const long long nH = (long long)k * n_features;
   const long long total = nH + (long long)n_samples * k;
   legacy_gauss_block(seeds[r], total, sh, [&](long long t, double z) {
-    const float v = (float)fabs(__dmul_rn(avg, z));
+    const T v = (T)fabs(__dmul_rn(avg, z));
     if (t < nH) {
       const long long c = t / n_features, g = t % n_features;
       H[(row0 + c) * ldH + g] = v;
@@ -42,12 +44,10 @@ rng_init_kernel(const uint32_t* __restrict__ seeds, const int* __restrict__ ks, 
   });
 }
 
-}  // namespace
-
 // Fills the packed initial factors on the device.  d_meta: device scratch of >= 4 * R ints + R doubles (8-byte aligned).
-int launch_rng_init(const uint32_t* seeds_host, const int* ks_host, const int* offs_host, const double* avgs_host, int R,
-                    int n_samples, int n_features, float* Wt, long long ldW, float* H, long long ldH, cnmf_handle_s* h,
-                    cudaStream_t s) {
+template <typename T>
+int rng_init(const uint32_t* seeds_host, const int* ks_host, const int* offs_host, const double* avgs_host, int R,
+             int n_samples, int n_features, T* Wt, long long ldW, T* H, long long ldH, cnmf_handle_s* h, cudaStream_t s) {
   const size_t bytes = sizeof(double) * R + sizeof(int) * 3 * (size_t)R;
   unsigned char* d = static_cast<unsigned char*>(h->dev_buf("rng.meta", bytes));
   unsigned char* hp = static_cast<unsigned char*>(h->host_buf("rng.meta", bytes));
@@ -67,10 +67,24 @@ int launch_rng_init(const uint32_t* seeds_host, const int* ks_host, const int* o
   const uint32_t* d_seed = reinterpret_cast<const uint32_t*>(d + sizeof(double) * R);
   const int* d_k = reinterpret_cast<const int*>(d + sizeof(double) * R + sizeof(int) * (size_t)R);
   const int* d_off = d_k + R;
-  rng_init_kernel<<<R, LEGACY_GAUSS_THREADS, 0, s>>>(d_seed, d_k, d_off, d_avg, n_samples, n_features, Wt, ldW, H, ldH);
+  rng_init_kernel<T><<<R, LEGACY_GAUSS_THREADS, 0, s>>>(d_seed, d_k, d_off, d_avg, n_samples, n_features, Wt, ldW, H, ldH);
   CNMF_CUDA_CHECK(cudaGetLastError());
   h->launches += 1;
   return 0;
+}
+
+}  // namespace
+
+int launch_rng_init(const uint32_t* seeds_host, const int* ks_host, const int* offs_host, const double* avgs_host, int R,
+                    int n_samples, int n_features, float* Wt, long long ldW, float* H, long long ldH, cnmf_handle_s* h,
+                    cudaStream_t s) {
+  return rng_init(seeds_host, ks_host, offs_host, avgs_host, R, n_samples, n_features, Wt, ldW, H, ldH, h, s);
+}
+
+int launch_rng_init(const uint32_t* seeds_host, const int* ks_host, const int* offs_host, const double* avgs_host, int R,
+                    int n_samples, int n_features, double* Wt, long long ldW, double* H, long long ldH, cnmf_handle_s* h,
+                    cudaStream_t s) {
+  return rng_init(seeds_host, ks_host, offs_host, avgs_host, R, n_samples, n_features, Wt, ldW, H, ldH, h, s);
 }
 
 }  // namespace cnmf

@@ -281,6 +281,11 @@ int require_dense(const cnmf_dataset_s* d, const char* what) {
                    "step only (col_stats, project_rows, from_columns, transposed Frobenius refit)");
     return -3;
   }
+  if (d && d->precision == CNMF_PRECISION_FP64) {
+    set_last_error(std::string(what) + " is not available on float64 datasets: they support shape, ld, sums, "
+                   "col_stats, solve_bytes_per_row and the _f64 entry points");
+    return -3;
+  }
   return 0;
 }
 

@@ -9,7 +9,8 @@ import numpy as np
 
 from . import _lib
 from ._lib import (LOSS_FROBENIUS, LOSS_ITAKURA_SAITO, LOSS_KULLBACK_LEIBLER, NmfParams, PRECISION_FP32,
-                   PRECISION_F16X2, PRECISION_TF32X3, PRECISION_TF32X3_GENERAL, SOLVER_CD, SOLVER_MU, check, f32c, ptr)
+                   PRECISION_F16X2, PRECISION_FP64, PRECISION_TF32X3, PRECISION_TF32X3_GENERAL, SOLVER_CD, SOLVER_MU,
+                   check, f32c, f64c, ptr)
 
 # default: split-operand tensor-core products with fp32-class accuracy -- 2 f16 passes when X is recognised as
 # scaled integer counts (what the reference factorizes), 3 tf32 passes otherwise
@@ -18,11 +19,29 @@ _DEFAULT_PRECISION = PRECISION_F16X2
 
 def precision_code(p):
     """'fp32' | 'tf32x3' (default; 2-pass products when X is scaled integer counts) | 'f16x2' (like tf32x3, but the
-    2-pass products of scaled-integer-count matrices run on f16 MMAs) | 'tf32x3-general' (always 3-pass)."""
-    if p in (PRECISION_FP32, PRECISION_TF32X3, PRECISION_TF32X3_GENERAL, PRECISION_F16X2):
+    2-pass products of scaled-integer-count matrices run on f16 MMAs) | 'tf32x3-general' (always 3-pass) | 'fp64'
+    (X, factors and products in float64 on the fp64 tensor cores: the reference's own float64 numbers)."""
+    if p in (PRECISION_FP32, PRECISION_TF32X3, PRECISION_TF32X3_GENERAL, PRECISION_F16X2, PRECISION_FP64):
         return p
     return {"fp32": PRECISION_FP32, "tf32x3": PRECISION_TF32X3, "tf32x3-general": PRECISION_TF32X3_GENERAL,
-            "f16x2": PRECISION_F16X2}[p]
+            "f16x2": PRECISION_F16X2, "fp64": PRECISION_FP64}[p]
+
+
+def is_fp64(precision):
+    return precision is not None and precision_code(precision) == PRECISION_FP64
+
+
+def check_fp64_supported(precision, beta_loss="frobenius", rng="device"):
+    """What precision='fp64' does not cover is refused where the user states it: beta_loss other than frobenius, and the
+    host random generator (fp64 starts come from the device generator or the NNDSVD family)."""
+    if not is_fp64(precision):
+        return
+    if loss_code(beta_loss) != LOSS_FROBENIUS:
+        raise NotImplementedError("cnmf_b200: precision='fp64' supports beta_loss='frobenius' only (got %r)"
+                                  % (beta_loss,))
+    if rng == "host":
+        raise NotImplementedError("cnmf_b200: precision='fp64' draws its random starts on the device; rng='host' "
+                                  "serves the float precisions only")
 
 
 def _params_precision(p):
@@ -58,8 +77,8 @@ def init_code(init, ks, n_samples, n_features):
     return _lib.INIT_CODES[which.pop()]
 
 
-def nndsvd_starts(X, ks, seeds, init):
-    """Packed starting factors (W^T rows: sum ks x cells, H rows: sum ks x genes; fp32) of every restart (k, seed) for
+def nndsvd_starts(X, ks, seeds, init, dtype=np.float32):
+    """Packed starting factors (W^T rows: sum ks x cells, H rows: sum ks x genes; dtype) of every restart (k, seed) for
     init in {'nndsvd', 'nndsvda', 'nndsvdar', None}: scikit-learn's `_initialize_nmf` as the reference's call reaches it
     (cnmf.py:672), restated in cnmf_b200/nndsvd.py.  One randomized SVD per restart on the host (threads: LAPACK / BLAS
     release the GIL).  Dataset.nndsvd_init_dev computes the same starts on the GPU."""
@@ -69,8 +88,8 @@ def nndsvd_starts(X, ks, seeds, init):
     ks = [int(k) for k in ks]
     n, g = X.shape
     offs = np.concatenate([[0], np.cumsum(ks)]).astype(np.int64)
-    W0 = np.empty((int(offs[-1]), n), np.float32)
-    H0 = np.empty((int(offs[-1]), g), np.float32)
+    W0 = np.empty((int(offs[-1]), n), dtype)
+    H0 = np.empty((int(offs[-1]), g), dtype)
 
     def one(r):
         which = resolve_init(init, ks[r], n, g)
@@ -114,6 +133,7 @@ def make_params(nmf_kwargs, n_samples, n_features, precision, for_refit=False):
     rng = nmf_kwargs.get("rng", "device")
     if rng not in ("device", "host"):
         raise ValueError("rng must be 'device' or 'host'")
+    check_fp64_supported(precision, beta, rng)
     p.reserved = 1 if rng == "host" else 0          # bit 0: draw the random init on the host
     p.max_iter = int(nmf_kwargs.get("max_iter", 1000))
     p.tol = float(nmf_kwargs.get("tol", 1e-4))
@@ -168,7 +188,8 @@ class Engine:
     def profile_get(self, kernel_class=0):
         """(total device ms, launches, algorithmic work) of a kernel class since profile(True):
         0 = batched GEMM (work in FLOPs), 1 = fused update kernels (work in bytes), 2 = sparse-dataset products
-        (work in bytes), 3 = fp64 GEMM of the NNDSVD starts (work in FLOPs)."""
+        (work in bytes), 3 = fp64 GEMM of the NNDSVD starts (work in FLOPs), 4 = fp64 GEMM of the float64 solver
+        (work in FLOPs)."""
         ms, n, fl = ctypes.c_double(), ctypes.c_longlong(), ctypes.c_double()
         check(self.lib.cnmf_profile_get_class(self._h, int(kernel_class), ctypes.byref(ms), ctypes.byref(n),
                                               ctypes.byref(fl)))
@@ -197,7 +218,11 @@ class Engine:
         """X (any scipy sparse matrix or an ndarray) resident on the GPU as canonical float32 CSC, 8 bytes per stored
         entry; no dense copy is made on the host or the device.  Serves the consensus step's TPM uses: sums, col_stats,
         project_rows, from_columns (returns a dense dataset) and refit(transposed=True) with the Frobenius loss; and
-        prepare's uses of raw counts: tpm_stats, col_stats, from_columns.  Everything else raises CnmfError."""
+        prepare's uses of raw counts: tpm_stats, col_stats, from_columns.  Everything else raises CnmfError.
+        precision='fp64' has no sparse form."""
+        if is_fp64(precision):
+            raise NotImplementedError("cnmf_b200: precision='fp64' needs a dense dataset; sparse (CSC) datasets hold "
+                                      "float32 values")
         import scipy.sparse as sp
         C = sp.csc_matrix(X, dtype=np.float32)
         if not C.has_canonical_format:          # sorted row indices, no duplicates: the library does not sort
@@ -325,12 +350,14 @@ class Engine:
 
 
 class Dataset:
-    """A cells x genes matrix resident on the GPU (norm_counts.X / tpm.X of the reference)."""
+    """A cells x genes matrix resident on the GPU (norm_counts.X / tpm.X of the reference).  precision='fp64' keeps X
+    in float64 and runs everything in float64: factorize / refit / project_rows then take and return float64 arrays."""
 
     def __init__(self, engine, X, precision=_DEFAULT_PRECISION, stream=None, _handle=None, sparse=False):
         self.engine = engine
         self.lib = engine.lib
         self.precision = precision_code(precision)
+        self.fp64 = self.precision == PRECISION_FP64
         self.sparse = sparse        # CSC-resident (Engine.sparse_dataset)
         self._d = ctypes.c_void_p()
         if _handle is not None:
@@ -338,10 +365,15 @@ class Dataset:
         else:
             if hasattr(X, "toarray"):       # scipy sparse: the CUDA path is dense (DESIGN.md)
                 X = X.toarray()
-            X = f32c(X)
-            n, g = X.shape
-            check(self.lib.cnmf_dataset_create(engine._h, ptr(X), n, g, g, 0, self.precision, stream,
-                                               ctypes.byref(self._d)))
+            if self.fp64:
+                X = f64c(X)
+                n, g = X.shape
+                check(self.lib.cnmf_dataset_create_f64(engine._h, ptr(X), n, g, g, 0, stream, ctypes.byref(self._d)))
+            else:
+                X = f32c(X)
+                n, g = X.shape
+                check(self.lib.cnmf_dataset_create(engine._h, ptr(X), n, g, g, 0, self.precision, stream,
+                                                   ctypes.byref(self._d)))
         n, g = ctypes.c_int(), ctypes.c_int()
         check(self.lib.cnmf_dataset_shape(self._d, ctypes.byref(n), ctypes.byref(g)))
         self.shape = (n.value, g.value)
@@ -503,6 +535,16 @@ class Dataset:
         check(self.lib.cnmf_dataset_from_columns(self._d, ptr(cols), ptr(scale), len(cols), None, ctypes.byref(out)))
         return Dataset(self.engine, None, self.precision, _handle=out)
 
+    def from_columns_div(self, cols, divisor):
+        """float64 datasets: new float64 dataset X[:, cols] / divisor, each entry one IEEE division (bit for bit what
+        numpy gives for X[:, cols] / divisor on the host)."""
+        cols = np.ascontiguousarray(cols, dtype=np.int32)
+        div = f64c(divisor)
+        assert div.shape == cols.shape
+        out = ctypes.c_void_p()
+        check(self.lib.cnmf_dataset_from_columns_f64(self._d, ptr(cols), ptr(div), len(cols), None, ctypes.byref(out)))
+        return Dataset(self.engine, None, self.precision, _handle=out)
+
     def params(self, nmf_kwargs):
         return make_params(nmf_kwargs, self.shape[0], self.shape[1], self.precision)
 
@@ -517,16 +559,28 @@ class Dataset:
         n, g = self.shape
         p = self.params(nmf_kwargs)
         self._check_loss(p)
-        spectra = np.empty((SK, g), np.float32)
-        usages = np.empty((SK, n), np.float32) if return_usages else None
+        dt = np.float64 if self.fp64 else np.float32
+        spectra = np.empty((SK, g), dt)
+        usages = np.empty((SK, n), dt) if return_usages else None
         n_iter = np.zeros(R, np.int32)
         err = np.zeros(R, np.float64)
         init = nmf_kwargs.get("init", "random")
         if W0 is None and init != "random" and X_host is not None:
             # NNDSVD family (cnmf.py:1252 / SK _nmf.py:309-369) on the host: starting factors from cnmf_b200.nndsvd, one
             # randomized SVD per restart (the seed enters through its test matrix), then the ordinary batched solve
-            W0, H0 = nndsvd_starts(X_host, ks, seeds, init)
-        if W0 is None:
+            W0, H0 = nndsvd_starts(X_host, ks, seeds, init, dtype=dt)
+        if self.fp64:
+            if W0 is None:
+                p.reserved |= init_code(init, ks, n, g) << 1
+                seeds = np.ascontiguousarray(seeds, dtype=np.uint32)
+                check(self.lib.cnmf_factorize_f64(self._d, R, ptr(ks), ptr(seeds), ctypes.byref(p), ptr(spectra),
+                                                  ptr(usages), ptr(n_iter), ptr(err), None))
+            else:
+                W0, H0 = f64c(W0), f64c(H0)
+                assert W0.shape == (SK, n) and H0.shape == (SK, g)
+                check(self.lib.cnmf_factorize_init_f64(self._d, R, ptr(ks), ptr(W0), ptr(H0), ctypes.byref(p),
+                                                       ptr(spectra), ptr(usages), ptr(n_iter), ptr(err), None))
+        elif W0 is None:
             p.reserved |= init_code(init, ks, n, g) << 1
             seeds = np.ascontiguousarray(seeds, dtype=np.uint32)
             check(self.lib.cnmf_factorize(self._d, R, ptr(ks), ptr(seeds), ctypes.byref(p), ptr(spectra), ptr(usages),
@@ -544,25 +598,27 @@ class Dataset:
     def refit(self, fixed, nmf_kwargs, transposed=False):
         """NMF with `fixed` held constant (update_H=False).  transposed=False: fixed = H (k x genes),
         returns W (cells x k).  transposed=True: fixed = W^T (k x cells), returns H^T (genes x k)."""
-        fixed = f32c(fixed)
+        fixed = f64c(fixed) if self.fp64 else f32c(fixed)
         k = fixed.shape[0]
         n, g = self.shape
         n_r, n_c = (g, n) if transposed else (n, g)
         assert fixed.shape[1] == n_c
         p = make_params(nmf_kwargs, n_r, n_c, self.precision, for_refit=True)
         self._check_loss(p)
-        out = np.empty((n_r, k), np.float32)
+        out = np.empty((n_r, k), fixed.dtype)
         it = ctypes.c_int32(0)
         err = ctypes.c_double(0)
-        check(self.lib.cnmf_refit(self._d, 1 if transposed else 0, k, ptr(fixed), ctypes.byref(p), ptr(out),
-                                  ctypes.byref(it), ctypes.byref(err), None))
+        fn = self.lib.cnmf_refit_f64 if self.fp64 else self.lib.cnmf_refit
+        check(fn(self._d, 1 if transposed else 0, k, ptr(fixed), ctypes.byref(p), ptr(out), ctypes.byref(it),
+                 ctypes.byref(err), None))
         return out, int(it.value), float(err.value)
 
     def project_rows(self, Ut):
         """Ut (k x cells) @ X -> (k x genes)."""
-        Ut = f32c(Ut)
+        Ut = f64c(Ut) if self.fp64 else f32c(Ut)
         k = Ut.shape[0]
         assert Ut.shape[1] == self.shape[0]
-        out = np.empty((k, self.shape[1]), np.float32)
-        check(self.lib.cnmf_project_rows(self._d, k, ptr(Ut), ptr(out), None))
+        out = np.empty((k, self.shape[1]), Ut.dtype)
+        fn = self.lib.cnmf_project_rows_f64 if self.fp64 else self.lib.cnmf_project_rows
+        check(fn(self._d, k, ptr(Ut), ptr(out), None))
         return out

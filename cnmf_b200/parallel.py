@@ -193,7 +193,11 @@ def factorize_sharded(ds, ks_all, seeds_all, nmf_kwargs, comm=None, X_host=None)
     """The multi-GPU factorize: this rank's jobs (idx % world == rank, cnmf.py:52-53) in one batched solve whose
     spectra stay in HBM, then ONE NCCL all-gather of the per-rank slabs (cnmf_allgather_spectra).  No host staging:
     random and NNDSVD starts are computed on the device (X_host: take the NNDSVD starts from the host instead).
-    Returns (ShardedSpectra, n_iter of the local jobs, local job indices)."""
+    Returns (ShardedSpectra, n_iter of the local jobs, local job indices).  Float64 datasets (precision='fp64') are
+    refused: the slabs and the all-gather are float32."""
+    if getattr(ds, "fp64", False):
+        raise NotImplementedError("cnmf_b200: the sharded multi-GPU factorize gathers float32 spectra; precision='fp64' "
+                                  "runs on one GPU per process (cNMF.factorize)")
     import torch
     rank, world, _ = dist_info()
     _, max_rows, _, per_rank = _slab_layout(ks_all, world)

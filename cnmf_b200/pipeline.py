@@ -73,10 +73,13 @@ def tpm_dataset(eng, X, precision, beta_loss="frobenius"):
     """The resident TPM matrix for consensus (refit_spectra, the OLS z-scores and the HVG refit, cnmf.py:950-969):
     dense as everywhere else when it fits, else CSC (Engine.sparse_dataset).  A sparse TPM supports the Frobenius
     refits only: a KL / IS run that would need it raises NotImplementedError before anything is built."""
-    from .engine import LOSS_FROBENIUS, loss_code
+    from .engine import LOSS_FROBENIUS, is_fp64, loss_code
     n, g = X.shape
     if fits_dense(eng, X.shape, precision):
         return eng.dataset(X, precision=precision)
+    if is_fp64(precision):
+        raise NotImplementedError("cnmf_b200: the %d x %d TPM matrix does not fit on the device in dense float64 form, "
+                                  "and precision='fp64' has no sparse datasets" % (n, g))
     if loss_code(beta_loss) != LOSS_FROBENIUS:
         raise NotImplementedError("cnmf_b200: the %d x %d TPM matrix does not fit on the device in dense form, and the "
                                   "sparse KL / IS refit is not implemented (beta_loss=%r)" % (n, g, beta_loss))
@@ -134,6 +137,9 @@ class cNMF:
     """Same constructor, attributes and methods as the reference class (cnmf.py:265)."""
 
     def __init__(self, output_dir=".", name=None, precision="f16x2", device=None):
+        """precision (cnmf_b200 extension): 'f16x2' (default), 'tf32x3', 'tf32x3-general', 'fp32', or 'fp64' -- X,
+        factorize and every refit in float64 as the reference computes (beta_loss='frobenius'; the consensus kernels
+        that compare spectra stay float32)."""
         self.output_dir = output_dir
         if name is None:
             name = "%s_%s" % (datetime.datetime.now().strftime("%Y_%m_%d"), uuid.uuid4().hex[:6])
@@ -177,8 +183,12 @@ class cNMF:
         exact integer counts); the normalised matrix stays in HBM for factorize().  Raises without a GPU.  Counts
         stored sparse (and densify=False) whose dense dataset would not fit (TPM_DENSE_FRACTION) stay CSC on the device
         and CSR on the host, so an atlas needs no cells x all-genes dense matrix anywhere."""
-        from .engine import check_supported
+        from .engine import check_fp64_supported, check_supported, is_fp64
         check_supported(components, init, beta_loss)                  # fail here, not hours later in factorize
+        check_fp64_supported(self.precision, beta_loss)
+        if on_device and is_fp64(self.precision):
+            raise NotImplementedError("cnmf_b200: prepare(on_device=True) runs on float counts datasets; "
+                                      "precision='fp64' prepares on the host (on_device=False)")
         counts = cio.read_counts(counts_fn)
         # the reference keeps X sparse (CSR) unless --densify: text / npz inputs are converted to CSR, .h5ad keeps
         # what the file holds (cnmf.py:383-405).  The CUDA path is dense, but the two branches differ in one rule
@@ -622,8 +632,8 @@ class cNMF:
         return usage, scores, tpm, top_genes
 
 
-def main():
-    """`cnmf {prepare,factorize,combine,consensus,k_selection_plot}` with the reference's flags (cnmf.py:1213-1294)."""
+def build_parser():
+    """The command line of main(): the reference's flags (cnmf.py:1213-1294) and the cnmf_b200 extensions."""
     import argparse
     ap = argparse.ArgumentParser()
     ap.add_argument("command", type=str, choices=["prepare", "factorize", "combine", "consensus", "k_selection_plot"])
@@ -651,10 +661,16 @@ def main():
     ap.add_argument("--build-reference", dest="build_reference", action="store_true", default=True)
     ap.add_argument("--prepare-on-device", dest="prepare_on_device", action="store_true", default=False,
                     help="[cnmf_b200] prepare: cell totals, TPM gene statistics and the HVG matrix computed on the GPU")
-    ap.add_argument("--precision", type=str, choices=["f16x2", "tf32x3", "fp32"], default="f16x2",
+    ap.add_argument("--precision", type=str, choices=["f16x2", "tf32x3", "fp32", "fp64"], default="f16x2",
                     help="[cnmf_b200] big products: split-fp16 wgmma MMAs for scaled-integer-count matrices, split-TF32 "
-                         "otherwise (default); split-TF32 always; or FFMA fp32")
-    a = ap.parse_args()
+                         "otherwise (default); split-TF32 always; FFMA fp32; or everything in float64 on the fp64 "
+                         "tensor cores (frobenius loss)")
+    return ap
+
+
+def main(argv=None):
+    """`cnmf {prepare,factorize,combine,consensus,k_selection_plot}` with the reference's flags (cnmf.py:1213-1294)."""
+    a = build_parser().parse_args(argv)
     obj = cNMF(output_dir=a.output_dir, name=a.name, precision=a.precision)
     if a.command == "prepare":
         obj.prepare(a.counts, components=a.components, n_iter=a.n_iter, densify=a.densify, tpm_fn=a.tpm, seed=a.seed,

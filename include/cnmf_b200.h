@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define CNMF_B200_ABI_VERSION 12
+#define CNMF_B200_ABI_VERSION 13
 #define CNMF_MAX_COMPONENTS 32          /* largest n_components per restart on the CUDA path */
 
 typedef struct cnmf_handle_s* cnmf_handle_t;
@@ -41,7 +41,11 @@ enum { CNMF_PRECISION_FP32 = 0, CNMF_PRECISION_TF32X3 = 1, CNMF_PRECISION_TF32X3
        /* dataset_create only: like TF32X3, but when X is recognised as scaled integer counts the big products run as
         * 2 f16 tensor-core passes (integer operand exact in fp16, factor = two fp16 pieces of its row-normalised
         * values: the same 22 significant bits as the tf32 pair at twice the MMA rate); params.precision stays TF32X3 */
-       CNMF_PRECISION_F16X2 = 3 };
+       CNMF_PRECISION_F16X2 = 3,
+       /* float64 datasets (cnmf_dataset_create_f64 / cnmf_dataset_from_columns_f64) and their params: X, factors,
+        * products and every sum in fp64 (fp64 tensor-core GEMM), Frobenius loss with MU or CD, as scikit-learn computes
+        * on a float64 X.  Reached through the _f64 entry points only. */
+       CNMF_PRECISION_FP64 = 4 };
 
 /* yaml 'beta_loss' (cnmf.py:622, CLI --beta-loss cnmf.py:1251).  'frobenius' (or 2) runs the tensor-core path with
  * either solver; 'kullback-leibler' (1) and 'itakura-saito' (0) run the multiplicative updates of sklearn
@@ -88,7 +92,8 @@ int cnmf_profile_get(cnmf_handle_t h, double* gemm_ms, long long* gemm_launches,
 /* same counters per kernel class: 0 = batched GEMM (work = algorithmic FLOPs), 1 = fused update kernels
  * (work = algorithmic bytes: factor read + product slices read + factor and tf32 pieces written), 2 = the product
  * of a sparse dataset, both of its kernels (work = algorithmic bytes: 8 per entry, col_ptr, staged U, output),
- * 3 = the fp64 GEMM of cnmf_nndsvd_init_dev (work = algorithmic FLOPs, 2*M*N*K per launch) */
+ * 3 = the fp64 GEMM of cnmf_nndsvd_init_dev (work = algorithmic FLOPs, 2*M*N*K per launch), 4 = the fp64 GEMM of
+ * the float64 solver (work = algorithmic FLOPs, 2*M*N*K per launch) */
 int cnmf_profile_get_class(cnmf_handle_t h, int kernel_class, double* ms, long long* launches, double* work);
 
 /* host wall-clock phases (ms) of the last cnmf_factorize, cnmf_factorize_seeds_dev, cnmf_factorize_init or
@@ -182,6 +187,30 @@ int cnmf_nndsvd_chunk_limit(cnmf_handle_t h, int max_restarts);
 /* test hook: the fp64 GEMM of cnmf_nndsvd_init_dev.  to_genes = 0: C_host (M x n_rows) = A_host (M x n_cols) X^T;
  * 1: C_host (M x n_cols) = A_host (M x n_rows) X.  Host arrays dense row-major fp64. */
 int cnmf_nndsvd_gemm_host(cnmf_dataset_t d, int to_genes, int M, const double* A_host, double* C_host, void* stream);
+
+/* ---- float64 datasets (CNMF_PRECISION_FP64) -------------------------------------------------------------------- */
+/* X (n_rows x n_cols, row stride ld, fp64) resident as one fp64 row-major copy, 8 bytes per entry, no transposed copy
+ * and no operand pieces.  Entry points that take or return floats refuse such a dataset (-3) and name their _f64
+ * form; the _f64 entry points refuse any other dataset.  Also supported on it: destroy, shape, ld, sums, col_stats,
+ * solve_bytes_per_row.  Supported: beta_loss = frobenius, MU and CD, random (device generator) and NNDSVD starts. */
+int cnmf_dataset_create_f64(cnmf_handle_t h, const double* X, int n_rows, int n_cols, long long ld, int src_is_device,
+                            void* stream, cnmf_dataset_t* out);
+/* new float64 dataset = src[:, cols] / divisor (cnmf.py:542, 967-969: X /= std), each entry one IEEE fp64 division */
+int cnmf_dataset_from_columns_f64(cnmf_dataset_t src, const int32_t* cols_host, const double* divisor_host, int n_cols,
+                                  void* stream, cnmf_dataset_t* out);
+/* cnmf_factorize, cnmf_factorize_init, cnmf_refit and cnmf_project_rows of a float64 dataset: the same arguments with
+ * fp64 factors and outputs; params.precision = CNMF_PRECISION_FP64.  The starting factors of cnmf_factorize_f64 are
+ * scikit-learn's random init drawn on the device (params.reserved bit 0 must be 0) or its NNDSVD starts (bits 1-2),
+ * both kept in fp64. */
+int cnmf_factorize_f64(cnmf_dataset_t d, int n_restarts, const int32_t* ks, const uint32_t* seeds,
+                       const cnmf_nmf_params* params, double* spectra_host, double* usages_host, int32_t* n_iter_host,
+                       double* err_host, void* stream);
+int cnmf_factorize_init_f64(cnmf_dataset_t d, int n_restarts, const int32_t* ks, const double* Wt0_host,
+                            const double* H0_host, const cnmf_nmf_params* params, double* spectra_host,
+                            double* usages_host, int32_t* n_iter_host, double* err_host, void* stream);
+int cnmf_refit_f64(cnmf_dataset_t d, int transposed, int k, const double* fixed_host, const cnmf_nmf_params* params,
+                   double* out_host, int32_t* n_iter_host, double* err_host, void* stream);
+int cnmf_project_rows_f64(cnmf_dataset_t d, int k, const double* Ut_host, double* out_host, void* stream);
 
 /* ---- batched factorize: replaces the restart loop of cNMF.factorize ---------------- */
 /* For r in [0, n_restarts): one NMF of the dataset with n_components = ks[r] and
