@@ -130,12 +130,22 @@ SIGNATURES = {
     "cnmf_kmeans_assign": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "cnmf_cluster_dist_sums": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _vp, _vp]),
     "cnmf_cluster_median": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _vp, _i, _vp]),
+    "cnmf_l2_normalize_rows_f64": (_i, [_vp, _vp, _i, _i, _i, _vp]),
+    "cnmf_local_density_f64": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "cnmf_col_stats_dev_f64": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
+    "cnmf_gather_rows_f64": (_i, [_vp, _vp, _i, _vp, _i, _i, _vp, _i, _vp]),
+    "cnmf_sq_dists_to_rows_f64": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _vp, _vp]),
+    "cnmf_kmeans_step_f64": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _pp(_c.c_int32), _pp(_c.c_int32), _pp(_d), _vp]),
+    "cnmf_kmeans_fit_f64": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _d, _vp, _vp, _i, _vp, _vp, _vp, _pp(_c.c_int32), _vp]),
+    "cnmf_kmeans_assign_f64": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "cnmf_cluster_dist_sums_f64": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _vp, _vp]),
+    "cnmf_cluster_median_f64": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _vp, _i, _vp]),
 }
 
 _lib = None
 
 
-ABI_VERSION = 13     # include/cnmf_b200.h CNMF_B200_ABI_VERSION
+ABI_VERSION = 14     # include/cnmf_b200.h CNMF_B200_ABI_VERSION
 
 
 def load():

@@ -51,29 +51,43 @@ def _torch():
 
 
 class SpectraMatrix:
-    """R x G fp32 matrix on the device (row stride ld = G padded to 32)."""
+    """R x G matrix on the device (row stride ld = G padded to 32), float32 or float64 (dtype).  A float64 matrix
+    (precision='fp64') runs every consensus kernel on its _f64 entry point: distances, densities, KMeans centres and
+    medians stay in float64."""
 
-    def __init__(self, engine, array=None, shape=None):
+    def __init__(self, engine, array=None, shape=None, dtype=np.float32):
         torch = _torch()
         self.engine = engine
         self.lib = engine.lib
+        self.dtype = np.dtype(dtype)
+        if self.dtype not in (np.float32, np.float64):
+            raise ValueError("SpectraMatrix: dtype must be float32 or float64, not %s" % self.dtype)
+        self.fp64 = self.dtype == np.float64
         if array is not None:
-            array = np.ascontiguousarray(array, dtype=np.float32)
+            array = np.ascontiguousarray(array, dtype=self.dtype)
             shape = array.shape
         self.R, self.G = int(shape[0]), int(shape[1])
         self.ld = (self.G + 31) // 32 * 32
-        self.t = torch.zeros((self.R, self.ld), dtype=torch.float32, device="cuda:%d" % engine.device)
+        self.t = torch.zeros((self.R, self.ld), dtype=self.torch_dtype, device="cuda:%d" % engine.device)
         if array is not None:
             self.t[:, :self.G].copy_(torch.from_numpy(array))     # H2D memcpy
 
+    @property
+    def torch_dtype(self):
+        return _torch().float64 if self.fp64 else _torch().float32
+
+    def fn(self, name):
+        """The library entry point `name` for this matrix's element type (name + '_f64' for a float64 matrix)."""
+        return getattr(self.lib, name + "_f64" if self.fp64 else name)
+
     @classmethod
-    def from_device_rows(cls, engine, src_ptr, ld_src, rows, n_cols):
-        """Rows `rows` of a device-resident slab (e.g. the all-gathered spectra of every restart) as a new matrix:
-        a device-side row gather, no trip through the host."""
+    def from_device_rows(cls, engine, src_ptr, ld_src, rows, n_cols, dtype=np.float32):
+        """Rows `rows` of a device-resident slab of `dtype` (e.g. the all-gathered spectra of every restart) as a new
+        matrix: a device-side row gather, no trip through the host."""
         rows = np.ascontiguousarray(rows, dtype=np.int32)
-        out = cls(engine, shape=(len(rows), n_cols))
-        check(engine.lib.cnmf_gather_rows(engine._h, ctypes.c_void_p(int(src_ptr)), int(ld_src), ptr(rows), len(rows),
-                                          int(n_cols), out.p, out.ld, None))
+        out = cls(engine, shape=(len(rows), n_cols), dtype=dtype)
+        check(out.fn("cnmf_gather_rows")(engine._h, ctypes.c_void_p(int(src_ptr)), int(ld_src), ptr(rows), len(rows),
+                                         int(n_cols), out.p, out.ld, None))
         return out
 
     @property
@@ -84,14 +98,14 @@ class SpectraMatrix:
         return self.t[:, :self.G].cpu().numpy()
 
     def l2_normalize(self):
-        check(self.lib.cnmf_l2_normalize_rows(self.engine._h, self.p, self.R, self.G, self.ld, None))
+        check(self.fn("cnmf_l2_normalize_rows")(self.engine._h, self.p, self.R, self.G, self.ld, None))
         return self
 
     def local_density(self, n_neighbors, return_dist=False):
         torch = _torch()
-        dens = torch.empty(self.R, dtype=torch.float32, device=self.t.device)
-        D = torch.empty((self.R, self.R), dtype=torch.float32, device=self.t.device) if return_dist else None
-        check(self.lib.cnmf_local_density(self.engine._h, self.p, self.R, self.G, self.ld, int(n_neighbors),
+        dens = torch.empty(self.R, dtype=self.torch_dtype, device=self.t.device)
+        D = torch.empty((self.R, self.R), dtype=self.torch_dtype, device=self.t.device) if return_dist else None
+        check(self.fn("cnmf_local_density")(self.engine._h, self.p, self.R, self.G, self.ld, int(n_neighbors),
                                           ctypes.c_void_p(dens.data_ptr()),
                                           ctypes.c_void_p(D.data_ptr()) if D is not None else None, None))
         torch.cuda.synchronize(self.t.device)
@@ -99,15 +113,15 @@ class SpectraMatrix:
 
     def take_rows(self, idx):
         idx = np.ascontiguousarray(idx, dtype=np.int32)
-        out = SpectraMatrix(self.engine, shape=(len(idx), self.G))
-        check(self.lib.cnmf_gather_rows(self.engine._h, self.p, self.ld, ptr(idx), len(idx), self.G, out.p, out.ld, None))
+        out = SpectraMatrix(self.engine, shape=(len(idx), self.G), dtype=self.dtype)
+        check(self.fn("cnmf_gather_rows")(self.engine._h, self.p, self.ld, ptr(idx), len(idx), self.G, out.p, out.ld, None))
         return out
 
     def sq_dists_to_rows(self, idx):
         idx = np.ascontiguousarray(idx, dtype=np.int32)
-        out = np.empty((len(idx), self.R), np.float32)
-        check(self.lib.cnmf_sq_dists_to_rows(self.engine._h, self.p, self.R, self.G, self.ld, ptr(idx), len(idx),
-                                             ptr(out), None))
+        out = np.empty((len(idx), self.R), self.dtype)
+        check(self.fn("cnmf_sq_dists_to_rows")(self.engine._h, self.p, self.R, self.G, self.ld, ptr(idx), len(idx),
+                                               ptr(out), None))
         return out.astype(np.float64)
 
 
@@ -173,7 +187,7 @@ def kmeans(S, k, n_init=10, random_state=1, max_iter=300, tol=1e-4):
     # tolerance: mean of the per-feature variances * tol (sklearn _kmeans.py:285-293)
     mean = np.empty(G)
     var = np.empty(G)
-    check(lib.cnmf_col_stats_dev(h, S.p, R, G, S.ld, ptr(mean), ptr(var), None))
+    check(S.fn("cnmf_col_stats_dev")(h, S.p, R, G, S.ld, ptr(mean), ptr(var), None))
     tol_abs = float(var.mean()) * tol
     if k <= 32 and n_init <= 32 and R * 8 <= 200 * 1024:
         rng = np.random.RandomState(random_state)
@@ -182,8 +196,9 @@ def kmeans(S, k, n_init=10, random_state=1, max_iter=300, tol=1e-4):
         inertia = np.empty(n_init, np.float64)
         n_it = np.zeros(n_init, np.int32)
         fallback = ctypes.c_int32(0)
-        check(lib.cnmf_kmeans_fit(h, S.p, R, G, S.ld, int(k), int(n_init), int(max_iter), tol_abs, ptr(first), ptr(unif),
-                                  int(n_trials), ptr(labels_all), ptr(inertia), ptr(n_it), ctypes.byref(fallback), None))
+        check(S.fn("cnmf_kmeans_fit")(h, S.p, R, G, S.ld, int(k), int(n_init), int(max_iter), tol_abs, ptr(first),
+                                      ptr(unif), int(n_trials), ptr(labels_all), ptr(inertia), ptr(n_it),
+                                      ctypes.byref(fallback), None))
         if not fallback.value:
             STATS["lloyd_iters"] = STATS.get("lloyd_iters", 0) + int(n_it.sum())
             best = None
@@ -197,7 +212,8 @@ def kmeans(S, k, n_init=10, random_state=1, max_iter=300, tol=1e-4):
 
 def _kmeans_per_run(S, k, n_init, random_state, max_iter, tol_abs):
     """One run at a time, k-means++ draws and the empty-cluster relocation rule on the host (sklearn
-    _k_means_common.pyx:167-211), distances and Lloyd steps on the device."""
+    _k_means_common.pyx:167-211), distances and Lloyd steps on the device.  A float32 matrix runs its E steps against an
+    fp32 copy of the fp64 centres; a float64 one against the fp64 centres themselves."""
     torch = _torch()
     lib, h = S.lib, S.engine._h
     rng = np.random.RandomState(random_state)
@@ -205,11 +221,11 @@ def _kmeans_per_run(S, k, n_init, random_state, max_iter, tol_abs):
 
     dev = S.t.device
     labels_t = torch.empty(R, dtype=torch.int32, device=dev)
-    mind_t = torch.empty(R, dtype=torch.float32, device=dev)
+    mind_t = torch.empty(R, dtype=S.torch_dtype, device=dev)
     # centres stay on the device across Lloyd iterations (fp64 master + fp32 copy for the E step, ping-pong):
     # an iteration returns three scalars instead of a K x G round trip
     C64 = [torch.empty((k, G), dtype=torch.float64, device=dev) for _ in range(2)]
-    C32 = [torch.empty((k, G), dtype=torch.float32, device=dev) for _ in range(2)]
+    C32 = None if S.fp64 else [torch.empty((k, G), dtype=torch.float32, device=dev) for _ in range(2)]
     sums_t = torch.empty((k, G), dtype=torch.float64, device=dev)
     counts_t = torch.empty(k, dtype=torch.int32, device=dev)
     vp = lambda t: ctypes.c_void_p(t.data_ptr())        # noqa: E731
@@ -223,14 +239,19 @@ def _kmeans_per_run(S, k, n_init, random_state, max_iter, tol_abs):
         centers = S.take_rows(idx).numpy().astype(np.float64)
         cur = 0
         C64[cur].copy_(torch.from_numpy(centers))
-        C32[cur].copy_(torch.from_numpy(np.ascontiguousarray(centers, dtype=np.float32)))
+        if C32 is not None:
+            C32[cur].copy_(torch.from_numpy(np.ascontiguousarray(centers, dtype=np.float32)))
         labels_t.fill_(-1)
         n_it = 0
         for n_it in range(max_iter):
             new = 1 - cur
-            check(lib.cnmf_kmeans_step(h, S.p, R, G, S.ld, k, vp(C32[cur]), vp(C64[cur]), vp(C64[new]), vp(C32[new]),
-                                       vp(labels_t), vp(mind_t), vp(sums_t), vp(counts_t), ctypes.byref(n_changed),
-                                       ctypes.byref(any_empty), ctypes.byref(shift), None))
+            flags = (vp(labels_t), vp(mind_t), vp(sums_t), vp(counts_t), ctypes.byref(n_changed),
+                     ctypes.byref(any_empty), ctypes.byref(shift), None)
+            if S.fp64:
+                check(lib.cnmf_kmeans_step_f64(h, S.p, R, G, S.ld, k, vp(C64[cur]), vp(C64[new]), *flags))
+            else:
+                check(lib.cnmf_kmeans_step(h, S.p, R, G, S.ld, k, vp(C32[cur]), vp(C64[cur]), vp(C64[new]),
+                                           vp(C32[new]), *flags))
             shift_tot = shift.value
             if any_empty.value:                       # rare: relocation rule on the host, sklearn _k_means_common.pyx:167-211
                 centers = C64[cur].cpu().numpy()
@@ -256,7 +277,8 @@ def _kmeans_per_run(S, k, n_init, random_state, max_iter, tol_abs):
                         nc[j] = nc[amax]
                 shift_tot = float(((nc - centers) ** 2).sum())
                 C64[new].copy_(torch.from_numpy(nc))
-                C32[new].copy_(torch.from_numpy(np.ascontiguousarray(nc, dtype=np.float32)))
+                if C32 is not None:
+                    C32[new].copy_(torch.from_numpy(np.ascontiguousarray(nc, dtype=np.float32)))
             cur = new
             if n_changed.value == 0:
                 break
@@ -264,11 +286,11 @@ def _kmeans_per_run(S, k, n_init, random_state, max_iter, tol_abs):
                 break
         STATS["lloyd_iters"] = STATS.get("lloyd_iters", 0) + n_it + 1
         centers = C64[cur].cpu().numpy()
-        c32 = np.ascontiguousarray(centers, dtype=np.float32)
+        ce = np.ascontiguousarray(centers, dtype=S.dtype)
         # final E step (labels consistent with the final centres) + inertia
-        check(lib.cnmf_kmeans_assign(h, S.p, R, G, S.ld, ptr(c32), k, ctypes.c_void_p(labels_t.data_ptr()),
-                                     None, None, ctypes.c_void_p(mind_t.data_ptr()), ctypes.byref(n_changed),
-                                     ctypes.byref(inertia), None))
+        check(S.fn("cnmf_kmeans_assign")(h, S.p, R, G, S.ld, ptr(ce), k, ctypes.c_void_p(labels_t.data_ptr()),
+                                         None, None, ctypes.c_void_p(mind_t.data_ptr()), ctypes.byref(n_changed),
+                                         ctypes.byref(inertia), None))
         labels = labels_t.cpu().numpy().copy()
         if best is None or (inertia.value < best[1] and not _same_clustering(labels, best[0], k)):
             best = (labels, float(inertia.value), centers.copy(), n_it + 1)
@@ -279,8 +301,8 @@ def _kmeans_per_run(S, k, n_init, random_state, max_iter, tol_abs):
 def cluster_medians(S, labels_t, k):
     """cnmf.py:913-916 on the device; returns K x G float64 (rows sum to 1)."""
     torch = _torch()
-    M = torch.empty((k, S.ld), dtype=torch.float32, device=S.t.device)
-    check(S.lib.cnmf_cluster_median(S.engine._h, S.p, S.R, S.G, S.ld, ctypes.c_void_p(labels_t.data_ptr()), k,
+    M = torch.empty((k, S.ld), dtype=S.torch_dtype, device=S.t.device)
+    check(S.fn("cnmf_cluster_median")(S.engine._h, S.p, S.R, S.G, S.ld, ctypes.c_void_p(labels_t.data_ptr()), k,
                                     ctypes.c_void_p(M.data_ptr()), S.ld, None))
     torch.cuda.synchronize(S.t.device)
     return M[:, :S.G].cpu().numpy().astype(np.float64)
@@ -290,8 +312,8 @@ def silhouette(S, labels, labels_t, k):
     """sklearn.metrics.silhouette_score(l2_spectra, labels, metric='euclidean') (cnmf.py:923): the R x R
     distances and the per-sample per-cluster distance sums come from the GPU, the O(R*K) rest is numpy."""
     sums = np.empty((S.R, k), np.float64)
-    check(S.lib.cnmf_cluster_dist_sums(S.engine._h, S.p, S.R, S.G, S.ld, ctypes.c_void_p(labels_t.data_ptr()), k,
-                                       ptr(sums), None))
+    check(S.fn("cnmf_cluster_dist_sums")(S.engine._h, S.p, S.R, S.G, S.ld, ctypes.c_void_p(labels_t.data_ptr()), k,
+                                         ptr(sums), None))
     counts = np.bincount(labels, minlength=k).astype(np.float64)
     own = counts[labels]
     idx = np.arange(S.R)
@@ -352,7 +374,9 @@ def _consensus_numerics(eng, merged, k, norm_ds, kw, density_threshold=0.5, n_ne
         phases[name] = phases.get(name, 0.0) + 1e3 * (now - t_last[0])
         t_last[0] = now
 
-    S = merged if isinstance(merged, SpectraMatrix) else SpectraMatrix(eng, merged)
+    # a float64 analysis (precision='fp64') keeps the spectra in float64 through every consensus kernel
+    dtype = np.float64 if getattr(norm_ds, "fp64", False) else np.float32
+    S = merged if isinstance(merged, SpectraMatrix) else SpectraMatrix(eng, merged, dtype=dtype)
     S.l2_normalize()                                                            # cnmf.py:882
     R = S.R
     if n_neighbors is None:

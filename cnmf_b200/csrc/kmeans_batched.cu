@@ -18,6 +18,7 @@
 #include <algorithm>
 #include <chrono>
 #include <cstring>
+#include <type_traits>
 #include <vector>
 
 #include "engine.h"
@@ -42,8 +43,9 @@ __device__ __forceinline__ T kb_block_sum_all(T v, T* smem /* >= 33 */) {
   return smem[32];
 }
 
+template <typename T>
 struct KmState {
-  const float* S; int R, G, ld, K, n_init, n_trials, row_blocks;
+  const T* S; int R, G, ld, K, n_init, n_trials, row_blocks;
   double* closest;      // [n_init][R]
   double* newd;         // [n_init][n_trials][R]
   double* part;         // [n_init][n_trials][row_blocks]
@@ -53,45 +55,52 @@ struct KmState {
   const double* unif;   // [n_init][K-1][n_trials]
 };
 
-// squared distance of row r to `NC` rows: fp32 differences, fp64 accumulation, rounded to fp32 (what the per-run path
+// four consecutive elements as one load
+template <typename T> struct KbVec4;
+template <> struct KbVec4<float> { using type = float4; };
+struct __align__(32) kb_double4a { double x, y, z, w; };
+template <> struct KbVec4<double> { using type = kb_double4a; };
+
+// squared distance of row r to `NC` rows: differences in T, fp64 accumulation, rounded to T (what the per-run path
 // hands to the host: cand_dist_kernel)
-template <int NC>
-__device__ __forceinline__ void row_dists(const float* __restrict__ S, int G, int ld, int r, const int* idx, int n_c,
+template <typename T, int NC>
+__device__ __forceinline__ void row_dists(const T* __restrict__ S, int G, int ld, int r, const int* idx, int n_c,
                                           int lane, double (&out)[NC]) {
-  const float4* row = reinterpret_cast<const float4*>(S + (long long)r * ld);
-  const float4* cand[NC];
+  using V4 = typename KbVec4<T>::type;
+  const V4* row = reinterpret_cast<const V4*>(S + (long long)r * ld);
+  const V4* cand[NC];
 #pragma unroll
-  for (int c = 0; c < NC; ++c) cand[c] = reinterpret_cast<const float4*>(S + (long long)idx[c < n_c ? c : 0] * ld);
+  for (int c = 0; c < NC; ++c) cand[c] = reinterpret_cast<const V4*>(S + (long long)idx[c < n_c ? c : 0] * ld);
   double acc[NC];
 #pragma unroll
   for (int c = 0; c < NC; ++c) acc[c] = 0.0;
   const int g4 = G / 4;
   for (int q = lane; q < g4; q += 32) {
-    const float4 x = row[q];
+    const V4 x = row[q];
 #pragma unroll
     for (int c = 0; c < NC; ++c) {
-      const float4 y = cand[c][q];
-      const float d0 = x.x - y.x, d1 = x.y - y.y, d2 = x.z - y.z, d3 = x.w - y.w;
+      const V4 y = cand[c][q];
+      const T d0 = x.x - y.x, d1 = x.y - y.y, d2 = x.z - y.z, d3 = x.w - y.w;
       acc[c] += (double)d0 * d0 + (double)d1 * d1 + (double)d2 * d2 + (double)d3 * d3;
     }
   }
   for (int g = 4 * g4 + lane; g < G; g += 32) {
-    const float x = S[(long long)r * ld + g];
+    const T x = S[(long long)r * ld + g];
 #pragma unroll
     for (int c = 0; c < NC; ++c) {
-      const float d = x - S[(long long)idx[c < n_c ? c : 0] * ld + g];
+      const T d = x - S[(long long)idx[c < n_c ? c : 0] * ld + g];
       acc[c] += (double)d * d;
     }
   }
 #pragma unroll
-  for (int c = 0; c < NC; ++c) out[c] = (double)(float)warp_sum(acc[c]);
+  for (int c = 0; c < NC; ++c) out[c] = (double)(T)warp_sum(acc[c]);
 }
 
 // step 0: closest = distances to the first centre.  step > 0: newd[j] = min(closest, distance to candidate j).
 // Per block: fixed-order partial sums of what was written (potentials).
-template <int NC>
+template <typename T, int NC>
 __global__ void __launch_bounds__(256)
-kpp_eval_kernel(KmState st, int first) {
+kpp_eval_kernel(KmState<T> st, int first) {
   __shared__ double sm[8][NC];
   const int t = blockIdx.y;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -102,7 +111,7 @@ kpp_eval_kernel(KmState st, int first) {
 #pragma unroll
   for (int c = 0; c < NC; ++c) d[c] = 0.0;
   if (r < st.R) {
-    row_dists<NC>(st.S, st.G, st.ld, r, idx, n_c, lane, d);
+    row_dists<T, NC>(st.S, st.G, st.ld, r, idx, n_c, lane, d);
     if (first) {
       if (lane == 0) st.closest[(long long)t * st.R + r] = d[0];
     } else {
@@ -128,8 +137,9 @@ kpp_eval_kernel(KmState st, int first) {
 
 // one block per run: potentials of the candidates (fixed-order sums), argmin (first minimum wins), commit the winner,
 // then the next candidates: searchsorted(cumsum(closest), uniform * pot) with numpy's sequential float64 cumsum
+template <typename T>
 __global__ void __launch_bounds__(256)
-kpp_select_kernel(KmState st, int step /* centre being committed: 0 = the first one */) {
+kpp_select_kernel(KmState<T> st, int step /* centre being committed: 0 = the first one */) {
   extern __shared__ double cl_s[];            // R doubles
   __shared__ double cpot[8];
   __shared__ int s_best;
@@ -202,23 +212,26 @@ kpp_select_kernel(KmState st, int step /* centre being committed: 0 = the first 
     if (j < st.n_trials) st.cand[t * 8 + j] = found[j] < 0 ? st.R - 1 : found[j];   // np.clip
 }
 
+// C64: the fp64 centres; CT: their fp32 copy for the E step (T = float only: with T = double the E step reads C64)
+template <typename T>
 __global__ void __launch_bounds__(256)
-kpp_gather_centres_kernel(KmState st, double* __restrict__ C64, float* __restrict__ C32) {
+kpp_gather_centres_kernel(KmState<T> st, double* __restrict__ C64, T* __restrict__ CT) {
   const int k = blockIdx.x, t = blockIdx.y;
-  const float* src = st.S + (long long)st.centre_idx[(long long)t * st.K + k] * st.ld;
+  const T* src = st.S + (long long)st.centre_idx[(long long)t * st.K + k] * st.ld;
   const long long o = ((long long)t * st.K + k) * st.G;
   for (int g = threadIdx.x; g < st.G; g += blockDim.x) {
-    const float v = src[g];
-    C32[o + g] = v;
+    const T v = src[g];
+    if constexpr (!std::is_same<T, double>::value) CT[o + g] = v;
     C64[o + g] = (double)v;
   }
 }
 
 // ---------------------------------------------------------------- Lloyd, all runs at once
+template <typename T>
 struct LloydState {
-  const float* S; int R, G, ld, K, n_init;
+  const T* S; int R, G, ld, K, n_init;
   int* labels;        // [n_init][R]
-  float* mind;        // [n_init][R]
+  T* mind;            // [n_init][R]
   int* counts;        // [n_init][K]
   int* order;         // [n_init][K][R]
   double* sums;       // [n_init][K][G]
@@ -227,28 +240,30 @@ struct LloydState {
   double* inertia;    // [n_init]
 };
 
-// E step: one warp per row (arithmetic of kmeans_assign_kernel); `final_pass` assigns against every run's final centres
+// E step: one warp per row (arithmetic of kmeans_assign_kernel); `final_pass` assigns against every run's final centres.
+// CEa / CEb: the two ping-pong centre buffers the E step reads (fp32 copies for T = float, the fp64 centres for double)
+template <typename T>
 __global__ void __launch_bounds__(256)
-kmb_assign_kernel(LloydState st, const float* __restrict__ C32a, const float* __restrict__ C32b, int parity, int final_pass) {
+kmb_assign_kernel(LloydState<T> st, const T* __restrict__ CEa, const T* __restrict__ CEb, int parity, int final_pass) {
   const int t = blockIdx.y;
   int* fl = st.flags + t * 4;
   const bool done = fl[2] != 0;
   if (!final_pass && done) return;
   // centres this run reads: the live parity while iterating; after it stopped, the buffer its last step wrote
   const int buf = final_pass ? (fl[3] & 1) : parity;
-  const float* C = (buf ? C32b : C32a) + (long long)t * st.K * st.G;
+  const T* C = (buf ? CEb : CEa) + (long long)t * st.K * st.G;
   const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (row >= st.R) return;
-  const float* x = st.S + (long long)row * st.ld;
-  float best = 0.f;
+  const T* x = st.S + (long long)row * st.ld;
+  T best = T(0);
   int bl = 0;
   for (int c = 0; c < st.K; ++c) {
-    const float* cc = C + (long long)c * st.G;
-    float a = 0.f;
+    const T* cc = C + (long long)c * st.G;
+    T a = T(0);
     for (int g = lane; g < st.G; g += 32) {
-      const float d = x[g] - cc[g];
-      a = fmaf(d, d, a);
+      const T d = x[g] - cc[g];
+      a = fma(d, d, a);
     }
     a = warp_sum(a);
     if (c == 0 || a < best) {   // strict '<': first minimum wins (sklearn _k_means_lloyd.pyx:205-209)
@@ -266,8 +281,9 @@ kmb_assign_kernel(LloydState st, const float* __restrict__ C32a, const float* __
 
 // stable counting sort of the row indices by label (members of cluster c in row order): 1024 rows at a time, ranks
 // from warp ballots, warp offsets from a per-cluster scan over the 32 warps
+template <typename T>
 __global__ void __launch_bounds__(1024)
-kmb_members_kernel(LloydState st) {
+kmb_members_kernel(LloydState<T> st) {
   __shared__ int base[32];            // members of cluster c placed so far
   __shared__ int wtot[32][33];        // [cluster][warp]
   const int t = blockIdx.x;
@@ -304,8 +320,9 @@ kmb_members_kernel(LloydState st) {
 }
 
 // M step: per-cluster column sums in fp64, members visited in row order (arithmetic of cluster_sums_kernel)
+template <typename T>
 __global__ void __launch_bounds__(128)
-kmb_sums_kernel(LloydState st) {
+kmb_sums_kernel(LloydState<T> st) {
   const int c = blockIdx.y, t = blockIdx.z;
   if (st.flags[t * 4 + 2]) return;
   const int g = blockIdx.x * blockDim.x + threadIdx.x;
@@ -317,10 +334,12 @@ kmb_sums_kernel(LloydState st) {
   st.sums[((long long)t * st.K + c) * st.G + g] = a;
 }
 
-// new centre = sums * (1 / count), squared shift against the current one (arithmetic of centre_update_kernel)
+// new centre = sums * (1 / count), squared shift against the current one (arithmetic of centre_update_kernel);
+// CT_new: the fp32 copy for the next E step (T = float only)
+template <typename T>
 __global__ void __launch_bounds__(256)
-kmb_centre_update_kernel(LloydState st, const double* __restrict__ C64_cur, double* __restrict__ C64_new,
-                         float* __restrict__ C32_new) {
+kmb_centre_update_kernel(LloydState<T> st, const double* __restrict__ C64_cur, double* __restrict__ C64_new,
+                         T* __restrict__ CT_new) {
   __shared__ double sm[33];
   const int j = blockIdx.x, t = blockIdx.y;
   if (st.flags[t * 4 + 2]) return;
@@ -340,7 +359,7 @@ kmb_centre_update_kernel(LloydState st, const double* __restrict__ C64_cur, doub
     const double d = nv - C64_cur[o + g];
     acc += d * d;
     C64_new[o + g] = nv;
-    C32_new[o + g] = (float)nv;
+    if constexpr (!std::is_same<T, double>::value) CT_new[o + g] = (T)nv;
   }
   acc = kb_block_sum_all(acc, sm);
   if (threadIdx.x == 0) st.shift_part[t * st.K + j] = acc;
@@ -348,7 +367,8 @@ kmb_centre_update_kernel(LloydState st, const double* __restrict__ C64_cur, doub
 
 // the stopping rule of the per-run loop, per run: stop when no label changed or the total shift <= tol
 // (sklearn _kmeans.py:700-715); flags[3] = iterations run = index of the buffer that holds the final centres (parity)
-__global__ void kmb_check_kernel(LloydState st, double tol_abs, int max_iter) {
+template <typename T>
+__global__ void kmb_check_kernel(LloydState<T> st, double tol_abs, int max_iter) {
   const int t = threadIdx.x;
   if (t >= st.n_init) return;
   int* fl = st.flags + t * 4;
@@ -361,26 +381,23 @@ __global__ void kmb_check_kernel(LloydState st, double tol_abs, int max_iter) {
   fl[0] = 0;
 }
 
+template <typename T>
 __global__ void __launch_bounds__(256)
-kmb_inertia_kernel(LloydState st) {
+kmb_inertia_kernel(LloydState<T> st) {
   __shared__ double sm[33];
   const int t = blockIdx.x;
-  const float* v = st.mind + (long long)t * st.R;
+  const T* v = st.mind + (long long)t * st.R;
   double a = 0.0;
   for (int i = threadIdx.x; i < st.R; i += blockDim.x) a += (double)v[i];
   a = kb_block_sum_all(a, sm);
   if (threadIdx.x == 0) st.inertia[t] = a;
 }
 
-}  // namespace
-}  // namespace cnmf
-
-using namespace cnmf;
-
-extern "C" int cnmf_kmeans_fit(cnmf_handle_t h, const float* S_dev, int R, int G, int ld, int K, int n_init, int max_iter,
-                               double tol_abs, const int32_t* first_idx_host, const double* uniforms_host, int n_trials,
-                               int32_t* labels_host /* n_init x R */, double* inertia_host /* n_init */,
-                               int32_t* n_iter_host /* n_init */, int32_t* needs_host_path, void* stream) {
+template <typename T>
+int kmeans_fit(cnmf_handle_t h, const T* S_dev, int R, int G, int ld, int K, int n_init, int max_iter, double tol_abs,
+               const int32_t* first_idx_host, const double* uniforms_host, int n_trials,
+               int32_t* labels_host /* n_init x R */, double* inertia_host /* n_init */, int32_t* n_iter_host /* n_init */,
+               int32_t* needs_host_path, void* stream) {
   CNMF_REQUIRE(h && S_dev && first_idx_host && labels_host && inertia_host && needs_host_path, "kmeans_fit: NULL argument");
   CNMF_REQUIRE(R > 0 && G > 0 && ld >= G && ld % 4 == 0 && K >= 1 && K <= 32 && n_init >= 1 && n_init <= 32 &&
                    n_trials >= 1 && n_trials <= 8 && (K == 1 || uniforms_host) && max_iter >= 1,
@@ -390,7 +407,7 @@ extern "C" int cnmf_kmeans_fit(cnmf_handle_t h, const float* S_dev, int R, int G
   CNMF_CUDA_CHECK(cudaSetDevice(h->device));
   const int row_blocks = (R + 7) / 8;
   const size_t nR = (size_t)n_init * R, nKG = (size_t)n_init * K * G;
-  KmState st{};
+  KmState<T> st{};
   st.S = S_dev; st.R = R; st.G = G; st.ld = ld; st.K = K; st.n_init = n_init; st.n_trials = n_trials; st.row_blocks = row_blocks;
   st.closest = static_cast<double*>(h->dev_buf("kmb.closest", nR * 8));
   st.newd = static_cast<double*>(h->dev_buf("kmb.newd", nR * n_trials * 8));
@@ -401,18 +418,20 @@ extern "C" int cnmf_kmeans_fit(cnmf_handle_t h, const float* S_dev, int R, int G
   const size_t n_unif = (size_t)n_init * (K > 1 ? K - 1 : 1) * n_trials;
   double* d_unif = static_cast<double*>(h->dev_buf("kmb.unif", n_unif * 8));
   double* C64 = static_cast<double*>(h->dev_buf("kmb.C64", 2 * nKG * 8));
-  float* C32 = static_cast<float*>(h->dev_buf("kmb.C32", 2 * nKG * 4));
-  LloydState ls{};
+  // the ping-pong centres the E step reads: an fp32 copy for T = float, the fp64 centres themselves for T = double
+  T* CE = std::is_same<T, double>::value ? reinterpret_cast<T*>(C64)
+                                         : static_cast<T*>(h->dev_buf("kmb.C32", 2 * nKG * sizeof(T)));
+  LloydState<T> ls{};
   ls.S = S_dev; ls.R = R; ls.G = G; ls.ld = ld; ls.K = K; ls.n_init = n_init;
   ls.labels = static_cast<int*>(h->dev_buf("kmb.labels", nR * 4));
-  ls.mind = static_cast<float*>(h->dev_buf("kmb.mind", nR * 4));
+  ls.mind = static_cast<T*>(h->dev_buf("kmb.mind", nR * sizeof(T)));
   ls.counts = static_cast<int*>(h->dev_buf("kmb.counts", (size_t)n_init * K * 4));
   ls.order = static_cast<int*>(h->dev_buf("kmb.order", nR * K * 4));
   ls.sums = static_cast<double*>(h->dev_buf("kmb.sums", nKG * 8));
   ls.shift_part = static_cast<double*>(h->dev_buf("kmb.shift", (size_t)n_init * K * 8));
   ls.flags = static_cast<int*>(h->dev_buf("kmb.flags", (size_t)n_init * 4 * 4));
   ls.inertia = static_cast<double*>(h->dev_buf("kmb.inertia", (size_t)n_init * 8));
-  if (!st.closest || !st.newd || !st.part || !st.cand || !st.centre_idx || !st.pot || !d_unif || !C64 || !C32 ||
+  if (!st.closest || !st.newd || !st.part || !st.cand || !st.centre_idx || !st.pot || !d_unif || !C64 || !CE ||
       !ls.labels || !ls.mind || !ls.counts || !ls.order || !ls.sums || !ls.shift_part || !ls.flags || !ls.inertia)
     return -2;
   st.unif = d_unif;
@@ -437,17 +456,17 @@ extern "C" int cnmf_kmeans_fit(cnmf_handle_t h, const float* S_dev, int R, int G
   const size_t sel_smem = (size_t)R * sizeof(double);
   static bool sel_attr[64] = {};
   if (sel_smem > 48 * 1024 && !sel_attr[h->device & 63]) {
-    CNMF_CUDA_CHECK(cudaFuncSetAttribute(kpp_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    CNMF_CUDA_CHECK(cudaFuncSetAttribute(kpp_select_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     sel_attr[h->device & 63] = true;
   }
   const dim3 eval_grid(row_blocks, n_init);
-  kpp_eval_kernel<8><<<eval_grid, 256, 0, s>>>(st, 1);
-  kpp_select_kernel<<<n_init, 256, sel_smem, s>>>(st, 0);
+  kpp_eval_kernel<T, 8><<<eval_grid, 256, 0, s>>>(st, 1);
+  kpp_select_kernel<T><<<n_init, 256, sel_smem, s>>>(st, 0);
   for (int step = 1; step < K; ++step) {
-    kpp_eval_kernel<8><<<eval_grid, 256, 0, s>>>(st, 0);
-    kpp_select_kernel<<<n_init, 256, sel_smem, s>>>(st, step);
+    kpp_eval_kernel<T, 8><<<eval_grid, 256, 0, s>>>(st, 0);
+    kpp_select_kernel<T><<<n_init, 256, sel_smem, s>>>(st, step);
   }
-  kpp_gather_centres_kernel<<<dim3(K, n_init), 256, 0, s>>>(st, C64, C32);
+  kpp_gather_centres_kernel<T><<<dim3(K, n_init), 256, 0, s>>>(st, C64, CE);
   h->launches += 2 * K + 1;
 
   if (h->profile) {                 // phase timing for bench / probes (cnmf_last_timing: rng = seeding, solve = Lloyd)
@@ -463,12 +482,12 @@ extern "C" int cnmf_kmeans_fit(cnmf_handle_t h, const float* S_dev, int R, int G
   int it = 0;
   while (!all_done && it < max_iter) {
     const int cur = it & 1, nxt = cur ^ 1;
-    kmb_assign_kernel<<<assign_grid, 256, 0, s>>>(ls, C32, C32 + nKG, cur, 0);
-    kmb_members_kernel<<<n_init, 1024, 0, s>>>(ls);
-    kmb_sums_kernel<<<dim3((G + 127) / 128, K, n_init), 128, 0, s>>>(ls);
-    kmb_centre_update_kernel<<<dim3(K, n_init), 256, 0, s>>>(ls, C64 + (size_t)cur * nKG, C64 + (size_t)nxt * nKG,
-                                                             C32 + (size_t)nxt * nKG);
-    kmb_check_kernel<<<1, 32, 0, s>>>(ls, tol_abs, max_iter);
+    kmb_assign_kernel<T><<<assign_grid, 256, 0, s>>>(ls, CE, CE + nKG, cur, 0);
+    kmb_members_kernel<T><<<n_init, 1024, 0, s>>>(ls);
+    kmb_sums_kernel<T><<<dim3((G + 127) / 128, K, n_init), 128, 0, s>>>(ls);
+    kmb_centre_update_kernel<T><<<dim3(K, n_init), 256, 0, s>>>(ls, C64 + (size_t)cur * nKG, C64 + (size_t)nxt * nKG,
+                                                                CE + (size_t)nxt * nKG);
+    kmb_check_kernel<T><<<1, 32, 0, s>>>(ls, tol_abs, max_iter);
     h->launches += 5;
     ++it;
     CNMF_CUDA_CHECK(cudaMemcpyAsync(hb->flags, ls.flags, (size_t)n_init * 16, cudaMemcpyDeviceToHost, s));
@@ -492,8 +511,8 @@ extern "C" int cnmf_kmeans_fit(cnmf_handle_t h, const float* S_dev, int R, int G
     t_phase = clk::now();
   }
   // ---- final E step against every run's final centres + inertia (sklearn _kmeans.py:736-744)
-  kmb_assign_kernel<<<assign_grid, 256, 0, s>>>(ls, C32, C32 + nKG, 0, 1);
-  kmb_inertia_kernel<<<n_init, 256, 0, s>>>(ls);
+  kmb_assign_kernel<T><<<assign_grid, 256, 0, s>>>(ls, CE, CE + nKG, 0, 1);
+  kmb_inertia_kernel<T><<<n_init, 256, 0, s>>>(ls);
   h->launches += 2;
   CNMF_CUDA_CHECK(cudaGetLastError());
   CNMF_CUDA_CHECK(cudaMemcpyAsync(hb->inertia, ls.inertia, (size_t)n_init * 8, cudaMemcpyDeviceToHost, s));
@@ -505,4 +524,25 @@ extern "C" int cnmf_kmeans_fit(cnmf_handle_t h, const float* S_dev, int R, int G
     if (n_iter_host) n_iter_host[t] = hb->flags[t * 4 + 3];
   }
   return 0;
+}
+
+}  // namespace
+}  // namespace cnmf
+
+using namespace cnmf;
+
+extern "C" int cnmf_kmeans_fit(cnmf_handle_t h, const float* S_dev, int R, int G, int ld, int K, int n_init, int max_iter,
+                               double tol_abs, const int32_t* first_idx_host, const double* uniforms_host, int n_trials,
+                               int32_t* labels_host, double* inertia_host, int32_t* n_iter_host,
+                               int32_t* needs_host_path, void* stream) {
+  return kmeans_fit(h, S_dev, R, G, ld, K, n_init, max_iter, tol_abs, first_idx_host, uniforms_host, n_trials,
+                    labels_host, inertia_host, n_iter_host, needs_host_path, stream);
+}
+
+extern "C" int cnmf_kmeans_fit_f64(cnmf_handle_t h, const double* S_dev, int R, int G, int ld, int K, int n_init,
+                                   int max_iter, double tol_abs, const int32_t* first_idx_host,
+                                   const double* uniforms_host, int n_trials, int32_t* labels_host,
+                                   double* inertia_host, int32_t* n_iter_host, int32_t* needs_host_path, void* stream) {
+  return kmeans_fit(h, S_dev, R, G, ld, K, n_init, max_iter, tol_abs, first_idx_host, uniforms_host, n_trials,
+                    labels_host, inertia_host, n_iter_host, needs_host_path, stream);
 }

@@ -138,8 +138,8 @@ class cNMF:
 
     def __init__(self, output_dir=".", name=None, precision="f16x2", device=None):
         """precision (cnmf_b200 extension): 'f16x2' (default), 'tf32x3', 'tf32x3-general', 'fp32', or 'fp64' -- X,
-        factorize and every refit in float64 as the reference computes (beta_loss='frobenius'; the consensus kernels
-        that compare spectra stay float32)."""
+        factorize, the consensus kernels and every refit in float64 as the reference computes
+        (beta_loss='frobenius')."""
         self.output_dir = output_dir
         if name is None:
             name = "%s_%s" % (datetime.datetime.now().strftime("%Y_%m_%d"), uuid.uuid4().hex[:6])

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define CNMF_B200_ABI_VERSION 13
+#define CNMF_B200_ABI_VERSION 14
 #define CNMF_MAX_COMPONENTS 32          /* largest n_components per restart on the CUDA path */
 
 typedef struct cnmf_handle_s* cnmf_handle_t;
@@ -410,6 +410,35 @@ int cnmf_cluster_dist_sums(cnmf_handle_t h, const float* S_dev, int R, int G, in
  * (cnmf.py:916) -> M_dev (K x ldm). Asynchronous on `stream`. */
 int cnmf_cluster_median(cnmf_handle_t h, const float* S_dev, int R, int G, int ld, const int32_t* labels_dev, int K,
                         float* M_dev, int ldm, void* stream);
+
+/* ---- the same consensus kernels on a float64 S (precision="fp64"): S, distances, densities, centres and medians are
+ * double, every argument is otherwise that of the float entry point above.  Distances keep the direct sum (x - y)^2
+ * form (fp64 FMA), the radix selects of the density and the medians run over the 64-bit patterns, and the KMeans E step
+ * reads the fp64 centres themselves (cnmf_kmeans_step_f64 has no fp32 centre copy). */
+int cnmf_l2_normalize_rows_f64(cnmf_handle_t h, double* S_dev, int R, int G, int ld, void* stream);
+int cnmf_local_density_f64(cnmf_handle_t h, const double* S_dev, int R, int G, int ld, int n_neighbors,
+                           double* density_dev, double* D_dev, void* stream);
+int cnmf_col_stats_dev_f64(cnmf_handle_t h, const double* S_dev, int R, int G, int ld, double* mean_host,
+                           double* var_host, void* stream);
+int cnmf_gather_rows_f64(cnmf_handle_t h, const double* src_dev, int ld_src, const int32_t* idx_host, int n, int G,
+                         double* dst_dev, int ld_dst, void* stream);
+int cnmf_sq_dists_to_rows_f64(cnmf_handle_t h, const double* S_dev, int R, int G, int ld, const int32_t* idx_host,
+                              int n_c, double* out_host, void* stream);
+int cnmf_kmeans_assign_f64(cnmf_handle_t h, const double* S_dev, int R, int G, int ld, const double* centers_host,
+                           int K, int32_t* labels_dev, double* sums_host, int32_t* counts_host, double* mind_dev,
+                           int32_t* n_changed_host, double* inertia_host, void* stream);
+int cnmf_kmeans_step_f64(cnmf_handle_t h, const double* S_dev, int R, int G, int ld, int K, const double* C64_cur_dev,
+                         double* C64_new_dev, int32_t* labels_dev, double* mind_dev, double* sums_dev,
+                         int32_t* counts_dev, int32_t* n_changed_host, int32_t* any_empty_host, double* shift_host,
+                         void* stream);
+int cnmf_kmeans_fit_f64(cnmf_handle_t h, const double* S_dev, int R, int G, int ld, int K, int n_init, int max_iter,
+                        double tol_abs, const int32_t* first_idx_host, const double* uniforms_host, int n_trials,
+                        int32_t* labels_host, double* inertia_host, int32_t* n_iter_host, int32_t* needs_host_path,
+                        void* stream);
+int cnmf_cluster_dist_sums_f64(cnmf_handle_t h, const double* S_dev, int R, int G, int ld, const int32_t* labels_dev,
+                               int K, double* sums_host, void* stream);
+int cnmf_cluster_median_f64(cnmf_handle_t h, const double* S_dev, int R, int G, int ld, const int32_t* labels_dev,
+                            int K, double* M_dev, int ldm, void* stream);
 
 #ifdef __cplusplus
 }
