@@ -117,7 +117,7 @@ SIGNATURES = {
     "cnmf_factorize_dev": (_i, [_vp, _i, _vp, _vp, _vp, _pp(NmfParams), _vp, _vp, _vp, _vp]),
     "cnmf_refit": (_i, [_vp, _i, _i, _vp, _pp(NmfParams), _vp, _pp(_c.c_int32), _pp(_d), _vp]),
     "cnmf_project_rows": (_i, [_vp, _i, _vp, _vp, _vp]),
-    "cnmf_gemm_abt_host": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _pp(_c.c_float), _vp]),
+    "cnmf_gemm_abt_host": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp, _i, _pp(_c.c_float), _vp]),
     "cnmf_update_step_host": (_i, [_vp, _pp(UpdateStepArgs), _vp]),
     "cnmf_beta_step_host": (_i, [_vp, _pp(BetaStepArgs), _vp]),
     "cnmf_l2_normalize_rows": (_i, [_vp, _vp, _i, _i, _i, _vp]),
@@ -145,7 +145,7 @@ SIGNATURES = {
 _lib = None
 
 
-ABI_VERSION = 14     # include/cnmf_b200.h CNMF_B200_ABI_VERSION
+ABI_VERSION = 15     # include/cnmf_b200.h CNMF_B200_ABI_VERSION
 
 
 def load():

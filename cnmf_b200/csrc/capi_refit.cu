@@ -546,8 +546,8 @@ int cnmf_project_rows_f64(cnmf_dataset_t d, int k, const double* Ut_host, double
 // mean device time per launch in *ms_out (CUDA events).  Used by tests and by the roofline micro-bench.
 // Exact forms (b_exact, f16x2): A diag(k_scale) goes into the A pieces and out_col_scale onto C, as in the solver.
 int cnmf_gemm_abt_host(cnmf_handle_t h, int precision, const float* A, const float* B, int M, int N, int Kd, int splits,
-                       int b_exact, const float* k_scale, const float* out_col_scale, float* C, int reps, float* ms_out,
-                       void* stream) {
+                       int b_exact, const float* k_scale, const float* out_col_scale, int tile_n, float* C, int reps,
+                       float* ms_out, void* stream) {
   CNMF_REQUIRE(h && A && B && C && M > 0 && N > 0 && Kd > 0, "gemm_abt_host: bad arguments");
   const bool f16 = precision == CNMF_PRECISION_F16X2;    // B must hold integers <= 2048 (exact in fp16)
   CNMF_REQUIRE(!b_exact || f16 || precision == CNMF_PRECISION_TF32X3, "gemm_abt_host: b_exact needs tf32x3 or f16x2");
@@ -598,6 +598,7 @@ int cnmf_gemm_abt_host(cnmf_handle_t h, int precision, const float* A, const flo
   GemmArgs g{};
   g.M = M; g.N = N; g.Kd = Kd; g.lda = lda; g.ldb = lda; g.ldc = ldc;
   g.C = dC; g.c_split_stride = (long long)M * ldc; g.splits = splits; g.splits_effective = se;
+  g.tile_n = tile_n;
   const Operand Bop{dB, dBh, dBl, N, Kd, lda};
   cudaEvent_t e0, e1;
   CNMF_CUDA_CHECK(cudaEventCreate(&e0));

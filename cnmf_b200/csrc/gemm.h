@@ -25,6 +25,9 @@ struct GemmArgs {
   // multiply each finished MMA chain (128 elements, never straddling a group) by a_tile_scale[m * a_tiles + group]
   const float* a_tile_scale;
   int a_tiles;                // groups per row = ceil(Kd / 512)
+  // columns of C per output tile: 0 = the launcher's choice by shape; 128, or with b_exact 168 / 192, forces that width
+  // (tests and micro-benchmarks: every element is formed by the same chains in the same order whatever the width)
+  int tile_n;
 };
 
 // number of non-empty split-K slices for a reduction length Kd (k-blocks of 32 fp32 / 64 fp16 elements = 128 B)
@@ -34,7 +37,7 @@ int gemm_effective_splits(int Kd, int splits, int f16 = 0);
 // restart's result does not depend on the batch it is solved in
 int gemm_fixed_splits(int Kd, int f16 = 0);
 
-// wgmma / TMA path (gemm_tf32x3.cu), 128 x 128 output tiles
+// wgmma / TMA path (gemm_tf32x3.cu), 128- or 192-row and 128- to 192-column output tiles
 int gemm_tf32x3(const GemmArgs& g, cudaStream_t stream);
 
 // plain fp32 FFMA path (gemm_simt.cu): A = A_hi, B = B_hi exactly; same split-K contract

@@ -15,17 +15,17 @@
 //   X H^T   (sklearn _nmf.py:538, :380)  ->  A = H_batch (SK x G),   B = X   (cells x G)
 //   W^T X   (sklearn _nmf.py:634, :380)  ->  A = W^T_batch (SK x N), B = X^T (G x cells), split-K
 //
-// Structure (one CTA per SM, persistent over a static tile schedule of BM x 128 tiles, BM = 128 or 192; 128 + 2 BM
-// threads = 1 + BM / 64 warpgroups; the CTAs run in clusters of 2 whose tiles share an m-tile, and each CTA loads half
-// of the shared A panel and multicasts it to both):
+// Structure (one CTA per SM, persistent over a static tile schedule of 128 x BN tiles, BN = 128, 168 or 192; 384
+// threads = 3 warpgroups; the CTAs run in clusters of 2 whose tiles share an m-tile, and each CTA loads half of the
+// shared A panel and multicasts it to both):
 //   warpgroup 0     TMA producer (one thread): cp.async.bulk.tensor 2D, 128B-swizzled tiles, mbarrier full/empty ring,
 //                   a stage refilled only once both CTAs of the pair have released it
-//   warpgroups 1-   consumers: rows [64 (w - 1), 64 w) of the tile, wgmma.mma_async m64n128 from shared memory
+//   warpgroups 1-2  consumers: rows [64 (w - 1), 64 w) of the tile, wgmma.mma_async m64nBN from shared memory
 //                   descriptors, fp32 fragment in registers, float2 stores.  Named barriers make them take turns in a
 //                   ring issuing one k-block of MMAs each (ping-pong), so one warpgroup's chain drain and tile stores
 //                   run while the others' MMAs keep the tensor pipe busy.
-//   At BM = 192 (512 threads) setmaxnreg moves the producer to 32 registers and the consumers to 160.  The launcher
-//   picks BM by shape (gemm_tf32x3 below); measured on one H100 SXM (700 W), DESIGN.md section 4.1.
+//   At BN > 128 setmaxnreg moves the producer to 40 registers and the consumers to 232.  The launcher picks BN by
+//   shape (pick_tile_n below); measured on one H100 SXM (700 W), DESIGN.md section 4.1.
 //
 // Accumulation accuracy.  The tensor core does not round its running sum to nearest: a long chain of MMAs on
 // non-negative data is biased low by about 3e-8 relative per MMA (2.3e-5 at K = 2048), far outside the 1e-4 parity
@@ -49,21 +49,19 @@ namespace cnmf {
 
 namespace {
 
-// BM (rows of A per tile) is a template parameter: one consumer warpgroup per 64 rows, plus the producer warpgroup.
-constexpr int BN = 128;          // rows of B per tile (wgmma N)
+// BN (rows of B per tile, the wgmma N) is a template parameter.  BM rows of A per tile: one consumer warpgroup per 64.
+constexpr int BM = 128;
+constexpr int NUM_THREADS = 128 * (1 + BM / 64);
 constexpr int BK = 32;           // fp32 elements per k-block = 128 B = one swizzle row
 constexpr long long WAIT_TIMEOUT_CYCLES = 4000000000LL;   // ~2 s: a dead pipeline traps instead of hanging
 
-template <int BM>
-constexpr int num_threads() { return 128 * (1 + BM / 64); }
-
 // BEXACT: the B operand is exactly representable in tf32 / fp16 (e.g. integer counts), so it needs no "lo" piece:
-// 2 MMAs per k-step instead of 3.  Stages: 4 of 48 KB for the exact-B forms at BM = 128, 3 of 64 KB for them at
-// BM = 192 (24 KB per A piece), 3 of 64 KB for the general form (BM = 128 only).
-template <int BM, int STAGES, bool BEXACT>
+// 2 MMAs per k-step instead of 3.  Stages: 4 of 32 KB + BN * 128 B (48-56 KB) for the exact-B forms, 3 of 64 KB for
+// the general form (BN = 128 only).
+template <int BN, int STAGES, bool BEXACT>
 struct SmemLayout {
-  static constexpr int A_BYTES = BM * BK * 4;              // 16 KB (BM = 128) or 24 KB (BM = 192)
-  static constexpr int B_BYTES = BN * BK * 4;              // 16 KB
+  static constexpr int A_BYTES = BM * BK * 4;              // 16 KB
+  static constexpr int B_BYTES = BN * BK * 4;              // 16 KB (BN = 128) to 24 KB (BN = 192), a multiple of 1 KB
   static constexpr int STAGE_BYTES = 2 * A_BYTES + (BEXACT ? 1 : 2) * B_BYTES;
   static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;  // full[STAGES], empty[STAGES], peer_free[STAGES]
   static constexpr int TOTAL = BAR_OFFSET + 3 * STAGES * 8;
@@ -172,48 +170,44 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// D (64 x 128 fp32, warpgroup fragment) (+)= A (64 x k, smem) * B (128 x k, smem)^T, both K-major; acc = 0: D = A * B^T
-template <bool F16>
-__device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
-  if constexpr (F16) {
-    asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %66, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {"
-      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63 "
-      "}, %64, %65, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(adesc), "l"(bdesc), "r"(acc));
-  } else {
-    asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %66, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {"
-      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63 "
-      "}, %64, %65, p, 1, 1;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(adesc), "l"(bdesc), "r"(acc));
+// D (64 x N fp32, warpgroup fragment) (+)= A (64 x k, smem) * B (N x k, smem)^T, both K-major; acc = 0: D = A * B^T.
+// One wrapper per N: the fragment's N / 2 registers are the asm outputs %0 .. %(N/2 - 1), then the two descriptors and
+// the accumulate flag (at IA, IB, IACC).
+#define CNMF_R64                                                                      \
+  "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "            \
+  "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "  \
+  "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "  \
+  "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+#define CNMF_R84 CNMF_R64 ", %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, " \
+  "%80, %81, %82, %83"
+#define CNMF_R96 CNMF_R84 ", %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95"
+#define CNMF_D4(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3])
+#define CNMF_D8(i) CNMF_D4(i), CNMF_D4(i + 4)
+#define CNMF_D64 CNMF_D8(0), CNMF_D8(8), CNMF_D8(16), CNMF_D8(24), CNMF_D8(32), CNMF_D8(40), CNMF_D8(48), CNMF_D8(56)
+#define CNMF_D84 CNMF_D64, CNMF_D8(64), CNMF_D8(72), CNMF_D4(80)
+#define CNMF_D96 CNMF_D64, CNMF_D8(64), CNMF_D8(72), CNMF_D8(80), CNMF_D8(88)
+#define CNMF_WGMMA(N, REGS, IA, IB, IACC, ...)                                                                        \
+  template <bool F16>                                                                                                 \
+  __device__ __forceinline__ void wgmma_m64n##N(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, uint32_t acc) {    \
+    if constexpr (F16)                                                                                                \
+      asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" IACC ", 0;\n\t"                                          \
+                   "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32.f16.f16 {" REGS "}, %" IA ", %" IB                 \
+                   ", p, 1, 1, 0, 0;\n\t}"                                                                            \
+                   : __VA_ARGS__ : "l"(adesc), "l"(bdesc), "r"(acc));                                                 \
+    else                                                                                                              \
+      asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" IACC ", 0;\n\t"                                          \
+                   "wgmma.mma_async.sync.aligned.m64n" #N "k8.f32.tf32.tf32 {" REGS "}, %" IA ", %" IB ", p, 1, 1;\n\t}" \
+                   : __VA_ARGS__ : "l"(adesc), "l"(bdesc), "r"(acc));                                                 \
   }
+CNMF_WGMMA(128, CNMF_R64, "64", "65", "66", CNMF_D64)
+CNMF_WGMMA(168, CNMF_R84, "84", "85", "86", CNMF_D84)
+CNMF_WGMMA(192, CNMF_R96, "96", "97", "98", CNMF_D96)
+
+template <int BN, bool F16>
+__device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+  if constexpr (BN == 128) wgmma_m64n128<F16>(d, adesc, bdesc, acc);
+  else if constexpr (BN == 168) wgmma_m64n168<F16>(d, adesc, bdesc, acc);
+  else wgmma_m64n192<F16>(d, adesc, bdesc, acc);
 }
 
 // ------------------------------------------------------------------ tile order
@@ -247,19 +241,19 @@ __host__ __device__ __forceinline__ void decode_item(int w, const TileOrder& o, 
 // a k-step still 32 B = 16 elements (wgmma K of f16), so the smem / TMA / descriptor byte geometry is unchanged.
 //
 // Fragment of consumer thread (warp w of its warpgroup, lane l): d[4j + e] is row 16w + l/4 (+8 for e >= 2),
-// column 8j + 2(l%4) + (e & 1) of the warpgroup's 64 x 128 block.
-template <int BM, int STAGES, bool BEXACT, bool F16>
+// column 8j + 2(l%4) + (e & 1) of the warpgroup's 64 x BN block.
+template <int BN, int STAGES, bool BEXACT, bool F16>
 __device__ __forceinline__ void
 gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMap& tmB_hi, const CUtensorMap& tmB_lo,
           float* __restrict__ C, int M, int ldc, long long c_split_stride,
           const TileOrder& ord, int n_tiles, int splits, int total_kb, int kb_per_split, int chain_kb,
           const float* __restrict__ out_scale, const float* __restrict__ a_tile_scale, int a_tiles, int a_gshift) {
   static_assert(!F16 || BEXACT, "the fp16 path exists for exact integer B operands only");
-  static_assert(BM == 128 || BM == 192, "two or three consumer warpgroups");
+  static_assert(BN == 128 || (BEXACT && (BN == 168 || BN == 192)), "wide n-tiles in the exact-B forms only");
   constexpr int NC = BM / 64;                                   // consumer warpgroups
   constexpr int BKE = F16 ? 2 * BK : BK;                        // elements per k-block
   constexpr int KSTEP_BYTES = 32;                               // wgmma K: 8 tf32 or 16 fp16 elements
-  using L = SmemLayout<BM, STAGES, BEXACT>;
+  using L = SmemLayout<BN, STAGES, BEXACT>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;     // SWIZZLE_128B needs 1024 B alignment
 
@@ -286,11 +280,12 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
 
   const int items = ord.m_tiles * ord.n_pairs * splits;
 
-  // 512 threads (BM = 192) get 128 registers each at launch; the producer drops to 32 and the consumers rise to 160
-  // (128 * 32 + 384 * 160 = 65 536).  At 384 threads (BM = 128) everyone keeps the launch-wide 168.
-  constexpr bool REBALANCE = NC == 3;
+  // 384 threads get 168 registers each at launch, enough for BN = 128.  A wider tile's fragment and sums (2 x BN / 2
+  // floats) do not fit that, so the producer drops to 40 and the consumers rise to 232 (128 * 40 + 256 * 232 = 64 512,
+  // what the launch allocates).
+  constexpr bool REBALANCE = BN > 128;
   if (wg == 0) {
-    if constexpr (REBALANCE) setmaxnreg_dec<32>();
+    if constexpr (REBALANCE) setmaxnreg_dec<40>();
     // ===================== TMA producer =====================
     // Both CTAs of the pair need the whole BM-row A panel of the m-tile: each loads its BM/2-row half of A_hi and A_lo
     // once from L2 and multicasts it to the same stage offset in both CTAs; B is the CTA's own n-tile, a local load.
@@ -336,7 +331,7 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
     // tensor pipe.  All walk the same items, so they take the same number of turns; the last warpgroup's hand-off
     // before the first turn and warpgroup 1's sync after the last one pair the ends.  Only the issue time changes, not
     // which MMAs form a chain or the order of the sums.
-    if constexpr (REBALANCE) setmaxnreg_inc<160>();
+    if constexpr (REBALANCE) setmaxnreg_inc<232>();
     constexpr uint32_t TURN_BAR = 1, TURN_THREADS = 256;
     const int cw = wg - 1;                                      // rows [64 cw, 64 cw + 64) of the tile
     const uint32_t a_off = static_cast<uint32_t>(cw * 64 * 128);
@@ -351,15 +346,15 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
       const int kb0 = z * kb_per_split;
       const int kb1 = min(total_kb, kb0 + kb_per_split);
       const int row0 = mt * BM + cw * 64 + warp * 16 + (lane >> 2);   // and row0 + 8
-      float acc[64];
+      float acc[BN / 2];
 #pragma unroll
-      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
       // f16: power-of-two scale of this thread's two A rows for the scale group (2^a_gshift k-blocks) of a chain
       const float* sc_row0 = (F16 && a_tile_scale && row0 < M) ? a_tile_scale + static_cast<long long>(row0) * a_tiles : nullptr;
       const float* sc_row1 = (F16 && a_tile_scale && row0 + 8 < M) ? a_tile_scale + static_cast<long long>(row0 + 8) * a_tiles : nullptr;
       for (int c0 = kb0; c0 < kb1; c0 += chain_kb) {            // one short accumulation chain
         const int c1 = min(kb1, c0 + chain_kb);
-        float d[64];
+        float d[BN / 2];
         int prev = -1;
         for (int kb = c0; kb < c1; ++kb) {
           mbar_wait<false>(full_bar(stage), phase);
@@ -374,9 +369,9 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
           for (int k = 0; k < BK * 4 / KSTEP_BYTES; ++k) {
             const uint64_t koff = static_cast<uint64_t>((k * KSTEP_BYTES) >> 4);   // +32 B per k-step inside the swizzle row
             const uint32_t acc0 = (kb > c0 || k > 0) ? 1u : 0u;
-            wgmma_m64n128<F16>(d, a_lo + koff, b_hi + koff, acc0);     // small terms first
-            if constexpr (!BEXACT) wgmma_m64n128<F16>(d, a_hi + koff, b_lo + koff, 1u);
-            wgmma_m64n128<F16>(d, a_hi + koff, b_hi + koff, 1u);
+            wgmma_tile<BN, F16>(d, a_lo + koff, b_hi + koff, acc0);     // small terms first
+            if constexpr (!BEXACT) wgmma_tile<BN, F16>(d, a_hi + koff, b_lo + koff, 1u);
+            wgmma_tile<BN, F16>(d, a_hi + koff, b_hi + koff, 1u);
           }
           wgmma_commit();
           named_bar_arrive(next_bar, TURN_THREADS);
@@ -393,7 +388,7 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
           const float s0 = sc_row0 ? sc_row0[c0 >> a_gshift] : 1.f;
           const float s1 = sc_row1 ? sc_row1[c0 >> a_gshift] : 1.f;
 #pragma unroll
-          for (int i = 0; i < 64; i += 4) {
+          for (int i = 0; i < BN / 2; i += 4) {
             acc[i] = fmaf(d[i], s0, acc[i]);
             acc[i + 1] = fmaf(d[i + 1], s0, acc[i + 1]);
             acc[i + 2] = fmaf(d[i + 2], s1, acc[i + 2]);
@@ -401,19 +396,20 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
           }
         } else {
 #pragma unroll
-          for (int i = 0; i < 64; ++i) acc[i] += d[i];          // round-to-nearest fp32
+          for (int i = 0; i < BN / 2; ++i) acc[i] += d[i];          // round-to-nearest fp32
         }
       }
       if (nt >= n_tiles) continue;                              // second CTA of a pair past the last n-tile
       // Epilogue: a quad of lanes writes 32 contiguous bytes of a row per instruction (whole sectors).  The column
-      // scales are loaded EPI_J at a time ahead of their stores, so the epilogue waits for 2 load latencies, not for 16
-      // in a row, and fits better under the other warpgroup's last k-block (all 16 at once would need 168 registers
-      // and spill).
-      constexpr int EPI_J = 8;
+      // scales are loaded EPI_J at a time ahead of their stores, so the epilogue waits for 3 or fewer load latencies,
+      // not for BN / 8 in a row, and fits better under the other warpgroup's last k-block (all 16 of a 128-column tile
+      // at once would need 168 registers and spill).  EPI_J divides BN / 8: 8 (BN = 128, 192) or 7 (BN = 168).
+      constexpr int EPI_J = (BN / 8) % 8 == 0 ? 8 : 7;
+      static_assert((BN / 8) % EPI_J == 0, "column groups in whole batches");
       float* cbase = C + static_cast<long long>(z) * c_split_stride;
       const int colq = nt * BN + 2 * (lane & 3);
 #pragma unroll
-      for (int j0 = 0; j0 < 16; j0 += EPI_J) {
+      for (int j0 = 0; j0 < BN / 8; j0 += EPI_J) {
         float2 sc[EPI_J];
 #pragma unroll
         for (int j = 0; j < EPI_J; ++j) {                       // length >= ldc, zero padded
@@ -439,14 +435,14 @@ gemm_body(const CUtensorMap& tmA_hi, const CUtensorMap& tmA_lo, const CUtensorMa
   cluster_sync();                 // neither CTA exits while the peer may still write its shared memory or barriers
 }
 
-template <int BM, int STAGES, bool BEXACT, bool F16>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(num_threads<BM>(), 1)
+template <int BN, int STAGES, bool BEXACT, bool F16>
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NUM_THREADS, 1)
 gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                    const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
                    float* __restrict__ C, int M, int ldc, long long c_split_stride,
                    const TileOrder ord, int n_tiles, int splits, int total_kb, int kb_per_split, int chain_kb,
                    const float* __restrict__ out_scale, const float* __restrict__ a_tile_scale, int a_tiles, int a_gshift) {
-  gemm_body<BM, STAGES, BEXACT, F16>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, C, M, ldc, c_split_stride, ord, n_tiles, splits,
+  gemm_body<BN, STAGES, BEXACT, F16>(tmA_hi, tmA_lo, tmB_hi, tmB_lo, C, M, ldc, c_split_stride, ord, n_tiles, splits,
                                      total_kb, kb_per_split, chain_kb, out_scale, a_tile_scale, a_tiles, a_gshift);
 }
 
@@ -518,7 +514,7 @@ static double order_bytes(int q_tiles, int p_tiles, double q_panel, double p_pan
 
 // The tile order with the least modelled traffic, over both orientations and every balanced group size, with half of
 // the L2 as the budget of the resident panels (the other half holds the streamed operand and the output lines).
-// a_panel: bytes of one 128-row A panel of a slice, b_panel: of the 256 rows of B one n-pair covers, all pieces;
+// a_panel: bytes of one BM-row A panel of a slice, b_panel: of the 2 BN rows of B one n-pair covers, all pieces;
 // grid: the number of pairs (clusters) that run at once.  Ties keep the m-tile-fastest order, which is what a problem
 // whose factor operand fits the L2 gets.  The order decides only which CTA computes a tile when: every output element
 // is still formed by the same chains in the same order.
@@ -541,10 +537,9 @@ static TileOrder pick_tile_order(int m_tiles, int n_pairs, double a_panel, doubl
   return best;
 }
 
-template <int BM, int STAGES, bool BEXACT, bool F16>
+template <int BN, int STAGES, bool BEXACT, bool F16>
 int launch(const GemmArgs& g, cudaStream_t stream) {
-  using L = SmemLayout<BM, STAGES, BEXACT>;
-  constexpr int NUM_THREADS = num_threads<BM>();
+  using L = SmemLayout<BN, STAGES, BEXACT>;
   constexpr int BKE = F16 ? 2 * BK : BK;
   CUtensorMap mAh, mAl, mBh, mBl;
   int rc;
@@ -556,7 +551,9 @@ int launch(const GemmArgs& g, cudaStream_t stream) {
   CNMF_CUDA_CHECK(cudaGetDevice(&dev));
   CNMF_CUDA_CHECK(cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, dev));
   const int m_tiles = (g.M + BM - 1) / BM;
-  const int n_tiles = (g.N + BN - 1) / BN;
+  // The tiles cover the columns up to the next multiple of 32 (ldc permitting) whatever BN is: a 128-column tile
+  // grid always reaches that far, and the padding columns of a row-stride-padded output then hold zeros.
+  const int n_tiles = (std::min(g.ldc, (g.N + 31) / 32 * 32) + BN - 1) / BN;
   const int n_pairs = (n_tiles + 1) / 2;
   const int total_kb = (g.Kd + BKE - 1) / BKE;
   int splits = g.splits < 1 ? 1 : g.splits;
@@ -566,7 +563,7 @@ int launch(const GemmArgs& g, cudaStream_t stream) {
   splits = (total_kb + kb_per_split - 1) / kb_per_split;      // no empty slices
   if (splits != g.splits_effective) { set_last_error("gemm: splits_effective mismatch (use gemm_effective_splits)"); return -1; }
 
-  auto kern = gemm_tf32x3_kernel<BM, STAGES, BEXACT, F16>;
+  auto kern = gemm_tf32x3_kernel<BN, STAGES, BEXACT, F16>;
   // Per device (a second GPU in the same process needs its own calls): the shared-memory attribute, then how many
   // pairs fit at once (66 on a 132-SM H100 SXM).
   static int max_clusters[64] = {};
@@ -619,6 +616,33 @@ int gemm_effective_splits(int Kd, int splits, int f16) {
   return (total_kb + kb_per_split - 1) / kb_per_split;
 }
 
+// Output-tile width of an exact-B product (the general 3-pass form has 128-column tiles only).  The persistent grid
+// runs its pair items in ceil(items / pairs) rounds, and a pair item of a BN-column tile takes about 1.25 (BN = 168)
+// or 1.42 (BN = 192) times as long as a 128-column one, measured on the c3 products (DESIGN.md section 4.1), against
+// the 1.31 and 1.5 of their FLOPs, because the MMAs read less shared memory per FLOP the wider the tile.  So a width
+// costs its rounds times that; a wide width is taken when it saves at least 2 % (near-ties keep 128 columns).
+static int pick_tile_n(const GemmArgs& g) {
+  if (!g.b_exact) return 128;
+  int dev = 0, sms = 0;
+  CNMF_CUDA_CHECK(cudaGetDevice(&dev));
+  CNMF_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const long long pairs = std::max(1, sms / 2);
+  const long long m_items = static_cast<long long>((g.M + BM - 1) / BM) * g.splits_effective;
+  const int cols = std::min(g.ldc, (g.N + 31) / 32 * 32);      // what launch() covers
+  auto cost = [&](int bn, int per_item) {
+    const long long items = m_items * (((cols + bn - 1) / bn + 1) / 2);
+    return (items + pairs - 1) / pairs * per_item;
+  };
+  const long long narrow = cost(128, 100);
+  int best = 128;
+  long long best_cost = narrow * 98 / 100;
+  for (const auto& [bn, per_item] : {std::pair<int, int>{168, 125}, std::pair<int, int>{192, 142}}) {
+    const long long c = cost(bn, per_item);
+    if (c <= best_cost) { best_cost = c; best = bn; }
+  }
+  return best;
+}
+
 int gemm_tf32x3(const GemmArgs& g, cudaStream_t stream) {
   CNMF_REQUIRE(g.M > 0 && g.N > 0 && g.Kd > 0, "gemm: empty problem");
   CNMF_REQUIRE(g.lda % 4 == 0 && g.ldb % 4 == 0 && g.ldc % 4 == 0, "gemm: leading dimensions must be multiples of 4 floats");
@@ -626,18 +650,23 @@ int gemm_tf32x3(const GemmArgs& g, cudaStream_t stream) {
                 reinterpret_cast<uintptr_t>(g.B_hi) | reinterpret_cast<uintptr_t>(g.B_lo) |
                 reinterpret_cast<uintptr_t>(g.C) | reinterpret_cast<uintptr_t>(g.out_col_scale)) % 16 == 0,
                "gemm: pointers must be 16-byte aligned");
-  // Tile height, a shape rule: 192-row tiles (three consumer warpgroups; 17 % less L2 -> shared-memory operand feed
-  // per FLOP) for split-K products of at least 2 048 rows, where they measured 3-6 % faster; 128-row tiles elsewhere,
-  // where the 192-row form measured no faster (one slice) or lost to padding (fewer rows).  Results do not depend on
-  // the choice: every element is formed by the same chains in the same order.
-  const bool tall = g.splits_effective > 1 && g.M >= 2048;
+  // Results do not depend on the tile width: every element is formed by the same chains in the same order.
+  CNMF_REQUIRE(g.tile_n == 0 || g.tile_n == 128 || (g.b_exact && (g.tile_n == 168 || g.tile_n == 192)),
+               "gemm: tile_n must be 0 (the launcher's choice), 128, or 168 / 192 with an exact B");
+  const int bn = g.tile_n ? g.tile_n : pick_tile_n(g);
   if (g.f16) {
     CNMF_REQUIRE(g.b_exact, "gemm: the fp16 path needs an exact B operand");
     CNMF_REQUIRE(g.lda % 8 == 0 && g.ldb % 8 == 0, "gemm: fp16 leading dimensions must be multiples of 8 halves");
     CNMF_REQUIRE(!g.a_tile_scale || g.a_tiles * 512 >= g.Kd, "gemm: a_tiles does not cover the reduction length");
-    return tall ? launch<192, 3, true, true>(g, stream) : launch<128, 4, true, true>(g, stream);
+    if (bn == 168) return launch<168, 4, true, true>(g, stream);
+    if (bn == 192) return launch<192, 4, true, true>(g, stream);
+    return launch<128, 4, true, true>(g, stream);
   }
-  if (g.b_exact) return tall ? launch<192, 3, true, false>(g, stream) : launch<128, 4, true, false>(g, stream);
+  if (g.b_exact) {
+    if (bn == 168) return launch<168, 4, true, false>(g, stream);
+    if (bn == 192) return launch<192, 4, true, false>(g, stream);
+    return launch<128, 4, true, false>(g, stream);
+  }
   return launch<128, 3, false, false>(g, stream);
 }
 

@@ -244,10 +244,12 @@ class Engine:
         return int(peak.value)
 
     def gemm_abt(self, A, B, precision=PRECISION_TF32X3, splits=1, reps=1, b_exact=False, k_scale=None,
-                 out_col_scale=None):
+                 out_col_scale=None, tile_n=0):
         """C = A @ B.T through the solver's GEMM kernels (test / micro-benchmark hook).  The exact-count forms:
         b_exact (tf32x3; implied by f16x2) takes B as exact tf32 values, and then C = A diag(k_scale) B^T
-        diag(out_col_scale) with the scales applied where the solver applies a dataset's (either may be None)."""
+        diag(out_col_scale) with the scales applied where the solver applies a dataset's (either may be None).
+        tile_n: columns per output tile, 0 = the launcher's choice by shape; 128, or 168 / 192 in the exact forms,
+        forces that width."""
         A, B = f32c(A), f32c(B)
         M, Kd = A.shape
         N = B.shape[0]
@@ -261,7 +263,7 @@ class Engine:
         pc = precision_code(precision)
         pc = PRECISION_TF32X3 if pc == PRECISION_TF32X3_GENERAL else pc      # f16x2: B must hold integers <= 2048
         check(self.lib.cnmf_gemm_abt_host(self._h, pc, ptr(A), ptr(B), M, N, Kd, splits, 1 if b_exact else 0,
-                                          ptr(ks), ptr(cs), ptr(C), reps, ctypes.byref(ms), None))
+                                          ptr(ks), ptr(cs), int(tile_n), ptr(C), reps, ctypes.byref(ms), None))
         return C, float(ms.value)
 
     def update_step(self, ks, rids, done, n, F, num, gram_in, solver="mu", pieces=None, gram=None, want_scalar=False,

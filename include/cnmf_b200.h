@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define CNMF_B200_ABI_VERSION 14
+#define CNMF_B200_ABI_VERSION 15
 #define CNMF_MAX_COMPONENTS 32          /* largest n_components per restart on the CUDA path */
 
 typedef struct cnmf_handle_s* cnmf_handle_t;
@@ -276,10 +276,12 @@ int cnmf_project_rows(cnmf_dataset_t d, int k, const float* Ut_host, float* out_
  * The exact-count forms the solver runs on scaled-integer datasets: b_exact = 1 (tf32x3; implied by f16x2) takes B as
  * exact tf32 values (2 passes, no lo piece of B); then k_scale (length Kd, or NULL) is folded into the A pieces as the
  * solver folds the dataset's scale, A diag(k_scale), and out_col_scale (length N, or NULL) multiplies column n of C:
- * C = A diag(k_scale) B^T diag(out_col_scale).  The scales are refused without the exact form. */
+ * C = A diag(k_scale) B^T diag(out_col_scale).  The scales are refused without the exact form.
+ * tile_n: columns per output tile, 0 = chosen by shape as in the solver; 128, or 168 / 192 in the exact forms, forces
+ * that width (the result does not depend on it). */
 int cnmf_gemm_abt_host(cnmf_handle_t h, int precision, const float* A, const float* B, int M, int N, int Kd,
-                       int splits, int b_exact, const float* k_scale, const float* out_col_scale, float* C, int reps,
-                       float* ms_out, void* stream);
+                       int splits, int b_exact, const float* k_scale, const float* out_col_scale, int tile_n, float* C,
+                       int reps, float* ms_out, void* stream);
 
 /* test hook: ONE update launch of the batched solver (or the stand-alone Gram / <NUM, F> / piece launches that start a
  * solve) on host-supplied packed data, issued exactly as the solver issues it.  Slot s holds restart rids[s] with
