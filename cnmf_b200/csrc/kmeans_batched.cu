@@ -13,8 +13,13 @@
 // An empty cluster (sklearn's relocation rule, _k_means_common.pyx:167-211) is reported to the caller, which then runs
 // the per-run host-assisted path (cnmf_kmeans_step): it is rare and not worth a device implementation.
 //
-// Numerics are those of the per-run path this replaces (same kernels' arithmetic, same summation orders), so labels and
-// inertia are bit-identical to it -- and labels equal scikit-learn's on the parity fixtures.
+// The E step, the member-order centre sums, the centre update and the stopping rule have the arithmetic and summation
+// orders of the per-run path (cnmf_kmeans_step), so from the same k-means++ centres every run's labels, centres and
+// iteration count are those of the per-run path, and labels equal scikit-learn's on the parity fixtures.  Two sums are
+// associated differently, so they agree to rounding, not bit for bit: the candidate potentials (here blocks of 8 rows,
+// then the blocks in order; there host dot products) and the inertia (here 256 threads per run; there sum_kernel's one
+// block of 1024).  A potential that differs in its last bits can move a k-means++ draw only when a uniform lands within
+// those bits of a cumulative-sum boundary.
 #include <algorithm>
 #include <chrono>
 #include <cstring>
@@ -453,20 +458,26 @@ int kmeans_fit(cnmf_handle_t h, const T* S_dev, int R, int G, int ld, int K, int
     if (K > 1) CNMF_CUDA_CHECK(cudaMemcpyAsync(d_unif, uniforms_host, n_unif * 8, cudaMemcpyHostToDevice, s));
     CNMF_CUDA_CHECK(cudaStreamSynchronize(s));          // cidx goes out of scope
   }
+  // The select kernel keeps `closest` in dynamic shared memory.  Without an opt-in a launch may use at most 48 KB minus
+  // the kernel's static shared memory (cpot, s_best), so the limit is read from the function rather than assumed.
   const size_t sel_smem = (size_t)R * sizeof(double);
-  static bool sel_attr[64] = {};
-  if (sel_smem > 48 * 1024 && !sel_attr[h->device & 63]) {
+  cudaFuncAttributes sel_fa;
+  CNMF_CUDA_CHECK(cudaFuncGetAttributes(&sel_fa, kpp_select_kernel<T>));
+  if (sel_smem > (size_t)sel_fa.maxDynamicSharedSizeBytes)
     CNMF_CUDA_CHECK(cudaFuncSetAttribute(kpp_select_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    sel_attr[h->device & 63] = true;
-  }
+  // each select launch is checked at once: a refused launch raises before the next centre's eval reads candidates it
+  // never wrote
   const dim3 eval_grid(row_blocks, n_init);
   kpp_eval_kernel<T, 8><<<eval_grid, 256, 0, s>>>(st, 1);
   kpp_select_kernel<T><<<n_init, 256, sel_smem, s>>>(st, 0);
+  CNMF_CUDA_CHECK(cudaGetLastError());
   for (int step = 1; step < K; ++step) {
     kpp_eval_kernel<T, 8><<<eval_grid, 256, 0, s>>>(st, 0);
     kpp_select_kernel<T><<<n_init, 256, sel_smem, s>>>(st, step);
+    CNMF_CUDA_CHECK(cudaGetLastError());
   }
   kpp_gather_centres_kernel<T><<<dim3(K, n_init), 256, 0, s>>>(st, C64, CE);
+  CNMF_CUDA_CHECK(cudaGetLastError());
   h->launches += 2 * K + 1;
 
   if (h->profile) {                 // phase timing for bench / probes (cnmf_last_timing: rng = seeding, solve = Lloyd)

@@ -80,6 +80,34 @@ def test_kmeans_restatement_matches_sklearn():
     assert np.allclose(centers, km.cluster_centers_, atol=1e-12)
 
 
+@pytest.mark.parametrize("k,n_init,seed", [(1, 3, 0), (2, 10, 1), (5, 10, 2), (7, 4, 3)])
+def test_kmeans_device_order_restatement_matches_sklearn(k, n_init, seed):
+    """oracle/kmeans_device_ref.py (the batched fit in the device's order) in float64 against scikit-learn: every run's
+    k-means++ centre indices equal kmeans_plusplus' from the same RandomState stream, and the best run's labels equal
+    KMeans'.  Overlapping blobs, so Lloyd takes several iterations; no E-step decision is within 1e-9 of a tie."""
+    from sklearn.cluster import KMeans, kmeans_plusplus
+    from cnmf_b200.consensus import _kmeans_draws
+    from oracle import kmeans_device_ref as kd
+    rng = np.random.RandomState(40 + seed)
+    centres = rng.rand(max(k, 2) + 1, 12)
+    X = np.vstack([c + 0.25 * rng.randn(60, 12) for c in centres])
+    first, unif, n_trials = _kmeans_draws(np.random.RandomState(seed), X.shape[0], k, n_init)
+    tol_abs = float(np.var(X, axis=0).mean()) * 1e-4
+    runs = kd.kmeans_fit(X, k, first, unif, n_trials, 300, tol_abs)
+    sk_rng = np.random.RandomState(seed)
+    for r in runs:
+        _, idx = kmeans_plusplus(X, k, random_state=sk_rng)
+        assert np.array_equal(r["centre_idx"], idx)
+        assert r["min_gap"] > 1e-9 and not r["empty"]
+    assert len({r["n_iter"] for r in runs}) > 1 or n_init == 1 or k == 1
+    with warnings.catch_warnings():
+        warnings.simplefilter("ignore")
+        km = KMeans(n_clusters=k, n_init=n_init, random_state=seed).fit(X)
+    best = kd.best_run(runs, k)
+    assert np.array_equal(best["labels"], km.labels_)
+    assert abs(best["inertia"] - km.inertia_) <= 1e-10 * km.inertia_
+
+
 def test_distance_and_density_match_sklearn():
     from sklearn.metrics.pairwise import euclidean_distances
     rng = np.random.RandomState(0)
