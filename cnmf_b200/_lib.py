@@ -64,6 +64,31 @@ class BetaStepArgs(ctypes.Structure):
                 ("oth_sum", ctypes.c_void_p), ("last", ctypes.c_void_p), ("totals", ctypes.c_void_p)]
 
 
+UNIT_F64_UPDATE, UNIT_F64_GRAM, UNIT_F64_CROSS = 0, 1, 2
+
+
+class UpdateStepF64Args(ctypes.Structure):
+    """struct cnmf_update_step_f64_args (include/cnmf_b200.h): arguments of the cnmf_update_step_f64_host test hook."""
+    _fields_ = [("n_slots", ctypes.c_int32), ("n_rids", ctypes.c_int32),
+                ("ks", ctypes.c_void_p), ("rids", ctypes.c_void_p), ("done", ctypes.c_void_p),
+                ("n", ctypes.c_int32), ("op", ctypes.c_int32), ("solver", ctypes.c_int32),
+                ("want_scalar", ctypes.c_int32), ("l1", ctypes.c_double), ("l2", ctypes.c_double),
+                ("F", ctypes.c_void_p), ("num", ctypes.c_void_p), ("gram_in", ctypes.c_void_p),
+                ("gram_out", ctypes.c_void_p), ("scal_out", ctypes.c_void_p)]
+
+
+class ConvCheckArgs(ctypes.Structure):
+    """struct cnmf_conv_check_args (include/cnmf_b200.h): arguments of the cnmf_conv_check_host test hook."""
+    _fields_ = [("n_slots", ctypes.c_int32), ("n_rids", ctypes.c_int32),
+                ("ks", ctypes.c_void_p), ("rids", ctypes.c_void_p),
+                ("solver", ctypes.c_int32), ("it", ctypes.c_int32), ("max_iter", ctypes.c_int32),
+                ("tol", ctypes.c_double), ("normX2", ctypes.c_double),
+                ("cross", ctypes.c_void_p), ("gramA", ctypes.c_void_p), ("gramB", ctypes.c_void_p),
+                ("violA", ctypes.c_void_p), ("violB", ctypes.c_void_p),
+                ("done", ctypes.c_void_p), ("n_iter", ctypes.c_void_p),
+                ("err0", ctypes.c_void_p), ("prev", ctypes.c_void_p), ("last", ctypes.c_void_p)]
+
+
 _c = ctypes
 _vp, _i, _ll, _d = _c.c_void_p, _c.c_int, _c.c_longlong, _c.c_double
 _pp = _c.POINTER
@@ -120,6 +145,8 @@ SIGNATURES = {
     "cnmf_gemm_abt_host": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp, _i, _pp(_c.c_float), _vp]),
     "cnmf_update_step_host": (_i, [_vp, _pp(UpdateStepArgs), _vp]),
     "cnmf_beta_step_host": (_i, [_vp, _pp(BetaStepArgs), _vp]),
+    "cnmf_update_step_f64_host": (_i, [_vp, _pp(UpdateStepF64Args), _vp]),
+    "cnmf_conv_check_host": (_i, [_vp, _pp(ConvCheckArgs), _vp]),
     "cnmf_l2_normalize_rows": (_i, [_vp, _vp, _i, _i, _i, _vp]),
     "cnmf_local_density": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     "cnmf_col_stats_dev": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
@@ -145,7 +172,7 @@ SIGNATURES = {
 _lib = None
 
 
-ABI_VERSION = 15     # include/cnmf_b200.h CNMF_B200_ABI_VERSION
+ABI_VERSION = 16     # include/cnmf_b200.h CNMF_B200_ABI_VERSION
 
 
 def load():

@@ -1,12 +1,14 @@
 // Test hooks of the C ABI: one launch of the batched solver's update / Gram / <NUM, F> / piece kernels on host data
 // (cnmf_update_step_host, include/cnmf_b200.h).  It builds the FactorView / BatchMeta / FusedOut the solver builds
 // (nmf_engine.cu) and calls the same launch_* functions; no kernel code of its own.  cnmf_beta_step_host does the same
-// for the KL / IS solver (nmf_beta.cu).
+// for the KL / IS solver (nmf_beta.cu), cnmf_update_step_f64_host for the float64 solver (nmf_f64.cu), and
+// cnmf_conv_check_host runs the convergence kernels every solver shares.
 #include <algorithm>
 #include <vector>
 
 #include "engine.h"
 #include "nmf_beta.h"
+#include "nmf_f64.h"
 #include "nmf_kernels.cuh"
 
 using namespace cnmf;
@@ -245,6 +247,150 @@ extern "C" int cnmf_beta_step_host(cnmf_handle_t h, const cnmf_beta_step_args* a
     }
     a->totals[2 * r] = t;
     a->totals[2 * r + 1] = sx;
+  }
+  return 0;
+}
+
+// the slot tables of a unit launch: meta = off | k | rid per slot, done per rid; returns SK and kmax
+static int unit_slots(const int32_t* ks, const int32_t* rids, const int32_t* done, int R, int NR, const char* what,
+                      std::vector<int>& meta, int* SK, int* kmax) {
+  meta.assign(3 * R + NR, 0);
+  std::vector<char> seen(NR, 0);
+  *SK = *kmax = 0;
+  for (int s = 0; s < R; ++s) {
+    if (ks[s] < 1 || ks[s] > KMAX) {
+      set_last_error(std::string("invalid argument: ") + what + ": ks must be in [1, 32]");
+      return -1;
+    }
+    if (rids[s] < 0 || rids[s] >= NR || seen[rids[s]]) {
+      set_last_error(std::string("invalid argument: ") + what + ": rids must be distinct and < n_rids");
+      return -1;
+    }
+    seen[rids[s]] = 1;
+    meta[s] = *SK;
+    meta[R + s] = ks[s];
+    meta[2 * R + s] = rids[s];
+    *SK += ks[s];
+    *kmax = std::max(*kmax, ks[s]);
+  }
+  for (int r = 0; r < NR; ++r) meta[3 * R + r] = done ? done[r] : 0;
+  return 0;
+}
+
+// cnmf_update_step_f64_host: one launch of the float64 solver through its own f64_update / f64_gram / f64_cross, with
+// the partial-Gram stride the solver sets (kp = kmax rounded up to 4)
+extern "C" int cnmf_update_step_f64_host(cnmf_handle_t h, const cnmf_update_step_f64_args* a, void* stream) {
+  CNMF_REQUIRE(h && a && a->ks && a->rids && a->done && a->F, "update_step_f64: NULL argument");
+  CNMF_REQUIRE(a->n_slots >= 1 && a->n_rids >= 1 && a->n >= 1, "update_step_f64: bad sizes");
+  CNMF_REQUIRE(a->op == CNMF_UNIT_F64_UPDATE || a->op == CNMF_UNIT_F64_GRAM || a->op == CNMF_UNIT_F64_CROSS,
+               "update_step_f64: unknown op");
+  const bool upd = a->op == CNMF_UNIT_F64_UPDATE;
+  CNMF_REQUIRE(!upd || a->solver == CNMF_SOLVER_MU || a->solver == CNMF_SOLVER_CD, "update_step_f64: unknown solver");
+  CNMF_REQUIRE(!upd || (a->num && a->gram_in), "update_step_f64: num / gram_in missing");
+  CNMF_REQUIRE(a->op != CNMF_UNIT_F64_CROSS || (a->num && a->scal_out), "update_step_f64: num / scal_out missing");
+  CNMF_REQUIRE(a->op != CNMF_UNIT_F64_GRAM || a->gram_out, "update_step_f64: gram_out missing");
+  CNMF_REQUIRE(!(upd && a->want_scalar) || a->scal_out, "update_step_f64: scal_out missing");
+  const int R = a->n_slots, NR = a->n_rids;
+  std::vector<int> meta;
+  int SK = 0, kmax = 0;
+  CNMF_TRY(unit_slots(a->ks, a->rids, a->done, R, NR, "update_step_f64", meta, &SK, &kmax));
+  const int kp = round_up(kmax, 4);
+
+  cudaStream_t s = as_stream(stream);
+  CNMF_CUDA_CHECK(cudaSetDevice(h->device));
+  const int n = a->n, ld = pad_ld(n);
+  const size_t nf = (size_t)SK * ld, gsz = (size_t)NR * KMAX * KMAX;
+  const int chunks = f64_chunks(n), gchunks = f64_gram_chunks(n);
+  int* d_meta = static_cast<int*>(h->dev_buf("unit.meta", sizeof(int) * meta.size()));
+  double* d_F = static_cast<double*>(h->dev_buf("unit.F64", nf * 8));
+  double* d_num = static_cast<double*>(h->dev_buf("unit.num64", nf * 8));
+  double* d_gin = static_cast<double*>(h->dev_buf("unit.gram_in", sizeof(double) * gsz));
+  double* d_gout = static_cast<double*>(h->dev_buf("unit.gram_out", sizeof(double) * gsz));
+  double* d_scal = static_cast<double*>(h->dev_buf("unit.scal", sizeof(double) * NR));
+  double* d_gpart = static_cast<double*>(h->dev_buf("unit.gram_part", sizeof(double) * (size_t)NR * gchunks * kp * kp));
+  double* d_spart = static_cast<double*>(h->dev_buf("unit.scal_part", sizeof(double) * (size_t)NR * chunks));
+  if (!d_meta || !d_F || !d_num || !d_gin || !d_gout || !d_scal || !d_gpart || !d_spart) return -2;
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(d_meta, meta.data(), sizeof(int) * meta.size(), cudaMemcpyHostToDevice, s));
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(d_F, a->F, nf * 8, cudaMemcpyHostToDevice, s));
+  if (a->num) CNMF_CUDA_CHECK(cudaMemcpyAsync(d_num, a->num, nf * 8, cudaMemcpyHostToDevice, s));
+  if (a->gram_in) CNMF_CUDA_CHECK(cudaMemcpyAsync(d_gin, a->gram_in, sizeof(double) * gsz, cudaMemcpyHostToDevice, s));
+  if (a->gram_out) CNMF_CUDA_CHECK(cudaMemcpyAsync(d_gout, a->gram_out, sizeof(double) * gsz, cudaMemcpyHostToDevice, s));
+  if (a->scal_out) CNMF_CUDA_CHECK(cudaMemcpyAsync(d_scal, a->scal_out, sizeof(double) * NR, cudaMemcpyHostToDevice, s));
+
+  const BatchMeta b{d_meta, d_meta + R, d_meta + 2 * R, d_meta + 3 * R, R, kp};
+  const F64Launch L{h, s, SK};
+  const F64View f{d_F, n, ld};
+  if (upd)
+    CNMF_TRY(f64_update(L, a->solver == CNMF_SOLVER_CD, f, d_num, d_gin, b, a->l1, a->l2, d_spart,
+                        a->want_scalar ? d_scal : nullptr));
+  else if (a->op == CNMF_UNIT_F64_GRAM)
+    CNMF_TRY(f64_gram(L, f, b, d_gpart, d_gout));
+  else
+    CNMF_TRY(f64_cross(L, f, d_num, b, d_spart, d_scal));
+
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(a->F, d_F, nf * 8, cudaMemcpyDeviceToHost, s));
+  if (a->gram_out) CNMF_CUDA_CHECK(cudaMemcpyAsync(a->gram_out, d_gout, sizeof(double) * gsz, cudaMemcpyDeviceToHost, s));
+  if (a->scal_out) CNMF_CUDA_CHECK(cudaMemcpyAsync(a->scal_out, d_scal, sizeof(double) * NR, cudaMemcpyDeviceToHost, s));
+  CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
+  return 0;
+}
+
+// cnmf_conv_check_host: one mu_check_kernel / cd_check_kernel launch (launch_mu_check / launch_cd_check) on host state;
+// the state's done array is also the batch's, as in the solvers
+extern "C" int cnmf_conv_check_host(cnmf_handle_t h, const cnmf_conv_check_args* a, void* stream) {
+  CNMF_REQUIRE(h && a && a->ks && a->rids && a->done && a->n_iter && a->err0 && a->prev && a->last,
+               "conv_check: NULL argument");
+  CNMF_REQUIRE(a->n_slots >= 1 && a->n_rids >= 1, "conv_check: bad sizes");
+  CNMF_REQUIRE(a->solver == CNMF_SOLVER_MU || a->solver == CNMF_SOLVER_CD, "conv_check: unknown solver");
+  const bool mu = a->solver == CNMF_SOLVER_MU;
+  CNMF_REQUIRE(!mu || (a->cross && a->gramA && a->gramB), "conv_check: cross / gramA / gramB missing");
+  CNMF_REQUIRE(mu || a->violA, "conv_check: violA missing");
+  const int R = a->n_slots, NR = a->n_rids;
+  std::vector<int> meta;
+  int SK = 0, kmax = 0;
+  CNMF_TRY(unit_slots(a->ks, a->rids, nullptr, R, NR, "conv_check", meta, &SK, &kmax));
+  meta.resize(3 * R + 2 * NR);
+  for (int r = 0; r < NR; ++r) {
+    meta[3 * R + r] = a->done[r];
+    meta[3 * R + NR + r] = a->n_iter[r];
+  }
+
+  cudaStream_t s = as_stream(stream);
+  CNMF_CUDA_CHECK(cudaSetDevice(h->device));
+  const size_t gsz = (size_t)NR * KMAX * KMAX;
+  int* d_meta = static_cast<int*>(h->dev_buf("unit.meta", sizeof(int) * meta.size()));
+  double* d_state = static_cast<double*>(h->dev_buf("unit.conv_state", sizeof(double) * 6 * NR));
+  double* d_gram = static_cast<double*>(h->dev_buf("unit.conv_gram", sizeof(double) * 2 * gsz));
+  if (!d_meta || !d_state || !d_gram) return -2;
+  double *d_err0 = d_state, *d_prev = d_state + NR, *d_last = d_state + 2 * NR;
+  double *d_x = d_state + 3 * NR, *d_vb = d_state + 4 * NR;
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(d_meta, meta.data(), sizeof(int) * meta.size(), cudaMemcpyHostToDevice, s));
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(d_err0, a->err0, sizeof(double) * NR, cudaMemcpyHostToDevice, s));
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(d_prev, a->prev, sizeof(double) * NR, cudaMemcpyHostToDevice, s));
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(d_last, a->last, sizeof(double) * NR, cudaMemcpyHostToDevice, s));
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(d_x, mu ? a->cross : a->violA, sizeof(double) * NR, cudaMemcpyHostToDevice, s));
+  if (mu) {
+    CNMF_CUDA_CHECK(cudaMemcpyAsync(d_gram, a->gramA, sizeof(double) * gsz, cudaMemcpyHostToDevice, s));
+    CNMF_CUDA_CHECK(cudaMemcpyAsync(d_gram + gsz, a->gramB, sizeof(double) * gsz, cudaMemcpyHostToDevice, s));
+  } else if (a->violB) {
+    CNMF_CUDA_CHECK(cudaMemcpyAsync(d_vb, a->violB, sizeof(double) * NR, cudaMemcpyHostToDevice, s));
+  }
+
+  int* d_done = d_meta + 3 * R;
+  const BatchMeta b{d_meta, d_meta + R, d_meta + 2 * R, d_done, R, round_up(kmax, 4)};
+  const ConvState st{d_err0, d_prev, d_last, d_done, d_done + NR};
+  h->launches += 1;
+  if (mu) CNMF_TRY(launch_mu_check(st, d_x, d_gram, d_gram + gsz, a->normX2, b, a->it, a->tol, a->max_iter, s));
+  else CNMF_TRY(launch_cd_check(st, d_x, a->violB ? d_vb : nullptr, b, a->it, a->tol, a->max_iter, s));
+
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(meta.data(), d_meta, sizeof(int) * meta.size(), cudaMemcpyDeviceToHost, s));
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(a->err0, d_err0, sizeof(double) * NR, cudaMemcpyDeviceToHost, s));
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(a->prev, d_prev, sizeof(double) * NR, cudaMemcpyDeviceToHost, s));
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(a->last, d_last, sizeof(double) * NR, cudaMemcpyDeviceToHost, s));
+  CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
+  for (int r = 0; r < NR; ++r) {
+    a->done[r] = meta[3 * R + r];
+    a->n_iter[r] = meta[3 * R + NR + r];
   }
   return 0;
 }

@@ -17,23 +17,15 @@
 #include <cmath>
 #include <cstring>
 
-#include "engine.h"
-#include "nmf_kernels.cuh"
+#include "nmf_f64.h"
 
 namespace cnmf {
 
 namespace {
 
-constexpr int F64_THREADS = 256;
-constexpr int F64_ITEMS = F64_THREADS;      // items per block of the update / cross kernels (one per thread)
-constexpr int F64_GRAM_COLS = 2048;         // items per block of the Gram kernel
+constexpr int F64_THREADS = F64_ITEMS;      // one item per thread in the update / cross kernels
 constexpr int F64_GRAM_TILE = 64;           // items staged in shared memory per pass of the Gram kernel
 constexpr double EPSILON_F32_D = 1.1920928955078125e-07;   // np.finfo(np.float32).eps, sklearn _nmf.py:32
-
-struct F64View {
-  double* F;       // SK x ld
-  int n, ld;
-};
 
 // fixed-tree block sum of one value per thread (F64_THREADS threads); the result is valid in thread 0
 __device__ __forceinline__ double block_sum(double v, double* red) {
@@ -249,6 +241,37 @@ __global__ void sums64_final_kernel(const double* __restrict__ part, int nblocks
 
 }  // namespace
 
+int f64_gram(const F64Launch& L, const F64View& f, const BatchMeta& b, double* part, double* gram) {
+  const int gch = f64_gram_chunks(f.n);
+  gram64_kernel<<<dim3(gch, b.R), F64_THREADS, 0, L.s>>>(f, b, part);
+  CNMF_CUDA_CHECK(cudaGetLastError());
+  L.h->launches += 2;
+  return launch_finalize(part, gram, nullptr, nullptr, gch, b, L.s);
+}
+
+int f64_cross(const F64Launch& L, const F64View& f, const double* NUM, const BatchMeta& b, double* part, double* out) {
+  const int ch = f64_chunks(f.n);
+  cross64_kernel<<<dim3(ch, b.R), F64_THREADS, 0, L.s>>>(f, NUM, b, part);
+  CNMF_CUDA_CHECK(cudaGetLastError());
+  L.h->launches += 2;
+  return launch_finalize(nullptr, nullptr, part, out, ch, b, L.s);
+}
+
+int f64_update(const F64Launch& L, bool cd, const F64View& f, const double* NUM, const double* gram_in,
+               const BatchMeta& b, double l1, double l2, double* part, double* scal) {
+  const int ch = f64_chunks(f.n);
+  if (!scal) part = nullptr;
+  L.h->launches += 1;
+  const int slot = L.h->prof_begin(L.s, 8.0 * (double)L.SK * (double)f.n * 3.0, 1);
+  if (!cd) update64_kernel<false><<<dim3(ch, b.R), F64_THREADS, 0, L.s>>>(f, NUM, gram_in, b, l1, l2, part);
+  else update64_kernel<true><<<dim3(ch, b.R), F64_THREADS, 0, L.s>>>(f, NUM, gram_in, b, l1, l2, part);
+  L.h->prof_end(L.s, slot);
+  CNMF_CUDA_CHECK(cudaGetLastError());
+  if (!scal) return 0;
+  L.h->launches += 1;
+  return launch_finalize(nullptr, nullptr, part, scal, ch, b, L.s);
+}
+
 int matrix_sums_f64(cnmf_handle_s* h, const double* X, int rows, int cols, int ld, double* out_host, cudaStream_t s) {
   const int rpb = 64;
   const int nb = (rows + rpb - 1) / rpb;
@@ -300,9 +323,8 @@ int solve_batched_f64(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cn
     }
     return pos;
   };
-  // chunkings: functions of the item counts only
-  const int chunks_r = (v.n_r + F64_ITEMS - 1) / F64_ITEMS, chunks_c = (v.n_c + F64_ITEMS - 1) / F64_ITEMS;
-  const int gchunks_r = (v.n_r + F64_GRAM_COLS - 1) / F64_GRAM_COLS, gchunks_c = (v.n_c + F64_GRAM_COLS - 1) / F64_GRAM_COLS;
+  const int chunks_r = f64_chunks(v.n_r), chunks_c = f64_chunks(v.n_c);
+  const int gchunks_r = f64_gram_chunks(v.n_r), gchunks_c = f64_gram_chunks(v.n_c);
   const int chunks_cap = std::max(chunks_r, chunks_c), gchunks_cap = std::max(gchunks_r, gchunks_c);
 
   // ---- workspace
@@ -352,36 +374,18 @@ int solve_batched_f64(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cn
   auto fr = [&]() { return F64View{wFr, v.n_r, v.ld_r}; };
   auto fc = [&]() { return F64View{wFc, v.n_c, v.ld_c}; };
 
+  auto L = [&]() { return F64Launch{h, s, SK}; };
+
   auto gram = [&](const F64View& f, int side_is_c, const BatchMeta& b) -> int {
-    const int gch = side_is_c ? gchunks_c : gchunks_r;
-    double* part = side_is_c ? d_gpartC : d_gpartR;
-    gram64_kernel<<<dim3(gch, b.R), F64_THREADS, 0, s>>>(f, b, part);
-    CNMF_CUDA_CHECK(cudaGetLastError());
-    h->launches += 2;
-    return launch_finalize(part, side_is_c ? d_gramC : d_gramR, nullptr, nullptr, gch, b, s);
+    return f64_gram(L(), f, b, side_is_c ? d_gpartC : d_gpartR, side_is_c ? d_gramC : d_gramR);
   };
   auto cross = [&](const F64View& f, const double* NUM, int side_is_c, double* out, const BatchMeta& b) -> int {
-    const int ch = side_is_c ? chunks_c : chunks_r;
-    double* part = side_is_c ? d_scalB : d_scalA;
-    cross64_kernel<<<dim3(ch, b.R), F64_THREADS, 0, s>>>(f, NUM, b, part);
-    CNMF_CUDA_CHECK(cudaGetLastError());
-    h->launches += 2;
-    return launch_finalize(nullptr, nullptr, part, out, ch, b, s);
+    return f64_cross(L(), f, NUM, b, side_is_c ? d_scalB : d_scalA, out);
   };
   // update of one factor; scal (optional) receives MU <NUM, F_new> / CD sum |projected gradient| per restart
   auto update = [&](const F64View& f, const double* NUM, int side_is_c, const double* gram_in, double l1, double l2,
                     double* scal) -> int {
-    const int ch = side_is_c ? chunks_c : chunks_r;
-    double* part = scal ? (side_is_c ? d_scalB : d_scalA) : nullptr;
-    h->launches += 1;
-    const int slot = h->prof_begin(s, 8.0 * (double)SK * (double)f.n * 3.0, 1);
-    if (mu) update64_kernel<false><<<dim3(ch, R), F64_THREADS, 0, s>>>(f, NUM, gram_in, bm(), l1, l2, part);
-    else update64_kernel<true><<<dim3(ch, R), F64_THREADS, 0, s>>>(f, NUM, gram_in, bm(), l1, l2, part);
-    h->prof_end(s, slot);
-    CNMF_CUDA_CHECK(cudaGetLastError());
-    if (!scal) return 0;
-    h->launches += 1;
-    return launch_finalize(nullptr, nullptr, part, scal, ch, bm(), s);
+    return f64_update(L(), !mu, f, NUM, gram_in, bm(), l1, l2, side_is_c ? d_scalB : d_scalA, scal);
   };
   // NUM_r = Fc * X^T over the row items (reduction over n_c); NUM_c = Fr * X over the column items
   auto gemm = [&](bool rows) -> int {

@@ -633,7 +633,7 @@ int cnmf_nndsvd_chunk_limit(cnmf_handle_t h, int max_restarts) {
 
 int cnmf_nndsvd_gemm_host(cnmf_dataset_t d, int to_genes, int M, const double* A_host, double* C_host, void* stream) {
   CNMF_REQUIRE(d && A_host && C_host && M > 0, "nndsvd_gemm_host: bad arguments");
-  CNMF_TRY(require_dense(d, "nndsvd_gemm_host"));
+  if (d->sparse) CNMF_TRY(require_dense(d, "nndsvd_gemm_host"));
   CNMF_CUDA_CHECK(cudaSetDevice(d->h->device));
   cudaStream_t s = as_stream(stream);
   const int n_in = to_genes ? d->n_rows : d->n_cols, ld_in = to_genes ? d->ld_r : d->ld_c;
@@ -642,10 +642,15 @@ int cnmf_nndsvd_gemm_host(cnmf_dataset_t d, int to_genes, int M, const double* A
   CNMF_CUDA_CHECK(cudaMalloc(&a.p, (size_t)M * ld_in * 8));
   CNMF_CUDA_CHECK(cudaMalloc(&c.p, (size_t)M * ld_out * 8));
   CNMF_CUDA_CHECK(cudaMemsetAsync(a.p, 0, (size_t)M * ld_in * 8, s));
+  CNMF_CUDA_CHECK(cudaMemsetAsync(c.p, 0xff, (size_t)M * ld_out * 8, s));   // NaN pattern: unwritten outputs show up
   CNMF_CUDA_CHECK(cudaMemcpy2DAsync(a.p, (size_t)ld_in * 8, A_host, (size_t)n_in * 8, (size_t)n_in * 8, M,
                                     cudaMemcpyHostToDevice, s));
-  CNMF_TRY(launch_gemm_f64(static_cast<double*>(a.p), ld_in, M, d->X, d->n_rows, d->n_cols, d->ld_c, to_genes != 0,
-                           static_cast<double*>(c.p), ld_out, s));
+  const double* A = static_cast<double*>(a.p);
+  double* C = static_cast<double*>(c.p);
+  if (d->form == Form::FP64)     // float64 dataset: the <*, double> instantiation the float64 solver runs, on X64
+    CNMF_TRY(launch_gemm_f64(A, ld_in, M, d->X64, d->n_rows, d->n_cols, d->ld_c, to_genes != 0, C, ld_out, s));
+  else
+    CNMF_TRY(launch_gemm_f64(A, ld_in, M, d->X, d->n_rows, d->n_cols, d->ld_c, to_genes != 0, C, ld_out, s));
   d->h->launches += 1;
   CNMF_CUDA_CHECK(cudaMemcpy2DAsync(C_host, (size_t)n_out * 8, c.p, (size_t)ld_out * 8, (size_t)n_out * 8, M,
                                     cudaMemcpyDeviceToHost, s));

@@ -350,6 +350,63 @@ class Engine:
         check(self.lib.cnmf_beta_step_host(self._h, ctypes.byref(a), None))
         return dict(F=F, oth_sum=oth, last=lo, totals=tt)
 
+    def update_step_f64(self, ks, rids, done, n, F, op="update", num=None, gram_in=None, solver="mu", want_scalar=False,
+                        l1=0.0, l2=0.0, gram_out=None, scal_out=None):
+        """Test hook: one launch of the float64 solver on packed fp64 host data (slot s holds restart rids[s] with
+        ks[s] components; F and num are (sum ks) x ld with ld = ceil(n / 32) * 32, gram_in n_rids x 32 x 32).  op
+        'update' (solver 'mu' / 'cd'; with want_scalar also MU <NUM, F_new> / CD sum |projected gradient|), 'gram' (the
+        Gram of F) or 'cross' (<NUM, F>).  gram_out and scal_out are uploaded as given, so a caller can pre-fill them
+        with a sentinel; missing ones start as zeros.  Returns dict(F, gram, scal)."""
+        ks = np.ascontiguousarray(ks, np.int32)
+        rids = np.ascontiguousarray(rids, np.int32)
+        done = np.ascontiguousarray(done, np.int32)
+        F = f64c(F).copy()
+        SK, ld = F.shape
+        assert SK == int(ks.sum()) and ld == -(-int(n) // 32) * 32
+        num = None if num is None else f64c(num)
+        assert num is None or num.shape == (SK, ld)
+        n_rids = len(done)
+        gin = None if gram_in is None else f64c(gram_in)
+        assert gin is None or gin.shape == (n_rids, 32, 32)
+        g_out = np.zeros((n_rids, 32, 32)) if gram_out is None else f64c(gram_out).copy()
+        s_out = np.zeros(n_rids) if scal_out is None else f64c(scal_out).copy()
+        a = _lib.UpdateStepF64Args()
+        a.n_slots, a.n_rids, a.n = len(ks), n_rids, int(n)
+        a.ks, a.rids, a.done = ptr(ks), ptr(rids), ptr(done)
+        a.op = {"update": _lib.UNIT_F64_UPDATE, "gram": _lib.UNIT_F64_GRAM, "cross": _lib.UNIT_F64_CROSS}[op]
+        a.solver = {"mu": SOLVER_MU, "cd": SOLVER_CD}[solver]
+        a.want_scalar = 1 if want_scalar else 0
+        a.l1, a.l2 = float(l1), float(l2)
+        a.F, a.num, a.gram_in, a.gram_out, a.scal_out = ptr(F), ptr(num), ptr(gin), ptr(g_out), ptr(s_out)
+        check(self.lib.cnmf_update_step_f64_host(self._h, ctypes.byref(a), None))
+        return dict(F=F, gram=g_out, scal=s_out)
+
+    def conv_check(self, ks, rids, solver, it, tol, max_iter, done, n_iter, err0, prev, last, normX2=0.0, cross=None,
+                   gramA=None, gramB=None, violA=None, violB=None):
+        """Test hook: one launch of the shared convergence kernel (solver 'mu': mu_check_kernel, 'cd': cd_check_kernel)
+        on host state, with it / tol / max_iter as the solvers pass them.  Per-restart arrays have one entry per rid
+        (gramA / gramB n_rids x 32 x 32); the state (done, n_iter, err0, prev, last) is uploaded as given.  Returns
+        dict(done, n_iter, err0, prev, last) after the launch."""
+        ks = np.ascontiguousarray(ks, np.int32)
+        rids = np.ascontiguousarray(rids, np.int32)
+        st = dict(done=np.array(done, np.int32), n_iter=np.array(n_iter, np.int32), err0=np.array(err0, np.float64),
+                  prev=np.array(prev, np.float64), last=np.array(last, np.float64))
+        n_rids = len(st["done"])
+        assert all(len(v) == n_rids for v in st.values())
+        opt = {k: (None if v is None else f64c(v)) for k, v in
+               dict(cross=cross, gramA=gramA, gramB=gramB, violA=violA, violB=violB).items()}
+        a = _lib.ConvCheckArgs()
+        a.n_slots, a.n_rids = len(ks), n_rids
+        a.ks, a.rids = ptr(ks), ptr(rids)
+        a.solver = {"mu": SOLVER_MU, "cd": SOLVER_CD}[solver]
+        a.it, a.max_iter, a.tol, a.normX2 = int(it), int(max_iter), float(tol), float(normX2)
+        for k, v in opt.items():
+            setattr(a, k, ptr(v))
+        for k, v in st.items():
+            setattr(a, k, ptr(v))
+        check(self.lib.cnmf_conv_check_host(self._h, ctypes.byref(a), None))
+        return st
+
 
 class Dataset:
     """A cells x genes matrix resident on the GPU (norm_counts.X / tpm.X of the reference).  precision='fp64' keeps X
@@ -427,7 +484,9 @@ class Dataset:
                                             ctypes.c_void_p(H_ptr), None))
 
     def nndsvd_gemm(self, A, to_genes):
-        """float64 product of the NNDSVD starts (test hook): A (M x genes) @ X.T, or with to_genes A (M x cells) @ X."""
+        """The fp64 GEMM hook, for both element types of X (the NNDSVD starts on an fp32 X; the float64 solver's two
+        products and NNDSVD starts on a float64 X): A (M x genes) @ X.T, or with to_genes A (M x cells) @ X, in float64.
+        Sparse datasets are refused."""
         A = np.ascontiguousarray(A, dtype=np.float64)
         n, g = self.shape
         assert A.shape[1] == (n if to_genes else g)

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define CNMF_B200_ABI_VERSION 15
+#define CNMF_B200_ABI_VERSION 16
 #define CNMF_MAX_COMPONENTS 32          /* largest n_components per restart on the CUDA path */
 
 typedef struct cnmf_handle_s* cnmf_handle_t;
@@ -184,8 +184,10 @@ int cnmf_nndsvd_init_dev(cnmf_dataset_t d, int n_restarts, const int32_t* ks, co
 /* test hook: at most max_restarts restarts per chunk of cnmf_nndsvd_init_dev on this handle (0 = sized from the free
  * device memory only, the default) -- chunkings can then be compared without starving the device */
 int cnmf_nndsvd_chunk_limit(cnmf_handle_t h, int max_restarts);
-/* test hook: the fp64 GEMM of cnmf_nndsvd_init_dev.  to_genes = 0: C_host (M x n_rows) = A_host (M x n_cols) X^T;
- * 1: C_host (M x n_cols) = A_host (M x n_rows) X.  Host arrays dense row-major fp64. */
+/* test hook: the fp64 GEMM of cnmf_nndsvd_init_dev and of the float64 solver, on the dataset's own X: the fp32 X of an
+ * ordinary dataset, the fp64 X of a float64 one.  to_genes = 0: C_host (M x n_rows) = A_host (M x n_cols) X^T;
+ * 1: C_host (M x n_cols) = A_host (M x n_rows) X.  Host arrays dense row-major fp64.  The device output starts as NaN
+ * bytes, so an output the kernel does not write shows.  Sparse datasets: -3. */
 int cnmf_nndsvd_gemm_host(cnmf_dataset_t d, int to_genes, int M, const double* A_host, double* C_host, void* stream);
 
 /* ---- float64 datasets (CNMF_PRECISION_FP64) -------------------------------------------------------------------- */
@@ -355,6 +357,62 @@ typedef struct cnmf_beta_step_args {
   double* totals;               /* in/out (divergence): n_rids x 2 */
 } cnmf_beta_step_args;
 int cnmf_beta_step_host(cnmf_handle_t h, const cnmf_beta_step_args* args, void* stream);
+
+/* test hook: ONE launch of the float64 solver (nmf_f64.cu) on host-supplied packed fp64 data, through the launch
+ * functions the solver uses (batch layout, rids and done as for cnmf_update_step_host; ld = ceil(n / 32) * 32; the
+ * partial Grams use the solver's stride kp = max ks rounded up to 4).
+ *   op UPDATE: one MU or CD update of F with the other factor's Gram gram_in, l1 / l2; with want_scalar, MU <NUM, F_new>
+ *     or CD sum |projected gradient| per restart into scal_out, through finalize.
+ *   op GRAM: the Gram of F (gram64 + finalize) into gram_out.
+ *   op CROSS: <NUM, F> per restart (cross64 + finalize) into scal_out.
+ * Every array marked in/out is uploaded before the launch and downloaded after it. */
+enum { CNMF_UNIT_F64_UPDATE = 0, CNMF_UNIT_F64_GRAM = 1, CNMF_UNIT_F64_CROSS = 2 };
+typedef struct cnmf_update_step_f64_args {
+  int32_t n_slots;              /* restarts in the batch */
+  int32_t n_rids;               /* length of done / scal_out, and of gram_in / gram_out in 32 x 32 blocks */
+  const int32_t* ks;            /* [n_slots], 1..32 */
+  const int32_t* rids;          /* [n_slots], distinct, < n_rids */
+  const int32_t* done;          /* [n_rids] 1 = frozen restart: the launches skip it */
+  int32_t n;                    /* valid columns of the factor */
+  int32_t op;                   /* CNMF_UNIT_F64_* */
+  int32_t solver;               /* op UPDATE: CNMF_SOLVER_MU / CNMF_SOLVER_CD */
+  int32_t want_scalar;          /* op UPDATE: also the per-restart scalar */
+  double l1, l2;
+  double* F;                    /* in/out: (sum ks) x ld */
+  const double* num;            /* (sum ks) x ld (UPDATE, CROSS) */
+  const double* gram_in;        /* n_rids x 32 x 32 (UPDATE) */
+  double* gram_out;             /* in/out (GRAM): n_rids x 32 x 32 */
+  double* scal_out;             /* in/out (UPDATE with want_scalar, CROSS): n_rids */
+} cnmf_update_step_f64_args;
+int cnmf_update_step_f64_host(cnmf_handle_t h, const cnmf_update_step_f64_args* args, void* stream);
+
+/* test hook: ONE launch of the convergence kernel every solver shares, on host state (batch layout and rids as for
+ * cnmf_update_step_host; the state's done is also the batch's, as in the solvers).  it, tol and max_iter are what the
+ * solvers pass: MU it = 0 initialises err0 / prev, a check at it with tol > 0 and it % 10 == 0 passes tol, a forced check
+ * at it = max_iter passes -1; CD passes tol at every iteration.
+ *   MU: err = sqrt(max(normX2 - 2 cross + <gramA, gramB>, 0)) over the K x K block of each rid (32 x 32 blocks).
+ *   CD: viol = violA (+ violB when given).
+ * Frozen restarts (done = 1) are left alone. */
+typedef struct cnmf_conv_check_args {
+  int32_t n_slots;              /* restarts in the batch */
+  int32_t n_rids;               /* length of every per-restart array */
+  const int32_t* ks;            /* [n_slots], 1..32 */
+  const int32_t* rids;          /* [n_slots], distinct, < n_rids */
+  int32_t solver;               /* CNMF_SOLVER_MU / CNMF_SOLVER_CD */
+  int32_t it, max_iter;
+  double tol, normX2;
+  const double* cross;          /* MU: n_rids */
+  const double* gramA;          /* MU: n_rids x 32 x 32 */
+  const double* gramB;
+  const double* violA;          /* CD: n_rids */
+  const double* violB;          /* CD: n_rids, or NULL */
+  int32_t* done;                /* in/out: n_rids */
+  int32_t* n_iter;              /* in/out: n_rids */
+  double* err0;                 /* in/out: n_rids */
+  double* prev;
+  double* last;
+} cnmf_conv_check_args;
+int cnmf_conv_check_host(cnmf_handle_t h, const cnmf_conv_check_args* args, void* stream);
 
 /* ---- consensus kernels (cnmf.py:882-916) on a stacked-spectra matrix S (R x G, device, row stride ld) -- */
 /* rows / ||row||_2 in place (cnmf.py:882) */

@@ -1,5 +1,6 @@
 """ORACLE (test infrastructure) -- float64 references of ONE launch of the batched solver's kernels
-(cnmf_b200/csrc/nmf_kernels.cu) and bit-exact numpy restatements of the operand pieces the GEMM reads.
+(cnmf_b200/csrc/nmf_kernels.cu, and nmf_f64.cu for the float64 solver), the stopping decision of the solver loops, and
+bit-exact numpy restatements of the operand pieces the GEMM reads.
 
 Layout as in the kernels: a factor is K x n (components x items); `num` is the product the update divides by
 (X H^T for W, W^T X for H) summed over its split-K slices; `G` is the K x K Gram of the other factor.  The update
@@ -22,42 +23,75 @@ def gram_fp32(gram_in, K, diag_add=0.0):
     return G.astype(np.float64)
 
 
-def mu_half_step(F, num, G, l1=0.0, l2=0.0):
-    """One multiplicative update of F (SK/decomposition/_nmf.py:535-549,610-624 for W; :633-635,696-721 for H), float64:
-        den = G F + l1 + l2 F;   den < FLT_MIN -> float32 eps;   F_new = F * num / den.
-    The floor is the kernel's rule (its Newton quotient needs a normal denominator); scikit-learn maps only exact
-    zeros to eps, which is the same for every denominator a test builds."""
-    F = np.asarray(F, np.float64)
-    den = G @ F + l1 + l2 * F
-    den = np.where(den < FLT_MIN, EPSILON, den)
-    return F * np.asarray(num, np.float64) / den
+def mu_half_step(F, num, G, l1=0.0, l2=0.0, eps_rule="floor", dtype=np.float64):
+    """One multiplicative update of F (SK/decomposition/_nmf.py:535-549,610-624 for W; :633-635,696-721 for H):
+        den = G F + l1 + l2 F;   den -> float32 eps by eps_rule;   F_new = F * num / den.
+    eps_rule "floor" (the default) is the fp32 kernels' rule: den < FLT_MIN -> eps (their Newton quotient needs a normal
+    denominator).  "zero" is scikit-learn's own rule, which the float64 solver keeps: only den == 0 -> eps, a positive
+    denominator below FLT_MIN is used as it is.  The two agree on every denominator that is 0 or >= FLT_MIN.  dtype:
+    the arithmetic (np.longdouble gives a reference whose own rounding is far below float64's)."""
+    F = np.asarray(F, dtype)
+    den = np.asarray(G, dtype) @ F + dtype(l1) + dtype(l2) * F
+    if eps_rule == "floor":
+        den = np.where(den < FLT_MIN, dtype(EPSILON), den)
+    elif eps_rule == "zero":
+        den = np.where(den == 0, dtype(EPSILON), den)
+    else:
+        raise ValueError("eps_rule must be 'floor' or 'zero'")
+    return F * np.asarray(num, dtype) / den
 
 
-def cd_sweep(F, num, G, l1=0.0, l2=0.0, jacobi=False):
+def cd_sweep(F, num, G, l1=0.0, l2=0.0, jacobi=False, dtype=np.float64):
     """One coordinate-descent sweep over the K coordinates of every item (SK/decomposition/_cdnmf_fast.pyx:8-37 with
     shuffle=False; l1 subtracted from the product and l2 added to the Gram diagonal, SK/decomposition/_nmf.py:
-    379-385), float64.  G must be the Gram WITHOUT l2 (gram_fp32(..., diag_add=l2) gives the kernel's form; pass
-    l2=0 then).  Returns (F_new, violation, magnitude): violation = sum |projected gradient| over items and
-    coordinates, magnitude[t, j] = |num - l1| + sum_r |G[t, r] F[r, j]| of each gradient (what its rounding error
-    scales with).  jacobi=True evaluates every gradient from the OLD F (a wrong order, for tests that must tell
-    Gauss-Seidel from it)."""
-    F = np.array(F, np.float64)
-    num = np.asarray(num, np.float64)
-    G = np.asarray(G, np.float64) + l2 * np.eye(len(G))
+    379-385), in dtype (float64 by default).  G must be the Gram WITHOUT l2 (gram_fp32(..., diag_add=l2) gives the
+    kernel's form; pass l2=0 then).  Returns (F_new, violation, magnitude): violation = sum |projected gradient| over
+    items and coordinates (a Python float), magnitude[t, j] = |num - l1| + sum_r |G[t, r] F[r, j]| of each gradient
+    (what its rounding error scales with).  jacobi=True evaluates every gradient from the OLD F (a wrong order, for
+    tests that must tell Gauss-Seidel from it)."""
+    F = np.array(F, dtype)
+    num = np.asarray(num, dtype)
+    G = np.asarray(G, dtype) + dtype(l2) * np.eye(len(G), dtype=dtype)
+    l1 = dtype(l1)
     K = F.shape[0]
     F0 = F.copy()
-    viol = 0.0
+    viol = dtype(0.0)
     mag = np.zeros_like(F)
     for t in range(K):
         src = F0 if jacobi else F
         grad = l1 - num[t] + G[t] @ src
         mag[t] = np.abs(l1 - num[t]) + np.abs(G[t]) @ np.abs(src)
-        pg = np.where(src[t] == 0.0, np.minimum(0.0, grad), grad)
-        viol += float(np.abs(pg).sum())
+        pg = np.where(src[t] == 0.0, np.minimum(dtype(0.0), grad), grad)
+        viol += np.abs(pg).sum()
         h = G[t, t]
         if h != 0.0:
-            F[t] = np.maximum(src[t] - grad / h, 0.0)
-    return F, viol, mag
+            F[t] = np.maximum(src[t] - grad / h, dtype(0.0))
+    return F, float(viol), mag
+
+
+# ---------------------------------------------------------------------------------------- stopping decisions
+def mu_stop(it, err, err0, prev, tol, max_iter):
+    """The MU loop's decision after iteration it >= 1 (oracle/nmf_ref.py mu_frobenius, SK/decomposition/_nmf.py:
+    867-888): the error is looked at only when tol > 0 and it % 10 == 0; the restart stops when (prev - err) / err0 <
+    tol -- strict, and with numpy's IEEE quotient, so err0 == 0 gives NaN (never stops) or -inf (stops) -- and prev
+    advances to err only when it continues.  The loop ends after max_iter whatever the error.  err is not read at the
+    other iterations.  Returns (stop, prev)."""
+    if tol > 0 and it % 10 == 0:
+        with np.errstate(divide="ignore", invalid="ignore"):
+            q = (np.float64(prev) - np.float64(err)) / np.float64(err0)
+        if q < tol:
+            return True, prev
+        prev = err
+    return it >= max_iter, prev
+
+
+def cd_stop(it, viol, viol0, tol, max_iter):
+    """The CD loop's decision after iteration it >= 1 (oracle/nmf_ref.py cd_frobenius, SK/decomposition/_nmf.py:
+    504-516): iteration 1's violation becomes viol0; the restart stops when viol0 == 0 or viol / viol0 <= tol (not
+    strict), and after max_iter.  Returns (stop, viol0)."""
+    if it == 1:
+        viol0 = viol
+    return bool(viol0 == 0 or viol / viol0 <= tol or it >= max_iter), viol0
 
 
 # ---------------------------------------------------------------------------------------- operand pieces

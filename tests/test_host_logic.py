@@ -286,7 +286,8 @@ def test_binding_table_matches_header_prototypes():
     assert ver == _lib.ABI_VERSION == ctypes.CDLL(_lib.LIB_PATH).cnmf_abi_version()
     assert ctypes.sizeof(_lib.NmfParams) == 4 * 4 + 5 * 8 + 2 * 4
     # the test hooks' argument structs: the ctypes mirrors name the header's fields in the header's order
-    for cname, mirror in (("cnmf_update_step_args", _lib.UpdateStepArgs), ("cnmf_beta_step_args", _lib.BetaStepArgs)):
+    for cname, mirror in (("cnmf_update_step_args", _lib.UpdateStepArgs), ("cnmf_beta_step_args", _lib.BetaStepArgs),
+                          ("cnmf_update_step_f64_args", _lib.UpdateStepF64Args), ("cnmf_conv_check_args", _lib.ConvCheckArgs)):
         body = re.search(r"typedef struct %s \{(.*?)\}" % cname, header, flags=re.S).group(1)
         names = []
         for decl in (d.strip() for d in body.split(";") if d.strip()):

@@ -225,3 +225,97 @@ def test_beta_step_references_match_sklearn(beta, l1, l2):
             assert (WH[keep] < kernel_ref.EPSILON).any()
         elif b == 0:
             assert sx == keep.sum() and t >= 0
+
+
+def test_float64_eps_rule_matches_sklearn():
+    """kernel_ref.mu_half_step(eps_rule='zero') -- what tests/test_fp64_units.py holds the float64 MU kernel to --
+    against scikit-learn's _multiplicative_update_w on denominators that are exactly 0 (-> float32 eps) and positive
+    below FLT_MIN (used as they are), where the fp32 kernels' floor rule differs."""
+    from sklearn.decomposition import _nmf
+    from oracle import kernel_ref
+    rng = np.random.RandomState(3)
+    n, K = 40, 6
+    W = np.abs(rng.randn(n, K)) + 0.1
+    G = np.abs(rng.randn(K, K))
+    G = G @ G.T
+    G[2] = 0.0                           # den == 0 on row 2 of the update (sklearn reads G transposed: HHt = G.T)
+    G[4] = 1e-300 * np.abs(rng.rand(K))   # 0 < den < FLT_MIN on row 4
+    num = np.abs(rng.randn(K, n))
+    Wm, *_ = _nmf._multiplicative_update_w(np.zeros((n, 3)), W.copy(), np.zeros((K, 3)), 2, 0.0, 0.0, 1.0,
+                                           HHt=G.T.copy(), XHt=num.T.copy(), update_H=False)
+    ref = kernel_ref.mu_half_step(W.T, num, G, eps_rule="zero")
+    assert np.allclose(ref, Wm.T, rtol=1e-13, atol=0)
+    den = G @ W.T
+    assert (den[4] > 0).all() and (den[4] < kernel_ref.FLT_MIN).all()
+    assert np.array_equal(ref[2], W.T[2] * num[2] / kernel_ref.EPSILON)
+    floor = kernel_ref.mu_half_step(W.T, num, G)
+    assert np.array_equal(floor[2], ref[2]) and not np.allclose(floor[4], ref[4])
+    ld = kernel_ref.mu_half_step(W.T, num, G, eps_rule="zero", dtype=np.longdouble)
+    assert np.allclose(ld.astype(np.float64), ref, rtol=1e-15, atol=0)
+
+
+def _mu_replay(errors, tol, max_iter):
+    """n_iter of the MU loop driven by kernel_ref.mu_stop over errors[it] (it = 0 is the error at init)."""
+    from oracle import kernel_ref
+    prev = errors[0]
+    for it in range(1, max_iter + 1):
+        stop, prev = kernel_ref.mu_stop(it, errors.get(it), errors[0], prev, tol, max_iter)
+        if stop:
+            return it
+    raise AssertionError("mu_stop never stopped the loop")
+
+
+@pytest.mark.parametrize("tol,max_iter", [(1e-3, 400), (1e-2, 400), (1e-4, 13), (0.0, 25), (1e-4, 30)])
+def test_mu_stop_restates_the_mu_loop(golden, tol, max_iter):
+    """kernel_ref.mu_stop -- the decision the MU convergence kernel is held to -- replayed over the errors
+    nmf_ref.mu_frobenius evaluates gives its n_iter: checks at multiples of 10 only, strict <, the end at max_iter."""
+    X = golden["X"]
+    W, H = nmf_ref.init_random(X.mean(), X.shape[0], X.shape[1], 4, 11)
+    seen = []
+
+    def record(X_, W_, H_):
+        e = nmf_ref.frobenius_error(X_, W_, H_)
+        seen.append(e)
+        return e
+
+    _, _, n_iter = nmf_ref.mu_frobenius(X, W, H, tol=tol, max_iter=max_iter, error_fn=record)
+    errors = {0: seen[0]}
+    errors.update({10 * (i + 1): e for i, e in enumerate(seen[1:])})
+    assert _mu_replay(errors, tol, max_iter) == n_iter
+
+
+def test_mu_stop_edges():
+    """The branches the fixtures never reach: err0 == 0 with err == 0 (NaN quotient: runs on), the tol boundary
+    (equality continues), prev advancing only on a continue, no look at the error off the multiples of 10."""
+    from oracle import kernel_ref as kr
+    assert kr.mu_stop(10, 0.0, 0.0, 0.0, 1e-4, 100) == (False, 0.0)
+    assert kr.mu_stop(100, 0.0, 0.0, 0.0, 1e-4, 100) == (True, 0.0)
+    assert kr.mu_stop(10, 2.0, 4.0, 3.0, 0.25, 100) == (False, 2.0)        # (3 - 2) / 4 == tol: continues
+    assert kr.mu_stop(10, 2.0, 4.0, 3.0, np.nextafter(0.25, 1), 100) == (True, 3.0)
+    assert kr.mu_stop(13, None, 4.0, 3.0, 0.25, 13) == (True, 3.0)
+    assert kr.mu_stop(7, None, 4.0, 3.0, 0.25, 100) == (False, 3.0)
+
+
+@pytest.mark.parametrize("tol,max_iter,l2", [(1e-4, 200, 0.0), (1e-2, 200, 0.5), (0.0, 7, 0.0)])
+def test_cd_stop_restates_the_cd_loop(golden, tol, max_iter, l2):
+    """kernel_ref.cd_stop replayed over nmf_ref's own half-sweeps gives cd_frobenius's n_iter and factors (<=, viol0
+    from iteration 1), and an all-zero problem -- viol0 == 0 -- stops at iteration 1."""
+    from oracle import kernel_ref as kr
+    X = golden["X"]
+    W0, H0 = nmf_ref.init_random(X.mean(), X.shape[0], X.shape[1], 4, 5)
+    Wr, Hr, n_ref = nmf_ref.cd_frobenius(X, W0, H0, tol=tol, max_iter=max_iter, l2_reg_W=l2, l2_reg_H=l2)
+    W, Ht = W0.copy(), np.ascontiguousarray(H0.T.copy())
+    viol0 = None
+    for it in range(1, max_iter + 1):
+        HHt = Ht.T @ Ht + l2 * np.eye(4)
+        viol = nmf_ref._cd_sweep(W, HHt, X @ Ht)
+        WtW = W.T @ W + l2 * np.eye(4)
+        viol += nmf_ref._cd_sweep(Ht, WtW, X.T @ W)
+        stop, viol0 = kr.cd_stop(it, viol, viol0, tol, max_iter)
+        if stop:
+            break
+    assert it == n_ref and np.array_equal(W, Wr) and np.array_equal(Ht.T, Hr)
+    Z = np.zeros_like(X)
+    _, _, n_zero = nmf_ref.cd_frobenius(Z, np.zeros_like(W0), np.zeros_like(H0), tol=tol, max_iter=max_iter)
+    assert n_zero == 1 and kr.cd_stop(1, 0.0, None, tol, max_iter) == (True, 0.0)
+    assert kr.cd_stop(3, 0.25, 1.0, 0.25, 100)[0] and not kr.cd_stop(3, 0.25, 1.0, np.nextafter(0.25, 0), 100)[0]
