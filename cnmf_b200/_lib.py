@@ -77,6 +77,14 @@ class UpdateStepF64Args(ctypes.Structure):
                 ("gram_out", ctypes.c_void_p), ("scal_out", ctypes.c_void_p)]
 
 
+FORM_FP32, FORM_TF32, FORM_TF32_EXACT, FORM_F16_EXACT, FORM_FP64 = 0, 1, 2, 3, 4
+FORM_NAMES = {FORM_FP32: "fp32", FORM_TF32: "tf32", FORM_TF32_EXACT: "tf32_exact", FORM_F16_EXACT: "f16_exact",
+              FORM_FP64: "fp64"}
+# resident arrays of cnmf_dataset_operand_host
+OPERANDS = {"X": 0, "Xt": 1, "X_hi": 2, "X_lo": 3, "Xt_hi": 4, "Xt_lo": 5, "X_h16": 6, "Xt_h16": 7, "row_scale": 8,
+            "col_scale": 9}
+
+
 class ConvCheckArgs(ctypes.Structure):
     """struct cnmf_conv_check_args (include/cnmf_b200.h): arguments of the cnmf_conv_check_host test hook."""
     _fields_ = [("n_slots", ctypes.c_int32), ("n_rids", ctypes.c_int32),
@@ -147,6 +155,9 @@ SIGNATURES = {
     "cnmf_beta_step_host": (_i, [_vp, _pp(BetaStepArgs), _vp]),
     "cnmf_update_step_f64_host": (_i, [_vp, _pp(UpdateStepF64Args), _vp]),
     "cnmf_conv_check_host": (_i, [_vp, _pp(ConvCheckArgs), _vp]),
+    "cnmf_dataset_form": (_i, [_vp]),
+    "cnmf_dataset_operand_host": (_i, [_vp, _i, _vp, _ll]),
+    "cnmf_dataset_gemm_host": (_i, [_vp, _i, _i, _i, _vp, _vp, _pp(_i)]),
     "cnmf_l2_normalize_rows": (_i, [_vp, _vp, _i, _i, _i, _vp]),
     "cnmf_local_density": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     "cnmf_col_stats_dev": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
@@ -172,7 +183,7 @@ SIGNATURES = {
 _lib = None
 
 
-ABI_VERSION = 16     # include/cnmf_b200.h CNMF_B200_ABI_VERSION
+ABI_VERSION = 17     # include/cnmf_b200.h CNMF_B200_ABI_VERSION
 
 
 def load():

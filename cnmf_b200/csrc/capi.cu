@@ -267,7 +267,7 @@ int dataset_resolve_form(cnmf_dataset_s* d, bool exact, cudaStream_t s) {
   // exact-count detection: is X = diag(r) C diag(s) with C integer <= 2048 ?  (column scale first, then row scale).
   // The same condition for dense and CSC matrices, so that both give the same dataset.
   const bool may_be_exact = d->precision == CNMF_PRECISION_TF32X3 || d->precision == CNMF_PRECISION_F16X2;
-  if (may_be_exact && !exact && d->n_rows <= 65535 * 64) {
+  if (may_be_exact && !exact) {
     if (d->sparse) {
       CNMF_TRY(csc_detect_exact(d, s, &exact));
     } else {

@@ -2,7 +2,9 @@
 // (cnmf_update_step_host, include/cnmf_b200.h).  It builds the FactorView / BatchMeta / FusedOut the solver builds
 // (nmf_engine.cu) and calls the same launch_* functions; no kernel code of its own.  cnmf_beta_step_host does the same
 // for the KL / IS solver (nmf_beta.cu), cnmf_update_step_f64_host for the float64 solver (nmf_f64.cu), and
-// cnmf_conv_check_host runs the convergence kernels every solver shares.
+// cnmf_conv_check_host runs the convergence kernels every solver shares.  cnmf_dataset_form / cnmf_dataset_operand_host
+// read what dataset creation left resident, and cnmf_dataset_gemm_host runs one of the solver's products (view_gemm)
+// on a dataset.
 #include <algorithm>
 #include <vector>
 
@@ -392,5 +394,79 @@ extern "C" int cnmf_conv_check_host(cnmf_handle_t h, const cnmf_conv_check_args*
     a->done[r] = meta[3 * R + r];
     a->n_iter[r] = meta[3 * R + NR + r];
   }
+  return 0;
+}
+
+static_assert((int)Form::FP32 == CNMF_FORM_FP32 && (int)Form::TF32 == CNMF_FORM_TF32 &&
+                  (int)Form::TF32_EXACT == CNMF_FORM_TF32_EXACT && (int)Form::F16_EXACT == CNMF_FORM_F16_EXACT &&
+                  (int)Form::FP64 == CNMF_FORM_FP64,
+              "CNMF_FORM_* mirror cnmf::Form");
+
+extern "C" int cnmf_dataset_form(cnmf_dataset_t d) {
+  CNMF_REQUIRE(d, "dataset_form: NULL dataset");
+  return (int)d->form;
+}
+
+extern "C" int cnmf_dataset_operand_host(cnmf_dataset_t d, int which, void* out_host, long long bytes) {
+  CNMF_REQUIRE(d && out_host, "dataset_operand: NULL argument");
+  const long long nx = (long long)d->n_rows * d->ld_c, nxt = (long long)d->n_cols * d->ld_r;
+  const void* src = nullptr;
+  long long size = 0;
+  switch (which) {
+    case CNMF_OPERAND_X: src = d->X; size = 4 * nx; break;
+    case CNMF_OPERAND_XT: src = d->Xt; size = 4 * nxt; break;
+    case CNMF_OPERAND_X_HI: src = d->X_hi; size = 4 * nx; break;
+    case CNMF_OPERAND_X_LO: src = d->X_lo; size = 4 * nx; break;
+    case CNMF_OPERAND_XT_HI: src = d->Xt_hi; size = 4 * nxt; break;
+    case CNMF_OPERAND_XT_LO: src = d->Xt_lo; size = 4 * nxt; break;
+    case CNMF_OPERAND_X_H16: src = d->X_h16; size = 2 * nx; break;
+    case CNMF_OPERAND_XT_H16: src = d->Xt_h16; size = 2 * nxt; break;
+    case CNMF_OPERAND_ROW_SCALE: src = d->row_scale; size = 4LL * d->ld_r; break;
+    case CNMF_OPERAND_COL_SCALE: src = d->col_scale; size = 4LL * d->ld_c; break;
+    default: CNMF_REQUIRE(false, "dataset_operand: unknown array");
+  }
+  if (!src) {
+    set_last_error("dataset_operand: this dataset does not hold that array");
+    return -3;
+  }
+  CNMF_REQUIRE(bytes == size, "dataset_operand: bytes must be the array's size");
+  CNMF_CUDA_CHECK(cudaSetDevice(d->h->device));
+  CNMF_CUDA_CHECK(cudaMemcpy(out_host, src, (size_t)size, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+extern "C" int cnmf_dataset_gemm_host(cnmf_dataset_t d, int transposed, int side, int SK, const float* F_host,
+                                      float* out_host, int* splits_out) {
+  CNMF_REQUIRE(d && splits_out && (side == 0 || side == 1) && SK >= 1, "dataset_gemm: bad arguments");
+  CNMF_TRY(require_dense(d, "dataset_gemm"));
+  cnmf_handle_s* h = d->h;
+  const DataView v = make_view(d, transposed != 0);
+  const GemmPlan plan = view_gemm_plan(v, side, SK);
+  *splits_out = plan.splits;
+  if (!out_host) return 0;
+  CNMF_REQUIRE(F_host, "dataset_gemm: NULL factor");
+  // the factor is the other side's: Fc (n_c items, scale_c) for NUM_r, Fr (n_r items, scale_r) for NUM_c
+  const int n_in = side == 0 ? v.n_c : v.n_r, ld_in = side == 0 ? v.ld_c : v.ld_r;
+  const int n_out = side == 0 ? v.n_r : v.n_c, ld_out = side == 0 ? v.ld_r : v.ld_c;
+  const float* piece_scale = side == 0 ? v.scale_c : v.scale_r;
+  cudaStream_t s = nullptr;
+  CNMF_CUDA_CHECK(cudaSetDevice(h->device));
+  const size_t nf = (size_t)SK * ld_in, nc = (size_t)plan.splits * SK * ld_out;
+  const int ktiles = (ld_in + 511) / 512;
+  float* F = static_cast<float*>(h->dev_buf("unit.gemm_F", nf * 4));
+  float* F_hi = static_cast<float*>(h->dev_buf("unit.gemm_F_hi", nf * 4));
+  float* F_lo = static_cast<float*>(h->dev_buf("unit.gemm_F_lo", nf * 4));
+  float* ts = static_cast<float*>(h->dev_buf("unit.gemm_tile_scale", sizeof(float) * (size_t)SK * ktiles));
+  float* C = static_cast<float*>(h->dev_buf("unit.gemm_C", nc * 4));
+  if (!F || !F_hi || !F_lo || !ts || !C) return -2;
+  CNMF_CUDA_CHECK(cudaMemsetAsync(F, 0, nf * 4, s));
+  CNMF_CUDA_CHECK(cudaMemcpy2DAsync(F, (size_t)ld_in * 4, F_host, (size_t)n_in * 4, (size_t)n_in * 4, SK,
+                                    cudaMemcpyHostToDevice, s));
+  CNMF_TRY(make_pieces(v.form, F, SK, n_in, ld_in, piece_scale, F_hi, F_lo, ts, s));
+  h->launches += v.form == Form::FP32 ? 0 : 1;
+  CNMF_TRY(view_gemm(h, v, side, F, F_hi, F_lo, ts, SK, C, plan, s));
+  CNMF_CUDA_CHECK(cudaMemcpy2DAsync(out_host, (size_t)n_out * 4, C, (size_t)ld_out * 4, (size_t)n_out * 4,
+                                    (size_t)plan.splits * SK, cudaMemcpyDeviceToHost, s));
+  CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
   return 0;
 }

@@ -139,6 +139,19 @@ DataView make_view(const cnmf_dataset_s* d, bool transposed);
 // and tile scales from make_pieces; out_scale on the output columns of the exact forms) and launches the GEMM
 int form_gemm(Form form, GemmArgs g, const float* A, const float* A_hi, const float* A_lo, const float* a_tile_scale,
               const Operand& B, const float* out_scale, cudaStream_t s);
+// split-K plan of one of the solver's two products on a view: splits from gemm_fixed_splits (a function of the
+// reduction length only), slices of SK rows at the output's row stride
+struct GemmPlan {
+  int splits;
+  long long split_stride;   // elements
+};
+GemmPlan view_gemm_plan(const DataView& v, int side, int SK);
+// one of the solver's two products on a view, counted and profiled as a batched GEMM:
+//   side 0: NUM_r = Fc * B_rows^T (SK x ld_r per slice, output scale scale_r); F = Fc (SK x ld_c)
+//   side 1: NUM_c = Fr * B_cols^T (SK x ld_c per slice, output scale scale_c); F = Fr (SK x ld_r)
+// F_hi / F_lo / tile_scale: F's pieces for the view's form (make_pieces with the other side's scale)
+int view_gemm(cnmf_handle_s* h, const DataView& v, int side, const float* F, const float* F_hi, const float* F_lo,
+              const float* tile_scale, int SK, float* C, const GemmPlan& plan, cudaStream_t s);
 // operand pieces of F diag(scale) (rows x ld, n valid columns) for the form: none, tf32 split, or two fp16 pieces with
 // tile scales (rows x ceil(ld / 512)); at most one launch
 int make_pieces(Form form, const float* F, int rows, int n, int ld, const float* scale, float* hi, float* lo,

@@ -76,32 +76,30 @@ int make_pieces(Form form, const float* F, int rows, int n, int ld, const float*
   }
 }
 
-namespace {
+GemmPlan view_gemm_plan(const DataView& v, int side, int SK) {
+  const int f16 = v.form == Form::F16_EXACT ? 1 : 0;
+  return side == 0 ? GemmPlan{gemm_fixed_splits(v.n_c, f16), (long long)SK * v.ld_r}
+                   : GemmPlan{gemm_fixed_splits(v.n_r, f16), (long long)SK * v.ld_c};
+}
 
-struct GemmPlan {
-  int splits;
-  long long split_stride;   // elements
-};
-
-// C[z] (SK x N) = A (SK x Kd) * B (N x Kd)^T, counted and profiled as a batched GEMM
-int run_gemm(cnmf_handle_s* h, Form form, const float* A, const float* A_hi, const float* A_lo, const float* a_tile_scale,
-             int SK, int lda, const Operand& B, const float* out_scale, float* C, int ldc, const GemmPlan& plan,
-             cudaStream_t s) {
+int view_gemm(cnmf_handle_s* h, const DataView& v, int side, const float* F, const float* F_hi, const float* F_lo,
+              const float* tile_scale, int SK, float* C, const GemmPlan& plan, cudaStream_t s) {
+  const Operand& B = side == 0 ? v.B_rows : v.B_cols;
   GemmArgs g{};
   g.M = SK; g.N = B.rows; g.Kd = B.cols;
-  g.lda = lda; g.ldb = B.ld; g.ldc = ldc;
+  g.lda = side == 0 ? v.ld_c : v.ld_r;
+  g.ldb = B.ld;
+  g.ldc = side == 0 ? v.ld_r : v.ld_c;
   g.C = C;
   g.c_split_stride = plan.split_stride;
   g.splits = plan.splits;
   g.splits_effective = plan.splits;
   h->launches += 1;
   const int slot = h->prof_begin(s, 2.0 * (double)g.M * (double)g.N * (double)g.Kd);
-  const int rc = form_gemm(form, g, A, A_hi, A_lo, a_tile_scale, B, out_scale, s);
+  const int rc = form_gemm(v.form, g, F, F_hi, F_lo, tile_scale, B, side == 0 ? v.scale_r : v.scale_c, s);
   h->prof_end(s, slot);
   return rc;
 }
-
-}  // namespace
 
 int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_nmf_params& p, cudaStream_t s) {
   const int R0 = io.R;
@@ -177,10 +175,9 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
   float *NUMr = nullptr, *NUMc = nullptr;
   // the split-K factor is a function of the reduction length only (gemm_fixed_splits)
   auto plan_gemms = [&]() -> int {
-    plan_r.splits = io.num_rows ? 1 : gemm_fixed_splits(v.n_c, f16 ? 1 : 0);
-    plan_r.split_stride = (long long)SK * v.ld_r;
-    plan_c.splits = gemm_fixed_splits(v.n_r, f16 ? 1 : 0);
-    plan_c.split_stride = (long long)SK * v.ld_c;
+    plan_r = view_gemm_plan(v, 0, SK);
+    if (io.num_rows) plan_r.splits = 1;
+    plan_c = view_gemm_plan(v, 1, SK);
     return 0;
   };
   plan_gemms();
@@ -326,10 +323,10 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
   };
   auto gemm_rows = [&]() -> int {   // NUM_r = Fc * B_rows^T
     if (io.num_rows) return 0;      // computed by the caller
-    return run_gemm(h, v.form, wFc, wFc_hi, wFc_lo, d_rs_c, SK, v.ld_c, v.B_rows, v.scale_r, NUMr, v.ld_r, plan_r, s);
+    return view_gemm(h, v, 0, wFc, wFc_hi, wFc_lo, d_rs_c, SK, NUMr, plan_r, s);
   };
   auto gemm_cols = [&]() -> int {   // NUM_c = Fr * B_cols^T
-    return run_gemm(h, v.form, wFr, wFr_hi, wFr_lo, d_rs_r, SK, v.ld_r, v.B_cols, v.scale_c, NUMc, v.ld_c, plan_c, s);
+    return view_gemm(h, v, 1, wFr, wFr_hi, wFr_lo, d_rs_r, SK, NUMc, plan_c, s);
   };
 
   // gathers `cnt` restarts' rows: dst[dst_off[i] ..] <- src[src_off[i] ..].  Index triples go through a pinned

@@ -6,6 +6,8 @@
 
 #include <cuda_fp16.h>
 
+#include <algorithm>
+
 namespace cnmf {
 
 namespace {
@@ -61,19 +63,22 @@ __global__ void split_scaled_kernel(const float* __restrict__ src, float* __rest
   }
 }
 
-// positive floats order like their bit patterns: atomicMin on the int view
+// positive floats order like their bit patterns: atomicMin on the int view.  Blocks stride over 64-row strips
+// (gridDim.y is capped at 65 535): integer minima, so the result does not depend on which block takes a strip
 __global__ void min_positive_kernel(const float* __restrict__ X, int rows, int cols, int ld, int* __restrict__ col_min,
                                     int* __restrict__ row_min) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  const int r0 = blockIdx.y * 64;
   int cm = 0x7f800000;
-  for (int r = r0; r < min(rows, r0 + 64); ++r) {
-    const float v = (c < cols) ? X[(long long)r * ld + c] : 0.f;
-    int b = (v > 0.f) ? __float_as_int(v) : 0x7f800000;
-    cm = min(cm, b);
-    // row minimum: warp reduce then one atomic per warp
-    for (int o = 16; o > 0; o >>= 1) b = min(b, __shfl_xor_sync(0xffffffffu, b, o));
-    if ((threadIdx.x & 31) == 0 && b != 0x7f800000) atomicMin(&row_min[r], b);
+  for (long long r0 = blockIdx.y * 64LL; r0 < rows; r0 += gridDim.y * 64LL) {
+    const int r1 = (int)min((long long)rows, r0 + 64);
+    for (int r = (int)r0; r < r1; ++r) {
+      const float v = (c < cols) ? X[(long long)r * ld + c] : 0.f;
+      int b = (v > 0.f) ? __float_as_int(v) : 0x7f800000;
+      cm = min(cm, b);
+      // row minimum: warp reduce then one atomic per warp
+      for (int o = 16; o > 0; o >>= 1) b = min(b, __shfl_xor_sync(0xffffffffu, b, o));
+      if ((threadIdx.x & 31) == 0 && b != 0x7f800000) atomicMin(&row_min[r], b);
+    }
   }
   if (c < cols && cm != 0x7f800000) atomicMin(&col_min[c], cm);
 }
@@ -111,28 +116,34 @@ __global__ void fix_scale_kernel(float* __restrict__ v, int n, int n_pad) {
   v[i] = (isfinite(x) && x > 0.f && x < 1e30f) ? x : 1.f;   // rows / columns without a positive entry: any scale works
 }
 
+// 32 x 32 tiles; blocks stride over the row tiles (gridDim.y is capped at 65 535)
 __global__ void transpose_kernel(const float* __restrict__ src, int rows, int cols, int ld_src, float* __restrict__ dst,
                                  float* __restrict__ dst_hi, float* __restrict__ dst_lo, int ld_dst) {
   __shared__ float tile[32][33];
-  const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
-  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-    const int r = r0 + i, c = c0 + threadIdx.x;
-    tile[i][threadIdx.x] = (r < rows && c < cols) ? src[(long long)r * ld_src + c] : 0.f;
-  }
-  __syncthreads();
-  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-    const int c = c0 + i, r = r0 + threadIdx.x;      // dst row = c, dst col = r
-    if (c < cols && r < rows) {
-      const float v = tile[threadIdx.x][i];
-      const long long o = (long long)c * ld_dst + r;
-      if (dst) dst[o] = v;
-      if (dst_hi) {
-        float h, l;
-        split_tf32(v, h, l);
-        dst_hi[o] = h;
-        dst_lo[o] = l;
+  const int c0 = blockIdx.x * 32;
+  for (long long r0 = blockIdx.y * 32LL; r0 < rows; r0 += gridDim.y * 32LL) {
+    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+      const long long r = r0 + i;
+      const int c = c0 + threadIdx.x;
+      tile[i][threadIdx.x] = (r < rows && c < cols) ? src[r * ld_src + c] : 0.f;
+    }
+    __syncthreads();
+    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+      const int c = c0 + i;
+      const long long r = r0 + threadIdx.x;      // dst row = c, dst col = r
+      if (c < cols && r < rows) {
+        const float v = tile[threadIdx.x][i];
+        const long long o = (long long)c * ld_dst + r;
+        if (dst) dst[o] = v;
+        if (dst_hi) {
+          float h, l;
+          split_tf32(v, h, l);
+          dst_hi[o] = h;
+          dst_lo[o] = l;
+        }
       }
     }
+    __syncthreads();     // the tile is refilled for the next row block
   }
 }
 
@@ -1290,8 +1301,7 @@ int launch_to_half(const float* src, void* dst, long long n_elems, cudaStream_t 
 int launch_min_positive(const float* X, int rows, int cols, int ld, float* col_min, float* row_min, cudaStream_t s) {
   CNMF_CUDA_CHECK(cudaMemsetAsync(col_min, 0x7f, sizeof(float) * cols, s));   // 0x7f7f7f7f: a huge finite float
   CNMF_CUDA_CHECK(cudaMemsetAsync(row_min, 0x7f, sizeof(float) * rows, s));
-  dim3 grid((cols + 255) / 256, (rows + 63) / 64);
-  CNMF_REQUIRE(grid.y <= 65535, "min_positive: too many rows for one launch");
+  dim3 grid((cols + 255) / 256, std::min((rows + 63) / 64, 65535));
   min_positive_kernel<<<grid, 256, 0, s>>>(X, rows, cols, ld, reinterpret_cast<int*>(col_min), reinterpret_cast<int*>(row_min));
   CNMF_CUDA_CHECK(cudaGetLastError());
   return 0;
@@ -1319,8 +1329,7 @@ int launch_fix_scale(float* v, int n, int n_pad, cudaStream_t s) {
 
 int launch_transpose(const float* src, int rows, int cols, int ld_src, float* dst, float* dst_hi, float* dst_lo,
                      int ld_dst, cudaStream_t s) {
-  dim3 grid((cols + 31) / 32, (rows + 31) / 32), block(32, 8);
-  CNMF_REQUIRE(grid.y <= 65535, "transpose: too many rows for one launch");
+  dim3 grid((cols + 31) / 32, std::min((rows + 31) / 32, 65535)), block(32, 8);
   transpose_kernel<<<grid, block, 0, s>>>(src, rows, cols, ld_src, dst, dst_hi, dst_lo, ld_dst);
   CNMF_CUDA_CHECK(cudaGetLastError());
   return 0;

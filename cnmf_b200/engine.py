@@ -237,6 +237,13 @@ class Engine:
                                                precision_code(precision), stream, ctypes.byref(out)))
         return Dataset(self, None, precision, _handle=out, sparse=True)
 
+    def dataset_from_device(self, X_ptr, n_rows, n_cols, ld, precision=_DEFAULT_PRECISION, stream=None):
+        """Dataset of a float32 device matrix (n_rows x n_cols, row stride ld elements, e.g. torch.Tensor.data_ptr())."""
+        out = ctypes.c_void_p()
+        check(self.lib.cnmf_dataset_create(self._h, ctypes.c_void_p(X_ptr), int(n_rows), int(n_cols), int(ld), 1,
+                                           precision_code(precision), stream, ctypes.byref(out)))
+        return Dataset(self, None, precision, _handle=out)
+
     def dense_dataset_bytes(self, n_rows, n_cols, precision=_DEFAULT_PRECISION):
         """Worst-case device bytes dataset() of an n_rows x n_cols matrix needs while it is built."""
         peak = ctypes.c_longlong()
@@ -536,6 +543,46 @@ class Dataset:
     def f16(self):
         """True when the big products run as 2 f16 passes (exact dataset created with precision='f16x2')."""
         return self.lib.cnmf_dataset_is_exact(self._d) == 2
+
+    @property
+    def form(self):
+        """Operand form decided at creation: 'fp32', 'tf32', 'tf32_exact', 'f16_exact' or 'fp64' (sparse datasets: the
+        form their detection chose)."""
+        f = self.lib.cnmf_dataset_form(self._d)
+        if f < 0:
+            check(f)
+        return _lib.FORM_NAMES[f]
+
+    def operand(self, name):
+        """Test hook: copy of one resident array, padding included (None when the dataset does not hold it):
+        X, X_hi, X_lo (n_rows x ld_cols float32), Xt, Xt_hi, Xt_lo (n_cols x ld_rows float32), X_h16 / Xt_h16 (the
+        same shapes in float16), row_scale (ld_rows), col_scale (ld_cols)."""
+        ld_r, ld_c = self.ld()
+        n, g = self.shape
+        shape = {"X": (n, ld_c), "X_hi": (n, ld_c), "X_lo": (n, ld_c), "X_h16": (n, ld_c),
+                 "Xt": (g, ld_r), "Xt_hi": (g, ld_r), "Xt_lo": (g, ld_r), "Xt_h16": (g, ld_r),
+                 "row_scale": (ld_r,), "col_scale": (ld_c,)}[name]
+        out = np.empty(shape, np.float16 if name.endswith("h16") else np.float32)
+        rc = self.lib.cnmf_dataset_operand_host(self._d, _lib.OPERANDS[name], ptr(out), out.nbytes)
+        if rc == -3:
+            return None
+        check(rc)
+        return out
+
+    def gemm(self, F, side, transposed=False):
+        """Test hook: one of the solver's two products on this dataset's view, through the solver's own launch.
+        side 0: F (SK x n_c of the view) @ B_rows^T; side 1: F (SK x n_r of the view) @ B_cols^T (untransposed:
+        n_r = cells, n_c = genes).  Returns the raw split-K slices, splits x SK x n_out (their sum is the product)."""
+        F = f32c(F)
+        n_r, n_c = self.shape[::-1] if transposed else self.shape
+        assert F.ndim == 2 and F.shape[1] == (n_c if side == 0 else n_r)
+        splits = ctypes.c_int()
+        check(self.lib.cnmf_dataset_gemm_host(self._d, int(transposed), int(side), F.shape[0], None, None,
+                                              ctypes.byref(splits)))
+        out = np.empty((splits.value, F.shape[0], n_r if side == 0 else n_c), np.float32)
+        check(self.lib.cnmf_dataset_gemm_host(self._d, int(transposed), int(side), F.shape[0], ptr(F), ptr(out),
+                                              ctypes.byref(splits)))
+        return out
 
     def min(self):
         m = ctypes.c_float()

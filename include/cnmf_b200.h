@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define CNMF_B200_ABI_VERSION 16
+#define CNMF_B200_ABI_VERSION 17     /* 17: cnmf_dataset_form, cnmf_dataset_operand_host, cnmf_dataset_gemm_host */
 #define CNMF_MAX_COMPONENTS 32          /* largest n_components per restart on the CUDA path */
 
 typedef struct cnmf_handle_s* cnmf_handle_t;
@@ -413,6 +413,31 @@ typedef struct cnmf_conv_check_args {
   double* last;
 } cnmf_conv_check_args;
 int cnmf_conv_check_host(cnmf_handle_t h, const cnmf_conv_check_args* args, void* stream);
+
+/* test hooks: what a dataset holds and the solver's two products on it.
+ * cnmf_dataset_form returns the operand form decided at creation (CNMF_FORM_*; >= 0) or < 0 on error.  Sparse (CSC)
+ * datasets report the form their detection chose, which cnmf_dataset_from_columns passes on; they hold none of the
+ * dense operands themselves (cnmf_dataset_is_exact reports 0 for them). */
+enum { CNMF_FORM_FP32 = 0, CNMF_FORM_TF32 = 1, CNMF_FORM_TF32_EXACT = 2, CNMF_FORM_F16_EXACT = 3, CNMF_FORM_FP64 = 4 };
+int cnmf_dataset_form(cnmf_dataset_t d);
+/* copies one resident array, padding included, to out_host; bytes must be its exact size:
+ *   X, X_HI, X_LO (n_rows x ld_cols floats), XT, XT_HI, XT_LO (n_cols x ld_rows floats), X_H16 / XT_H16 (the same
+ *   shapes as fp16), ROW_SCALE (ld_rows floats), COL_SCALE (ld_cols floats).
+ * The exact forms hold their integer matrix C in X_HI and C^T in XT_HI (F16_EXACT: only as fp16, X_H16 / XT_H16).
+ * Returns -3 for an array this dataset does not hold. */
+enum { CNMF_OPERAND_X = 0, CNMF_OPERAND_XT = 1, CNMF_OPERAND_X_HI = 2, CNMF_OPERAND_X_LO = 3, CNMF_OPERAND_XT_HI = 4,
+       CNMF_OPERAND_XT_LO = 5, CNMF_OPERAND_X_H16 = 6, CNMF_OPERAND_XT_H16 = 7, CNMF_OPERAND_ROW_SCALE = 8,
+       CNMF_OPERAND_COL_SCALE = 9 };
+int cnmf_dataset_operand_host(cnmf_dataset_t d, int which, void* out_host, long long bytes);
+/* one of the batched solver's two products on the dataset's view (transposed as cnmf_refit's), through the solver's own
+ * launch: the factor's operand pieces for the dataset's form, then the split-K GEMM with the solver's split plan.
+ *   side 0: NUM_r = F * B_rows^T, F the column factor (SK x n_c of the view), out SK x n_r per slice
+ *   side 1: NUM_c = F * B_cols^T, F the row factor (SK x n_r of the view), out SK x n_c per slice
+ * (untransposed: n_r = n_rows, n_c = n_cols).  F_host is dense row-major; out_host receives the raw split-K slices,
+ * splits x SK x n_out, their sum being the product.  *splits_out = the number of slices; out_host may be NULL to ask
+ * for it alone.  Dense float datasets only. */
+int cnmf_dataset_gemm_host(cnmf_dataset_t d, int transposed, int side, int SK, const float* F_host, float* out_host,
+                           int* splits_out);
 
 /* ---- consensus kernels (cnmf.py:882-916) on a stacked-spectra matrix S (R x G, device, row stride ld) -- */
 /* rows / ||row||_2 in place (cnmf.py:882) */

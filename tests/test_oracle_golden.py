@@ -319,3 +319,72 @@ def test_cd_stop_restates_the_cd_loop(golden, tol, max_iter, l2):
     _, _, n_zero = nmf_ref.cd_frobenius(Z, np.zeros_like(W0), np.zeros_like(H0), tol=tol, max_iter=max_iter)
     assert n_zero == 1 and kr.cd_stop(1, 0.0, None, tol, max_iter) == (True, 0.0)
     assert kr.cd_stop(3, 0.25, 1.0, 0.25, 100)[0] and not kr.cd_stop(3, 0.25, 1.0, np.nextafter(0.25, 0), 100)[0]
+
+
+# ------------------------------------------------------------------------------------ dataset operand restatement
+def test_dataset_ref_detection_pins_todays_policy():
+    """oracle/dataset_ref.py restates exact-count detection (tests/test_dataset_units.py compares the device with it
+    bit for bit).  The reference's own matrices take the exact forms: the normalised HVG counts (counts / std) with a
+    column scale, TPM (counts * 1e6 / total) with a row scale.  A count of 2049, a column whose smallest count is 2 and
+    a matrix with both a row and a column scale take the general form."""
+    from cnmf_golden import load_golden
+    from oracle import dataset_ref as dr
+    g = load_golden("sim_mu")
+    X, tpm = g["X"].astype(np.float32), g["tpm"].astype(np.float32)
+    for precision, exact in (("tf32x3", "tf32_exact"), ("f16x2", "f16_exact")):
+        form, rs, cs = dr.decide(X, precision)
+        assert form == exact and rs is None and cs is not None
+        assert np.array_equal(dr.counts(X, rs, cs)[:, :X.shape[1]], g["counts"][:, g["hvg_idx"]])
+        form, rs, cs = dr.decide(tpm, precision)
+        assert form == exact and rs is not None and cs is None
+        assert np.array_equal(dr.counts(tpm, rs, cs)[:, :tpm.shape[1]], g["counts"])
+    assert dr.decide(X, "tf32x3-general") == ("tf32", None, None)
+    assert dr.decide(X, "fp32") == ("fp32", None, None)
+    rng = np.random.RandomState(0)
+    C = rng.poisson(3.0, (40, 30)).astype(np.float32)
+    C[:, 0] = np.maximum(C[:, 0], 1)
+    assert dr.decide(C, "tf32x3")[0] == "tf32_exact"
+    C2 = C.copy()
+    C2[5, 7] = 2049
+    assert dr.decide(C2, "tf32x3")[0] == "tf32"
+    C3 = C.copy()
+    C3[:, 4] = np.where(C3[:, 4] > 0, 2 * C3[:, 4] + 1, 0)         # odd counts ...
+    C3[np.flatnonzero(C3[:, 4])[0], 4] = 2                          # ... and one 2: the column scale 2 fails them
+    assert dr.decide(C3, "tf32x3")[0] == "tf32"
+    both = (C * (1.0 + rng.rand(40, 1)) * (1.0 + rng.rand(1, 30))).astype(np.float32)
+    assert dr.decide(both, "tf32x3")[0] == "tf32"
+    # the admission bound: 3e-7 n is admitted, 8e-7 n is not (n = 1000: far from the other rounding terms)
+    base = np.full((4, 4), 1000.0, np.float32)
+    base[0, 0] = 1.0
+    for rel, exact in ((3e-7, True), (8e-7, False)):
+        P = base.copy()
+        P[2, 3] = np.float32(1000.0 * (1.0 + rel))
+        assert (dr.decide(P, "tf32x3")[0] == "tf32_exact") == exact, rel
+
+
+def test_dataset_ref_to_tf32_is_cvt_rna():
+    """to_tf32 (the add-0x1000-and-mask form of common.cuh) is cvt.rna.tf32.f32: the nearest value with 10 stored
+    mantissa bits, ties away from zero, on a few thousand bit patterns (all exponents, the tie and its neighbours)."""
+    from oracle import dataset_ref as dr
+    rng = np.random.RandomState(1)
+    exps = rng.randint(1, 254, 4000).astype(np.uint32)
+    mant = rng.randint(0, 1 << 23, 4000).astype(np.uint32)
+    mant[:600] = (mant[:600] & ~np.uint32(0x1fff)) | np.uint32(0x1000)        # exact ties
+    mant[600:900] = (mant[600:900] & ~np.uint32(0x1fff)) | np.uint32(0x0fff)  # just below
+    mant[900:1200] = (mant[900:1200] & ~np.uint32(0x1fff)) | np.uint32(0x1001)  # just above
+    mant[1200:1300] = np.uint32(0x7fffff)                                     # carries into the exponent
+    sign = (rng.rand(4000) < 0.5).astype(np.uint32) << np.uint32(31)
+    bits = sign | (exps << np.uint32(23)) | mant
+    x = bits.view(np.float32)
+    got = dr.to_tf32(x)
+    # direct definition: |x| = m * 2^e with m = mant / 2^13 (step 1 of the kept mantissa), round half away from zero
+    ax = np.abs(x.astype(np.float64))
+    e = np.frexp(ax)[1] - 1                    # ax in [2^e, 2^(e + 1))
+    step = np.ldexp(1.0, e - 10)
+    want = np.sign(x) * np.floor(ax / step + 0.5) * step
+    assert np.array_equal(got.astype(np.float64), want)
+    assert (got.view(np.uint32) & np.uint32(0x1fff) == 0).all()
+    hi, lo = dr.split_tf32(x)
+    normal = (ax > 2.0 ** -100) & (ax < 2.0 ** 100)        # lo neither subnormal nor beyond fp32
+    assert np.array_equal(hi, got)
+    assert (np.abs(x.astype(np.float64) - hi - lo) <= ax * 2.0 ** -22)[normal].all()
