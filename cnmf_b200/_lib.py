@@ -82,7 +82,7 @@ FORM_NAMES = {FORM_FP32: "fp32", FORM_TF32: "tf32", FORM_TF32_EXACT: "tf32_exact
               FORM_FP64: "fp64"}
 # resident arrays of cnmf_dataset_operand_host
 OPERANDS = {"X": 0, "Xt": 1, "X_hi": 2, "X_lo": 3, "Xt_hi": 4, "Xt_lo": 5, "X_h16": 6, "Xt_h16": 7, "row_scale": 8,
-            "col_scale": 9}
+            "col_scale": 9, "csc_col_ptr": 10, "csc_row_idx": 11, "csc_values": 12}
 
 
 class ConvCheckArgs(ctypes.Structure):
@@ -116,6 +116,9 @@ SIGNATURES = {
     "cnmf_last_timing": (_i, [_vp, _pp(_d), _pp(_d), _pp(_d), _pp(_d)]),
     "cnmf_dataset_create": (_i, [_vp, _vp, _i, _i, _ll, _i, _i, _vp, _pp(_vp)]),
     "cnmf_dataset_create_csc": (_i, [_vp, _i, _i, _ll, _vp, _vp, _vp, _i, _vp, _pp(_vp)]),
+    "cnmf_dataset_create_csr": (_i, [_vp, _i, _i, _ll, _vp, _vp, _vp, _i, _vp, _pp(_vp)]),
+    "cnmf_dataset_create_from_csr": (_i, [_vp, _i, _i, _ll, _vp, _vp, _vp, _i, _vp, _pp(_vp)]),
+    "cnmf_dataset_create_from_csr_f64": (_i, [_vp, _i, _i, _ll, _vp, _vp, _vp, _vp, _pp(_vp)]),
     "cnmf_dataset_dense_bytes": (_i, [_i, _i, _i, _pp(_ll)]),
     "cnmf_dataset_from_columns": (_i, [_vp, _vp, _vp, _i, _vp, _pp(_vp)]),
     "cnmf_dataset_destroy": (_i, [_vp]),
@@ -183,7 +186,7 @@ SIGNATURES = {
 _lib = None
 
 
-ABI_VERSION = 17     # include/cnmf_b200.h CNMF_B200_ABI_VERSION
+ABI_VERSION = 18     # include/cnmf_b200.h CNMF_B200_ABI_VERSION
 
 
 def load():

@@ -391,29 +391,175 @@ int require_f64(const cnmf_dataset_s* d, const char* what) {
 
 extern "C" {
 
-int cnmf_dataset_create(cnmf_handle_t h, const float* X, int n_rows, int n_cols, long long ld, int src_is_device,
-                        int precision, void* stream, cnmf_dataset_t* out) {
-  CNMF_REQUIRE(h && X && out, "dataset_create: NULL argument");
-  CNMF_REQUIRE(n_rows > 0 && n_cols > 0 && ld >= n_cols, "dataset_create: bad shape");
-  CNMF_REQUIRE(precision == CNMF_PRECISION_FP32 || precision == CNMF_PRECISION_TF32X3 ||
-                   precision == CNMF_PRECISION_TF32X3_GENERAL || precision == CNMF_PRECISION_F16X2,
-               "dataset_create: bad precision");
-  cudaStream_t s = as_stream(stream);
+}  // extern "C"
+
+namespace {
+
+bool float_precision(int precision) {
+  return precision == CNMF_PRECISION_FP32 || precision == CNMF_PRECISION_TF32X3 ||
+         precision == CNMF_PRECISION_TF32X3_GENERAL || precision == CNMF_PRECISION_F16X2;
+}
+
+// Every dense dataset creator: the staging array (X, or X64 for CNMF_PRECISION_FP64; n_rows x ld_c) is zero-filled,
+// fill(d, X) writes the matrix into it on stream s, then the forms and sums are built from it.  cudaError_t from fill
+// is reported as an upload failure; a library status is passed on.
+template <class T, class Fill>
+int create_dense(cnmf_handle_t h, int n_rows, int n_cols, int precision, cudaStream_t s, cnmf_dataset_t* out, Fill fill) {
   CNMF_CUDA_CHECK(cudaSetDevice(h->device));
   auto* d = new cnmf_dataset_s(h, n_rows, n_cols, precision);
-  int rc = dataset_alloc(d, &d->X, (size_t)n_rows * d->ld_c);
+  const size_t nx = (size_t)n_rows * d->ld_c;
+  float* buf = nullptr;
+  int rc = dataset_alloc(d, &buf, nx * sizeof(T) / sizeof(float));
+  T* X = reinterpret_cast<T*>(buf);
   if (rc == 0) {
-    cudaError_t e = cudaMemsetAsync(d->X, 0, (size_t)n_rows * d->ld_c * sizeof(float), s);
-    if (e == cudaSuccess)
-      e = cudaMemcpy2DAsync(d->X, (size_t)d->ld_c * sizeof(float), X, (size_t)ld * sizeof(float),
-                            (size_t)n_cols * sizeof(float), n_rows,
-                            src_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s);
+    const cudaError_t e = cudaMemsetAsync(X, 0, nx * sizeof(T), s);
     if (e != cudaSuccess) {
       set_last_error(std::string("dataset upload failed: ") + cudaGetErrorString(e));
       rc = -2;
     }
   }
-  if (rc == 0) rc = dataset_finish(d, s);
+  if (rc == 0) rc = fill(d, X);
+  if (rc == 0 && precision == CNMF_PRECISION_FP64) {
+    d->form = Form::FP64;
+    d->X64 = reinterpret_cast<double*>(buf);
+    double sums[2] = {0.0, 0.0};
+    rc = matrix_sums_f64(h, d->X64, n_rows, n_cols, d->ld_c, sums, s);
+    d->sum = sums[0];
+    d->sum_sq = sums[1];
+  } else if (rc == 0) {
+    d->X = buf;
+    rc = dataset_finish(d, s);
+  }
+  if (rc != 0) {
+    cudaStreamSynchronize(s);
+    cnmf_dataset_destroy(d);
+    return rc;
+  }
+  *out = d;
+  return 0;
+}
+
+// fill of a host or device matrix with row stride ld
+template <class T>
+auto copy_fill(const T* src, long long ld, int n_rows, int n_cols, bool src_is_device, cudaStream_t s) {
+  return [=](cnmf_dataset_s* d, T* X) {
+    const cudaError_t e = cudaMemcpy2DAsync(X, (size_t)d->ld_c * sizeof(T), src, (size_t)ld * sizeof(T),
+                                            (size_t)n_cols * sizeof(T), n_rows,
+                                            src_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s);
+    if (e != cudaSuccess) {
+      set_last_error(std::string("dataset upload failed: ") + cudaGetErrorString(e));
+      return -2;
+    }
+    return 0;
+  };
+}
+
+// most stored entries staged on the device at a time while a host CSR matrix is scattered into a dense one
+constexpr long long CSR_STAGE_ENTRIES = 1LL << 24;
+
+// fill of a canonical host CSR matrix (checked by the caller): row_ptr is uploaded whole, the entries in slices of
+// whole rows of at most CSR_STAGE_ENTRIES (or one row) each, each slice scattered into X (stream order keeps a slice's
+// upload behind the previous scatter); the staging is freed before the dataset's other forms are built
+template <class T>
+auto csr_fill(const int64_t* row_ptr, const int32_t* col_idx, const T* values, const char* what, cudaStream_t s) {
+  return [=](cnmf_dataset_s* d, T* X) {
+    const int n = d->n_rows;
+    long long stage = 0;     // entries of the largest slice
+    std::vector<int> cuts{0};
+    while (cuts.back() < n) {
+      const int r0 = cuts.back();
+      // last row end within the budget, at least one row
+      const int r1 = std::max(r0 + 1, (int)(std::upper_bound(row_ptr + r0 + 1, row_ptr + n + 1,
+                                                              row_ptr[r0] + CSR_STAGE_ENTRIES) - row_ptr) - 1);
+      stage = std::max<long long>(stage, row_ptr[r1] - row_ptr[r0]);
+      cuts.push_back(r1);
+    }
+    DeviceTemp rp, ci, va;
+    CNMF_TRY(rp.alloc(sizeof(long long) * ((size_t)n + 1), std::string(what) + ": row_ptr"));
+    CNMF_TRY(ci.alloc(sizeof(int) * (size_t)stage, std::string(what) + ": column indices"));
+    CNMF_TRY(va.alloc(sizeof(T) * (size_t)stage, std::string(what) + ": values"));
+    CNMF_CUDA_CHECK(cudaMemcpyAsync(rp.p, row_ptr, sizeof(long long) * ((size_t)n + 1), cudaMemcpyHostToDevice, s));
+    for (size_t i = 0; i + 1 < cuts.size(); ++i) {
+      const int r0 = cuts[i], r1 = cuts[i + 1];
+      const long long base = row_ptr[r0], cnt = row_ptr[r1] - base;
+      if (cnt == 0) continue;
+      CNMF_CUDA_CHECK(cudaMemcpyAsync(ci.p, col_idx + base, sizeof(int) * cnt, cudaMemcpyHostToDevice, s));
+      CNMF_CUDA_CHECK(cudaMemcpyAsync(va.p, values + base, sizeof(T) * cnt, cudaMemcpyHostToDevice, s));
+      CNMF_TRY(csr_scatter_rows(rp.as<long long>(), base, ci.as<int>(), va.as<T>(), r0, r1, X, d->ld_c, s));
+      d->h->launches += 1;
+    }
+    CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
+    return 0;
+  };
+}
+
+}  // namespace
+
+extern "C" {
+
+int cnmf_dataset_create(cnmf_handle_t h, const float* X, int n_rows, int n_cols, long long ld, int src_is_device,
+                        int precision, void* stream, cnmf_dataset_t* out) {
+  CNMF_REQUIRE(h && X && out, "dataset_create: NULL argument");
+  CNMF_REQUIRE(n_rows > 0 && n_cols > 0 && ld >= n_cols, "dataset_create: bad shape");
+  CNMF_REQUIRE(float_precision(precision), "dataset_create: bad precision");
+  cudaStream_t s = as_stream(stream);
+  return create_dense<float>(h, n_rows, n_cols, precision, s, out,
+                             copy_fill(X, ld, n_rows, n_cols, src_is_device != 0, s));
+}
+
+int cnmf_dataset_create_from_csr(cnmf_handle_t h, int n_rows, int n_cols, long long nnz, const int64_t* row_ptr,
+                                 const int32_t* col_idx, const float* values, int precision, void* stream,
+                                 cnmf_dataset_t* out) {
+  CNMF_REQUIRE(h && row_ptr && out && (nnz == 0 || (col_idx && values)), "dataset_create_from_csr: NULL argument");
+  CNMF_REQUIRE(n_rows > 0 && n_cols > 0 && nnz >= 0, "dataset_create_from_csr: bad shape");
+  CNMF_REQUIRE(float_precision(precision), "dataset_create_from_csr: bad precision");
+  CNMF_TRY(check_csr("dataset_create_from_csr", n_rows, n_cols, nnz, row_ptr, col_idx));
+  cudaStream_t s = as_stream(stream);
+  return create_dense<float>(h, n_rows, n_cols, precision, s, out,
+                             csr_fill(row_ptr, col_idx, values, "dataset_create_from_csr", s));
+}
+
+int cnmf_dataset_create_from_csr_f64(cnmf_handle_t h, int n_rows, int n_cols, long long nnz, const int64_t* row_ptr,
+                                     const int32_t* col_idx, const double* values, void* stream, cnmf_dataset_t* out) {
+  CNMF_REQUIRE(h && row_ptr && out && (nnz == 0 || (col_idx && values)), "dataset_create_from_csr_f64: NULL argument");
+  CNMF_REQUIRE(n_rows > 0 && n_cols > 0 && nnz >= 0, "dataset_create_from_csr_f64: bad shape");
+  CNMF_TRY(check_csr("dataset_create_from_csr_f64", n_rows, n_cols, nnz, row_ptr, col_idx));
+  cudaStream_t s = as_stream(stream);
+  return create_dense<double>(h, n_rows, n_cols, CNMF_PRECISION_FP64, s, out,
+                              csr_fill(row_ptr, col_idx, values, "dataset_create_from_csr_f64", s));
+}
+
+int cnmf_dataset_create_csr(cnmf_handle_t h, int n_rows, int n_cols, long long nnz, const int64_t* row_ptr,
+                            const int32_t* col_idx, const float* values, int precision, void* stream,
+                            cnmf_dataset_t* out) {
+  CNMF_REQUIRE(h && row_ptr && out && (nnz == 0 || (col_idx && values)), "dataset_create_csr: NULL argument");
+  CNMF_REQUIRE(n_rows > 0 && n_cols > 0 && nnz >= 0, "dataset_create_csr: bad shape");
+  CNMF_REQUIRE(float_precision(precision), "dataset_create_csr: bad precision");
+  CNMF_TRY(check_csr("dataset_create_csr", n_rows, n_cols, nnz, row_ptr, col_idx));
+  cudaStream_t s = as_stream(stream);
+  CNMF_CUDA_CHECK(cudaSetDevice(h->device));
+  auto* d = new cnmf_dataset_s(h, n_rows, n_cols, precision);
+  d->sparse = true;
+  d->nnz = nnz;
+  int rc = 0;
+  {
+    DeviceTemp rp, ci, va;      // the CSR upload, released before return
+    rc = rp.alloc(sizeof(long long) * ((size_t)n_rows + 1), "dataset_create_csr: row_ptr");
+    if (rc == 0) rc = ci.alloc(sizeof(int) * (size_t)nnz, "dataset_create_csr: column indices");
+    if (rc == 0) rc = va.alloc(sizeof(float) * (size_t)nnz, "dataset_create_csr: values");
+    cudaError_t e = cudaSuccess;
+    if (rc == 0) e = cudaMemcpyAsync(rp.p, row_ptr, sizeof(long long) * ((size_t)n_rows + 1), cudaMemcpyHostToDevice, s);
+    if (rc == 0 && e == cudaSuccess && nnz > 0)
+      e = cudaMemcpyAsync(ci.p, col_idx, sizeof(int) * (size_t)nnz, cudaMemcpyHostToDevice, s);
+    if (rc == 0 && e == cudaSuccess && nnz > 0)
+      e = cudaMemcpyAsync(va.p, values, sizeof(float) * (size_t)nnz, cudaMemcpyHostToDevice, s);
+    if (e != cudaSuccess) {
+      set_last_error(std::string("dataset_create_csr: upload failed: ") + cudaGetErrorString(e));
+      rc = -2;
+    }
+    if (rc == 0) rc = csr_to_csc(d, rp.as<long long>(), ci.as<int>(), va.as<float>(), s);
+    cudaStreamSynchronize(s);
+  }
   if (rc != 0) {
     cnmf_dataset_destroy(d);
     return rc;
@@ -452,34 +598,8 @@ int cnmf_dataset_create_f64(cnmf_handle_t h, const double* X, int n_rows, int n_
   CNMF_REQUIRE(h && X && out, "dataset_create_f64: NULL argument");
   CNMF_REQUIRE(n_rows > 0 && n_cols > 0 && ld >= n_cols, "dataset_create_f64: bad shape");
   cudaStream_t s = as_stream(stream);
-  CNMF_CUDA_CHECK(cudaSetDevice(h->device));
-  auto* d = new cnmf_dataset_s(h, n_rows, n_cols, CNMF_PRECISION_FP64);
-  d->form = Form::FP64;
-  const size_t nx = (size_t)n_rows * d->ld_c;
-  float* buf = nullptr;
-  int rc = dataset_alloc(d, &buf, 2 * nx);
-  if (rc == 0) {
-    d->X64 = reinterpret_cast<double*>(buf);
-    cudaError_t e = cudaMemsetAsync(d->X64, 0, nx * sizeof(double), s);
-    if (e == cudaSuccess)
-      e = cudaMemcpy2DAsync(d->X64, (size_t)d->ld_c * sizeof(double), X, (size_t)ld * sizeof(double),
-                            (size_t)n_cols * sizeof(double), n_rows,
-                            src_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s);
-    if (e != cudaSuccess) {
-      set_last_error(std::string("dataset upload failed: ") + cudaGetErrorString(e));
-      rc = -2;
-    }
-  }
-  double sums[2] = {0.0, 0.0};
-  if (rc == 0) rc = matrix_sums_f64(h, d->X64, n_rows, n_cols, d->ld_c, sums, s);
-  if (rc != 0) {
-    cnmf_dataset_destroy(d);
-    return rc;
-  }
-  d->sum = sums[0];
-  d->sum_sq = sums[1];
-  *out = d;
-  return 0;
+  return create_dense<double>(h, n_rows, n_cols, CNMF_PRECISION_FP64, s, out,
+                              copy_fill(X, ld, n_rows, n_cols, src_is_device != 0, s));
 }
 
 int cnmf_dataset_min(cnmf_dataset_t d, float* min_host, void* stream) {

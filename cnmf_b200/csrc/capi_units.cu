@@ -423,6 +423,9 @@ extern "C" int cnmf_dataset_operand_host(cnmf_dataset_t d, int which, void* out_
     case CNMF_OPERAND_XT_H16: src = d->Xt_h16; size = 2 * nxt; break;
     case CNMF_OPERAND_ROW_SCALE: src = d->row_scale; size = 4LL * d->ld_r; break;
     case CNMF_OPERAND_COL_SCALE: src = d->col_scale; size = 4LL * d->ld_c; break;
+    case CNMF_OPERAND_CSC_COL_PTR: src = d->col_ptr; size = 8LL * (d->n_cols + 1); break;
+    case CNMF_OPERAND_CSC_ROW_IDX: src = d->row_idx; size = 4LL * d->nnz; break;
+    case CNMF_OPERAND_CSC_VALUES: src = d->vals; size = 4LL * d->nnz; break;
     default: CNMF_REQUIRE(false, "dataset_operand: unknown array");
   }
   if (!src) {

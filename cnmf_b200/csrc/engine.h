@@ -223,6 +223,46 @@ int csc_gather_cols(const cnmf_dataset_s* d, const int* cols, const float* scale
 // device totals (n_rows): fp64 row sums; col_sums (2 x n_cols): per column sum(v), sum(v^2) of v = x * target_sum /
 // (row total), 0 for a row without counts.  Fixed reduction order, no floating-point atomics.  Does not synchronise.
 int csc_tpm_sums(const cnmf_dataset_s* d, double target_sum, double* totals, double* col_sums, cudaStream_t s);
+// a temporary device array outside the handle's pool, freed when it goes out of scope: the owner synchronises the
+// stream that uses it first
+struct DeviceTemp {
+  void* p = nullptr;
+  DeviceTemp() = default;
+  DeviceTemp(const DeviceTemp&) = delete;
+  DeviceTemp& operator=(const DeviceTemp&) = delete;
+  ~DeviceTemp() {
+    if (p) cudaFree(p);
+  }
+  int alloc(size_t bytes, const std::string& what) {
+    const cudaError_t e = cudaMalloc(&p, bytes < 256 ? 256 : bytes);
+    if (e != cudaSuccess) {
+      p = nullptr;
+      set_last_error(what + ": cudaMalloc(" + std::to_string(bytes) + " bytes) failed: " + cudaGetErrorString(e));
+      return -2;
+    }
+    return 0;
+  }
+  template <class T>
+  T* as() const { return static_cast<T*>(p); }
+};
+// a host CSR matrix (row_ptr from 0 to nnz, col_idx strictly increasing within each row and in [0, n_cols)) checked
+// before any device work: the device kernels below rely on it
+int check_csr(const char* what, int n_rows, int n_cols, long long nnz, const int64_t* row_ptr, const int32_t* col_idx);
+// A sparse dataset d (shape, precision, nnz and sparse set) from a canonical CSR matrix in device arrays: the canonical
+// CSC arrays of d (owned by d) by a column histogram per block of CSR_ROW_BLOCK rows, a per-column scan over the
+// blocks, a 64-bit scan of the column totals into d->col_ptr, and a scatter in which each row block walks its rows in
+// order -- no atomic decides a position, so the row indices of a column come out increasing -- then the chunk table,
+// column sums and form as cnmf_dataset_create_csc makes them.  The row block grows when the per-block count table
+// (blocks x n_cols ints, freed before return) would exceed CSR_COUNT_BUDGET ints.  Synchronises.
+constexpr int CSR_ROW_BLOCK = 256;
+constexpr long long CSR_COUNT_BUDGET = 1LL << 25;
+int csr_to_csc(cnmf_dataset_s* d, const long long* row_ptr, const int* col_idx, const float* vals, cudaStream_t s);
+// rows [r0, r1) of a canonical CSR matrix into a zeroed dense matrix: X[r][col_idx[j]] = vals[j], with row_ptr[r] -
+// base indexing col_idx / vals (a staged slice).  Does not synchronise.
+int csr_scatter_rows(const long long* row_ptr, long long base, const int* col_idx, const float* vals, int r0, int r1,
+                     float* X, int ld, cudaStream_t s);
+int csr_scatter_rows(const long long* row_ptr, long long base, const int* col_idx, const double* vals, int r0, int r1,
+                     double* X, int ld, cudaStream_t s);
 
 // ---- NNDSVD starts on the device: gemm_f64.cu, nndsvd.cu
 // C (M x n_out, row stride ldc) = A (M x K, row stride lda) * op(X) in fp64 for the dataset matrix X (n_rows x n_cols,

@@ -271,6 +271,134 @@ __global__ void __launch_bounds__(WARPS * 32) csc_gather_cols_kernel(const long 
   for (long long j = col_ptr[src] + lane; j < col_ptr[src + 1]; j += 32) dst[(long long)row_idx[j] * ld_dst + c] = vals[j] * f;
 }
 
+// CSR -> CSC (csr_to_csc).  Row block b holds rows [b * rb, min((b + 1) * rb, n_rows)); its entries are one contiguous
+// range of the CSR arrays.  cnt[b * n_cols + c]: entries of column c in block b.
+// Pass 1: the counts.  Integer atomics only count; no position depends on their order.
+__global__ void csr_block_hist_kernel(const long long* __restrict__ row_ptr, const int* __restrict__ col_idx, int n_rows,
+                                      int n_cols, int rb, int* __restrict__ cnt) {
+  const long long r0 = (long long)blockIdx.x * rb, r1 = min(r0 + rb, (long long)n_rows);
+  int* c = cnt + (long long)blockIdx.x * n_cols;
+  for (long long j = row_ptr[r0] + threadIdx.x; j < row_ptr[r1]; j += blockDim.x) atomicAdd(&c[col_idx[j]], 1);
+}
+
+// Pass 2, one thread per column: the counts become exclusive prefixes over the blocks (where block b's entries of the
+// column start within it) and col_tot[c] the column's length
+__global__ void csr_block_scan_kernel(int* __restrict__ cnt, int n_blocks, int n_cols, long long* __restrict__ col_tot) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= n_cols) return;
+  int run = 0;
+  for (int b = 0; b < n_blocks; ++b) {
+    int* p = cnt + (long long)b * n_cols + c;
+    const int t = *p;
+    *p = run;
+    run += t;
+  }
+  col_tot[c] = run;
+}
+
+// Pass 3, one block: out[0..n] = exclusive prefix sums of in[0..n-1], 64-bit (col_ptr from the column lengths)
+constexpr int SCAN_THREADS = 1024;
+__global__ void __launch_bounds__(SCAN_THREADS) exclusive_scan_ll_kernel(const long long* __restrict__ in, int n,
+                                                                         long long* __restrict__ out) {
+  __shared__ long long part[SCAN_THREADS];
+  const long long per = (n + SCAN_THREADS - 1) / SCAN_THREADS;
+  const long long beg = threadIdx.x * per, end = min(beg + per, (long long)n);
+  long long s = 0;
+  for (long long i = beg; i < end; ++i) s += in[i];
+  part[threadIdx.x] = s;
+  __syncthreads();
+  for (int o = 1; o < SCAN_THREADS; o <<= 1) {      // inclusive scan of the thread totals
+    const long long v = threadIdx.x >= o ? part[threadIdx.x - o] : 0;
+    __syncthreads();
+    part[threadIdx.x] += v;
+    __syncthreads();
+  }
+  long long run = threadIdx.x > 0 ? part[threadIdx.x - 1] : 0;
+  for (long long i = beg; i < end; ++i) {
+    out[i] = run;
+    run += in[i];
+  }
+  if (threadIdx.x == SCAN_THREADS - 1) out[n] = part[SCAN_THREADS - 1];
+}
+
+// Pass 4: block b walks its rows in order; the entries of one canonical row have distinct columns, so the threads of a
+// row never share a cursor (next[b * n_cols + c], block b's next slot in column c), and the barrier orders the rows:
+// each column receives its rows in increasing order.
+__global__ void csr_block_scatter_kernel(const long long* __restrict__ row_ptr, const int* __restrict__ col_idx,
+                                         const float* __restrict__ vals, int n_rows, int n_cols, int rb,
+                                         const long long* __restrict__ col_ptr, int* next, int* __restrict__ row_out,
+                                         float* __restrict__ val_out) {
+  const int r0 = (int)min((long long)blockIdx.x * rb, (long long)n_rows);
+  const int r1 = (int)min((long long)r0 + rb, (long long)n_rows);
+  int* nx = next + (long long)blockIdx.x * n_cols;
+  for (int r = r0; r < r1; ++r) {
+    for (long long j = row_ptr[r] + threadIdx.x; j < row_ptr[r + 1]; j += blockDim.x) {
+      const int c = col_idx[j];
+      const long long p = col_ptr[c] + nx[c];
+      nx[c] += 1;
+      row_out[p] = r;
+      val_out[p] = vals[j];
+    }
+    __syncthreads();
+  }
+}
+
+// one warp per row of [r0, r1): X[r][col_idx[j]] = vals[j] (a canonical row: no two lanes write one element)
+template <class T>
+__global__ void __launch_bounds__(WARPS * 32) csr_scatter_rows_kernel(const long long* __restrict__ row_ptr,
+                                                                      long long base, const int* __restrict__ col_idx,
+                                                                      const T* __restrict__ vals, int r0, int r1,
+                                                                      T* __restrict__ X, int ld) {
+  const long long r = r0 + (long long)blockIdx.x * WARPS + (threadIdx.x >> 5);
+  if (r >= r1) return;
+  T* row = X + r * ld;
+  const long long end = row_ptr[r + 1] - base;
+  for (long long j = row_ptr[r] - base + (threadIdx.x & 31); j < end; j += 32) row[col_idx[j]] = vals[j];
+}
+
+template <class T>
+int launch_csr_scatter_rows(const long long* row_ptr, long long base, const int* col_idx, const T* vals, int r0, int r1,
+                            T* X, int ld, cudaStream_t s) {
+  if (r1 <= r0) return 0;
+  const unsigned blocks = (unsigned)((r1 - r0 + WARPS - 1) / WARPS);
+  csr_scatter_rows_kernel<T><<<blocks, WARPS * 32, 0, s>>>(row_ptr, base, col_idx, vals, r0, r1, X, ld);
+  CNMF_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+// device arrays owned by d (from the handle's pool when one fits), typed
+template <class T>
+int alloc_owned(cnmf_dataset_s* d, T** p, size_t count) {
+  float* q = nullptr;
+  const int rc = dataset_alloc(d, &q, (count * sizeof(T) + 3) / 4);
+  *p = reinterpret_cast<T*>(q);
+  return rc;
+}
+
+// chunk table of csc_project_kernel from a host col_ptr, which is checked monotone on the way
+int csc_item_table(const int64_t* col_ptr, int n_cols, std::vector<int>* item_ptr) {
+  item_ptr->assign(n_cols + 1, 0);
+  long long items = 0;
+  for (int c = 0; c < n_cols; ++c) {
+    CNMF_REQUIRE(col_ptr[c + 1] >= col_ptr[c], "CSC dataset: col_ptr is not monotone");
+    (*item_ptr)[c] = (int)items;
+    items += (col_ptr[c + 1] - col_ptr[c] + CSC_CHUNK - 1) / CSC_CHUNK;
+    CNMF_REQUIRE(items < (1LL << 31), "CSC dataset: too many entries");
+  }
+  (*item_ptr)[n_cols] = (int)items;
+  return 0;
+}
+
+// the rest of every CSC dataset creation once its three arrays are resident: chunk table, column sums, form
+int csc_finish(cnmf_dataset_s* d, const std::vector<int>& item_ptr, cudaStream_t s) {
+  d->n_items = item_ptr[d->n_cols];
+  CNMF_TRY(alloc_owned(d, &d->item_ptr, (size_t)d->n_cols + 1));
+  CNMF_TRY(alloc_owned(d, &d->col_sums, 2 * (size_t)d->n_cols));
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(d->item_ptr, item_ptr.data(), sizeof(int) * (d->n_cols + 1), cudaMemcpyHostToDevice, s));
+  CNMF_TRY(csc_col_stats(d, s));    // synchronises: item_ptr may go out of scope afterwards
+  return dataset_resolve_form(d, false, s);
+}
+
 }  // namespace
 
 namespace cnmf {
@@ -387,6 +515,60 @@ int stage_rows(cnmf_handle_s* h, const float* F, int k, int n, int ld, int kp, f
   return 0;
 }
 
+int check_csr(const char* what, int n_rows, int n_cols, long long nnz, const int64_t* row_ptr, const int32_t* col_idx) {
+  const std::string w(what);
+  CNMF_REQUIRE(row_ptr[0] == 0 && row_ptr[n_rows] == nnz, w + ": row_ptr must start at 0 and end at nnz");
+  for (int r = 0; r < n_rows; ++r) {
+    CNMF_REQUIRE(row_ptr[r + 1] >= row_ptr[r], w + ": row_ptr is not monotone");
+    for (long long j = row_ptr[r]; j < row_ptr[r + 1]; ++j) {
+      CNMF_REQUIRE(col_idx[j] >= 0 && col_idx[j] < n_cols, w + ": column index out of range");
+      CNMF_REQUIRE(j == row_ptr[r] || col_idx[j] > col_idx[j - 1],
+                   w + ": column indices must increase within a row (canonical CSR: sorted, no duplicates)");
+    }
+  }
+  return 0;
+}
+
+int csr_to_csc(cnmf_dataset_s* d, const long long* row_ptr, const int* col_idx, const float* vals, cudaStream_t s) {
+  cnmf_handle_s* h = d->h;
+  const int n_rows = d->n_rows, n_cols = d->n_cols;
+  const long long max_blocks = std::max(1LL, CSR_COUNT_BUDGET / n_cols);
+  long long rb = CSR_ROW_BLOCK;
+  if ((n_rows + rb - 1) / rb > max_blocks) rb = (n_rows + max_blocks - 1) / max_blocks;
+  const int n_blocks = (int)((n_rows + rb - 1) / rb);
+  CNMF_TRY(alloc_owned(d, &d->col_ptr, (size_t)n_cols + 1));
+  CNMF_TRY(alloc_owned(d, &d->row_idx, (size_t)d->nnz));
+  CNMF_TRY(alloc_owned(d, &d->vals, (size_t)d->nnz));
+  DeviceTemp cnt, col_tot;
+  CNMF_TRY(cnt.alloc(sizeof(int) * (size_t)n_blocks * n_cols, "dataset_create_csr: block counts"));
+  CNMF_TRY(col_tot.alloc(sizeof(long long) * (size_t)n_cols, "dataset_create_csr: column lengths"));
+  CNMF_CUDA_CHECK(cudaMemsetAsync(cnt.p, 0, sizeof(int) * (size_t)n_blocks * n_cols, s));
+  csr_block_hist_kernel<<<n_blocks, 256, 0, s>>>(row_ptr, col_idx, n_rows, n_cols, (int)rb, cnt.as<int>());
+  csr_block_scan_kernel<<<(n_cols + 255) / 256, 256, 0, s>>>(cnt.as<int>(), n_blocks, n_cols, col_tot.as<long long>());
+  exclusive_scan_ll_kernel<<<1, SCAN_THREADS, 0, s>>>(col_tot.as<long long>(), n_cols, d->col_ptr);
+  csr_block_scatter_kernel<<<n_blocks, 256, 0, s>>>(row_ptr, col_idx, vals, n_rows, n_cols, (int)rb, d->col_ptr,
+                                                     cnt.as<int>(), d->row_idx, d->vals);
+  h->launches += 4;
+  CNMF_CUDA_CHECK(cudaGetLastError());
+  std::vector<int64_t> col_ptr(n_cols + 1);
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(col_ptr.data(), d->col_ptr, sizeof(long long) * (n_cols + 1), cudaMemcpyDeviceToHost,
+                                  s));
+  CNMF_CUDA_CHECK(cudaStreamSynchronize(s));      // the count table is released on return
+  std::vector<int> item_ptr;
+  CNMF_TRY(csc_item_table(col_ptr.data(), n_cols, &item_ptr));
+  return csc_finish(d, item_ptr, s);
+}
+
+int csr_scatter_rows(const long long* row_ptr, long long base, const int* col_idx, const float* vals, int r0, int r1,
+                     float* X, int ld, cudaStream_t s) {
+  return launch_csr_scatter_rows(row_ptr, base, col_idx, vals, r0, r1, X, ld, s);
+}
+
+int csr_scatter_rows(const long long* row_ptr, long long base, const int* col_idx, const double* vals, int r0, int r1,
+                     double* X, int ld, cudaStream_t s) {
+  return launch_csr_scatter_rows(row_ptr, base, col_idx, vals, r0, r1, X, ld, s);
+}
+
 }  // namespace cnmf
 
 extern "C" {
@@ -400,16 +582,8 @@ int cnmf_dataset_create_csc(cnmf_handle_t h, int n_rows, int n_cols, long long n
                    precision == CNMF_PRECISION_TF32X3_GENERAL || precision == CNMF_PRECISION_F16X2,
                "dataset_create_csc: bad precision");
   CNMF_REQUIRE(col_ptr[0] == 0 && col_ptr[n_cols] == nnz, "dataset_create_csc: col_ptr must start at 0 and end at nnz");
-  // chunk table of csc_project_kernel, built while col_ptr is checked
-  std::vector<int> item_ptr(n_cols + 1);
-  long long items = 0;
-  for (int c = 0; c < n_cols; ++c) {
-    CNMF_REQUIRE(col_ptr[c + 1] >= col_ptr[c], "dataset_create_csc: col_ptr is not monotone");
-    item_ptr[c] = (int)items;
-    items += (col_ptr[c + 1] - col_ptr[c] + CSC_CHUNK - 1) / CSC_CHUNK;
-    CNMF_REQUIRE(items < (1LL << 31), "dataset_create_csc: too many entries");
-  }
-  item_ptr[n_cols] = (int)items;
+  std::vector<int> item_ptr;
+  CNMF_TRY(csc_item_table(col_ptr, n_cols, &item_ptr));
   for (long long j = 0; j < nnz; ++j)
     CNMF_REQUIRE(row_idx[j] >= 0 && row_idx[j] < n_rows, "dataset_create_csc: row index out of range");
   cudaStream_t s = as_stream(stream);
@@ -417,13 +591,6 @@ int cnmf_dataset_create_csc(cnmf_handle_t h, int n_rows, int n_cols, long long n
   auto* d = new cnmf_dataset_s(h, n_rows, n_cols, precision);
   d->sparse = true;
   d->nnz = nnz;
-  d->n_items = (int)items;
-  auto alloc = [&](auto** p, size_t bytes) {
-    float* q = nullptr;
-    const int rc = dataset_alloc(d, &q, (bytes + 3) / 4);
-    *p = reinterpret_cast<std::remove_pointer_t<decltype(p)>>(q);
-    return rc;
-  };
   auto upload = [&](void* dst, const void* src, size_t bytes) {
     if (bytes == 0) return 0;
     const cudaError_t e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, s);
@@ -433,17 +600,13 @@ int cnmf_dataset_create_csc(cnmf_handle_t h, int n_rows, int n_cols, long long n
     }
     return 0;
   };
-  int rc = alloc(&d->col_ptr, sizeof(long long) * (n_cols + 1));
-  if (rc == 0) rc = alloc(&d->row_idx, sizeof(int) * (size_t)nnz);
-  if (rc == 0) rc = alloc(&d->vals, sizeof(float) * (size_t)nnz);
-  if (rc == 0) rc = alloc(&d->item_ptr, sizeof(int) * (n_cols + 1));
-  if (rc == 0) rc = alloc(&d->col_sums, sizeof(double) * 2 * (size_t)n_cols);
+  int rc = alloc_owned(d, &d->col_ptr, (size_t)n_cols + 1);
+  if (rc == 0) rc = alloc_owned(d, &d->row_idx, (size_t)nnz);
+  if (rc == 0) rc = alloc_owned(d, &d->vals, (size_t)nnz);
   if (rc == 0) rc = upload(d->col_ptr, col_ptr, sizeof(long long) * (n_cols + 1));
   if (rc == 0) rc = upload(d->row_idx, row_idx, sizeof(int) * (size_t)nnz);
   if (rc == 0) rc = upload(d->vals, values, sizeof(float) * (size_t)nnz);
-  if (rc == 0) rc = upload(d->item_ptr, item_ptr.data(), sizeof(int) * (n_cols + 1));
-  if (rc == 0) rc = csc_col_stats(d, s);    // synchronises: item_ptr may go out of scope afterwards
-  if (rc == 0) rc = dataset_resolve_form(d, false, s);
+  if (rc == 0) rc = csc_finish(d, item_ptr, s);
   if (rc != 0) {
     cudaStreamSynchronize(s);
     cnmf_dataset_destroy(d);

@@ -157,6 +157,16 @@ def loss_code(beta):
                                   "'itakura-saito' (0) on the CUDA path (got %r)" % (beta,))
 
 
+def _csr_arrays(C, dtype):
+    """(row_ptr int64, col_idx int32, values as dtype) of the scipy CSR matrix C in canonical form: column indices sorted
+    within each row, duplicates summed in C's own dtype (C itself is left as it is)."""
+    if not C.has_canonical_format:
+        C = C.copy()
+        C.sum_duplicates()
+    return (np.ascontiguousarray(C.indptr, dtype=np.int64), np.ascontiguousarray(C.indices, dtype=np.int32),
+            np.ascontiguousarray(C.data, dtype=dtype))
+
+
 class Engine:
     """One per process and GPU: owns the library handle and its cached device workspace."""
 
@@ -219,11 +229,19 @@ class Engine:
         entry; no dense copy is made on the host or the device.  Serves the consensus step's TPM uses: sums, col_stats,
         project_rows, from_columns (returns a dense dataset) and refit(transposed=True) with the Frobenius loss; and
         prepare's uses of raw counts: tpm_stats, col_stats, from_columns.  Everything else raises CnmfError.
-        precision='fp64' has no sparse form."""
+        precision='fp64' has no sparse form.  A CSR matrix is transposed on the device (only its stored entries are
+        copied); any other input is converted to CSC on the host."""
         if is_fp64(precision):
             raise NotImplementedError("cnmf_b200: precision='fp64' needs a dense dataset; sparse (CSC) datasets hold "
                                       "float32 values")
         import scipy.sparse as sp
+        out = ctypes.c_void_p()
+        if sp.issparse(X) and X.format == "csr":
+            n, g = X.shape
+            row_ptr, col_idx, vals = _csr_arrays(sp.csr_matrix(X, dtype=np.float32), np.float32)
+            check(self.lib.cnmf_dataset_create_csr(self._h, n, g, int(row_ptr[-1]), ptr(row_ptr), ptr(col_idx),
+                                                   ptr(vals), precision_code(precision), stream, ctypes.byref(out)))
+            return Dataset(self, None, precision, _handle=out, sparse=True)
         C = sp.csc_matrix(X, dtype=np.float32)
         if not C.has_canonical_format:          # sorted row indices, no duplicates: the library does not sort
             C = C.copy()
@@ -232,7 +250,6 @@ class Engine:
         col_ptr = np.ascontiguousarray(C.indptr, dtype=np.int64)
         row_idx = np.ascontiguousarray(C.indices, dtype=np.int32)
         vals = np.ascontiguousarray(C.data, dtype=np.float32)
-        out = ctypes.c_void_p()
         check(self.lib.cnmf_dataset_create_csc(self._h, n, g, int(col_ptr[-1]), ptr(col_ptr), ptr(row_idx), ptr(vals),
                                                precision_code(precision), stream, ctypes.byref(out)))
         return Dataset(self, None, precision, _handle=out, sparse=True)
@@ -428,9 +445,20 @@ class Dataset:
         self._d = ctypes.c_void_p()
         if _handle is not None:
             self._d = _handle
+        elif hasattr(X, "toarray"):
+            # scipy sparse: the stored entries go to the device and are scattered into the dense dataset there -- the
+            # same dataset X.toarray() would give, without a cells x genes array on the host
+            import scipy.sparse as sp
+            n, g = X.shape
+            row_ptr, col_idx, vals = _csr_arrays(sp.csr_matrix(X), np.float64 if self.fp64 else np.float32)
+            nnz = int(row_ptr[-1])
+            if self.fp64:
+                check(self.lib.cnmf_dataset_create_from_csr_f64(engine._h, n, g, nnz, ptr(row_ptr), ptr(col_idx),
+                                                                ptr(vals), stream, ctypes.byref(self._d)))
+            else:
+                check(self.lib.cnmf_dataset_create_from_csr(engine._h, n, g, nnz, ptr(row_ptr), ptr(col_idx), ptr(vals),
+                                                            self.precision, stream, ctypes.byref(self._d)))
         else:
-            if hasattr(X, "toarray"):       # scipy sparse: the CUDA path is dense (DESIGN.md)
-                X = X.toarray()
             if self.fp64:
                 X = f64c(X)
                 n, g = X.shape
@@ -556,13 +584,23 @@ class Dataset:
     def operand(self, name):
         """Test hook: copy of one resident array, padding included (None when the dataset does not hold it):
         X, X_hi, X_lo (n_rows x ld_cols float32), Xt, Xt_hi, Xt_lo (n_cols x ld_rows float32), X_h16 / Xt_h16 (the
-        same shapes in float16), row_scale (ld_rows), col_scale (ld_cols)."""
+        same shapes in float16), row_scale (ld_rows), col_scale (ld_cols); on sparse datasets csc_col_ptr (n_cols + 1,
+        int64), csc_row_idx (nnz, int32), csc_values (nnz)."""
         ld_r, ld_c = self.ld()
         n, g = self.shape
-        shape = {"X": (n, ld_c), "X_hi": (n, ld_c), "X_lo": (n, ld_c), "X_h16": (n, ld_c),
-                 "Xt": (g, ld_r), "Xt_hi": (g, ld_r), "Xt_lo": (g, ld_r), "Xt_h16": (g, ld_r),
-                 "row_scale": (ld_r,), "col_scale": (ld_c,)}[name]
-        out = np.empty(shape, np.float16 if name.endswith("h16") else np.float32)
+        if name == "csc_col_ptr":
+            shape, dtype = (g + 1,), np.int64
+        elif name in ("csc_row_idx", "csc_values"):
+            col_ptr = self.operand("csc_col_ptr")
+            if col_ptr is None:
+                return None
+            shape, dtype = (int(col_ptr[-1]),), np.int32 if name == "csc_row_idx" else np.float32
+        else:
+            shape = {"X": (n, ld_c), "X_hi": (n, ld_c), "X_lo": (n, ld_c), "X_h16": (n, ld_c),
+                     "Xt": (g, ld_r), "Xt_hi": (g, ld_r), "Xt_lo": (g, ld_r), "Xt_h16": (g, ld_r),
+                     "row_scale": (ld_r,), "col_scale": (ld_c,)}[name]
+            dtype = np.float16 if name.endswith("h16") else np.float32
+        out = np.empty(shape, dtype)
         rc = self.lib.cnmf_dataset_operand_host(self._d, _lib.OPERANDS[name], ptr(out), out.nbytes)
         if rc == -3:
             return None

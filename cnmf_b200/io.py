@@ -106,13 +106,76 @@ def read_matrix(path):
     raise FileNotFoundError(path)
 
 
+def make_index_unique(names, join="-"):
+    """anndata.utils.make_index_unique: the first occurrence keeps its name, each later duplicate v becomes v-1, v-2, ...
+    (one counter per name), skipping any candidate already present."""
+    names = pd.Index(names)
+    if names.is_unique:
+        return names
+    values = names.values.copy()
+    dup = names.duplicated(keep="first")
+    taken = set(values)
+    counter = {}
+    renamed = []
+    for v in values[dup]:
+        while True:
+            counter[v] = counter.get(v, 0) + 1
+            candidate = v + join + str(counter[v])
+            if candidate not in taken:
+                taken.add(candidate)
+                renamed.append(candidate)
+                break
+    values[dup] = renamed
+    return pd.Index(values)
+
+
+def _read_tsv_column(path, col):
+    if not os.path.exists(path):
+        raise FileNotFoundError(path)
+    # names are the file's text (no NA parsing): 10x identifiers and symbols are strings
+    return pd.read_csv(path, header=None, sep="\t", dtype=str, keep_default_na=False, usecols=[col])[col].values
+
+
+def read_10x_mtx(path):
+    """scanpy.read_10x_mtx(path) with its defaults (var_names='gene_symbols', make_unique=True, gex_only=True) as a
+    CellGeneMatrix holding canonical float32 CSR (cells x genes).  The legacy (Cell Ranger 2) layout, recognised by
+    genes.tsv, is matrix.mtx / genes.tsv / barcodes.tsv; otherwise matrix.mtx.gz / features.tsv.gz / barcodes.tsv.gz,
+    of which only the 'Gene Expression' features are kept.  The genes x cells matrix is cast to float32 before its
+    duplicates are summed, as scanpy's read_mtx does.  Needs scipy only."""
+    import scipy.io
+    import scipy.sparse as sp
+    legacy = os.path.isfile(os.path.join(path, "genes.tsv"))
+    suffix = "" if legacy else ".gz"
+    mtx = os.path.join(path, "matrix.mtx" + suffix)
+    features = os.path.join(path, ("genes" if legacy else "features") + ".tsv" + suffix)
+    barcodes = os.path.join(path, "barcodes.tsv" + suffix)
+    for fn in (mtx, features, barcodes):
+        if not os.path.exists(fn):
+            raise FileNotFoundError(fn)
+    with warnings.catch_warnings():        # scipy >= 1.18 announces sparse arrays as mmread's future return type
+        warnings.simplefilter("ignore", DeprecationWarning)
+        M = scipy.io.mmread(mtx)
+    X = sp.csr_matrix(sp.coo_matrix(M).astype(np.float32).T)      # duplicates summed here
+    var_names = make_index_unique(_read_tsv_column(features, 1))
+    obs_names = _read_tsv_column(barcodes, 0)
+    if len(var_names) != X.shape[1] or len(obs_names) != X.shape[0]:
+        raise ValueError("%s is %d genes x %d cells, but %s names %d and %s %d" % (
+            mtx, X.shape[1], X.shape[0], features, len(var_names), barcodes, len(obs_names)))
+    if not legacy:
+        gex = _read_tsv_column(features, 2) == "Gene Expression"
+        X, var_names = X[:, np.flatnonzero(gex)], var_names[gex]
+    X.sum_duplicates()            # canonical: sorted column indices (a no-op when they already are)
+    return CellGeneMatrix(X, obs_names, var_names)
+
+
 def read_counts(counts_fn):
-    """Input counts as accepted by the reference's prepare() (cnmf.py:383-402): .h5ad, df.npz, or tab-delimited text.
-    10x .mtx directories need scanpy and are not supported here."""
+    """Input counts as accepted by the reference's prepare() (cnmf.py:383-414): .h5ad, df.npz, tab-delimited text, or
+    10x Matrix Market output given as <dir>/matrix.mtx or <dir>/matrix.mtx.gz: the directory is read as
+    scanpy.read_10x_mtx reads it (read_10x_mtx), whatever the file name."""
     if counts_fn.endswith(".h5ad"):
         return read_matrix(counts_fn)
     if counts_fn.endswith(".mtx") or counts_fn.endswith(".mtx.gz"):
-        raise NotImplementedError("10x mtx input needs scanpy.read_10x_mtx, which is outside the accelerated path")
+        return read_10x_mtx(os.path.dirname(counts_fn))
     if counts_fn.endswith(".npz"):
         df = load_df_from_npz(counts_fn)
     else:

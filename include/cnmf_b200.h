@@ -28,7 +28,8 @@
 extern "C" {
 #endif
 
-#define CNMF_B200_ABI_VERSION 17     /* 17: cnmf_dataset_form, cnmf_dataset_operand_host, cnmf_dataset_gemm_host */
+#define CNMF_B200_ABI_VERSION 18     /* 18: cnmf_dataset_create_csr, cnmf_dataset_create_from_csr / _f64, the CSC arrays
+                                      * of cnmf_dataset_operand_host */
 #define CNMF_MAX_COMPONENTS 32          /* largest n_components per restart on the CUDA path */
 
 typedef struct cnmf_handle_s* cnmf_handle_t;
@@ -107,6 +108,14 @@ int cnmf_last_timing(cnmf_handle_t h, double* rng_ms, double* h2d_ms, double* so
  * sum(X), sum(X^2).  `src_is_device` = 0: X is host memory (copied H2D inside the call). */
 int cnmf_dataset_create(cnmf_handle_t h, const float* X, int n_rows, int n_cols, long long ld,
                         int src_is_device, int precision, void* stream, cnmf_dataset_t* out);
+/* cnmf_dataset_create of the dense form of a canonical host CSR matrix (row_ptr[n_rows + 1] int64 from 0 to nnz;
+ * col_idx int32 in [0, n_cols), strictly increasing within a row -- checked; values fp32) without forming it on the
+ * host: the zeroed device matrix receives the stored entries, which cross PCIe in slices of at most 2^24 entries, then
+ * the form and the operands are built as cnmf_dataset_create builds them -- the dataset is bit-identical to the one
+ * cnmf_dataset_create makes of the dense matrix.  The staged slices are freed before the operands are built. */
+int cnmf_dataset_create_from_csr(cnmf_handle_t h, int n_rows, int n_cols, long long nnz, const int64_t* row_ptr,
+                                 const int32_t* col_idx, const float* values, int precision, void* stream,
+                                 cnmf_dataset_t* out);
 /* A cells x genes matrix kept sparse on the device: canonical CSC from the host (col_ptr[n_cols + 1] int64, monotone,
  * from 0 to nnz; row_idx int32 in [0, n_rows), increasing and unique within a column -- scipy.sparse tocsc() gives
  * exactly that; the order is not checked; values fp32), 8 bytes per stored entry.  For the TPM matrix of the consensus
@@ -117,6 +126,14 @@ int cnmf_dataset_create(cnmf_handle_t h, const float* X, int n_rows, int n_cols,
  * cnmf_dataset_is_exact reports 0 (no tensor-core product runs on it). */
 int cnmf_dataset_create_csc(cnmf_handle_t h, int n_rows, int n_cols, long long nnz, const int64_t* col_ptr,
                             const int32_t* row_idx, const float* values, int precision, void* stream,
+                            cnmf_dataset_t* out);
+/* The same sparse dataset from a canonical host CSR matrix (row_ptr[n_rows + 1] int64 from 0 to nnz; col_idx int32 in
+ * [0, n_cols), strictly increasing within a row -- checked; values fp32), transposed on the device: the CSC arrays
+ * are bit-identical to what cnmf_dataset_create_csc gets from scipy's tocsc() of the same matrix, and every result on
+ * the dataset is too.  Only the stored entries cross PCIe (12 bytes each).  The CSR upload (12 bytes per entry) and a
+ * count table of at most 128 MB are freed before the call returns. */
+int cnmf_dataset_create_csr(cnmf_handle_t h, int n_rows, int n_cols, long long nnz, const int64_t* row_ptr,
+                            const int32_t* col_idx, const float* values, int precision, void* stream,
                             cnmf_dataset_t* out);
 /* worst-case device bytes cnmf_dataset_create of an n_rows x n_cols matrix at `precision` needs while the dataset is
  * built, over the forms it can take (exact f16, exact tf32, general): what a caller compares with free memory to
@@ -197,6 +214,10 @@ int cnmf_nndsvd_gemm_host(cnmf_dataset_t d, int to_genes, int M, const double* A
  * solve_bytes_per_row.  Supported: beta_loss = frobenius, MU and CD, random (device generator) and NNDSVD starts. */
 int cnmf_dataset_create_f64(cnmf_handle_t h, const double* X, int n_rows, int n_cols, long long ld, int src_is_device,
                             void* stream, cnmf_dataset_t* out);
+/* cnmf_dataset_create_from_csr for float64 datasets: fp64 values, scattered into the zeroed fp64 X; bit-identical to
+ * cnmf_dataset_create_f64 of the dense matrix */
+int cnmf_dataset_create_from_csr_f64(cnmf_handle_t h, int n_rows, int n_cols, long long nnz, const int64_t* row_ptr,
+                                     const int32_t* col_idx, const double* values, void* stream, cnmf_dataset_t* out);
 /* new float64 dataset = src[:, cols] / divisor (cnmf.py:542, 967-969: X /= std), each entry one IEEE fp64 division */
 int cnmf_dataset_from_columns_f64(cnmf_dataset_t src, const int32_t* cols_host, const double* divisor_host, int n_cols,
                                   void* stream, cnmf_dataset_t* out);
@@ -422,12 +443,14 @@ enum { CNMF_FORM_FP32 = 0, CNMF_FORM_TF32 = 1, CNMF_FORM_TF32_EXACT = 2, CNMF_FO
 int cnmf_dataset_form(cnmf_dataset_t d);
 /* copies one resident array, padding included, to out_host; bytes must be its exact size:
  *   X, X_HI, X_LO (n_rows x ld_cols floats), XT, XT_HI, XT_LO (n_cols x ld_rows floats), X_H16 / XT_H16 (the same
- *   shapes as fp16), ROW_SCALE (ld_rows floats), COL_SCALE (ld_cols floats).
+ *   shapes as fp16), ROW_SCALE (ld_rows floats), COL_SCALE (ld_cols floats); on sparse (CSC) datasets CSC_COL_PTR
+ *   (n_cols + 1 int64), CSC_ROW_IDX (nnz int32), CSC_VALUES (nnz floats), nnz being the last entry of CSC_COL_PTR.
  * The exact forms hold their integer matrix C in X_HI and C^T in XT_HI (F16_EXACT: only as fp16, X_H16 / XT_H16).
  * Returns -3 for an array this dataset does not hold. */
 enum { CNMF_OPERAND_X = 0, CNMF_OPERAND_XT = 1, CNMF_OPERAND_X_HI = 2, CNMF_OPERAND_X_LO = 3, CNMF_OPERAND_XT_HI = 4,
        CNMF_OPERAND_XT_LO = 5, CNMF_OPERAND_X_H16 = 6, CNMF_OPERAND_XT_H16 = 7, CNMF_OPERAND_ROW_SCALE = 8,
-       CNMF_OPERAND_COL_SCALE = 9 };
+       CNMF_OPERAND_COL_SCALE = 9, CNMF_OPERAND_CSC_COL_PTR = 10, CNMF_OPERAND_CSC_ROW_IDX = 11,
+       CNMF_OPERAND_CSC_VALUES = 12 };
 int cnmf_dataset_operand_host(cnmf_dataset_t d, int which, void* out_host, long long bytes);
 /* one of the batched solver's two products on the dataset's view (transposed as cnmf_refit's), through the solver's own
  * launch: the factor's operand pieces for the dataset's form, then the split-K GEMM with the solver's split plan.
