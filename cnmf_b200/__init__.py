@@ -6,5 +6,6 @@ Importing this package needs neither a GPU nor the compiled library; using it do
 """
 from .io import load_df_from_npz, save_df_to_npz, save_df_to_text  # noqa: F401
 from .pipeline import cNMF, main  # noqa: F401
+from .preprocess import Preprocess  # noqa: F401
 
 __version__ = "0.1.0"

@@ -181,12 +181,16 @@ SIGNATURES = {
     "cnmf_kmeans_assign_f64": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "cnmf_cluster_dist_sums_f64": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _vp, _vp]),
     "cnmf_cluster_median_f64": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _vp, _i, _vp]),
+    "cnmf_moe_grams": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp]),
+    "cnmf_moe_correct": (_i, [_vp, _vp, _i, _i, _i, _ll, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _ll, _i, _vp, _vp, _vp]),
+    "cnmf_scale_quantile_ceiling": (_i, [_vp, _vp, _i, _i, _i, _ll, _i, _vp, _vp, _ll, _d, _i, _ll, _ll, _d, _vp, _ll,
+                                         _i, _pp(_d), _vp]),
 }
 
 _lib = None
 
 
-ABI_VERSION = 18     # include/cnmf_b200.h CNMF_B200_ABI_VERSION
+ABI_VERSION = 19     # include/cnmf_b200.h CNMF_B200_ABI_VERSION
 
 
 def load():

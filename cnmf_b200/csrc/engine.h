@@ -42,10 +42,10 @@ struct cnmf_handle_s {
   size_t ev_used = 0;
   // kernel classes: 0 = batched GEMM (work = algorithmic FLOPs), 1 = fused update kernels (work = algorithmic bytes),
   // 2 = sparse products csc_project (work = algorithmic bytes), 3 = fp64 GEMM of the NNDSVD starts (work = FLOPs),
-  // 4 = fp64 GEMM of the float64 solver (work = FLOPs)
-  static constexpr int PROF_CLASSES = 5;
-  double prof_ms[PROF_CLASSES] = {0.0, 0.0, 0.0, 0.0, 0.0}, prof_work[PROF_CLASSES] = {0.0, 0.0, 0.0, 0.0, 0.0};
-  long long prof_launches[PROF_CLASSES] = {0, 0, 0, 0, 0};
+  // 4 = fp64 GEMM of the float64 solver (work = FLOPs), 5 = fp64 GEMMs of the Harmony ridge correction (work = FLOPs)
+  static constexpr int PROF_CLASSES = 6;
+  double prof_ms[PROF_CLASSES] = {}, prof_work[PROF_CLASSES] = {};
+  long long prof_launches[PROF_CLASSES] = {};
   int nndsvd_chunk_restarts = 0;                // > 0: at most this many restarts per chunk of the NNDSVD starts
   double t_rng_ms = 0, t_h2d_ms = 0, t_solve_ms = 0, t_d2h_ms = 0;   // host wall-clock phases of the last factorize
   int prof_begin(cudaStream_t s, double work, int cls = 0);    // start event (recorded or shared); returns slot or -1
@@ -274,6 +274,13 @@ int launch_gemm_f64(const double* A, int lda, int M, const float* X, int n_rows,
 // float64 dataset): same tiles, same reduction order
 int launch_gemm_f64(const double* A, int lda, int M, const double* X, int n_rows, int n_cols, int ldx, bool to_genes,
                     double* C, int ldc, cudaStream_t s);
+// the same product cut along its reduction into slices of k_chunk elements (a multiple of 16): slice z accumulates
+// reduction elements [z * k_chunk, (z + 1) * k_chunk) in ascending order into C + z * c_split_stride.  The caller sums
+// the slices in a fixed order.  Does not synchronise.
+int launch_gemm_f64_split(const double* A, int lda, int M, const float* X, int n_rows, int n_cols, int ldx,
+                          bool to_genes, int k_chunk, double* C, int ldc, long long c_split_stride, cudaStream_t s);
+int launch_gemm_f64_split(const double* A, int lda, int M, const double* X, int n_rows, int n_cols, int ldx,
+                          bool to_genes, int k_chunk, double* C, int ldc, long long c_split_stride, cudaStream_t s);
 // scikit-learn's NNDSVD starting factors of every restart (ks[r], seeds[r]) for init = CNMF_INIT_NNDSVD / NNDSVDA /
 // NNDSVDAR into packed padded Wt (sum ks x ld_r) and H (sum ks x ld_c); synchronises
 int nndsvd_starts_dev(cnmf_dataset_s* d, int R, const int* ks, const uint32_t* seeds, int init, float* Wt, float* H,

@@ -50,7 +50,18 @@ __device__ __forceinline__ void load8(const double* p, double (&r)[8]) {
 template <bool TO_GENES, typename TX>
 __global__ void __launch_bounds__(F64_THREADS)
 gemm_f64_kernel(const double* __restrict__ A, int lda, int M, int K, const TX* __restrict__ X, int ldx, int n_rows,
-                double* __restrict__ C, int ldc, int n_out) {
+                double* __restrict__ C, int ldc, int n_out, int k_chunk, long long c_split_stride) {
+  // split-K slice blockIdx.z: reduction elements [z * k_chunk, (z + 1) * k_chunk), its own C slice.  One slice (the
+  // solver's products) is the whole reduction.
+  {
+    const int kz0 = blockIdx.z * k_chunk;
+    const int kn = min(k_chunk, K - kz0);
+    A += kz0;
+    X += TO_GENES ? (long long)kz0 * ldx : (long long)kz0;
+    if (TO_GENES) n_rows = kn;
+    K = kn;
+    C += blockIdx.z * c_split_stride;
+  }
   __shared__ double As[F64_BM][F64_PAD];
   __shared__ double Bs[F64_BN][F64_PAD];      // [output item][k]
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -152,16 +163,20 @@ gemm_f64_kernel(const double* __restrict__ A, int lda, int M, int K, const TX* _
 
 template <typename TX>
 int gemm_f64_launch(const double* A, int lda, int M, const TX* X, int n_rows, int n_cols, int ldx, bool to_genes,
-                    double* C, int ldc, cudaStream_t s) {
+                    double* C, int ldc, int k_chunk, long long c_split_stride, cudaStream_t s) {
   if (M <= 0) return 0;
   const int n_out = to_genes ? n_cols : n_rows;
   const int K = to_genes ? n_rows : n_cols;
-  dim3 grid((n_out + F64_BN - 1) / F64_BN, (M + F64_BM - 1) / F64_BM);
-  CNMF_REQUIRE(grid.y <= 65535, "fp64 GEMM: too many rows");
+  if (k_chunk <= 0) k_chunk = K;
+  const int splits = K > 0 ? (K + k_chunk - 1) / k_chunk : 1;
+  dim3 grid((n_out + F64_BN - 1) / F64_BN, (M + F64_BM - 1) / F64_BM, splits);
+  CNMF_REQUIRE(grid.y <= 65535 && grid.z <= 65535, "fp64 GEMM: too many rows or slices");
   if (to_genes)
-    gemm_f64_kernel<true, TX><<<grid, F64_THREADS, 0, s>>>(A, lda, M, K, X, ldx, n_rows, C, ldc, n_out);
+    gemm_f64_kernel<true, TX><<<grid, F64_THREADS, 0, s>>>(A, lda, M, K, X, ldx, n_rows, C, ldc, n_out, k_chunk,
+                                                           c_split_stride);
   else
-    gemm_f64_kernel<false, TX><<<grid, F64_THREADS, 0, s>>>(A, lda, M, K, X, ldx, n_rows, C, ldc, n_out);
+    gemm_f64_kernel<false, TX><<<grid, F64_THREADS, 0, s>>>(A, lda, M, K, X, ldx, n_rows, C, ldc, n_out, k_chunk,
+                                                            c_split_stride);
   CNMF_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
@@ -170,12 +185,24 @@ int gemm_f64_launch(const double* A, int lda, int M, const TX* X, int n_rows, in
 
 int launch_gemm_f64(const double* A, int lda, int M, const float* X, int n_rows, int n_cols, int ldx, bool to_genes,
                     double* C, int ldc, cudaStream_t s) {
-  return gemm_f64_launch(A, lda, M, X, n_rows, n_cols, ldx, to_genes, C, ldc, s);
+  return gemm_f64_launch(A, lda, M, X, n_rows, n_cols, ldx, to_genes, C, ldc, 0, 0, s);
 }
 
 int launch_gemm_f64(const double* A, int lda, int M, const double* X, int n_rows, int n_cols, int ldx, bool to_genes,
                     double* C, int ldc, cudaStream_t s) {
-  return gemm_f64_launch(A, lda, M, X, n_rows, n_cols, ldx, to_genes, C, ldc, s);
+  return gemm_f64_launch(A, lda, M, X, n_rows, n_cols, ldx, to_genes, C, ldc, 0, 0, s);
+}
+
+int launch_gemm_f64_split(const double* A, int lda, int M, const float* X, int n_rows, int n_cols, int ldx,
+                          bool to_genes, int k_chunk, double* C, int ldc, long long c_split_stride, cudaStream_t s) {
+  CNMF_REQUIRE(k_chunk > 0 && k_chunk % F64_BK == 0, "fp64 GEMM: split-K slices must be whole K tiles");
+  return gemm_f64_launch(A, lda, M, X, n_rows, n_cols, ldx, to_genes, C, ldc, k_chunk, c_split_stride, s);
+}
+
+int launch_gemm_f64_split(const double* A, int lda, int M, const double* X, int n_rows, int n_cols, int ldx,
+                          bool to_genes, int k_chunk, double* C, int ldc, long long c_split_stride, cudaStream_t s) {
+  CNMF_REQUIRE(k_chunk > 0 && k_chunk % F64_BK == 0, "fp64 GEMM: split-K slices must be whole K tiles");
+  return gemm_f64_launch(A, lda, M, X, n_rows, n_cols, ldx, to_genes, C, ldc, k_chunk, c_split_stride, s);
 }
 
 }  // namespace cnmf

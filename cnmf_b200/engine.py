@@ -199,7 +199,7 @@ class Engine:
         """(total device ms, launches, algorithmic work) of a kernel class since profile(True):
         0 = batched GEMM (work in FLOPs), 1 = fused update kernels (work in bytes), 2 = sparse-dataset products
         (work in bytes), 3 = fp64 GEMM of the NNDSVD starts (work in FLOPs), 4 = fp64 GEMM of the float64 solver
-        (work in FLOPs)."""
+        (work in FLOPs), 5 = fp64 GEMMs of the Harmony ridge correction (work in FLOPs)."""
         ms, n, fl = ctypes.c_double(), ctypes.c_longlong(), ctypes.c_double()
         check(self.lib.cnmf_profile_get_class(self._h, int(kernel_class), ctypes.byref(ms), ctypes.byref(n),
                                               ctypes.byref(fl)))

@@ -28,8 +28,8 @@
 extern "C" {
 #endif
 
-#define CNMF_B200_ABI_VERSION 18     /* 18: cnmf_dataset_create_csr, cnmf_dataset_create_from_csr / _f64, the CSC arrays
-                                      * of cnmf_dataset_operand_host */
+#define CNMF_B200_ABI_VERSION 19     /* 19: cnmf_moe_grams, cnmf_moe_correct, cnmf_scale_quantile_ceiling; profile
+                                      * class 5 */
 #define CNMF_MAX_COMPONENTS 32          /* largest n_components per restart on the CUDA path */
 
 typedef struct cnmf_handle_s* cnmf_handle_t;
@@ -94,7 +94,8 @@ int cnmf_profile_get(cnmf_handle_t h, double* gemm_ms, long long* gemm_launches,
  * (work = algorithmic bytes: factor read + product slices read + factor and tf32 pieces written), 2 = the product
  * of a sparse dataset, both of its kernels (work = algorithmic bytes: 8 per entry, col_ptr, staged U, output),
  * 3 = the fp64 GEMM of cnmf_nndsvd_init_dev (work = algorithmic FLOPs, 2*M*N*K per launch), 4 = the fp64 GEMM of
- * the float64 solver (work = algorithmic FLOPs, 2*M*N*K per launch) */
+ * the float64 solver (work = algorithmic FLOPs, 2*M*N*K per launch), 5 = the fp64 GEMMs of cnmf_moe_grams and
+ * cnmf_moe_correct (work = algorithmic FLOPs, 2*M*N*K per launch) */
 int cnmf_profile_get_class(cnmf_handle_t h, int kernel_class, double* ms, long long* launches, double* work);
 
 /* host wall-clock phases (ms) of the last cnmf_factorize, cnmf_factorize_seeds_dev, cnmf_factorize_init or
@@ -547,6 +548,39 @@ int cnmf_cluster_dist_sums_f64(cnmf_handle_t h, const double* S_dev, int R, int 
                                int K, double* sums_host, void* stream);
 int cnmf_cluster_median_f64(cnmf_handle_t h, const double* S_dev, int R, int G, int ld, const int32_t* labels_dev,
                             int K, double* M_dev, int ldm, void* stream);
+
+/* ---- preprocessing: Harmony's ridge correction and variance scaling (preprocess.py:9-29) ------ */
+/* Harmony's mixture-of-experts ridge correction of a cells x genes matrix X (moe_correct_ridge on Z_orig = X^T).
+ * Host inputs: R (K x n_cells) soft cluster assignments, Phi (n_phi x n_cells) design with row 0 the intercept of
+ * ones, lamb (n_phi x n_phi) ridge penalty; all row-major fp64, 1 <= n_phi <= 64.  With P_i = Phi * R[i, :] (per cell):
+ *   cnmf_moe_grams:   A_out (K x n_phi x n_phi, host) = P_i Phi^T + lamb, fp64 on the fp64 tensor cores in a fixed
+ *                     split-K order.  The caller inverts the K small systems.
+ *   cnmf_moe_correct: W_i = A_inv_i (P_i X) with row 0 zeroed, then X_out = X - sum_i W_i^T P_i, subtracted one
+ *                     cluster at a time per element with the cluster's term in fp64 and rounded to X's element type
+ *                     after each cluster.  dtype 0 = float32, 1 = float64 (X, X_out and X_cos_out).  X (row stride ld)
+ *                     and X_out / X_cos_out (row stride ld_out) are host or device memory as the flags say.
+ *                     clamp_zero != 0 writes max(x, 0).  X_cos_out (optional) = each cell's row of X_out divided by
+ *                     its L2 norm (Z_cos; meaningful with clamp_zero = 0).  W_last (optional, host, n_phi x n_genes)
+ *                     = W of the last cluster.
+ * No floating-point atomics: repeated calls give identical bits.  Both synchronise. */
+int cnmf_moe_grams(cnmf_handle_t h, const double* R, const double* Phi, const double* lamb, int K, int n_phi,
+                   int n_cells, double* A_out, void* stream);
+int cnmf_moe_correct(cnmf_handle_t h, const void* X, int dtype, int n_cells, int n_genes, long long ld,
+                     int src_is_device, const double* R, const double* Phi, const double* A_inv, int K, int n_phi,
+                     int clamp_zero, void* X_out, long long ld_out, int dst_is_device, void* X_cos_out,
+                     double* W_last, void* stream);
+/* stdscale_quantile_celing: X / std per column (ddof = 1, a zero std maps to 1, the division in fp64 rounded to the
+ * element type), clipped at max_value when clip != 0; then, when k_lo >= 0, every value above the quantile threshold
+ * is set to it.  The threshold is numpy's linear-method lerp in the element type of the values of ranks k_lo and k_hi
+ * (ascending over all n_rows * n_cols entries, found exactly by a radix select on the float bits) with weight gamma;
+ * the caller derives k_lo, k_hi and gamma from the quantile as np.quantile does.  thresh_out (optional) receives it.
+ * csr_row_ptr != NULL: X is the values array (nnz) of a host CSR matrix (csr_row_ptr: n_rows + 1 entries from 0,
+ * csr_col_idx: nnz), densified on the device.  dtype as for cnmf_moe_correct.  Synchronises. */
+int cnmf_scale_quantile_ceiling(cnmf_handle_t h, const void* X, int dtype, int n_rows, int n_cols, long long ld,
+                                int src_is_device, const long long* csr_row_ptr, const int* csr_col_idx,
+                                long long nnz, double max_value, int clip, long long k_lo, long long k_hi,
+                                double gamma, void* X_out, long long ld_out, int dst_is_device, double* thresh_out,
+                                void* stream);
 
 #ifdef __cplusplus
 }
