@@ -643,6 +643,8 @@ int cnmf_random_init_host(uint32_t seed, double avg, int n_samples, int n_featur
   return 0;
 }
 
+}  // extern "C"
+
 // ----------------------------------------------------------------------------- factorize
 namespace {
 
@@ -650,14 +652,16 @@ using clk = std::chrono::steady_clock;
 double ms_since(clk::time_point t0) { return std::chrono::duration<double, std::milli>(clk::now() - t0).count(); }
 
 // the restarts of one batched solve: n_components and first packed row of each, and the packed factors
-// (Fr = W^T rows, SK x ld_r; Fc = H rows, SK x ld_c)
+// (Fr = W^T rows, SK x ld_r; Fc = H rows, SK x ld_c) in the dataset's element type T
+template <class T>
 struct Batch {
   std::vector<int> ks, off;
   int SK = 0;
-  float *Fr = nullptr, *Fc = nullptr;
+  T *Fr = nullptr, *Fc = nullptr;
 };
 
-int pack_restarts(int n_restarts, const int32_t* ks_in, const std::string& what, Batch* b) {
+template <class T>
+int pack_restarts(int n_restarts, const int32_t* ks_in, const std::string& what, Batch<T>* b) {
   b->ks.assign(ks_in, ks_in + n_restarts);
   b->off.resize(n_restarts);
   b->SK = 0;
@@ -700,17 +704,32 @@ int check_params(cnmf_dataset_s* d, const cnmf_nmf_params* p) {
   return 0;
 }
 
+// parameters of the float64 factorize entry points: float64 dataset, Frobenius loss
+int check_params_f64(cnmf_dataset_s* d, const cnmf_nmf_params* p, const std::string& what) {
+  CNMF_REQUIRE(d && p, "NULL dataset or params");
+  CNMF_TRY(require_f64(d, what.c_str()));
+  CNMF_TRY(check_params_precision(d, p));
+  CNMF_REQUIRE(p->reserved2 == 0, "params.reserved2 must be 0");
+  if (p->beta_loss != CNMF_LOSS_FROBENIUS) {
+    set_last_error("cnmf_" + what + "_f64: float64 datasets support beta_loss = frobenius only");
+    return -3;
+  }
+  return 0;
+}
+
 // start of every factorize entry point: parameters and arguments checked (args_ok: the entry point's own pointers),
 // restarts packed, factor buffers allocated on the handle's device, phase timings reset
+template <class T>
 int begin_factorize(cnmf_dataset_s* d, const cnmf_nmf_params* p, int n_restarts, const int32_t* ks_in, bool args_ok,
-                    const std::string& what, Batch* b) {
-  CNMF_TRY(check_params(d, p));
-  CNMF_REQUIRE(args_ok && n_restarts > 0 && ks_in, what + ": bad arguments");
+                    const std::string& what, Batch<T>* b) {
+  constexpr bool f64 = sizeof(T) == 8;
+  CNMF_TRY(f64 ? check_params_f64(d, p, what) : check_params(d, p));
+  CNMF_REQUIRE(args_ok && n_restarts > 0 && ks_in, what + (f64 ? "_f64" : "") + ": bad arguments");
   CNMF_TRY(pack_restarts(n_restarts, ks_in, what, b));
   cnmf_handle_s* h = d->h;
   CNMF_CUDA_CHECK(cudaSetDevice(h->device));
-  b->Fr = static_cast<float*>(h->dev_buf("fac.Fr", (size_t)b->SK * d->ld_r * 4));
-  b->Fc = static_cast<float*>(h->dev_buf("fac.Fc", (size_t)b->SK * d->ld_c * 4));
+  b->Fr = static_cast<T*>(h->dev_buf(f64 ? "fac.Fr64" : "fac.Fr", (size_t)b->SK * d->ld_r * sizeof(T)));
+  b->Fc = static_cast<T*>(h->dev_buf(f64 ? "fac.Fc64" : "fac.Fc", (size_t)b->SK * d->ld_c * sizeof(T)));
   if (!b->Fr || !b->Fc) return -2;
   h->t_rng_ms = h->t_h2d_ms = h->t_solve_ms = h->t_d2h_ms = 0;
   return 0;
@@ -718,20 +737,21 @@ int begin_factorize(cnmf_dataset_s* d, const cnmf_nmf_params* p, int n_restarts,
 
 // sklearn's random starts of every restart (the legacy MT19937 / polar-gauss stream), generated in place on the device
 // into packed, padded Wt / H.  No host synchronisation: launch_rng_init stages its arguments itself.
-int rng_starts_dev(cnmf_dataset_s* d, const Batch& b, const uint32_t* seeds, float* Wt, float* H, cudaStream_t s) {
+template <class T>
+int rng_starts_dev(cnmf_dataset_s* d, const Batch<T>& b, const uint32_t* seeds, T* Wt, T* H, cudaStream_t s) {
   const int R = (int)b.ks.size();
   const double mean = d->sum / ((double)d->n_rows * (double)d->n_cols);
   std::vector<double> avgs(R);
   for (int r = 0; r < R; ++r) avgs[r] = std::sqrt(mean / b.ks[r]);
-  CNMF_CUDA_CHECK(cudaMemsetAsync(Wt, 0, (size_t)b.SK * d->ld_r * 4, s));
-  CNMF_CUDA_CHECK(cudaMemsetAsync(H, 0, (size_t)b.SK * d->ld_c * 4, s));
+  CNMF_CUDA_CHECK(cudaMemsetAsync(Wt, 0, (size_t)b.SK * d->ld_r * sizeof(T), s));
+  CNMF_CUDA_CHECK(cudaMemsetAsync(H, 0, (size_t)b.SK * d->ld_c * sizeof(T), s));
   return launch_rng_init(seeds, b.ks.data(), b.off.data(), avgs.data(), R, d->n_rows, d->n_cols, Wt, d->ld_r, H, d->ld_c,
                          d->h, s);
 }
 
 // the same starts drawn on the host (bit-exact numpy legacy stream) into b.Fr / b.Fc, in groups through a pinned
 // staging buffer
-int rng_starts_host(cnmf_dataset_s* d, const Batch& b, const uint32_t* seeds, cudaStream_t s) {
+int rng_starts_host(cnmf_dataset_s* d, const Batch<float>& b, const uint32_t* seeds, cudaStream_t s) {
   cnmf_handle_s* h = d->h;
   const std::vector<int>& ks = b.ks;
   const std::vector<int>& off = b.off;
@@ -775,13 +795,21 @@ int rng_starts_host(cnmf_dataset_s* d, const Batch& b, const uint32_t* seeds, cu
   return 0;
 }
 
-// end of every factorize entry point: the solve from the starts in b.Fr / b.Fc (full fp32), then its results out.
-// Null outputs are skipped; spectra_dev gets SK rows of dev_cols floats at row stride ld_dev.
-int solve_and_copy_out(cnmf_dataset_s* d, const Batch& b, const cnmf_nmf_params& p, float* spectra_host,
-                       float* usages_host, float* spectra_dev, long long ld_dev, int dev_cols, int32_t* n_iter_host,
-                       double* err_host, cudaStream_t s) {
+// float64 datasets take their starts from the device generator or the NNDSVD family only
+int rng_starts_host(cnmf_dataset_s*, const Batch<double>&, const uint32_t*, cudaStream_t) {
+  set_last_error("cnmf_factorize_f64: the host random generator (params.reserved bit 0) serves float datasets only");
+  return -3;
+}
+
+// end of every factorize entry point: the solve from the starts in b.Fr / b.Fc, then its results out.
+// Null outputs are skipped; spectra_dev gets SK rows of dev_cols elements at row stride ld_dev.
+template <class T>
+int solve_and_copy_out(cnmf_dataset_s* d, const Batch<T>& b, const cnmf_nmf_params& p, T* spectra_host, T* usages_host,
+                       T* spectra_dev, long long ld_dev, int dev_cols, int32_t* n_iter_host, double* err_host,
+                       cudaStream_t s) {
   cnmf_handle_s* h = d->h;
-  SolveIO io;
+  constexpr size_t e = sizeof(T);
+  SolveIO<T> io;
   io.R = (int)b.ks.size();
   io.ks = b.ks;
   io.Fr = b.Fr;
@@ -792,14 +820,14 @@ int solve_and_copy_out(cnmf_dataset_s* d, const Batch& b, const cnmf_nmf_params&
   h->t_solve_ms = ms_since(t_solve);
   auto t_d2h = clk::now();
   if (spectra_dev)      // result stays in HBM (multi-GPU path: the slab goes straight into the NCCL all-gather)
-    CNMF_CUDA_CHECK(cudaMemcpy2DAsync(spectra_dev, (size_t)ld_dev * 4, b.Fc, (size_t)d->ld_c * 4, (size_t)dev_cols * 4,
+    CNMF_CUDA_CHECK(cudaMemcpy2DAsync(spectra_dev, (size_t)ld_dev * e, b.Fc, (size_t)d->ld_c * e, (size_t)dev_cols * e,
                                       b.SK, cudaMemcpyDeviceToDevice, s));
   if (spectra_host)
-    CNMF_CUDA_CHECK(cudaMemcpy2DAsync(spectra_host, (size_t)d->n_cols * 4, b.Fc, (size_t)d->ld_c * 4,
-                                      (size_t)d->n_cols * 4, b.SK, cudaMemcpyDeviceToHost, s));
+    CNMF_CUDA_CHECK(cudaMemcpy2DAsync(spectra_host, (size_t)d->n_cols * e, b.Fc, (size_t)d->ld_c * e,
+                                      (size_t)d->n_cols * e, b.SK, cudaMemcpyDeviceToHost, s));
   if (usages_host)
-    CNMF_CUDA_CHECK(cudaMemcpy2DAsync(usages_host, (size_t)d->n_rows * 4, b.Fr, (size_t)d->ld_r * 4,
-                                      (size_t)d->n_rows * 4, b.SK, cudaMemcpyDeviceToHost, s));
+    CNMF_CUDA_CHECK(cudaMemcpy2DAsync(usages_host, (size_t)d->n_rows * e, b.Fr, (size_t)d->ld_r * e,
+                                      (size_t)d->n_rows * e, b.SK, cudaMemcpyDeviceToHost, s));
   CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
   h->t_d2h_ms = ms_since(t_d2h);
   for (int r = 0; r < io.R; ++r) {
@@ -809,64 +837,11 @@ int solve_and_copy_out(cnmf_dataset_s* d, const Batch& b, const cnmf_nmf_params&
   return 0;
 }
 
-// start of the float64 factorize entry points: as begin_factorize, with fp64 factor buffers
-int begin_factorize_f64(cnmf_dataset_s* d, const cnmf_nmf_params* p, int n_restarts, const int32_t* ks_in, bool args_ok,
-                        const std::string& what, Batch* b, double** Fr, double** Fc) {
-  CNMF_REQUIRE(d && p, "NULL dataset or params");
-  CNMF_TRY(require_f64(d, what.c_str()));
-  CNMF_TRY(check_params_precision(d, p));
-  CNMF_REQUIRE(p->reserved2 == 0, "params.reserved2 must be 0");
-  if (p->beta_loss != CNMF_LOSS_FROBENIUS) {
-    set_last_error("cnmf_" + what + "_f64: float64 datasets support beta_loss = frobenius only");
-    return -3;
-  }
-  CNMF_REQUIRE(args_ok && n_restarts > 0 && ks_in, what + "_f64: bad arguments");
-  CNMF_TRY(pack_restarts(n_restarts, ks_in, what, b));
-  cnmf_handle_s* h = d->h;
-  CNMF_CUDA_CHECK(cudaSetDevice(h->device));
-  *Fr = static_cast<double*>(h->dev_buf("fac.Fr64", (size_t)b->SK * d->ld_r * 8));
-  *Fc = static_cast<double*>(h->dev_buf("fac.Fc64", (size_t)b->SK * d->ld_c * 8));
-  if (!*Fr || !*Fc) return -2;
-  h->t_rng_ms = h->t_h2d_ms = h->t_solve_ms = h->t_d2h_ms = 0;
-  return 0;
-}
-
-// the float64 solve from the starts in Fr / Fc, then its results out (null outputs skipped)
-int solve_and_copy_out_f64(cnmf_dataset_s* d, const Batch& b, double* Fr, double* Fc, const cnmf_nmf_params& p,
-                           double* spectra_host, double* usages_host, int32_t* n_iter_host, double* err_host,
-                           cudaStream_t s) {
-  cnmf_handle_s* h = d->h;
-  SolveIO io;
-  io.R = (int)b.ks.size();
-  io.ks = b.ks;
-  io.Fr64 = Fr;
-  io.Fc64 = Fc;
-  io.update_cols = true;
-  auto t_solve = clk::now();
-  CNMF_TRY(solve_batched(h, make_view(d, false), io, p, s));
-  h->t_solve_ms = ms_since(t_solve);
-  auto t_d2h = clk::now();
-  if (spectra_host)
-    CNMF_CUDA_CHECK(cudaMemcpy2DAsync(spectra_host, (size_t)d->n_cols * 8, Fc, (size_t)d->ld_c * 8,
-                                      (size_t)d->n_cols * 8, b.SK, cudaMemcpyDeviceToHost, s));
-  if (usages_host)
-    CNMF_CUDA_CHECK(cudaMemcpy2DAsync(usages_host, (size_t)d->n_rows * 8, Fr, (size_t)d->ld_r * 8,
-                                      (size_t)d->n_rows * 8, b.SK, cudaMemcpyDeviceToHost, s));
-  CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
-  h->t_d2h_ms = ms_since(t_d2h);
-  for (int r = 0; r < io.R; ++r) {
-    if (n_iter_host) n_iter_host[r] = io.n_iter[r];
-    if (err_host) err_host[r] = io.err[r];
-  }
-  return 0;
-}
-
-}  // namespace
-
-static int factorize_impl(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, const uint32_t* seeds,
-                          const cnmf_nmf_params* p, float* spectra_host, float* usages_host, int32_t* n_iter_host,
-                          double* err_host, void* stream, float* spectra_dev, long long ld_dev) {
-  Batch b;
+template <class T>
+int factorize_impl(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, const uint32_t* seeds,
+                          const cnmf_nmf_params* p, T* spectra_host, T* usages_host, int32_t* n_iter_host,
+                          double* err_host, void* stream, T* spectra_dev, long long ld_dev) {
+  Batch<T> b;
   CNMF_TRY(begin_factorize(d, p, n_restarts, ks_in, seeds && (spectra_host || spectra_dev), "factorize", &b));
   CNMF_REQUIRE(!spectra_dev || ld_dev >= d->n_cols, "factorize: device output row stride too small");
   cudaStream_t s = as_stream(stream);
@@ -887,12 +862,37 @@ static int factorize_impl(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in
                             s);
 }
 
+// the starts Wt0_host / H0_host (n_rows / n_cols elements per row, SK rows each) padded into the packed factors
+template <class T>
+int factorize_init_impl(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, const T* Wt0_host,
+                               const T* H0_host, const cnmf_nmf_params* p, T* spectra_host, T* usages_host,
+                               int32_t* n_iter_host, double* err_host, void* stream) {
+  Batch<T> b;
+  CNMF_TRY(begin_factorize(d, p, n_restarts, ks_in, Wt0_host && H0_host && spectra_host, "factorize_init", &b));
+  cudaStream_t s = as_stream(stream);
+  constexpr size_t e = sizeof(T);
+  auto t_h2d = clk::now();
+  CNMF_CUDA_CHECK(cudaMemsetAsync(b.Fr, 0, (size_t)b.SK * d->ld_r * e, s));
+  CNMF_CUDA_CHECK(cudaMemsetAsync(b.Fc, 0, (size_t)b.SK * d->ld_c * e, s));
+  CNMF_CUDA_CHECK(cudaMemcpy2DAsync(b.Fr, (size_t)d->ld_r * e, Wt0_host, (size_t)d->n_rows * e, (size_t)d->n_rows * e,
+                                    b.SK, cudaMemcpyHostToDevice, s));
+  CNMF_CUDA_CHECK(cudaMemcpy2DAsync(b.Fc, (size_t)d->ld_c * e, H0_host, (size_t)d->n_cols * e, (size_t)d->n_cols * e,
+                                    b.SK, cudaMemcpyHostToDevice, s));
+  CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
+  d->h->t_h2d_ms = ms_since(t_h2d);
+  return solve_and_copy_out<T>(d, b, *p, spectra_host, usages_host, nullptr, 0, 0, n_iter_host, err_host, s);
+}
+
+}  // namespace
+
+extern "C" {
+
 int cnmf_factorize(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, const uint32_t* seeds,
                    const cnmf_nmf_params* p, float* spectra_host, float* usages_host, int32_t* n_iter_host,
                    double* err_host, void* stream) {
   CNMF_TRY(require_f32(d, "factorize"));
   CNMF_REQUIRE(spectra_host, "factorize: spectra_host is NULL");
-  return factorize_impl(d, n_restarts, ks_in, seeds, p, spectra_host, usages_host, n_iter_host, err_host, stream, nullptr, 0);
+  return factorize_impl<float>(d, n_restarts, ks_in, seeds, p, spectra_host, usages_host, n_iter_host, err_host, stream, nullptr, 0);
 }
 
 int cnmf_factorize_seeds_dev(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, const uint32_t* seeds,
@@ -900,7 +900,8 @@ int cnmf_factorize_seeds_dev(cnmf_dataset_t d, int n_restarts, const int32_t* ks
                              double* err_host, void* stream) {
   CNMF_TRY(require_dense(d, "factorize_seeds_dev"));
   CNMF_REQUIRE(spectra_dev, "factorize_seeds_dev: spectra_dev is NULL");
-  return factorize_impl(d, n_restarts, ks_in, seeds, p, nullptr, nullptr, n_iter_host, err_host, stream, spectra_dev, ld_out);
+  return factorize_impl<float>(d, n_restarts, ks_in, seeds, p, nullptr, nullptr, n_iter_host, err_host, stream, spectra_dev,
+                               ld_out);
 }
 
 int cnmf_last_timing(cnmf_handle_t h, double* rng_ms, double* h2d_ms, double* solve_ms, double* d2h_ms) {
@@ -916,79 +917,34 @@ int cnmf_factorize_init(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, 
                         const float* H0_host, const cnmf_nmf_params* p, float* spectra_host, float* usages_host,
                         int32_t* n_iter_host, double* err_host, void* stream) {
   CNMF_TRY(require_f32(d, "factorize_init"));
-  Batch b;
-  CNMF_TRY(begin_factorize(d, p, n_restarts, ks_in, Wt0_host && H0_host && spectra_host, "factorize_init", &b));
-  cudaStream_t s = as_stream(stream);
-  auto t_h2d = clk::now();
-  CNMF_CUDA_CHECK(cudaMemsetAsync(b.Fr, 0, (size_t)b.SK * d->ld_r * 4, s));
-  CNMF_CUDA_CHECK(cudaMemsetAsync(b.Fc, 0, (size_t)b.SK * d->ld_c * 4, s));
-  CNMF_CUDA_CHECK(cudaMemcpy2DAsync(b.Fr, (size_t)d->ld_r * 4, Wt0_host, (size_t)d->n_rows * 4, (size_t)d->n_rows * 4,
-                                    b.SK, cudaMemcpyHostToDevice, s));
-  CNMF_CUDA_CHECK(cudaMemcpy2DAsync(b.Fc, (size_t)d->ld_c * 4, H0_host, (size_t)d->n_cols * 4, (size_t)d->n_cols * 4,
-                                    b.SK, cudaMemcpyHostToDevice, s));
-  CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
-  d->h->t_h2d_ms = ms_since(t_h2d);
-  return solve_and_copy_out(d, b, *p, spectra_host, usages_host, nullptr, 0, 0, n_iter_host, err_host, s);
+  return factorize_init_impl(d, n_restarts, ks_in, Wt0_host, H0_host, p, spectra_host, usages_host, n_iter_host, err_host,
+                             stream);
 }
 
 int cnmf_factorize_dev(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, const float* Wt0_dev,
                        const float* H0_dev, const cnmf_nmf_params* p, float* spectra_dev, int32_t* n_iter_host,
                        double* err_host, void* stream) {
-  Batch b;
+  Batch<float> b;
   CNMF_TRY(begin_factorize(d, p, n_restarts, ks_in, Wt0_dev && H0_dev && spectra_dev, "factorize_dev", &b));
   cudaStream_t s = as_stream(stream);
   CNMF_CUDA_CHECK(cudaMemcpyAsync(b.Fr, Wt0_dev, (size_t)b.SK * d->ld_r * 4, cudaMemcpyDeviceToDevice, s));
   CNMF_CUDA_CHECK(cudaMemcpyAsync(b.Fc, H0_dev, (size_t)b.SK * d->ld_c * 4, cudaMemcpyDeviceToDevice, s));
   // spectra_dev has the layout of H0_dev: whole padded rows, the zero padding included
-  return solve_and_copy_out(d, b, *p, nullptr, nullptr, spectra_dev, d->ld_c, d->ld_c, n_iter_host, err_host, s);
+  return solve_and_copy_out<float>(d, b, *p, nullptr, nullptr, spectra_dev, d->ld_c, d->ld_c, n_iter_host, err_host, s);
 }
 
 int cnmf_factorize_f64(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, const uint32_t* seeds,
                        const cnmf_nmf_params* p, double* spectra_host, double* usages_host, int32_t* n_iter_host,
                        double* err_host, void* stream) {
-  Batch b;
-  double *Fr = nullptr, *Fc = nullptr;
-  CNMF_TRY(begin_factorize_f64(d, p, n_restarts, ks_in, seeds && spectra_host, "factorize", &b, &Fr, &Fc));
-  cudaStream_t s = as_stream(stream);
-  const int init = (p->reserved >> 1) & 3;
-  auto t_init = clk::now();
-  if (init != CNMF_INIT_RANDOM) {
-    CNMF_TRY(nndsvd_starts_dev(d, n_restarts, b.ks.data(), seeds, init, Fr, Fc, s));
-  } else {
-    if (p->reserved & 1) {
-      set_last_error("cnmf_factorize_f64: the host random generator (params.reserved bit 0) serves float datasets only");
-      return -3;
-    }
-    const double mean = d->sum / ((double)d->n_rows * (double)d->n_cols);
-    std::vector<double> avgs(n_restarts);
-    for (int r = 0; r < n_restarts; ++r) avgs[r] = std::sqrt(mean / b.ks[r]);
-    CNMF_CUDA_CHECK(cudaMemsetAsync(Fr, 0, (size_t)b.SK * d->ld_r * 8, s));
-    CNMF_CUDA_CHECK(cudaMemsetAsync(Fc, 0, (size_t)b.SK * d->ld_c * 8, s));
-    CNMF_TRY(launch_rng_init(seeds, b.ks.data(), b.off.data(), avgs.data(), n_restarts, d->n_rows, d->n_cols, Fr, d->ld_r,
-                             Fc, d->ld_c, d->h, s));
-  }
-  d->h->t_rng_ms = ms_since(t_init);
-  return solve_and_copy_out_f64(d, b, Fr, Fc, *p, spectra_host, usages_host, n_iter_host, err_host, s);
+  return factorize_impl<double>(d, n_restarts, ks_in, seeds, p, spectra_host, usages_host, n_iter_host, err_host, stream,
+                                nullptr, 0);
 }
 
 int cnmf_factorize_init_f64(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, const double* Wt0_host,
                             const double* H0_host, const cnmf_nmf_params* p, double* spectra_host, double* usages_host,
                             int32_t* n_iter_host, double* err_host, void* stream) {
-  Batch b;
-  double *Fr = nullptr, *Fc = nullptr;
-  CNMF_TRY(begin_factorize_f64(d, p, n_restarts, ks_in, Wt0_host && H0_host && spectra_host, "factorize_init", &b, &Fr,
-                               &Fc));
-  cudaStream_t s = as_stream(stream);
-  auto t_h2d = clk::now();
-  CNMF_CUDA_CHECK(cudaMemsetAsync(Fr, 0, (size_t)b.SK * d->ld_r * 8, s));
-  CNMF_CUDA_CHECK(cudaMemsetAsync(Fc, 0, (size_t)b.SK * d->ld_c * 8, s));
-  CNMF_CUDA_CHECK(cudaMemcpy2DAsync(Fr, (size_t)d->ld_r * 8, Wt0_host, (size_t)d->n_rows * 8, (size_t)d->n_rows * 8, b.SK,
-                                    cudaMemcpyHostToDevice, s));
-  CNMF_CUDA_CHECK(cudaMemcpy2DAsync(Fc, (size_t)d->ld_c * 8, H0_host, (size_t)d->n_cols * 8, (size_t)d->n_cols * 8, b.SK,
-                                    cudaMemcpyHostToDevice, s));
-  CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
-  d->h->t_h2d_ms = ms_since(t_h2d);
-  return solve_and_copy_out_f64(d, b, Fr, Fc, *p, spectra_host, usages_host, n_iter_host, err_host, s);
+  return factorize_init_impl(d, n_restarts, ks_in, Wt0_host, H0_host, p, spectra_host, usages_host, n_iter_host, err_host,
+                             stream);
 }
 
 int cnmf_random_init_dev(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in, const uint32_t* seeds, float* Wt_dev,
@@ -997,7 +953,7 @@ int cnmf_random_init_dev(cnmf_dataset_t d, int n_restarts, const int32_t* ks_in,
   CNMF_TRY(require_dense(d, "random_init_dev"));
   cudaStream_t s = as_stream(stream);
   CNMF_CUDA_CHECK(cudaSetDevice(d->h->device));
-  Batch b;
+  Batch<float> b;
   CNMF_TRY(pack_restarts(n_restarts, ks_in, "random_init_dev", &b));
   CNMF_TRY(rng_starts_dev(d, b, seeds, Wt_dev, H_dev, s));
   CNMF_CUDA_CHECK(cudaStreamSynchronize(s));

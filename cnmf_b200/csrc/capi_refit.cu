@@ -319,7 +319,7 @@ int cnmf_refit(cnmf_dataset_t d, int transposed, int k, const float* fixed_host,
     CNMF_CUDA_CHECK(cudaGetLastError());
     h->launches += 1;
   }  // 'cd': zeros (sklearn _nmf.py:1227-1228)
-  SolveIO io;
+  SolveIO<float> io;
   io.R = 1;
   io.ks = {k};
   io.Fr = Fr;
@@ -503,11 +503,11 @@ int cnmf_refit_f64(cnmf_dataset_t d, int transposed, int k, const double* fixed_
     CNMF_TRY(fill_f64(Fr, std::sqrt(mean / k), k, v.n_r, v.ld_r, s));
     h->launches += 1;
   }  // 'cd': zeros (sklearn _nmf.py:1227-1228)
-  SolveIO io;
+  SolveIO<double> io;
   io.R = 1;
   io.ks = {k};
-  io.Fr64 = Fr;
-  io.Fc64 = Fc;
+  io.Fr = Fr;
+  io.Fc = Fc;
   io.update_cols = false;
   CNMF_TRY(solve_batched(h, v, io, *p, s));
   transpose64_kernel<<<NUM_SMS * 4, 256, 0, s>>>(Fr, k, v.n_r, v.ld_r, T);

@@ -171,29 +171,30 @@ int require_f32(const cnmf_dataset_s* d, const char* what);
 // -3 with a message naming the float entry point `what` when d is not a float64 dataset (_f64 entry points)
 int require_f64(const cnmf_dataset_s* d, const char* what);
 
+// one batched solve: T = float on the float forms, double on FP64
+template <class T>
 struct SolveIO {
   int R = 0;
   std::vector<int> ks;      // per restart
-  // packed device factors (SK x ld), full fp32: row factor Fr (e.g. W^T), column factor Fc (e.g. H).  The solver
-  // makes their operand pieces itself.
-  float *Fr = nullptr, *Fc = nullptr;
+  // packed device factors (SK x ld) in the dataset's element type: row factor Fr (e.g. W^T), column factor Fc (e.g. H).
+  // The solver makes their operand pieces itself.
+  T *Fr = nullptr, *Fc = nullptr;
   bool update_cols = true;  // false: Fc fixed (refit)
   // the row product, computed by the caller (refits of sparse datasets: NUM_r = Fc * X^T, SK x ld_r, one split).
-  // Requires update_cols = false; the solver then runs no GEMM and reads no B operand.
+  // Requires update_cols = false; the solver then runs no GEMM and reads no B operand.  Float forms only.
   const float* num_rows = nullptr;
-  // FP64 datasets: the packed factors in fp64 (same slot layout); Fr / Fc and num_rows are unused
-  double *Fr64 = nullptr, *Fc64 = nullptr;
   std::vector<int> n_iter;  // out
   std::vector<double> last; // out: last convergence statistic (mu: error, cd: violation)
   std::vector<double> err;  // out: final ||X - Fr^T Fc||_F
 };
 
-// Runs the batched solver in place on io.Fr / io.Fc.
-int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_nmf_params& p, cudaStream_t s);
+// Runs the batched solver in place on io.Fr / io.Fc: float factors on the float forms (beta_loss KL / IS go to
+// solve_batched_beta), double factors on FP64 (Frobenius only).  The Frobenius solves of both share one driver (solve.h).
+int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO<float>& io, const cnmf_nmf_params& p, cudaStream_t s);
+int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO<double>& io, const cnmf_nmf_params& p, cudaStream_t s);
 // beta_loss = kullback-leibler / itakura-saito (nmf_beta.cu); reached through solve_batched
-int solve_batched_beta(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_nmf_params& p, cudaStream_t s);
-// float64 datasets (form FP64, Frobenius loss, MU and CD; nmf_f64.cu): io.Fr64 / io.Fc64; reached through solve_batched
-int solve_batched_f64(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_nmf_params& p, cudaStream_t s);
+int solve_batched_beta(cnmf_handle_s* h, const DataView& v, SolveIO<float>& io, const cnmf_nmf_params& p,
+                       cudaStream_t s);
 // out[0] = sum(X), out[1] = sum(X^2) of a float64 dataset matrix, fp64 in an order fixed by the shape (synchronises)
 int matrix_sums_f64(cnmf_handle_s* h, const double* X, int rows, int cols, int ld, double* out_host, cudaStream_t s);
 // p[r, j] = v for r < rows, j < n (row stride ld); does not synchronise

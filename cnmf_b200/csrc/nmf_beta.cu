@@ -438,7 +438,7 @@ int beta_check(const BetaLaunch& L, int mode, const BetaSide& sd, const BatchMet
   return 0;
 }
 
-int solve_batched_beta(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_nmf_params& p, cudaStream_t s) {
+int solve_batched_beta(cnmf_handle_s* h, const DataView& v, SolveIO<float>& io, const cnmf_nmf_params& p, cudaStream_t s) {
   const int R = io.R;
   CNMF_REQUIRE(R > 0 && (int)io.ks.size() == R, "solve: bad restart list");
   CNMF_REQUIRE(p.solver == CNMF_SOLVER_MU, "beta_loss other than frobenius needs solver 'mu' (sklearn _nmf.py:1195-1199)");

@@ -15,7 +15,9 @@
 
 #include "engine.h"
 #include "gemm.h"
+#include "nmf_f64.h"
 #include "nmf_kernels.cuh"
+#include "solve.h"
 
 namespace cnmf {
 
@@ -101,16 +103,258 @@ int view_gemm(cnmf_handle_s* h, const DataView& v, int side, const float* F, con
   return rc;
 }
 
-int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_nmf_params& p, cudaStream_t s) {
+// gather member of the batched solve's state (solve.h): rows of E go through launch_gather_rows as ld * sizeof(E) / 4
+// floats, a bit copy
+template <class T>
+template <class E>
+int FroSolve<T>::gather(const E* src, E* dst, const std::vector<int>& so, const std::vector<int>& dof,
+                        const std::vector<int>& kk, int ld_e) {
+  const int cnt = (int)kk.size();
+  if (cnt == 0 || !src || !dst) return 0;
+  if (gslot == GATHER_SLOTS) {
+    CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
+    gslot = 0;
+  }
+  int* hm = h_gidx + (size_t)gslot * 3 * R0;
+  int* dm = d_gidx + (size_t)gslot * 3 * R0;
+  ++gslot;
+  std::memcpy(hm, so.data(), sizeof(int) * cnt);
+  std::memcpy(hm + R0, dof.data(), sizeof(int) * cnt);
+  std::memcpy(hm + 2 * R0, kk.data(), sizeof(int) * cnt);
+  CNMF_CUDA_CHECK(cudaMemcpyAsync(dm, hm, sizeof(int) * 3 * R0, cudaMemcpyHostToDevice, s));
+  h->launches += 1;
+  return launch_gather_rows(reinterpret_cast<const float*>(src), dm, reinterpret_cast<float*>(dst), dm + R0, dm + 2 * R0,
+                            cnt, ld_e * (int)(sizeof(E) / sizeof(float)), s);
+}
+
+namespace {
+
+// The float forms' ops of the batched solve: products through view_gemm with the split-K plan of view_gemm_plan, the
+// update kernels with their fused outputs (Gram when kp == 16, otherwise a stand-alone Gram follows), and the factors'
+// operand pieces -- tf32 hi / lo written by the update kernels, or on f16 datasets the two fp16 pieces (same buffers).
+// Block plans follow the live restart count.  Compaction saves 128-row GEMM tiles.
+struct F32Ops {
+  using T = float;
+  static constexpr int tile_rows = 128;
+  static constexpr const char* buf_tag = "";
+  static int pick_kp(int kmax) { return kmax <= 16 ? 16 : 32; }
+
+  FroSolve<float>& b;
+  const DataView& v;
+  bool cd;
+  float l1[2], l2[2];
+  const bool tf32, f16;     // the factors have operand pieces; they are fp16 pieces
+  bool fused_gram;          // the update kernels emit the Gram of the factor they write (nmf_kernels.cu)
+  // tf32 pieces are written by the update kernels; the fp16 pieces need the row maximum first and come from
+  // emit_pieces() after the update (the hi / lo buffers then hold halves)
+  bool upd_pieces;
+  // f16: the Gram-fused update kernels (K <= 16, factor being iterated) emit the fp16 pieces themselves, per 512-column
+  // tile; everything else (initial factors, compaction, K > 16) goes through emit_pieces(), which normalises the same
+  // 512-column groups and writes the same bits
+  bool emit_in_update;
+  int cpb[2] = {}, gcpb[2] = {}, chunks[2] = {}, ktiles[2] = {};
+  int chunks_cap;           // finest chunking possible
+  size_t gram_part_elems;
+  GemmPlan plan[2];         // plan[0]: NUM_r = Fc * B_rows^T (reduce over n_c); plan[1]: NUM_c = Fr * B_cols^T
+  float *hi[2] = {}, *lo[2] = {}, *alt_hi[2] = {}, *alt_lo[2] = {};
+  float* tile_scale[2] = {};   // f16: power-of-two scales of the pieces, [packed row][512-element group]
+
+  const float* scale(int side) const { return side ? v.scale_c : v.scale_r; }
+
+  F32Ops(FroSolve<float>& b_, const cnmf_nmf_params& p)
+      : b(b_), v(b_.v), cd(p.solver == CNMF_SOLVER_CD), tf32(v.form != Form::FP32), f16(v.form == Form::F16_EXACT) {
+    l1[0] = (float)p.l1_reg_W; l2[0] = (float)p.l2_reg_W; l1[1] = (float)p.l1_reg_H; l2[1] = (float)p.l2_reg_H;
+    fused_gram = b.kp == 16;
+    upd_pieces = tf32 && !f16;
+    emit_in_update = f16 && b.kp == 16 && b.io.update_cols;
+    // block granularity of the streaming kernels: update kernels 3 blocks of 128 threads per SM resident, a block walks
+    // 1-4 tiles -> aim for >= 8 blocks per SM; stand-alone Gram kernel: 1 block/SM resident and a fixed-cost block
+    // reduction -> long blocks, about two waves
+    const int tile = upd_tile_cols(b.kp);
+    for (int side = 0; side < 2; ++side) {
+      gcpb[side] = pick_cols_per_block(b.n(side), b.R0, 8192, 1024, b.h->sm_count * 2);
+      ktiles[side] = (b.ld(side) + 511) / 512;
+    }
+    chunks_cap = std::max((v.n_r + tile - 1) / tile, (v.n_c + tile - 1) / tile);
+    const int gchunks_max = std::max((v.n_r + gcpb[0] - 1) / gcpb[0], (v.n_c + gcpb[1] - 1) / gcpb[1]);
+    size_t fused_part_slots = 0;   // slot-indexed partials of the fused kernels: max over live counts of R * chunks
+    for (int r = 1; r <= b.R0; ++r) {
+      plan_blocks(r);
+      fused_part_slots = std::max(fused_part_slots, (size_t)r * std::max(chunks[0], chunks[1]));
+    }
+    plan_blocks(b.R0);
+    gram_part_elems = std::max((size_t)b.R0 * std::max(gchunks_max, std::max((v.n_r + 1023) / 1024, (v.n_c + 1023) / 1024)),
+                               fused_part_slots) * b.kp * b.kp;
+    plan_gemms();
+  }
+  // the update kernels' chunking follows the number of LIVE restarts (re-planned after every compaction): with few
+  // restarts left a block should hold one tile, so that the work spreads over many SMs
+  void plan_blocks(int r_live) {
+    const int tile = upd_tile_cols(b.kp);
+    for (int side = 0; side < 2; ++side) {
+      cpb[side] = pick_cols_per_block(b.n(side), r_live, 4 * tile, tile, b.h->sm_count * 8);
+      chunks[side] = (b.n(side) + cpb[side] - 1) / cpb[side];
+    }
+  }
+  // the split-K factor is a function of the reduction length only (gemm_fixed_splits)
+  void plan_gemms() {
+    plan[0] = view_gemm_plan(v, 0, b.SK);
+    if (b.io.num_rows) plan[0].splits = 1;
+    plan[1] = view_gemm_plan(v, 1, b.SK);
+  }
+
+  int alloc() {
+    // the rows never exceed SK0
+    const size_t need_r = (size_t)plan[0].splits * (size_t)b.SK0 * v.ld_r;
+    const size_t need_c = (size_t)plan[1].splits * (size_t)b.SK0 * v.ld_c;
+    b.NUM[0] = b.io.num_rows ? const_cast<float*>(b.io.num_rows)
+                             : static_cast<float*>(b.h->dev_buf("solve.NUMr", sizeof(float) * need_r));
+    b.NUM[1] = b.io.update_cols ? static_cast<float*>(b.h->dev_buf("solve.NUMc", sizeof(float) * need_c)) : nullptr;
+    if (!b.NUM[0] || (b.io.update_cols && !b.NUM[1])) return -2;
+    if (tf32) {
+      const size_t nr = (size_t)b.SK0 * v.ld_r, nc = (size_t)b.SK0 * v.ld_c;
+      hi[0] = static_cast<float*>(b.h->dev_buf("solve.Fr_hi", nr * 4));
+      lo[0] = static_cast<float*>(b.h->dev_buf("solve.Fr_lo", nr * 4));
+      hi[1] = static_cast<float*>(b.h->dev_buf("solve.Fc_hi", nc * 4));
+      lo[1] = static_cast<float*>(b.h->dev_buf("solve.Fc_lo", nc * 4));
+      if (!hi[0] || !lo[0] || !hi[1] || !lo[1]) return -2;
+    }
+    if (f16) {
+      tile_scale[0] = static_cast<float*>(b.h->dev_buf("solve.rowscale_r", sizeof(float) * (size_t)b.SK0 * ktiles[0]));
+      tile_scale[1] = static_cast<float*>(b.h->dev_buf("solve.rowscale_c", sizeof(float) * (size_t)b.SK0 * ktiles[1]));
+      if (!tile_scale[0] || !tile_scale[1]) return -2;
+    }
+    return 0;
+  }
+
+  FactorView view(int side) const {
+    FactorView f{};
+    f.F = b.F[side];
+    // the fixed factor of a refit is never rewritten
+    const bool pieces = upd_pieces && (side == 0 || b.io.update_cols);
+    f.F_hi = pieces ? hi[side] : nullptr;
+    f.F_lo = pieces ? lo[side] : nullptr;
+    f.n = b.n(side); f.ld = b.ld(side); f.piece_scale = scale(side);
+    if (emit_in_update) { f.P_hi = hi[side]; f.P_mid = lo[side]; f.tile_scale = tile_scale[side]; f.n_ktiles = ktiles[side]; }
+    f.cpb = cpb[side]; f.gcpb = gcpb[side];
+    return f;
+  }
+  int pieces(int side) {
+    return make_pieces(v.form, b.F[side], b.SK, b.n(side), b.ld(side), scale(side), hi[side], lo[side], tile_scale[side], b.s);
+  }
+  int emit_pieces(int side) {   // fp16 pieces + row scales of a factor that was just (re)written
+    if (!f16) return 0;
+    b.h->launches += 1;
+    const int slot = b.h->prof_begin(b.s, 8.0 * (double)b.SK * (double)b.n(side), 1);   // fp32 in, two fp16 pieces out
+    const int rc = pieces(side);
+    b.h->prof_end(b.s, slot);
+    return rc;
+  }
+  int start() {
+    if (upd_pieces) {              // tf32 pieces of the starting factors; afterwards the update kernels write them
+      CNMF_TRY(pieces(0));
+      CNMF_TRY(pieces(1));
+      b.h->launches += 2;
+    }
+    CNMF_TRY(emit_pieces(0));      // f16: fp16 pieces of the starting factors
+    return emit_pieces(1);
+  }
+
+  int gemm(int side) {
+    if (side == 0 && b.io.num_rows) return 0;   // computed by the caller
+    const int o = 1 - side;                     // the factor multiplied
+    return view_gemm(b.h, v, side, b.F[o], hi[o], lo[o], tile_scale[o], b.SK, b.NUM[side], plan[side], b.s);
+  }
+  // stand-alone Gram: partial launch + finalize (initial factors, fixed factors of a refit, batches with K > 16)
+  int gram(int side, const BatchMeta& m) {
+    b.h->launches += 2;
+    const FactorView f = view(side);
+    CNMF_TRY(launch_gram_partial(f, m, b.gram_part[side], b.s));
+    return launch_finalize(b.gram_part[side], b.gram[side], nullptr, nullptr, gram_chunks(f), m, b.s);
+  }
+  int grams(const BatchMeta& m) {
+    b.h->launches += 4;
+    CNMF_TRY(launch_gram_partial(view(0), m, b.gram_part[0], b.s));
+    CNMF_TRY(launch_gram_partial(view(1), m, b.gram_part[1], b.s));
+    CNMF_TRY(launch_finalize(b.gram_part[0], b.gram[0], nullptr, nullptr, gram_chunks(view(0)), m, b.s));
+    return launch_finalize(b.gram_part[1], b.gram[1], nullptr, nullptr, gram_chunks(view(1)), m, b.s);
+  }
+  int cross(int side, const BatchMeta& m, double* out) {
+    b.h->launches += 2;
+    CNMF_TRY(launch_cross(view(side), b.NUM[side], plan[side].splits, plan[side].split_stride, m, b.scal_part[side], b.s));
+    return launch_finalize(nullptr, nullptr, b.scal_part[side], out, chunks[side], m, b.s);
+  }
+  int update(int side, bool want_gram, bool want_scal, double* scal) {
+    const FactorView f = view(side);
+    FusedOut out{};
+    if (want_gram && fused_gram) {
+      out.gram_part = b.gram_part[side];
+      out.gram = b.gram[side];
+    }
+    out.scal_part = want_scal ? b.scal_part[side] : nullptr;
+    out.scal = scal;
+    out.counter = b.d_ticket;
+    const GemmPlan& pl = plan[side];
+    // algorithmic bytes: factor read, product slices read, factor (+ pieces: two tf32 pieces = 2 floats per element,
+    // two fp16 pieces = 1) written
+    const int piece_floats = f.F_hi ? 2 : ((f.P_hi && out.gram_part) ? 1 : 0);
+    b.h->launches += 1;
+    const int slot = b.h->prof_begin(b.s, 4.0 * (double)b.SK * (double)f.n * (double)(2 + pl.splits + piece_floats), 1);
+    const double* gram_in = b.gram[1 - side];
+    const int rc = cd ? launch_cd_update(f, b.NUM[side], pl.splits, pl.split_stride, gram_in, b.bm(), l1[side], l2[side], out, b.s)
+                      : launch_mu_update(f, b.NUM[side], pl.splits, pl.split_stride, gram_in, b.bm(), l1[side], l2[side], out, b.s);
+    b.h->prof_end(b.s, slot);
+    if (rc != 0 || !b.io.update_cols) return rc;   // a refit never multiplies by the factor it updates
+    if (f.P_hi && out.gram_part) return 0;         // the Gram-fused kernel emitted the pieces of every tile it wrote
+    return emit_pieces(side);
+  }
+
+  // the live restarts' pieces follow their factors to the packed front of the alternates (tf32; f16 pieces are
+  // emitted again by repack)
+  int compact(const std::vector<int>& src, const std::vector<int>& dst, const std::vector<int>& k) {
+    if (tf32 && !alt_hi[0]) {
+      const size_t nr = (size_t)b.SK0 * v.ld_r, nc = (size_t)b.SK0 * v.ld_c;
+      alt_hi[0] = static_cast<float*>(b.h->dev_buf("solve.alt.Fr_hi", nr * 4));
+      alt_lo[0] = static_cast<float*>(b.h->dev_buf("solve.alt.Fr_lo", nr * 4));
+      alt_hi[1] = static_cast<float*>(b.h->dev_buf("solve.alt.Fc_hi", nc * 4));
+      alt_lo[1] = static_cast<float*>(b.h->dev_buf("solve.alt.Fc_lo", nc * 4));
+      if (!alt_hi[0] || !alt_lo[0] || !alt_hi[1] || !alt_lo[1]) return -2;
+    }
+    if (upd_pieces)
+      for (int side = 0; side < 2; ++side) {
+        CNMF_TRY(b.gather(hi[side], alt_hi[side], src, dst, k, b.ld(side)));
+        CNMF_TRY(b.gather(lo[side], alt_lo[side], src, dst, k, b.ld(side)));
+      }
+    for (int side = 0; side < 2; ++side) {
+      std::swap(hi[side], alt_hi[side]);
+      std::swap(lo[side], alt_lo[side]);
+    }
+    return 0;
+  }
+  // after a compaction: plans and f16 pieces follow the new packing
+  int repack() {
+    plan_gemms();
+    plan_blocks(b.R);
+    CNMF_TRY(emit_pieces(0));
+    return emit_pieces(1);
+  }
+};
+
+// One Frobenius batched solve (MU or CD, factorize or refit) on the ops of the factor element type.
+//
+// One outer iteration of sklearn's solvers (MU: _nmf.py:826-879, CD: _nmf.py:491-516) becomes
+//   NUM_r = Fc * X^T,  Fr <- update(Fr, NUM_r, Gram(Fc)),  NUM_c = Fr * X,  Fc <- update(Fc, NUM_c, Gram(Fr)).
+// Convergence is evaluated on the device per restart; converged restarts are frozen and the host only polls the flags,
+// dropping them from the packed arrays (compaction) when that saves a GEMM tile.
+template <class Ops>
+int solve_frobenius(cnmf_handle_s* h, const DataView& v, SolveIO<typename Ops::T>& io, const cnmf_nmf_params& p,
+                    cudaStream_t s) {
+  using T = typename Ops::T;
   const int R0 = io.R;
-  if (v.form == Form::FP64) return solve_batched_f64(h, v, io, p, s);
-  if (p.beta_loss != CNMF_LOSS_FROBENIUS) return solve_batched_beta(h, v, io, p, s);
   CNMF_REQUIRE(R0 > 0 && (int)io.ks.size() == R0, "solve: bad restart list");
   CNMF_REQUIRE(p.solver == CNMF_SOLVER_MU || p.solver == CNMF_SOLVER_CD, "solve: unknown solver");
   CNMF_REQUIRE(p.max_iter >= 1, "solve: max_iter must be >= 1");
   CNMF_REQUIRE(!io.num_rows || !io.update_cols, "solve: a caller-computed row product needs update_cols = false");
-  const bool tf32 = v.form != Form::FP32;        // the factors have operand pieces
-  const bool f16 = v.form == Form::F16_EXACT;
   const bool mu = p.solver == CNMF_SOLVER_MU;
 
   // ---- slot tables (host mirrors); slot s holds restart rid[s] at packed rows [off[s], off[s]+k[s])
@@ -123,8 +367,12 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
     SK0 += io.ks[r];
     kmax = std::max(kmax, io.ks[r]);
   }
-  int R = R0, SK = SK0;     // live slots / live packed rows
-  const int kp = kmax <= 16 ? 16 : 32;
+  FroSolve<T> b{h, v, io, s};
+  b.R0 = b.R = R0;
+  b.SK0 = b.SK = SK0;
+  b.kp = Ops::pick_kp(kmax);
+  b.F[0] = io.Fr;
+  b.F[1] = io.Fc;
   // packed layout of a list of restarts: each one's rows follow the previous one's
   auto pack_offsets = [&](const std::vector<int>& kk, std::vector<int>& offs) -> int {
     int pos = 0;
@@ -135,375 +383,162 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
     }
     return pos;
   };
-  // block granularity of the streaming kernels, fixed for the whole solve (partial buffers are sized by it)
-  // update kernels: 3 blocks of 128 threads per SM resident, a block walks 1-4 tiles -> aim for >= 8 blocks per SM;
-  // stand-alone Gram kernel: 1 block/SM resident and a fixed-cost block reduction -> long blocks, about two waves
-  const int tile = upd_tile_cols(kp);
-  // the update kernels' chunking follows the number of LIVE restarts (re-planned after every compaction): with few
-  // restarts left a block should hold one tile, so that the work spreads over many SMs
-  int cpb_r = 0, cpb_c = 0, chunks_r = 0, chunks_c = 0;
-  auto plan_blocks = [&](int r_live) {
-    cpb_r = pick_cols_per_block(v.n_r, r_live, 4 * tile, tile, h->sm_count * 8);
-    cpb_c = pick_cols_per_block(v.n_c, r_live, 4 * tile, tile, h->sm_count * 8);
-    chunks_r = (v.n_r + cpb_r - 1) / cpb_r;
-    chunks_c = (v.n_c + cpb_c - 1) / cpb_c;
-  };
-  const int gcpb_r = pick_cols_per_block(v.n_r, R0, 8192, 1024, h->sm_count * 2);
-  const int gcpb_c = pick_cols_per_block(v.n_c, R0, 8192, 1024, h->sm_count * 2);
-  const int chunks_cap = std::max((v.n_r + tile - 1) / tile, (v.n_c + tile - 1) / tile);   // finest chunking possible
-  const int gchunks_max = std::max((v.n_r + gcpb_r - 1) / gcpb_r, (v.n_c + gcpb_c - 1) / gcpb_c);
-  size_t fused_part_slots = 0;      // slot-indexed partials of the fused kernels: max over live counts of R * chunks
-  for (int r = 1; r <= R0; ++r) {
-    plan_blocks(r);
-    fused_part_slots = std::max(fused_part_slots, (size_t)r * std::max(chunks_r, chunks_c));
-  }
-  plan_blocks(R0);
-  const bool fuse = kp == 16;   // the update kernels emit the Gram of the factor they write (nmf_kernels.cu)
+  Ops ops(b, p);
 
   // ---- workspace
   int* d_meta = static_cast<int*>(h->dev_buf("solve.meta", sizeof(int) * 8 * R0));
   double* d_state = static_cast<double*>(h->dev_buf("solve.state", sizeof(double) * 8 * R0));
   double* d_gram = static_cast<double*>(h->dev_buf("solve.gram", sizeof(double) * 2 * R0 * KMAX * KMAX));
-  // per-block Gram partials of each factor (summed by the last block of the producing launch)
-  const size_t gpart_elems = std::max((size_t)R0 * std::max(gchunks_max, std::max((v.n_r + 1023) / 1024, (v.n_c + 1023) / 1024)),
-                                     fused_part_slots) * kp * kp;
-  double* d_gram_part = static_cast<double*>(h->dev_buf("solve.gram_part", sizeof(double) * 2 * gpart_elems));
-  double* d_scal_part = static_cast<double*>(h->dev_buf("solve.scal_part", sizeof(double) * 2 * (size_t)R0 * chunks_cap));
+  double* d_gram_part = static_cast<double*>(h->dev_buf("solve.gram_part", sizeof(double) * 2 * ops.gram_part_elems));
+  double* d_scal_part =
+      static_cast<double*>(h->dev_buf("solve.scal_part", sizeof(double) * 2 * (size_t)R0 * ops.chunks_cap));
   if (!d_meta || !d_state || !d_gram || !d_gram_part || !d_scal_part) return -2;
+  CNMF_TRY(ops.alloc());
 
-  GemmPlan plan_r, plan_c;   // plan_r: NUM_r = Fc * B_rows^T (reduce over n_c); plan_c: NUM_c = Fr * B_cols^T
-  float *NUMr = nullptr, *NUMc = nullptr;
-  // the split-K factor is a function of the reduction length only (gemm_fixed_splits)
-  auto plan_gemms = [&]() -> int {
-    plan_r = view_gemm_plan(v, 0, SK);
-    if (io.num_rows) plan_r.splits = 1;
-    plan_c = view_gemm_plan(v, 1, SK);
-    return 0;
-  };
-  plan_gemms();
-  // size the product buffers: the split-K factor depends on the reduction length only, the rows never exceed SK0
-  {
-    const size_t need_r = (size_t)plan_r.splits * (size_t)SK0 * v.ld_r;
-    const size_t need_c = (size_t)plan_c.splits * (size_t)SK0 * v.ld_c;
-    NUMr = io.num_rows ? const_cast<float*>(io.num_rows) : static_cast<float*>(h->dev_buf("solve.NUMr", sizeof(float) * need_r));
-    NUMc = io.update_cols ? static_cast<float*>(h->dev_buf("solve.NUMc", sizeof(float) * need_c)) : nullptr;
-    if (!NUMr || (io.update_cols && !NUMc)) return -2;
-  }
-
-  int* d_off = d_meta;             // [slots]
-  int* d_k = d_meta + R0;          // [slots]
-  int* d_rid = d_meta + 2 * R0;    // [slots]
-  int* d_done = d_meta + 3 * R0;   // [rid]
+  b.d_off = d_meta;                // [slots]
+  b.d_k = d_meta + R0;             // [slots]
+  b.d_rid = d_meta + 2 * R0;       // [slots]
+  b.d_done = d_meta + 3 * R0;      // [rid]
   int* d_niter = d_meta + 4 * R0;  // [rid]
-  int* d_ticket = d_meta + 5 * R0; // [rid] last-block tickets of the fused update kernels (self-resetting)
+  b.d_ticket = d_meta + 5 * R0;    // [rid] last-block tickets of the fused update kernels (self-resetting)
   auto upload_slots = [&]() -> int {
     std::vector<int> hm(3 * R0, 0);
-    std::memcpy(hm.data(), s_off.data(), sizeof(int) * R);
-    std::memcpy(hm.data() + R0, s_k.data(), sizeof(int) * R);
-    std::memcpy(hm.data() + 2 * R0, s_rid.data(), sizeof(int) * R);
+    std::memcpy(hm.data(), s_off.data(), sizeof(int) * b.R);
+    std::memcpy(hm.data() + R0, s_k.data(), sizeof(int) * b.R);
+    std::memcpy(hm.data() + 2 * R0, s_rid.data(), sizeof(int) * b.R);
     CNMF_CUDA_CHECK(cudaMemcpyAsync(d_meta, hm.data(), sizeof(int) * 3 * R0, cudaMemcpyHostToDevice, s));
     CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
     return 0;
   };
   CNMF_TRY(upload_slots());
-  CNMF_CUDA_CHECK(cudaMemsetAsync(d_done, 0, sizeof(int) * 3 * R0, s));   // done, n_iter, tickets
+  CNMF_CUDA_CHECK(cudaMemsetAsync(b.d_done, 0, sizeof(int) * 3 * R0, s));   // done, n_iter, tickets
   CNMF_CUDA_CHECK(cudaMemsetAsync(d_state, 0, sizeof(double) * 8 * R0, s));
-  ConvState st{d_state, d_state + R0, d_state + 2 * R0, d_done, d_niter};
+  ConvState st{d_state, d_state + R0, d_state + 2 * R0, b.d_done, d_niter};
   double* d_crossA = d_state + 3 * R0;   // finalised scalars: cross / violation of the row half
   double* d_crossB = d_state + 4 * R0;   // ... of the column half
-  double* d_gramR = d_gram;                            // Gram of Fr (e.g. W^T W), by rid
-  double* d_gramC = d_gram + (size_t)R0 * KMAX * KMAX; // Gram of Fc (e.g. H H^T), by rid
-  double* d_scalA = d_scal_part;
-  double* d_scalB = d_scal_part + (size_t)R0 * chunks_cap;
-  double* d_gpartR = d_gram_part;                      // partials of Gram(Fr)
-  double* d_gpartC = d_gram_part + gpart_elems;        // partials of Gram(Fc)
+  b.gram[0] = d_gram;                                // Gram of Fr (e.g. W^T W), by rid
+  b.gram[1] = d_gram + (size_t)R0 * KMAX * KMAX;     // Gram of Fc (e.g. H H^T), by rid
+  b.scal_part[0] = d_scal_part;
+  b.scal_part[1] = d_scal_part + (size_t)R0 * ops.chunks_cap;
+  b.gram_part[0] = d_gram_part;
+  b.gram_part[1] = d_gram_part + ops.gram_part_elems;
 
-  // working factor arrays (start in the caller's buffers; compaction ping-pongs to "solve.alt.*") and their operand
-  // pieces: tf32 hi / lo, or on f16 datasets the two fp16 pieces in the same buffers
-  float *wFr = io.Fr, *wFr_hi = nullptr, *wFr_lo = nullptr, *wFc = io.Fc, *wFc_hi = nullptr, *wFc_lo = nullptr;
-  if (tf32) {
-    const size_t nr = (size_t)SK0 * v.ld_r, nc = (size_t)SK0 * v.ld_c;
-    wFr_hi = static_cast<float*>(h->dev_buf("solve.Fr_hi", nr * 4));
-    wFr_lo = static_cast<float*>(h->dev_buf("solve.Fr_lo", nr * 4));
-    wFc_hi = static_cast<float*>(h->dev_buf("solve.Fc_hi", nc * 4));
-    wFc_lo = static_cast<float*>(h->dev_buf("solve.Fc_lo", nc * 4));
-    if (!wFr_hi || !wFr_lo || !wFc_hi || !wFc_lo) return -2;
-  }
-  float *aFr = nullptr, *aFr_hi = nullptr, *aFr_lo = nullptr, *aFc = nullptr, *aFc_hi = nullptr, *aFc_lo = nullptr;
-  float *resFr = nullptr, *resFc = nullptr;   // final factors of restarts that were compacted away (original offsets)
+  b.h_gidx = static_cast<int*>(h->host_buf("solve.gather_idx", sizeof(int) * 3 * (size_t)R0 * b.GATHER_SLOTS));
+  b.d_gidx = static_cast<int*>(h->dev_buf("solve.gather_didx", sizeof(int) * 3 * (size_t)R0 * b.GATHER_SLOTS));
+  if (!b.h_gidx || !b.d_gidx) return -2;
+
+  // working factors start in the caller's buffers; compaction ping-pongs them with the alternates and parks the
+  // final factors of the restarts it removes in the result slabs (original offsets)
+  T* alt[2] = {};
+  T* res[2] = {};
   bool compacted = false;
-
-  auto bm = [&]() { return BatchMeta{d_off, d_k, d_rid, d_done, R, kp}; };
-  float* d_rs_r = nullptr;   // f16: power-of-two scales of the Fr / Fc pieces, [packed row][512-element group]
-  float* d_rs_c = nullptr;
-  if (f16) {
-    d_rs_r = static_cast<float*>(h->dev_buf("solve.rowscale_r", sizeof(float) * (size_t)SK0 * ((v.ld_r + 511) / 512)));
-    d_rs_c = static_cast<float*>(h->dev_buf("solve.rowscale_c", sizeof(float) * (size_t)SK0 * ((v.ld_c + 511) / 512)));
-    if (!d_rs_r || !d_rs_c) return -2;
-  }
-  // tf32 pieces are written by the update kernels; the fp16 pieces need the row maximum first and come from
-  // emit_pieces() after the update (the hi / lo buffers then hold halves)
-  const bool upd_pieces = tf32 && !f16;
-  // f16: the Gram-fused update kernels (K <= 16, factor being iterated) emit the fp16 pieces themselves, per 512-column
-  // tile; everything else (initial factors, compaction, K > 16) goes through emit_pieces(), which normalises the same
-  // 512-column groups and writes the same bits
-  const int ktiles_r = (v.ld_r + 511) / 512, ktiles_c = (v.ld_c + 511) / 512;
-  const bool emit_in_update = f16 && kp == 16 && io.update_cols;
-  auto fr = [&]() {
-    FactorView f{};
-    f.F = wFr; f.F_hi = upd_pieces ? wFr_hi : nullptr; f.F_lo = upd_pieces ? wFr_lo : nullptr;
-    f.n = v.n_r; f.ld = v.ld_r; f.piece_scale = v.scale_r;
-    if (emit_in_update) { f.P_hi = wFr_hi; f.P_mid = wFr_lo; f.tile_scale = d_rs_r; f.n_ktiles = ktiles_r; }
-    f.cpb = cpb_r; f.gcpb = gcpb_r;
-    return f;
-  };
-  auto fc = [&]() {
-    FactorView f{};
-    f.F = wFc; f.F_hi = upd_pieces ? wFc_hi : nullptr; f.F_lo = upd_pieces ? wFc_lo : nullptr;
-    f.n = v.n_c; f.ld = v.ld_c; f.piece_scale = v.scale_c;
-    if (emit_in_update) { f.P_hi = wFc_hi; f.P_mid = wFc_lo; f.tile_scale = d_rs_c; f.n_ktiles = ktiles_c; }
-    f.cpb = cpb_c; f.gcpb = gcpb_c;
-    if (!io.update_cols) { f.F_hi = nullptr; f.F_lo = nullptr; }   // never rewritten
-    return f;
-  };
-  // side: 0 = row factor Fr, 1 = column factor Fc.  Stand-alone Gram: partial launch + finalize (initial factors,
-  // fixed factors of a refit, batches with K > 16).
-  auto gram_full = [&](const FactorView& f, int side_is_c) -> int {
-    h->launches += 2;
-    double* part = side_is_c ? d_gpartC : d_gpartR;
-    CNMF_TRY(launch_gram_partial(f, bm(), part, s));
-    return launch_finalize(part, side_is_c ? d_gramC : d_gramR, nullptr, nullptr, gram_chunks(f), bm(), s);
-  };
-  auto gram_after = [&](const FactorView& f, int side_is_c) -> int {   // Gram of a factor the update kernel just wrote
-    return fuse ? 0 : gram_full(f, side_is_c);
-  };
-  auto pieces = [&](int side_is_c) -> int {
-    return side_is_c ? make_pieces(v.form, wFc, SK, v.n_c, v.ld_c, v.scale_c, wFc_hi, wFc_lo, d_rs_c, s)
-                     : make_pieces(v.form, wFr, SK, v.n_r, v.ld_r, v.scale_r, wFr_hi, wFr_lo, d_rs_r, s);
-  };
-  auto emit_pieces = [&](int side_is_c) -> int {   // fp16 pieces + row scales of a factor that was just (re)written
-    if (!f16) return 0;
-    h->launches += 1;
-    const int n = side_is_c ? v.n_c : v.n_r;
-    const int slot = h->prof_begin(s, 8.0 * (double)SK * (double)n, 1);   // fp32 in, two fp16 pieces out
-    const int rc = pieces(side_is_c);
-    h->prof_end(s, slot);
-    return rc;
-  };
-  // algorithmic bytes of one update launch: factor read, product slices read, factor (+ tf32 pieces) written
-  // (pieces: two tf32 pieces = 2 floats per element, two fp16 pieces = 1)
-  auto upd_bytes = [&](int n_items, int nsplit, int piece_floats) {
-    return 4.0 * (double)SK * (double)n_items * (double)(2 + nsplit + piece_floats);
-  };
-  auto update = [&](bool cd, const FactorView& f, const float* NUM, const GemmPlan& pl, const double* gram_in, float l1,
-                    float l2, const FusedOut& out) -> int {
-    h->launches += 1;
-    const int slot = h->prof_begin(s, upd_bytes(f.n, pl.splits, f.F_hi ? 2 : ((f.P_hi && out.gram_part) ? 1 : 0)), 1);
-    const int rc = cd ? launch_cd_update(f, NUM, pl.splits, pl.split_stride, gram_in, bm(), l1, l2, out, s)
-                      : launch_mu_update(f, NUM, pl.splits, pl.split_stride, gram_in, bm(), l1, l2, out, s);
-    h->prof_end(s, slot);
-    if (rc != 0 || !io.update_cols) return rc;   // a refit never multiplies by the factor it updates
-    if (f.P_hi && out.gram_part) return 0;       // the Gram-fused kernel emitted the pieces of every tile it wrote
-    return emit_pieces(f.F == wFc ? 1 : 0);
-  };
-  auto fused_out = [&](int side_is_c, bool want_gram, double* scal_part, double* scal) {
-    FusedOut o{};
-    if (want_gram && fuse) {
-      o.gram_part = side_is_c ? d_gpartC : d_gpartR;
-      o.gram = side_is_c ? d_gramC : d_gramR;
-    }
-    o.scal_part = scal_part;
-    o.scal = scal;
-    o.counter = d_ticket;
-    return o;
-  };
-  auto finalize_scal = [&](const double* part, double* out, int chunks) -> int {
-    h->launches += 1;
-    return launch_finalize(nullptr, nullptr, part, out, chunks, bm(), s);
-  };
-  auto gemm_rows = [&]() -> int {   // NUM_r = Fc * B_rows^T
-    if (io.num_rows) return 0;      // computed by the caller
-    return view_gemm(h, v, 0, wFc, wFc_hi, wFc_lo, d_rs_c, SK, NUMr, plan_r, s);
-  };
-  auto gemm_cols = [&]() -> int {   // NUM_c = Fr * B_cols^T
-    return view_gemm(h, v, 1, wFr, wFr_hi, wFr_lo, d_rs_r, SK, NUMc, plan_c, s);
-  };
-
-  // gathers `cnt` restarts' rows: dst[dst_off[i] ..] <- src[src_off[i] ..].  Index triples go through a pinned
-  // ring of GATHER_SLOTS entries so that consecutive gathers need no host synchronisation in between; the
-  // caller synchronises the stream before the ring wraps (upload_slots / the final sync do).
-  constexpr int GATHER_SLOTS = 12;
-  int* h_gidx = static_cast<int*>(h->host_buf("solve.gather_idx", sizeof(int) * 3 * (size_t)R0 * GATHER_SLOTS));
-  int* d_gidx = static_cast<int*>(h->dev_buf("solve.gather_didx", sizeof(int) * 3 * (size_t)R0 * GATHER_SLOTS));
-  if (!h_gidx || !d_gidx) return -2;
-  int gslot = 0;
-  auto gather = [&](const float* src, float* dst, const std::vector<int>& so, const std::vector<int>& dof,
-                    const std::vector<int>& kk, int ld) -> int {
-    const int cnt = (int)kk.size();
-    if (cnt == 0 || !src || !dst) return 0;
-    if (gslot == GATHER_SLOTS) {
-      CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
-      gslot = 0;
-    }
-    int* hm = h_gidx + (size_t)gslot * 3 * R0;
-    int* dm = d_gidx + (size_t)gslot * 3 * R0;
-    ++gslot;
-    std::memcpy(hm, so.data(), sizeof(int) * cnt);
-    std::memcpy(hm + R0, dof.data(), sizeof(int) * cnt);
-    std::memcpy(hm + 2 * R0, kk.data(), sizeof(int) * cnt);
-    CNMF_CUDA_CHECK(cudaMemcpyAsync(dm, hm, sizeof(int) * 3 * R0, cudaMemcpyHostToDevice, s));
-    h->launches += 1;
-    return launch_gather_rows(src, dm, dst, dm + R0, dm + 2 * R0, cnt, ld, s);
+  auto gram_after = [&](int side) -> int {   // Gram of a factor the update kernel just wrote
+    return ops.fused_gram ? 0 : ops.gram(side, b.bm());
   };
 
   const double normX2 = v.sum_sq;
   double* d_cd_err = d_state + 7 * R0;
+  // CD: ||X - Fr^T Fc||_F of the restarts still packed, in the trace form, into d_cd_err
   auto cd_final_error = [&]() -> int {
     int* d_zero = static_cast<int*>(h->dev_buf("solve.zero", sizeof(int) * 2 * R0));
     if (!d_zero) return -2;
     CNMF_CUDA_CHECK(cudaMemsetAsync(d_zero, 0, sizeof(int) * 2 * R0, s));
-    BatchMeta bm0{d_off, d_k, d_rid, d_zero, R, kp};
-    h->launches += 7;
-    CNMF_TRY(launch_gram_partial(fr(), bm0, d_gpartR, s));
-    CNMF_TRY(launch_gram_partial(fc(), bm0, d_gpartC, s));
-    CNMF_TRY(launch_finalize(d_gpartR, d_gramR, nullptr, nullptr, gram_chunks(fr()), bm0, s));
-    CNMF_TRY(launch_finalize(d_gpartC, d_gramC, nullptr, nullptr, gram_chunks(fc()), bm0, s));
-    if (io.update_cols) {
-      CNMF_TRY(launch_cross(fc(), NUMc, plan_c.splits, plan_c.split_stride, bm0, d_scalB, s));
-      CNMF_TRY(launch_finalize(nullptr, nullptr, d_scalB, d_crossB, chunks_c, bm0, s));
-    } else {
-      CNMF_TRY(launch_cross(fr(), NUMr, plan_r.splits, plan_r.split_stride, bm0, d_scalA, s));
-      CNMF_TRY(launch_finalize(nullptr, nullptr, d_scalA, d_crossB, chunks_r, bm0, s));
-    }
+    BatchMeta bm0{b.d_off, b.d_k, b.d_rid, d_zero, b.R, b.kp};
+    CNMF_TRY(ops.grams(bm0));
+    CNMF_TRY(ops.cross(io.update_cols ? 1 : 0, bm0, d_crossB));
     ConvState scratch{d_state + 5 * R0, d_state + 6 * R0, d_cd_err, d_zero, d_zero + R0};
-    return launch_mu_check(scratch, d_crossB, d_gramR, d_gramC, normX2, bm0, 0, 0.0, p.max_iter, s);
+    h->launches += 1;
+    return launch_mu_check(scratch, d_crossB, b.gram[0], b.gram[1], normX2, bm0, 0, 0.0, p.max_iter, s);
   };
 
   std::vector<int> h_done(R0, 0);
-  // Drop converged restarts from the packed arrays when that saves a 128-row GEMM tile (or >= 1/8 of the rows).
+  // Drop converged restarts from the packed arrays when that saves a GEMM tile (or >= 1/8 of the rows).
   auto maybe_compact = [&]() -> int {
     if (!io.update_cols) return 0;
-    int live_rows = 0;
-    for (int sl = 0; sl < R; ++sl)
-      if (!h_done[s_rid[sl]]) live_rows += s_k[sl];
-    if (live_rows == SK || live_rows == 0) return 0;
-    std::vector<int> lk, lo;
-    for (int sl = 0; sl < R; ++sl)
-      if (!h_done[s_rid[sl]]) lk.push_back(s_k[sl]);
-    const int new_rows = pack_offsets(lk, lo);              // rows of the packed live set
-    const bool saves_tile = (new_rows + 127) / 128 < (SK + 127) / 128;
-    if (!saves_tile && new_rows > SK - SK / 8) return 0;
-    if (!mu) CNMF_TRY(cd_final_error());    // restarts leaving the packed arrays get their ||X - WH||_F now
-    if (!aFr) {
-      const size_t nr = (size_t)SK0 * v.ld_r, nc = (size_t)SK0 * v.ld_c;
-      aFr = static_cast<float*>(h->dev_buf("solve.alt.Fr", nr * 4));
-      aFc = static_cast<float*>(h->dev_buf("solve.alt.Fc", nc * 4));
-      resFr = static_cast<float*>(h->dev_buf("solve.res.Fr", nr * 4));
-      resFc = static_cast<float*>(h->dev_buf("solve.res.Fc", nc * 4));
-      if (!aFr || !aFc || !resFr || !resFc) return -2;
-      if (tf32) {
-        aFr_hi = static_cast<float*>(h->dev_buf("solve.alt.Fr_hi", nr * 4));
-        aFr_lo = static_cast<float*>(h->dev_buf("solve.alt.Fr_lo", nr * 4));
-        aFc_hi = static_cast<float*>(h->dev_buf("solve.alt.Fc_hi", nc * 4));
-        aFc_lo = static_cast<float*>(h->dev_buf("solve.alt.Fc_lo", nc * 4));
-        if (!aFr_hi || !aFr_lo || !aFc_hi || !aFc_lo) return -2;
-      }
-    }
-    std::vector<int> f_src, f_dst, f_k, l_src, l_dst, l_k, n_off, n_k, n_rid;
-    for (int sl = 0; sl < R; ++sl) {
+    std::vector<int> f_src, f_dst, f_k, l_src, l_dst, l_k, n_rid;
+    for (int sl = 0; sl < b.R; ++sl) {
       const int rid = s_rid[sl];
       if (h_done[rid]) {
         f_src.push_back(s_off[sl]); f_dst.push_back(off0[rid]); f_k.push_back(s_k[sl]);
       } else {
-        l_src.push_back(s_off[sl]); l_k.push_back(s_k[sl]);
-        n_k.push_back(s_k[sl]); n_rid.push_back(rid);
+        l_src.push_back(s_off[sl]); l_k.push_back(s_k[sl]); n_rid.push_back(rid);
       }
     }
-    const int pos = pack_offsets(l_k, l_dst);
-    n_off = l_dst;
-    CNMF_TRY(gather(wFr, resFr, f_src, f_dst, f_k, v.ld_r));       // finished restarts -> result slabs
-    CNMF_TRY(gather(wFc, resFc, f_src, f_dst, f_k, v.ld_c));
-    CNMF_TRY(gather(wFr, aFr, l_src, l_dst, l_k, v.ld_r));          // live restarts -> packed front of the alt buffers
-    CNMF_TRY(gather(wFc, aFc, l_src, l_dst, l_k, v.ld_c));
-    if (upd_pieces) {
-      CNMF_TRY(gather(wFr_hi, aFr_hi, l_src, l_dst, l_k, v.ld_r));
-      CNMF_TRY(gather(wFr_lo, aFr_lo, l_src, l_dst, l_k, v.ld_r));
-      CNMF_TRY(gather(wFc_hi, aFc_hi, l_src, l_dst, l_k, v.ld_c));
-      CNMF_TRY(gather(wFc_lo, aFc_lo, l_src, l_dst, l_k, v.ld_c));
+    const int new_rows = pack_offsets(l_k, l_dst);   // rows of the packed live set
+    const int SK = b.SK, tr = Ops::tile_rows;
+    if (new_rows == SK || new_rows == 0) return 0;
+    const bool saves_tile = (new_rows + tr - 1) / tr < (SK + tr - 1) / tr;
+    if (!saves_tile && new_rows > SK - SK / 8) return 0;
+    if (!mu) CNMF_TRY(cd_final_error());    // restarts leaving the packed arrays get their ||X - WH||_F now
+    if (!alt[0]) {
+      const std::string tag = Ops::buf_tag;
+      const size_t nr = (size_t)SK0 * v.ld_r * sizeof(T), nc = (size_t)SK0 * v.ld_c * sizeof(T);
+      alt[0] = static_cast<T*>(h->dev_buf("solve.alt.Fr" + tag, nr));
+      alt[1] = static_cast<T*>(h->dev_buf("solve.alt.Fc" + tag, nc));
+      res[0] = static_cast<T*>(h->dev_buf("solve.res.Fr" + tag, nr));
+      res[1] = static_cast<T*>(h->dev_buf("solve.res.Fc" + tag, nc));
+      if (!alt[0] || !alt[1] || !res[0] || !res[1]) return -2;
     }
-    std::swap(wFr, aFr); std::swap(wFr_hi, aFr_hi); std::swap(wFr_lo, aFr_lo);
-    std::swap(wFc, aFc); std::swap(wFc_hi, aFc_hi); std::swap(wFc_lo, aFc_lo);
-    R = (int)n_k.size();
-    SK = pos;
-    std::copy(n_off.begin(), n_off.end(), s_off.begin());
-    std::copy(n_k.begin(), n_k.end(), s_k.begin());
+    CNMF_TRY(b.gather(b.F[0], res[0], f_src, f_dst, f_k, v.ld_r));    // finished restarts -> result slabs
+    CNMF_TRY(b.gather(b.F[1], res[1], f_src, f_dst, f_k, v.ld_c));
+    CNMF_TRY(b.gather(b.F[0], alt[0], l_src, l_dst, l_k, v.ld_r));    // live restarts -> packed front of the alternates
+    CNMF_TRY(b.gather(b.F[1], alt[1], l_src, l_dst, l_k, v.ld_c));
+    CNMF_TRY(ops.compact(l_src, l_dst, l_k));
+    std::swap(b.F[0], alt[0]);
+    std::swap(b.F[1], alt[1]);
+    b.R = (int)l_k.size();
+    b.SK = new_rows;
+    std::copy(l_dst.begin(), l_dst.end(), s_off.begin());
+    std::copy(l_k.begin(), l_k.end(), s_k.begin());
     std::copy(n_rid.begin(), n_rid.end(), s_rid.begin());
     CNMF_TRY(upload_slots());      // synchronises the stream: the gather ring can be reused
-    gslot = 0;
-    plan_gemms();
-    plan_blocks(R);
-    CNMF_TRY(emit_pieces(0));      // f16: pieces and row scales follow the new packing
-    CNMF_TRY(emit_pieces(1));
+    b.gslot = 0;
+    CNMF_TRY(ops.repack());
     compacted = true;
     return 0;
   };
 
   auto poll_all_done = [&]() -> int {   // 1 = all done, 0 = not yet, <0 error
-    CNMF_CUDA_CHECK(cudaMemcpyAsync(h_done.data(), d_done, sizeof(int) * R0, cudaMemcpyDeviceToHost, s));
+    CNMF_CUDA_CHECK(cudaMemcpyAsync(h_done.data(), b.d_done, sizeof(int) * R0, cudaMemcpyDeviceToHost, s));
     CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
-    for (int sl = 0; sl < R; ++sl)
+    for (int sl = 0; sl < b.R; ++sl)
       if (!h_done[s_rid[sl]]) return maybe_compact();
     return 1;
   };
 
-  const float l1W = (float)p.l1_reg_W, l2W = (float)p.l2_reg_W, l1H = (float)p.l1_reg_H, l2H = (float)p.l2_reg_H;
-  int it = 0;
-  if (upd_pieces) {                // tf32 pieces of the starting factors; afterwards the update kernels write them
-    CNMF_TRY(pieces(0));
-    CNMF_TRY(pieces(1));
-    h->launches += 2;
-  }
-  CNMF_TRY(emit_pieces(0));        // f16: fp16 pieces of the starting factors
-  CNMF_TRY(emit_pieces(1));
-
+  CNMF_TRY(ops.start());
   if (mu) {
     // ---------------- multiplicative update (sklearn _nmf.py:726-888) ----------------
-    CNMF_TRY(gram_full(fc(), 1));
-    CNMF_TRY(gram_full(fr(), 0));
-    if (io.update_cols) {
-      CNMF_TRY(gemm_cols());
-      h->launches += 1;
-      CNMF_TRY(launch_cross(fc(), NUMc, plan_c.splits, plan_c.split_stride, bm(), d_scalB, s));
-      CNMF_TRY(finalize_scal(d_scalB, d_crossB, chunks_c));
-    } else {
-      CNMF_TRY(gemm_rows());          // H fixed: X H^T is computed once (sklearn caches XHt, _nmf.py:537-548)
-      h->launches += 1;
-      CNMF_TRY(launch_cross(fr(), NUMr, plan_r.splits, plan_r.split_stride, bm(), d_scalA, s));
-      CNMF_TRY(finalize_scal(d_scalA, d_crossB, chunks_r));
-    }
+    CNMF_TRY(ops.gram(1, b.bm()));
+    CNMF_TRY(ops.gram(0, b.bm()));
+    // the starting error from <NUM_c, Fc>, or on a refit from <NUM_r, Fr>: H fixed, X H^T is computed once (sklearn
+    // caches XHt, _nmf.py:537-548)
+    const int first = io.update_cols ? 1 : 0;
+    CNMF_TRY(ops.gemm(first));
+    CNMF_TRY(ops.cross(first, b.bm(), d_crossB));
     h->launches += 1;
-    CNMF_TRY(launch_mu_check(st, d_crossB, d_gramR, d_gramC, normX2, bm(), 0, p.tol, p.max_iter, s));
+    CNMF_TRY(launch_mu_check(st, d_crossB, b.gram[0], b.gram[1], normX2, b.bm(), 0, p.tol, p.max_iter, s));
 
-    // one iteration = GEMM, update(+Gram), GEMM, update(+Gram): the update kernels leave the finalised Gram of the
-    // factor they wrote (and, at check iterations, <NUM, F>) behind, so nothing else sits between the GEMMs
-    for (it = 1; it <= p.max_iter; ++it) {
+    // one iteration = GEMM, update(+Gram), GEMM, update(+Gram): the float update kernels leave the finalised Gram of
+    // the factor they wrote (and, at check iterations, <NUM, F>) behind, so nothing else sits between the GEMMs
+    for (int it = 1; it <= p.max_iter; ++it) {
       const bool check = (p.tol > 0 && it % 10 == 0) || it == p.max_iter;
       if (io.update_cols) {
-        CNMF_TRY(gemm_rows());
-        CNMF_TRY(update(false, fr(), NUMr, plan_r, d_gramC, l1W, l2W, fused_out(0, true, nullptr, nullptr)));
-        CNMF_TRY(gram_after(fr(), 0));
-        CNMF_TRY(gemm_cols());
-        CNMF_TRY(update(false, fc(), NUMc, plan_c, d_gramR, l1H, l2H, fused_out(1, true, check ? d_scalB : nullptr, d_crossB)));
-        CNMF_TRY(gram_after(fc(), 1));
+        CNMF_TRY(ops.gemm(0));
+        CNMF_TRY(ops.update(0, true, false, nullptr));
+        CNMF_TRY(gram_after(0));
+        CNMF_TRY(ops.gemm(1));
+        CNMF_TRY(ops.update(1, true, check, d_crossB));
+        CNMF_TRY(gram_after(1));
       } else {
-        CNMF_TRY(update(false, fr(), NUMr, plan_r, d_gramC, l1W, l2W, fused_out(0, check, check ? d_scalA : nullptr, d_crossB)));
-        if (check) CNMF_TRY(gram_after(fr(), 0));
+        CNMF_TRY(ops.update(0, check, check, d_crossB));
+        if (check) CNMF_TRY(gram_after(0));
       }
       if (check) {
         h->launches += 1;
         // at it == max_iter with it % 10 != 0 sklearn does not test; tol = -1 makes the test never fire
         const double tol_eff = (p.tol > 0 && it % 10 == 0) ? p.tol : -1.0;
-        CNMF_TRY(launch_mu_check(st, d_crossB, d_gramR, d_gramC, normX2, bm(), it, tol_eff, p.max_iter, s));
+        CNMF_TRY(launch_mu_check(st, d_crossB, b.gram[0], b.gram[1], normX2, b.bm(), it, tol_eff, p.max_iter, s));
         const int all = poll_all_done();
         if (all < 0) return all;
         if (all) break;
@@ -512,18 +547,18 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
   } else {
     // ---------------- coordinate descent (sklearn _nmf.py:399-518, shuffle=False) ----------------
     const int poll_every = 4;
-    for (it = 1; it <= p.max_iter; ++it) {
-      if (it == 1) CNMF_TRY(gram_full(fc(), 1));     // afterwards: left behind by the sweep over Fc
-      if (io.update_cols || it == 1) CNMF_TRY(gemm_rows());
-      CNMF_TRY(update(true, fr(), NUMr, plan_r, d_gramC, l1W, l2W, fused_out(0, io.update_cols, d_scalA, d_crossA)));
+    for (int it = 1; it <= p.max_iter; ++it) {
+      if (it == 1) CNMF_TRY(ops.gram(1, b.bm()));     // afterwards: left behind by the sweep over Fc
+      if (io.update_cols || it == 1) CNMF_TRY(ops.gemm(0));
+      CNMF_TRY(ops.update(0, io.update_cols, true, d_crossA));
       if (io.update_cols) {
-        CNMF_TRY(gram_after(fr(), 0));
-        CNMF_TRY(gemm_cols());
-        CNMF_TRY(update(true, fc(), NUMc, plan_c, d_gramR, l1H, l2H, fused_out(1, true, d_scalB, d_crossB)));
-        CNMF_TRY(gram_after(fc(), 1));
+        CNMF_TRY(gram_after(0));
+        CNMF_TRY(ops.gemm(1));
+        CNMF_TRY(ops.update(1, true, true, d_crossB));
+        CNMF_TRY(gram_after(1));
       }
       h->launches += 1;
-      CNMF_TRY(launch_cd_check(st, d_crossA, io.update_cols ? d_crossB : nullptr, bm(), it, p.tol, p.max_iter, s));
+      CNMF_TRY(launch_cd_check(st, d_crossA, io.update_cols ? d_crossB : nullptr, b.bm(), it, p.tol, p.max_iter, s));
       if (it % poll_every == 0 || it == p.max_iter) {
         const int all = poll_all_done();
         if (all < 0) return all;
@@ -543,12 +578,13 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
 
   // ---- put every restart's final factors back at its original rows of the caller's buffers
   if (compacted) {
+    const int R = b.R;
     std::vector<int> so(s_off.begin(), s_off.begin() + R), ko(s_k.begin(), s_k.begin() + R), dof(R);
     for (int sl = 0; sl < R; ++sl) dof[sl] = off0[s_rid[sl]];
-    CNMF_TRY(gather(wFr, resFr, so, dof, ko, v.ld_r));
-    CNMF_TRY(gather(wFc, resFc, so, dof, ko, v.ld_c));
-    CNMF_CUDA_CHECK(cudaMemcpyAsync(io.Fr, resFr, (size_t)SK0 * v.ld_r * 4, cudaMemcpyDeviceToDevice, s));
-    CNMF_CUDA_CHECK(cudaMemcpyAsync(io.Fc, resFc, (size_t)SK0 * v.ld_c * 4, cudaMemcpyDeviceToDevice, s));
+    CNMF_TRY(b.gather(b.F[0], res[0], so, dof, ko, v.ld_r));
+    CNMF_TRY(b.gather(b.F[1], res[1], so, dof, ko, v.ld_c));
+    CNMF_CUDA_CHECK(cudaMemcpyAsync(io.Fr, res[0], (size_t)SK0 * v.ld_r * sizeof(T), cudaMemcpyDeviceToDevice, s));
+    CNMF_CUDA_CHECK(cudaMemcpyAsync(io.Fc, res[1], (size_t)SK0 * v.ld_c * sizeof(T), cudaMemcpyDeviceToDevice, s));
   }
 
   io.n_iter.assign(R0, 0);
@@ -560,6 +596,20 @@ int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_n
   CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
   // per-launch event pairs are folded into the totals lazily (cnmf_profile_get*), not inside the solve
   return 0;
+}
+
+}  // namespace
+
+int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO<float>& io, const cnmf_nmf_params& p, cudaStream_t s) {
+  CNMF_REQUIRE(v.form != Form::FP64, "solve: float64 datasets solve with float64 factors");
+  if (p.beta_loss != CNMF_LOSS_FROBENIUS) return solve_batched_beta(h, v, io, p, s);
+  return solve_frobenius<F32Ops>(h, v, io, p, s);
+}
+
+int solve_batched(cnmf_handle_s* h, const DataView& v, SolveIO<double>& io, const cnmf_nmf_params& p, cudaStream_t s) {
+  CNMF_REQUIRE(v.form == Form::FP64 && v.X64, "solve: the float64 solver needs a float64 dataset");
+  CNMF_REQUIRE(p.beta_loss == CNMF_LOSS_FROBENIUS, "solve: float64 datasets support beta_loss = frobenius only");
+  return solve_frobenius<F64Ops>(h, v, io, p, s);
 }
 
 }  // namespace cnmf

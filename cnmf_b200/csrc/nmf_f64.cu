@@ -1,5 +1,6 @@
-// Batched NMF solver of float64 datasets (precision "fp64"): the Frobenius MU and CD iterations of nmf_engine.cu with
-// every value in fp64 -- factors, products, Grams, scalars -- as scikit-learn computes on the reference's float64 X.
+// Kernels and ops of the batched solve on float64 datasets (precision "fp64"): the Frobenius MU and CD iterations of
+// solve_frobenius (nmf_engine.cu) with every value in fp64 -- factors, products, Grams, scalars -- as scikit-learn
+// computes on the reference's float64 X.
 //
 // One outer iteration, all restarts together (packed slot layout of nmf_kernels.cuh, factors as doubles):
 //   NUM_r = Fc * X^T            gemm_f64 (DMMA), M = sum k, reduction over n_c in ascending K tiles
@@ -292,295 +293,55 @@ int fill_f64(double* p, double v, int rows, int n, int ld, cudaStream_t s) {
   return 0;
 }
 
-int solve_batched_f64(cnmf_handle_s* h, const DataView& v, SolveIO& io, const cnmf_nmf_params& p, cudaStream_t s) {
-  const int R0 = io.R;
-  CNMF_REQUIRE(v.form == Form::FP64 && v.X64, "solve: the float64 solver needs a float64 dataset");
-  CNMF_REQUIRE(p.beta_loss == CNMF_LOSS_FROBENIUS, "solve: float64 datasets support beta_loss = frobenius only");
-  CNMF_REQUIRE(R0 > 0 && (int)io.ks.size() == R0, "solve: bad restart list");
-  CNMF_REQUIRE(p.solver == CNMF_SOLVER_MU || p.solver == CNMF_SOLVER_CD, "solve: unknown solver");
-  CNMF_REQUIRE(p.max_iter >= 1, "solve: max_iter must be >= 1");
-  CNMF_REQUIRE(io.Fr64 && io.Fc64, "solve: float64 factors missing");
-  const bool mu = p.solver == CNMF_SOLVER_MU;
+F64Ops::F64Ops(FroSolve<double>& b_, const cnmf_nmf_params& p) : b(b_), cd(p.solver == CNMF_SOLVER_CD) {
+  l1[0] = p.l1_reg_W; l2[0] = p.l2_reg_W; l1[1] = p.l1_reg_H; l2[1] = p.l2_reg_H;
+  chunks[0] = f64_chunks(b.v.n_r);
+  chunks[1] = f64_chunks(b.v.n_c);
+  chunks_cap = std::max(chunks[0], chunks[1]);
+  gram_part_elems = (size_t)b.R0 * std::max(f64_gram_chunks(b.v.n_r), f64_gram_chunks(b.v.n_c)) * b.kp * b.kp;
+}
 
-  // ---- slot tables (host mirrors); slot s holds restart rid[s] at packed rows [off[s], off[s]+k[s])
-  std::vector<int> off0(R0), s_off(R0), s_k(io.ks), s_rid(R0);
-  int SK0 = 0, kmax = 0;
-  for (int r = 0; r < R0; ++r) {
-    CNMF_REQUIRE(io.ks[r] >= 1 && io.ks[r] <= KMAX, "solve: n_components must be in [1, 32] on the CUDA path");
-    off0[r] = s_off[r] = SK0;
-    s_rid[r] = r;
-    SK0 += io.ks[r];
-    kmax = std::max(kmax, io.ks[r]);
-  }
-  int R = R0, SK = SK0;
-  const int kp = round_up(kmax, 4);      // partial Gram stride kp * kp (finalize_kernel)
-  auto pack_offsets = [&](const std::vector<int>& kk, std::vector<int>& offs) -> int {
-    int pos = 0;
-    offs.clear();
-    for (int k : kk) {
-      offs.push_back(pos);
-      pos += k;
-    }
-    return pos;
-  };
-  const int chunks_r = f64_chunks(v.n_r), chunks_c = f64_chunks(v.n_c);
-  const int gchunks_r = f64_gram_chunks(v.n_r), gchunks_c = f64_gram_chunks(v.n_c);
-  const int chunks_cap = std::max(chunks_r, chunks_c), gchunks_cap = std::max(gchunks_r, gchunks_c);
+int F64Ops::alloc() {
+  b.NUM[0] = static_cast<double*>(b.h->dev_buf("solve.NUMr64", sizeof(double) * (size_t)b.SK0 * b.v.ld_r));
+  b.NUM[1] = b.io.update_cols ? static_cast<double*>(b.h->dev_buf("solve.NUMc64", sizeof(double) * (size_t)b.SK0 * b.v.ld_c))
+                              : nullptr;
+  return !b.NUM[0] || (b.io.update_cols && !b.NUM[1]) ? -2 : 0;
+}
 
-  // ---- workspace
-  int* d_meta = static_cast<int*>(h->dev_buf("solve.meta", sizeof(int) * 8 * R0));
-  double* d_state = static_cast<double*>(h->dev_buf("solve.state", sizeof(double) * 8 * R0));
-  double* d_gram = static_cast<double*>(h->dev_buf("solve.gram", sizeof(double) * 2 * R0 * KMAX * KMAX));
-  const size_t gpart_elems = (size_t)R0 * gchunks_cap * kp * kp;
-  double* d_gram_part = static_cast<double*>(h->dev_buf("solve.gram_part", sizeof(double) * 2 * gpart_elems));
-  double* d_scal_part = static_cast<double*>(h->dev_buf("solve.scal_part", sizeof(double) * 2 * (size_t)R0 * chunks_cap));
-  double* NUMr = static_cast<double*>(h->dev_buf("solve.NUMr64", sizeof(double) * (size_t)SK0 * v.ld_r));
-  double* NUMc = io.update_cols ? static_cast<double*>(h->dev_buf("solve.NUMc64", sizeof(double) * (size_t)SK0 * v.ld_c))
-                                : nullptr;
-  if (!d_meta || !d_state || !d_gram || !d_gram_part || !d_scal_part || !NUMr || (io.update_cols && !NUMc)) return -2;
+// NUM_r = Fc * X^T over the row items (reduction over n_c); NUM_c = Fr * X over the column items
+int F64Ops::gemm(int side) {
+  const DataView& v = b.v;
+  const bool rows = side == 0;
+  // untransposed: rows = cells, X^T products run over the genes (to_genes = false)
+  const bool to_genes = rows ? v.transposed : !v.transposed;
+  b.h->launches += 1;
+  const int slot = b.h->prof_begin(b.s, 2.0 * (double)b.SK * (double)v.n_r * (double)v.n_c, 4);
+  const int nrow_x = v.transposed ? v.n_c : v.n_r, ncol_x = v.transposed ? v.n_r : v.n_c;
+  const int ldx = v.transposed ? v.ld_r : v.ld_c;
+  const int rc = launch_gemm_f64(b.F[1 - side], b.ld(1 - side), b.SK, v.X64, nrow_x, ncol_x, ldx, to_genes, b.NUM[side],
+                                 b.ld(side), b.s);
+  b.h->prof_end(b.s, slot);
+  return rc;
+}
 
-  int* d_off = d_meta;
-  int* d_k = d_meta + R0;
-  int* d_rid = d_meta + 2 * R0;
-  int* d_done = d_meta + 3 * R0;
-  int* d_niter = d_meta + 4 * R0;
-  auto upload_slots = [&]() -> int {
-    std::vector<int> hm(3 * R0, 0);
-    std::memcpy(hm.data(), s_off.data(), sizeof(int) * R);
-    std::memcpy(hm.data() + R0, s_k.data(), sizeof(int) * R);
-    std::memcpy(hm.data() + 2 * R0, s_rid.data(), sizeof(int) * R);
-    CNMF_CUDA_CHECK(cudaMemcpyAsync(d_meta, hm.data(), sizeof(int) * 3 * R0, cudaMemcpyHostToDevice, s));
-    CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
-    return 0;
-  };
-  CNMF_TRY(upload_slots());
-  CNMF_CUDA_CHECK(cudaMemsetAsync(d_done, 0, sizeof(int) * 2 * R0, s));   // done, n_iter
-  CNMF_CUDA_CHECK(cudaMemsetAsync(d_state, 0, sizeof(double) * 8 * R0, s));
-  ConvState st{d_state, d_state + R0, d_state + 2 * R0, d_done, d_niter};
-  double* d_crossA = d_state + 3 * R0;
-  double* d_crossB = d_state + 4 * R0;
-  double* d_gramR = d_gram;
-  double* d_gramC = d_gram + (size_t)R0 * KMAX * KMAX;
-  double* d_scalA = d_scal_part;
-  double* d_scalB = d_scal_part + (size_t)R0 * chunks_cap;
-  double* d_gpartR = d_gram_part;
-  double* d_gpartC = d_gram_part + gpart_elems;
+int F64Ops::gram(int side, const BatchMeta& m) {
+  return f64_gram(F64Launch{b.h, b.s, b.SK}, F64View{b.F[side], b.n(side), b.ld(side)}, m, b.gram_part[side], b.gram[side]);
+}
 
-  double *wFr = io.Fr64, *wFc = io.Fc64;
-  double *aFr = nullptr, *aFc = nullptr, *resFr = nullptr, *resFc = nullptr;
-  bool compacted = false;
+int F64Ops::grams(const BatchMeta& m) {
+  CNMF_TRY(gram(0, m));
+  return gram(1, m);
+}
 
-  auto bm = [&]() { return BatchMeta{d_off, d_k, d_rid, d_done, R, kp}; };
-  auto fr = [&]() { return F64View{wFr, v.n_r, v.ld_r}; };
-  auto fc = [&]() { return F64View{wFc, v.n_c, v.ld_c}; };
+int F64Ops::cross(int side, const BatchMeta& m, double* out) {
+  return f64_cross(F64Launch{b.h, b.s, b.SK}, F64View{b.F[side], b.n(side), b.ld(side)}, b.NUM[side], m,
+                   b.scal_part[side], out);
+}
 
-  auto L = [&]() { return F64Launch{h, s, SK}; };
-
-  auto gram = [&](const F64View& f, int side_is_c, const BatchMeta& b) -> int {
-    return f64_gram(L(), f, b, side_is_c ? d_gpartC : d_gpartR, side_is_c ? d_gramC : d_gramR);
-  };
-  auto cross = [&](const F64View& f, const double* NUM, int side_is_c, double* out, const BatchMeta& b) -> int {
-    return f64_cross(L(), f, NUM, b, side_is_c ? d_scalB : d_scalA, out);
-  };
-  // update of one factor; scal (optional) receives MU <NUM, F_new> / CD sum |projected gradient| per restart
-  auto update = [&](const F64View& f, const double* NUM, int side_is_c, const double* gram_in, double l1, double l2,
-                    double* scal) -> int {
-    return f64_update(L(), !mu, f, NUM, gram_in, bm(), l1, l2, side_is_c ? d_scalB : d_scalA, scal);
-  };
-  // NUM_r = Fc * X^T over the row items (reduction over n_c); NUM_c = Fr * X over the column items
-  auto gemm = [&](bool rows) -> int {
-    const double* A = rows ? wFc : wFr;
-    const int lda = rows ? v.ld_c : v.ld_r;
-    double* C = rows ? NUMr : NUMc;
-    const int ldc = rows ? v.ld_r : v.ld_c;
-    // untransposed: rows = cells, X^T products run over the genes (to_genes = false)
-    const bool to_genes = rows ? v.transposed : !v.transposed;
-    h->launches += 1;
-    const int slot = h->prof_begin(s, 2.0 * (double)SK * (double)v.n_r * (double)v.n_c, 4);
-    const int nrow_x = v.transposed ? v.n_c : v.n_r, ncol_x = v.transposed ? v.n_r : v.n_c;
-    const int ldx = v.transposed ? v.ld_r : v.ld_c;
-    const int rc = launch_gemm_f64(A, lda, SK, v.X64, nrow_x, ncol_x, ldx, to_genes, C, ldc, s);
-    h->prof_end(s, slot);
-    return rc;
-  };
-
-  constexpr int GATHER_SLOTS = 12;
-  int* h_gidx = static_cast<int*>(h->host_buf("solve.gather_idx", sizeof(int) * 3 * (size_t)R0 * GATHER_SLOTS));
-  int* d_gidx = static_cast<int*>(h->dev_buf("solve.gather_didx", sizeof(int) * 3 * (size_t)R0 * GATHER_SLOTS));
-  if (!h_gidx || !d_gidx) return -2;
-  int gslot = 0;
-  // fp64 rows gathered as rows of 2 * ld floats: a bit copy
-  auto gather = [&](const double* src, double* dst, const std::vector<int>& so, const std::vector<int>& dof,
-                    const std::vector<int>& kk, int ld) -> int {
-    const int cnt = (int)kk.size();
-    if (cnt == 0) return 0;
-    if (gslot == GATHER_SLOTS) {
-      CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
-      gslot = 0;
-    }
-    int* hm = h_gidx + (size_t)gslot * 3 * R0;
-    int* dm = d_gidx + (size_t)gslot * 3 * R0;
-    ++gslot;
-    std::memcpy(hm, so.data(), sizeof(int) * cnt);
-    std::memcpy(hm + R0, dof.data(), sizeof(int) * cnt);
-    std::memcpy(hm + 2 * R0, kk.data(), sizeof(int) * cnt);
-    CNMF_CUDA_CHECK(cudaMemcpyAsync(dm, hm, sizeof(int) * 3 * R0, cudaMemcpyHostToDevice, s));
-    h->launches += 1;
-    return launch_gather_rows(reinterpret_cast<const float*>(src), dm, reinterpret_cast<float*>(dst), dm + R0, dm + 2 * R0,
-                              cnt, 2 * ld, s);
-  };
-
-  const double normX2 = v.sum_sq;
-  double* d_cd_err = d_state + 7 * R0;
-  // CD: ||X - Fr^T Fc||_F of the restarts still packed, in the trace form, into d_cd_err
-  auto cd_final_error = [&]() -> int {
-    int* d_zero = static_cast<int*>(h->dev_buf("solve.zero", sizeof(int) * 2 * R0));
-    if (!d_zero) return -2;
-    CNMF_CUDA_CHECK(cudaMemsetAsync(d_zero, 0, sizeof(int) * 2 * R0, s));
-    BatchMeta bm0{d_off, d_k, d_rid, d_zero, R, kp};
-    CNMF_TRY(gram(fr(), 0, bm0));
-    CNMF_TRY(gram(fc(), 1, bm0));
-    if (io.update_cols) CNMF_TRY(cross(fc(), NUMc, 1, d_crossB, bm0));
-    else CNMF_TRY(cross(fr(), NUMr, 0, d_crossB, bm0));
-    ConvState scratch{d_state + 5 * R0, d_state + 6 * R0, d_cd_err, d_zero, d_zero + R0};
-    h->launches += 1;
-    return launch_mu_check(scratch, d_crossB, d_gramR, d_gramC, normX2, bm0, 0, 0.0, p.max_iter, s);
-  };
-
-  std::vector<int> h_done(R0, 0);
-  // drop converged restarts from the packed arrays when that saves a 64-row GEMM tile (or >= 1/8 of the rows)
-  auto maybe_compact = [&]() -> int {
-    if (!io.update_cols) return 0;
-    std::vector<int> lk, lo;
-    for (int sl = 0; sl < R; ++sl)
-      if (!h_done[s_rid[sl]]) lk.push_back(s_k[sl]);
-    const int new_rows = pack_offsets(lk, lo);
-    if (new_rows == SK || new_rows == 0) return 0;
-    const bool saves_tile = (new_rows + 63) / 64 < (SK + 63) / 64;
-    if (!saves_tile && new_rows > SK - SK / 8) return 0;
-    if (!mu) CNMF_TRY(cd_final_error());    // restarts leaving the packed arrays get their ||X - WH||_F now
-    if (!aFr) {
-      const size_t nr = (size_t)SK0 * v.ld_r * 8, nc = (size_t)SK0 * v.ld_c * 8;
-      aFr = static_cast<double*>(h->dev_buf("solve.alt.Fr64", nr));
-      aFc = static_cast<double*>(h->dev_buf("solve.alt.Fc64", nc));
-      resFr = static_cast<double*>(h->dev_buf("solve.res.Fr64", nr));
-      resFc = static_cast<double*>(h->dev_buf("solve.res.Fc64", nc));
-      if (!aFr || !aFc || !resFr || !resFc) return -2;
-    }
-    std::vector<int> f_src, f_dst, f_k, l_src, l_dst, l_k, n_rid;
-    for (int sl = 0; sl < R; ++sl) {
-      const int rid = s_rid[sl];
-      if (h_done[rid]) {
-        f_src.push_back(s_off[sl]); f_dst.push_back(off0[rid]); f_k.push_back(s_k[sl]);
-      } else {
-        l_src.push_back(s_off[sl]); l_k.push_back(s_k[sl]); n_rid.push_back(rid);
-      }
-    }
-    const int pos = pack_offsets(l_k, l_dst);
-    CNMF_TRY(gather(wFr, resFr, f_src, f_dst, f_k, v.ld_r));
-    CNMF_TRY(gather(wFc, resFc, f_src, f_dst, f_k, v.ld_c));
-    CNMF_TRY(gather(wFr, aFr, l_src, l_dst, l_k, v.ld_r));
-    CNMF_TRY(gather(wFc, aFc, l_src, l_dst, l_k, v.ld_c));
-    std::swap(wFr, aFr);
-    std::swap(wFc, aFc);
-    R = (int)l_k.size();
-    SK = pos;
-    std::copy(l_dst.begin(), l_dst.end(), s_off.begin());
-    std::copy(l_k.begin(), l_k.end(), s_k.begin());
-    std::copy(n_rid.begin(), n_rid.end(), s_rid.begin());
-    CNMF_TRY(upload_slots());
-    gslot = 0;
-    compacted = true;
-    return 0;
-  };
-  auto poll_all_done = [&]() -> int {   // 1 = all done, 0 = not yet, <0 error
-    CNMF_CUDA_CHECK(cudaMemcpyAsync(h_done.data(), d_done, sizeof(int) * R0, cudaMemcpyDeviceToHost, s));
-    CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
-    for (int sl = 0; sl < R; ++sl)
-      if (!h_done[s_rid[sl]]) return maybe_compact();
-    return 1;
-  };
-
-  const double l1W = p.l1_reg_W, l2W = p.l2_reg_W, l1H = p.l1_reg_H, l2H = p.l2_reg_H;
-  if (mu) {
-    // ---------------- multiplicative update (sklearn _nmf.py:726-888) ----------------
-    CNMF_TRY(gram(fc(), 1, bm()));
-    CNMF_TRY(gram(fr(), 0, bm()));
-    if (io.update_cols) {
-      CNMF_TRY(gemm(false));
-      CNMF_TRY(cross(fc(), NUMc, 1, d_crossB, bm()));
-    } else {
-      CNMF_TRY(gemm(true));             // H fixed: X H^T is formed once (sklearn caches XHt, _nmf.py:537-548)
-      CNMF_TRY(cross(fr(), NUMr, 0, d_crossB, bm()));
-    }
-    h->launches += 1;
-    CNMF_TRY(launch_mu_check(st, d_crossB, d_gramR, d_gramC, normX2, bm(), 0, p.tol, p.max_iter, s));
-    for (int it = 1; it <= p.max_iter; ++it) {
-      const bool check = (p.tol > 0 && it % 10 == 0) || it == p.max_iter;
-      if (io.update_cols) {
-        CNMF_TRY(gemm(true));
-        CNMF_TRY(update(fr(), NUMr, 0, d_gramC, l1W, l2W, nullptr));
-        CNMF_TRY(gram(fr(), 0, bm()));
-        CNMF_TRY(gemm(false));
-        CNMF_TRY(update(fc(), NUMc, 1, d_gramR, l1H, l2H, check ? d_crossB : nullptr));
-        CNMF_TRY(gram(fc(), 1, bm()));
-      } else {
-        CNMF_TRY(update(fr(), NUMr, 0, d_gramC, l1W, l2W, check ? d_crossB : nullptr));
-        if (check) CNMF_TRY(gram(fr(), 0, bm()));
-      }
-      if (check) {
-        h->launches += 1;
-        const double tol_eff = (p.tol > 0 && it % 10 == 0) ? p.tol : -1.0;
-        CNMF_TRY(launch_mu_check(st, d_crossB, d_gramR, d_gramC, normX2, bm(), it, tol_eff, p.max_iter, s));
-        const int all = poll_all_done();
-        if (all < 0) return all;
-        if (all) break;
-      }
-    }
-  } else {
-    // ---------------- coordinate descent (sklearn _nmf.py:399-518, shuffle=False) ----------------
-    const int poll_every = 4;
-    for (int it = 1; it <= p.max_iter; ++it) {
-      if (it == 1) CNMF_TRY(gram(fc(), 1, bm()));
-      if (io.update_cols || it == 1) CNMF_TRY(gemm(true));
-      CNMF_TRY(update(fr(), NUMr, 0, d_gramC, l1W, l2W, d_crossA));
-      if (io.update_cols) {
-        CNMF_TRY(gram(fr(), 0, bm()));
-        CNMF_TRY(gemm(false));
-        CNMF_TRY(update(fc(), NUMc, 1, d_gramR, l1H, l2H, d_crossB));
-        CNMF_TRY(gram(fc(), 1, bm()));
-      }
-      h->launches += 1;
-      CNMF_TRY(launch_cd_check(st, d_crossA, io.update_cols ? d_crossB : nullptr, bm(), it, p.tol, p.max_iter, s));
-      if (it % poll_every == 0 || it == p.max_iter) {
-        const int all = poll_all_done();
-        if (all < 0) return all;
-        if (all) break;
-      }
-    }
-  }
-
-  double* d_err = st.last;
-  if (!mu) {
-    CNMF_TRY(cd_final_error());
-    d_err = d_cd_err;
-  }
-  if (compacted) {
-    std::vector<int> so(s_off.begin(), s_off.begin() + R), ko(s_k.begin(), s_k.begin() + R), dof(R);
-    for (int sl = 0; sl < R; ++sl) dof[sl] = off0[s_rid[sl]];
-    CNMF_TRY(gather(wFr, resFr, so, dof, ko, v.ld_r));
-    CNMF_TRY(gather(wFc, resFc, so, dof, ko, v.ld_c));
-    CNMF_CUDA_CHECK(cudaMemcpyAsync(io.Fr64, resFr, (size_t)SK0 * v.ld_r * 8, cudaMemcpyDeviceToDevice, s));
-    CNMF_CUDA_CHECK(cudaMemcpyAsync(io.Fc64, resFc, (size_t)SK0 * v.ld_c * 8, cudaMemcpyDeviceToDevice, s));
-  }
-  io.n_iter.assign(R0, 0);
-  io.last.assign(R0, 0.0);
-  io.err.assign(R0, 0.0);
-  CNMF_CUDA_CHECK(cudaMemcpyAsync(io.n_iter.data(), d_niter, sizeof(int) * R0, cudaMemcpyDeviceToHost, s));
-  CNMF_CUDA_CHECK(cudaMemcpyAsync(io.last.data(), st.last, sizeof(double) * R0, cudaMemcpyDeviceToHost, s));
-  CNMF_CUDA_CHECK(cudaMemcpyAsync(io.err.data(), d_err, sizeof(double) * R0, cudaMemcpyDeviceToHost, s));
-  CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
-  return 0;
+int F64Ops::update(int side, bool /* want_gram: the driver runs gram() after every update */, bool want_scal,
+                   double* scal) {
+  return f64_update(F64Launch{b.h, b.s, b.SK}, cd, F64View{b.F[side], b.n(side), b.ld(side)}, b.NUM[side],
+                    b.gram[1 - side], b.bm(), l1[side], l2[side], b.scal_part[side], want_scal ? scal : nullptr);
 }
 
 }  // namespace cnmf

@@ -1,8 +1,9 @@
-// Launches of the float64 solver (nmf_f64.cu), shared by solve_batched_f64 and the cnmf_update_step_f64_host test hook
-// (capi_units.cu), so that the hook runs exactly the launches the solver runs.
+// Launches of the float64 solver (nmf_f64.cu), shared by its ops in the batched solve (solve.h) and the
+// cnmf_update_step_f64_host test hook (capi_units.cu), so that the hook runs exactly the launches the solver runs.
 #pragma once
 #include "engine.h"
 #include "nmf_kernels.cuh"
+#include "solve.h"
 
 namespace cnmf {
 
@@ -33,5 +34,33 @@ int f64_cross(const F64Launch& L, const F64View& f, const double* NUM, const Bat
 // is its [rid][chunk] partials) receives MU <NUM, F_new> / CD sum |projected gradient| through finalize
 int f64_update(const F64Launch& L, bool cd, const F64View& f, const double* NUM, const double* gram_in,
                const BatchMeta& b, double l1, double l2, double* part, double* scal);
+
+// The FP64 ops of the batched solve: products through gemm_f64 (one slice), the update then a stand-alone Gram, block
+// plans fixed by the item counts, no operand pieces.  Compaction saves 64-row GEMM tiles.
+struct F64Ops {
+  using T = double;
+  static constexpr int tile_rows = 64;
+  static constexpr const char* buf_tag = "64";     // suffix of the workspace buffer names
+  static constexpr bool fused_gram = false;
+  static int pick_kp(int kmax) { return round_up(kmax, 4); }
+
+  FroSolve<double>& b;
+  bool cd;
+  double l1[2], l2[2];
+  int chunks[2];
+  int chunks_cap;            // partial scalars per restart and side
+  size_t gram_part_elems;    // Gram partials per side
+
+  F64Ops(FroSolve<double>& b, const cnmf_nmf_params& p);
+  int alloc();                                            // product buffers
+  int start() { return 0; }
+  int gemm(int side);                                     // NUM[side]
+  int gram(int side, const BatchMeta& m);                 // Gram of F[side]
+  int grams(const BatchMeta& m);                          // both Grams
+  int cross(int side, const BatchMeta& m, double* out);   // <NUM[side], F[side]>
+  int update(int side, bool want_gram, bool want_scal, double* scal);
+  int compact(const std::vector<int>&, const std::vector<int>&, const std::vector<int>&) { return 0; }
+  int repack() { return 0; }
+};
 
 }  // namespace cnmf

@@ -375,7 +375,7 @@ def mu_state(err0, prev, R=1):
 
 
 def mu_tol_eff(it, tol):
-    """what the solvers pass to mu_check_kernel at iteration it (nmf_f64.cu / nmf_engine.cu)"""
+    """what the batched solve passes to mu_check_kernel at iteration it (solve_frobenius, nmf_engine.cu)"""
     return tol if (tol > 0 and it % 10 == 0) else -1.0
 
 
