@@ -4,7 +4,7 @@
 // for the KL / IS solver (nmf_beta.cu), cnmf_update_step_f64_host for the float64 solver (nmf_f64.cu), and
 // cnmf_conv_check_host runs the convergence kernels every solver shares.  cnmf_dataset_form / cnmf_dataset_operand_host
 // read what dataset creation left resident, and cnmf_dataset_gemm_host runs one of the solver's products (view_gemm)
-// on a dataset.
+// on a dataset, or on a sparse one the transposed refit's product (stage_rows + csc_project).
 #include <algorithm>
 #include <vector>
 
@@ -441,8 +441,39 @@ extern "C" int cnmf_dataset_operand_host(cnmf_dataset_t d, int which, void* out_
 extern "C" int cnmf_dataset_gemm_host(cnmf_dataset_t d, int transposed, int side, int SK, const float* F_host,
                                       float* out_host, int* splits_out) {
   CNMF_REQUIRE(d && splits_out && (side == 0 || side == 1) && SK >= 1, "dataset_gemm: bad arguments");
-  CNMF_TRY(require_dense(d, "dataset_gemm"));
   cnmf_handle_s* h = d->h;
+  if (d->sparse) {
+    // the one product of the transposed refit on a CSC dataset, issued as cnmf_refit issues it: the factor in a zeroed
+    // SK x ld_c buffer, staged as rows (stage_rows), csc_project into a zeroed NUM_r at stride ld_r, one slice
+    if (!transposed || side != 0 || SK > KMAX) {
+      set_last_error("dataset_gemm: a sparse (CSC) dataset runs only the transposed refit's product (transposed = 1, "
+                     "side = 0, SK <= 32)");
+      return -3;
+    }
+    *splits_out = 1;
+    if (!out_host) return 0;
+    CNMF_REQUIRE(F_host, "dataset_gemm: NULL factor");
+    const DataView v = make_view(d, true);
+    cudaStream_t s = nullptr;
+    CNMF_CUDA_CHECK(cudaSetDevice(h->device));
+    const int kp = round_up(SK, 4);
+    const size_t nf = (size_t)SK * v.ld_c, nr = (size_t)SK * v.ld_r;
+    float* F = static_cast<float*>(h->dev_buf("unit.gemm_F", nf * 4));
+    float* U = static_cast<float*>(h->dev_buf("unit.gemm_U", (size_t)v.n_c * kp * 4));
+    float* NUM = static_cast<float*>(h->dev_buf("unit.gemm_C", nr * 4));
+    if (!F || !U || !NUM) return -2;
+    CNMF_CUDA_CHECK(cudaMemsetAsync(F, 0, nf * 4, s));
+    CNMF_CUDA_CHECK(cudaMemcpy2DAsync(F, (size_t)v.ld_c * 4, F_host, (size_t)v.n_c * 4, (size_t)v.n_c * 4, SK,
+                                      cudaMemcpyHostToDevice, s));
+    CNMF_CUDA_CHECK(cudaMemsetAsync(NUM, 0, nr * 4, s));
+    CNMF_TRY(stage_rows(h, F, SK, v.n_c, v.ld_c, kp, U, s));
+    CNMF_TRY(csc_project(d, U, SK, kp, NUM, v.ld_r, s));
+    CNMF_CUDA_CHECK(cudaMemcpy2DAsync(out_host, (size_t)v.n_r * 4, NUM, (size_t)v.ld_r * 4, (size_t)v.n_r * 4, SK,
+                                      cudaMemcpyDeviceToHost, s));
+    CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
+    return 0;
+  }
+  CNMF_TRY(require_dense(d, "dataset_gemm"));
   const DataView v = make_view(d, transposed != 0);
   const GemmPlan plan = view_gemm_plan(v, side, SK);
   *splits_out = plan.splits;

@@ -473,9 +473,13 @@ class Dataset:
         self.shape = (n.value, g.value)
 
     def close(self):
-        if self._d:
+        # cnmf_dataset_destroy hands the dataset's buffers back to its handle's pool, so it must not run once the
+        # handle is destroyed: it would write to freed host memory.  That happens after an explicit Engine.close, and
+        # when the garbage collector finalizes an Engine before a Dataset of the same reference cycle (a failed
+        # test's traceback holds both); the dataset's device memory then stays allocated until the process exits
+        if self._d and self.engine._h:
             self.lib.cnmf_dataset_destroy(self._d)
-            self._d = ctypes.c_void_p()
+        self._d = ctypes.c_void_p()
 
     def __del__(self):
         try:
@@ -610,7 +614,8 @@ class Dataset:
     def gemm(self, F, side, transposed=False):
         """Test hook: one of the solver's two products on this dataset's view, through the solver's own launch.
         side 0: F (SK x n_c of the view) @ B_rows^T; side 1: F (SK x n_r of the view) @ B_cols^T (untransposed:
-        n_r = cells, n_c = genes).  Returns the raw split-K slices, splits x SK x n_out (their sum is the product)."""
+        n_r = cells, n_c = genes).  Returns the raw split-K slices, splits x SK x n_out (their sum is the product).
+        Sparse datasets run the transposed refit's product only (transposed, side 0, SK <= 32; one slice)."""
         F = f32c(F)
         n_r, n_c = self.shape[::-1] if transposed else self.shape
         assert F.ndim == 2 and F.shape[1] == (n_c if side == 0 else n_r)

@@ -459,7 +459,9 @@ int cnmf_dataset_operand_host(cnmf_dataset_t d, int which, void* out_host, long 
  *   side 1: NUM_c = F * B_cols^T, F the row factor (SK x n_r of the view), out SK x n_c per slice
  * (untransposed: n_r = n_rows, n_c = n_cols).  F_host is dense row-major; out_host receives the raw split-K slices,
  * splits x SK x n_out, their sum being the product.  *splits_out = the number of slices; out_host may be NULL to ask
- * for it alone.  Dense float datasets only. */
+ * for it alone.  Dense float datasets, and sparse (CSC) ones for the one product their transposed refit runs
+ * (transposed = 1, side 0, SK <= 32): the factor staged as rows, then csc_project into the zeroed NUM_r, as cnmf_refit
+ * issues it, one slice; any other combination on a sparse dataset returns -3. */
 int cnmf_dataset_gemm_host(cnmf_dataset_t d, int transposed, int side, int SK, const float* F_host, float* out_host,
                            int* splits_out);
 

@@ -374,14 +374,22 @@ def test_products_scale_orientation(eng, precision):
 
 
 def test_products_need_a_dense_float_dataset(eng):
-    """The product hook refuses datasets the solver runs no tensor-core product on: float64 (gemm_f64 runs those) and
-    sparse (CSC) datasets."""
+    """The product hook refuses datasets the solver runs no tensor-core product on: float64 (gemm_f64 runs those), and
+    on sparse (CSC) datasets every product but the transposed refit's one (transposed, side 0, SK <= 32), which it runs
+    through csc_project in one slice."""
     from cnmf_b200._lib import CnmfError
     X = counts(np.random.RandomState(3), 40, 30)
-    F = np.ones((2, 30), np.float32)
-    for ds in (eng.dataset(X, "fp64"), make(eng, X, "tf32x3", "csc")):
-        with pytest.raises(CnmfError):
-            ds.gemm(F, 0)
+    with pytest.raises(CnmfError):
+        eng.dataset(X, "fp64").gemm(np.ones((2, 30), np.float32), 0)
+    ds = make(eng, X, "tf32x3", "csc")
+    for transposed, side, sk in ((False, 0, 2), (False, 1, 2), (True, 1, 2), (True, 0, 33)):
+        n_r, n_c = (30, 40) if transposed else (40, 30)
+        with pytest.raises(CnmfError, match="sparse"):
+            ds.gemm(np.ones((sk, n_c if side == 0 else n_r), np.float32), side, transposed)
+    F = np.random.RandomState(4).uniform(0.1, 1.0, (3, 40)).astype(np.float32)
+    sl = ds.gemm(F, 0, transposed=True)
+    assert sl.shape == (1, 3, 30)
+    assert np.allclose(sl[0], F.astype(np.float64) @ X, rtol=1e-6, atol=0)
 
 
 # ------------------------------------------------------------------------------------------------ row limits

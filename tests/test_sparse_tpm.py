@@ -86,7 +86,7 @@ def test_primitives_match_float64(eng, shape):
 
 
 @pytest.mark.parametrize("solver", ["mu", "cd"])
-@pytest.mark.parametrize("k", [1, 9, 32])
+@pytest.mark.parametrize("k", [1, 6, 9, 14, 19, 23, 27, 32])
 def test_transposed_refit_matches_oracle_and_dense(eng, solver, k):
     from oracle import nmf_ref
     T = ragged_csc(2500, 300, 0.08, 11, True)
@@ -99,10 +99,11 @@ def test_transposed_refit_matches_oracle_and_dense(eng, solver, k):
     Hr, itr = nmf_ref.refit(Td.T.astype(np.float64), W.T.astype(np.float64), solver, max_iter=400)
     assert it == itr and rel(Ht, Hr) < TOL_SPECTRA, (it, itr, rel(Ht, Hr))
     # the dense dataset's product runs as 2 f16 passes (fp32-class, ~2^-22 relative) where the sparse one is exact
-    # in fp64; with 32 components MU carries that rounding to 1.4e-6
+    # in fp64; the solve carries that rounding further the more components it has: measured on an H100, up to
+    # 9.2e-7 at k <= 9 and 1.2e-6 (k = 14) to 1.7e-6 (k = 32, CD) above
     dds = eng.dataset(Td)
     Htd, itd, _ = dds.refit(np.ascontiguousarray(W.T), kw, transposed=True)
-    assert itd == it and rel(Ht, Htd) < (2e-6 if k == 32 else 1e-6), (itd, it, rel(Ht, Htd))
+    assert itd == it and rel(Ht, Htd) < (2e-6 if k >= 14 else 1e-6), (itd, it, rel(Ht, Htd))
     sds.close()
     dds.close()
 
