@@ -25,6 +25,8 @@ namespace {
 constexpr int MOE_TILE = 64;      // apply kernel: 64 cells x 64 genes per block, 4 x 4 per thread
 constexpr int MOE_ROWS = 32;      // rows of P / W staged in shared memory per step
 constexpr int SEL_THREADS = 256;
+constexpr int MOM_LOADS = 12;     // column moments: rows each staging lane loads per step
+constexpr int MOM_ROWS = 7 * MOM_LOADS;   // rows of a 32-column strip staged per step by warps 1-7
 
 // split-K plan of the products over cells: slices of a fixed length that depends on N only
 int moe_chunk(int n) {
@@ -169,53 +171,66 @@ __global__ void moe_cos_kernel(const T* __restrict__ X, int ld, int N, int G, co
 
 // ---- variance scaling with a quantile ceiling
 
-// per column sum(x) and sum(x^2) in fp64 over the rows of one slice, fixed order
+// per column sum(x) and sum(x^2) in fp64, each one sequential chain in row order with every square rounded before it is
+// added: the order of numpy's axis-0 sum of a 2-D array, so that mean, mean(x^2) and the std that cancels between them
+// are the reference's bit for bit.  The chains of a 32-column strip run in warp 0 while warps 1-7 stage the next
+// MOM_ROWS rows of the strip in shared memory, each lane issuing all its MOM_LOADS loads before it stores any.
 template <typename T>
-__global__ void col_moments_kernel(const T* __restrict__ X, int ld, int N, int G, int rows_per_slice,
-                                   double* __restrict__ part) {
-  __shared__ double s1[8][33], s2[8][33];
-  const int c = blockIdx.x * 32 + threadIdx.x;
-  const int r0 = blockIdx.y * rows_per_slice, r1 = min(N, r0 + rows_per_slice);
-  double a = 0.0, q = 0.0;
-  if (c < G)
-    for (int r = r0 + threadIdx.y; r < r1; r += 8) {
-      const double v = (double)X[(long long)r * ld + c];
-      a += v;
-      q += v * v;
+__global__ void __launch_bounds__(256) col_moments_kernel(const T* __restrict__ X, int ld, int N, int G,
+                                                          double* __restrict__ sum, double* __restrict__ sumsq) {
+  __shared__ T tile[2][MOM_ROWS][32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int c = blockIdx.x * 32 + lane;
+  const int tiles = (N + MOM_ROWS - 1) / MOM_ROWS;
+  auto stage = [&](int t) {
+    T v[MOM_LOADS];
+#pragma unroll
+    for (int j = 0; j < MOM_LOADS; ++j) {
+      const int r = t * MOM_ROWS + (warp - 1) + 7 * j;
+      v[j] = (r < N && c < G) ? X[(long long)r * ld + c] : T(0);
     }
-  s1[threadIdx.y][threadIdx.x] = a;
-  s2[threadIdx.y][threadIdx.x] = q;
+#pragma unroll
+    for (int j = 0; j < MOM_LOADS; ++j) tile[t & 1][(warp - 1) + 7 * j][lane] = v[j];
+  };
+  if (warp > 0) stage(0);
   __syncthreads();
-  if (threadIdx.y == 0 && c < G) {
-    for (int y = 1; y < 8; ++y) {
-      a += s1[y][threadIdx.x];
-      q += s2[y][threadIdx.x];
+  double a = 0.0, q = 0.0;
+  for (int t = 0; t < tiles; ++t) {
+    if (warp > 0) {
+      if (t + 1 < tiles) stage(t + 1);
+    } else {
+      const int rn = min(MOM_ROWS, N - t * MOM_ROWS);
+      for (int r = 0; r < rn; ++r) {
+        const double v = (double)tile[t & 1][r][lane];
+        a = __dadd_rn(a, v);
+        q = __dadd_rn(q, __dmul_rn(v, v));
+      }
     }
-    part[(long long)blockIdx.y * 2 * G + c] = a;
-    part[(long long)blockIdx.y * 2 * G + G + c] = q;
+    __syncthreads();
+  }
+  if (warp == 0 && c < G) {
+    sum[c] = a;
+    sumsq[c] = q;
   }
 }
 
-// std of each column from the slice partials: ddof = 1, a zero std maps to 1
-__global__ void col_std_kernel(const double* __restrict__ part, int slices, int N, int G, double* __restrict__ sd) {
+// std of each column from its moments as the reference forms it, sqrt((msq - mean^2) * (N / (N - 1))) with every
+// operation rounded on its own (no contraction); a zero std maps to 1
+__global__ void col_std_kernel(const double* __restrict__ sum, const double* __restrict__ sumsq, int N, int G,
+                               double* __restrict__ sd) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= G) return;
-  double a = 0.0, q = 0.0;
-  for (int z = 0; z < slices; ++z) {
-    a += part[(long long)z * 2 * G + c];
-    q += part[(long long)z * 2 * G + G + c];
-  }
-  const double mean = a / N, msq = q / N;
-  double var = msq - mean * mean;
-  var *= (double)N / (double)(N - 1);
+  const double mean = sum[c] / (double)N, msq = sumsq[c] / (double)N;
+  const double var = __dmul_rn(__dsub_rn(msq, __dmul_rn(mean, mean)), (double)N / (double)(N - 1));
   double s = sqrt(var);
   if (s == 0.0) s = 1.0;
   sd[c] = s;
 }
 
+// X / std rounded to T, clipped at max_value; *nan_seen = 1 when a result is NaN
 template <typename T>
 __global__ void scale_clip_kernel(T* __restrict__ X, int ld, int N, int G, const double* __restrict__ sd, int clip,
-                                  double max_value) {
+                                  double max_value, int* __restrict__ nan_seen) {
   const long long total = (long long)N * G;
   for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total;
        e += (long long)gridDim.x * blockDim.x) {
@@ -223,6 +238,7 @@ __global__ void scale_clip_kernel(T* __restrict__ X, int ld, int N, int G, const
     const int c = (int)(e - r * G);
     T v = (T)((double)X[r * ld + c] / sd[c]);
     if (clip && (double)v > max_value) v = (T)max_value;
+    if (v != v) *nan_seen = 1;
     X[r * ld + c] = v;
   }
 }
@@ -442,37 +458,44 @@ int scale_quantile(cnmf_handle_s* h, const void* X, int N, int G, long long ld, 
                    long long k_lo, long long k_hi, double gamma, void* X_out, long long ld_out, int dst_is_device,
                    double* thresh_out, cudaStream_t s) {
   const int ldp = pad_ld(G);
-  const int rows_per_slice = 2048;
-  const int slices = (N + rows_per_slice - 1) / rows_per_slice;
-  DeviceTemp xb, part, sd, hist, csr;
+  DeviceTemp xb, mom, sd, hist, flag, csr;
   CNMF_TRY(xb.alloc((size_t)N * ldp * sizeof(T), "scale_quantile_ceiling X"));
-  CNMF_TRY(part.alloc((size_t)slices * 2 * G * 8, "scale_quantile_ceiling moments"));
+  CNMF_TRY(mom.alloc((size_t)2 * G * 8, "scale_quantile_ceiling moments"));
   CNMF_TRY(sd.alloc((size_t)G * 8, "scale_quantile_ceiling std"));
   CNMF_TRY(hist.alloc(256 * 8, "scale_quantile_ceiling histogram"));
+  CNMF_TRY(flag.alloc(sizeof(int), "scale_quantile_ceiling NaN flag"));
   T* Xd = xb.as<T>();
   CNMF_TRY(stage_matrix<T>(X, N, G, ld, src_is_device, csr_row_ptr, csr_col_idx, nnz, Xd, ldp, &csr, s));
-  col_moments_kernel<T><<<dim3((G + 31) / 32, slices), dim3(32, 8), 0, s>>>(Xd, ldp, N, G, rows_per_slice,
-                                                                            part.as<double>());
+  CNMF_CUDA_CHECK(cudaMemsetAsync(flag.p, 0, sizeof(int), s));
+  col_moments_kernel<T><<<(G + 31) / 32, 256, 0, s>>>(Xd, ldp, N, G, mom.as<double>(), mom.as<double>() + G);
   CNMF_CUDA_CHECK(cudaGetLastError());
-  col_std_kernel<<<(G + 255) / 256, 256, 0, s>>>(part.as<double>(), slices, N, G, sd.as<double>());
+  col_std_kernel<<<(G + 255) / 256, 256, 0, s>>>(mom.as<double>(), mom.as<double>() + G, N, G, sd.as<double>());
   CNMF_CUDA_CHECK(cudaGetLastError());
   const long long total = (long long)N * G;
   scale_clip_kernel<T><<<grid_for(total, 256, h->sm_count), 256, 0, s>>>(Xd, ldp, N, G, sd.as<double>(), clip,
-                                                                         max_value);
+                                                                         max_value, flag.as<int>());
   CNMF_CUDA_CHECK(cudaGetLastError());
   h->launches += 3;
   if (k_lo >= 0) {
     CNMF_REQUIRE(k_lo < total && k_hi >= k_lo && k_hi < total, "scale_quantile_ceiling: rank out of range");
-    T a, b;
-    auto* hd = hist.as<unsigned long long>();
-    CNMF_TRY(radix_select<T>(h, Xd, ldp, N, G, k_lo, hd, &a, s));
-    b = a;
-    if (k_hi != k_lo) CNMF_TRY(radix_select<T>(h, Xd, ldp, N, G, k_hi, hd, &b, s));
-    const T thresh = numpy_lerp<T>(a, b, (T)gamma);
-    if (thresh_out) *thresh_out = (double)thresh;
-    ceiling_kernel<T><<<grid_for(total, 256, h->sm_count), 256, 0, s>>>(Xd, ldp, N, G, thresh);
-    CNMF_CUDA_CHECK(cudaGetLastError());
-    h->launches += 1;
+    int nan_seen = 0;
+    CNMF_CUDA_CHECK(cudaMemcpyAsync(&nan_seen, flag.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+    CNMF_CUDA_CHECK(cudaStreamSynchronize(s));
+    if (nan_seen) {
+      // np.quantile of values that include a NaN is NaN, and nothing compares above NaN: X stays as scaled
+      if (thresh_out) *thresh_out = std::nan("");
+    } else {
+      T a, b;
+      auto* hd = hist.as<unsigned long long>();
+      CNMF_TRY(radix_select<T>(h, Xd, ldp, N, G, k_lo, hd, &a, s));
+      b = a;
+      if (k_hi != k_lo) CNMF_TRY(radix_select<T>(h, Xd, ldp, N, G, k_hi, hd, &b, s));
+      const T thresh = numpy_lerp<T>(a, b, (T)gamma);
+      if (thresh_out) *thresh_out = (double)thresh;
+      ceiling_kernel<T><<<grid_for(total, 256, h->sm_count), 256, 0, s>>>(Xd, ldp, N, G, thresh);
+      CNMF_CUDA_CHECK(cudaGetLastError());
+      h->launches += 1;
+    }
   }
   CNMF_TRY(copy_out<T>(Xd, ldp, N, G, X_out, ld_out, dst_is_device, s));
   CNMF_CUDA_CHECK(cudaStreamSynchronize(s));

@@ -573,7 +573,8 @@ int cnmf_moe_correct(cnmf_handle_t h, const void* X, int dtype, int n_cells, int
                      double* W_last, void* stream);
 /* stdscale_quantile_celing: X / std per column (ddof = 1, a zero std maps to 1, the division in fp64 rounded to the
  * element type), clipped at max_value when clip != 0; then, when k_lo >= 0, every value above the quantile threshold
- * is set to it.  The threshold is numpy's linear-method lerp in the element type of the values of ranks k_lo and k_hi
+ * is set to it.  The moments are summed in row order (numpy's axis-0 order), so that the std is the reference's bit
+ * for bit.  A NaN anywhere in the scaled matrix makes the threshold NaN and leaves the matrix as scaled.  The threshold is numpy's linear-method lerp in the element type of the values of ranks k_lo and k_hi
  * (ascending over all n_rows * n_cols entries, found exactly by a radix select on the float bits) with weight gamma;
  * the caller derives k_lo, k_hi and gamma from the quantile as np.quantile does.  thresh_out (optional) receives it.
  * csr_row_ptr != NULL: X is the values array (nnz) of a host CSR matrix (csr_row_ptr: n_rows + 1 entries from 0,
